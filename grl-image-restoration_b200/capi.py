@@ -11,7 +11,7 @@ _PKG = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_PKG, "libgrl_b200.so")
 HEADER_PATH = os.path.join(os.path.dirname(_PKG), "include", "grl_b200.h")
 
-ABI_VERSION = 3
+ABI_VERSION = 4
 c_int, c_i64, c_f32, c_vp, c_sz = ctypes.c_int, ctypes.c_int64, ctypes.c_float, ctypes.c_void_p, ctypes.c_size_t
 
 
@@ -79,6 +79,9 @@ _SIGNATURES = {
     "grl_stripe_attn_workspace": (c_sz, [c_int, GrlGrid, GrlGrid, c_int, c_int]),
     "grl_stripe_attn_f32": (c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_int, GrlGrid, GrlGrid, c_int, c_int,
                                     c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_sz, c_vp]),
+    "grl_d8_index_host": (c_int, [c_int, c_int, c_int, c_int, c_vp]),
+    "grl_ens_gather_f32": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp]),
+    "grl_ens_merge_f32": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp]),
 }
 
 _lib = None

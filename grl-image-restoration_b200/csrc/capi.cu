@@ -328,4 +328,33 @@ int grl_psnr_f32(const float* restored, const float* target, int B, int C, int H
                      (cudaStream_t)stream);
 }
 
+// ---------------------------------------------------------------- x8 self-ensemble
+int grl_d8_index_host(int mode, int H, int W, int inverse, int32_t* out) {
+  GRL_REQUIRE(mode >= 0 && mode < 8 && H > 0 && W > 0 && (long long)H * W <= 0x7fffffffLL && out,
+              "d8_index: bad arguments mode=%d H=%d W=%d", mode, H, W);
+  const int Hv = d8_transposes(mode) ? W : H, Wv = d8_transposes(mode) ? H : W;
+  if (!inverse) {
+    for (int y = 0; y < Hv; ++y)
+      for (int x = 0; x < Wv; ++x) {
+        const Pix p = d8_src(mode, y, x, H, W);
+        out[(size_t)y * Wv + x] = p.y * W + p.x;
+      }
+  } else {
+    for (int y = 0; y < H; ++y)
+      for (int x = 0; x < W; ++x) {
+        const Pix p = d8_inv(mode, y, x, H, W);
+        out[(size_t)y * W + x] = p.y * Wv + p.x;
+      }
+  }
+  return GRL_OK;
+}
+
+int grl_ens_gather_f32(const float* x, int B, int C, int H, int W, int group, float* views, void* stream) {
+  return launch_ens_gather(x, B, C, H, W, group, views, (cudaStream_t)stream);
+}
+
+int grl_ens_merge_f32(const float* ya, const float* yb, int B, int C, int Hs, int Ws, float* y, void* stream) {
+  return launch_ens_merge(ya, yb, B, C, Hs, Ws, y, (cudaStream_t)stream);
+}
+
 }  // extern "C"

@@ -56,4 +56,25 @@ GRL_HD int rel_index(int qh, int qw, int kh, int kw, int qww, int kwh, int kww) 
 
 GRL_HD int windows_per_image(const GrlGrid& g) { return (g.H / g.wh) * (g.W / g.ww); }
 
+// The 8 dihedral views of augment_img_tensor4 (utils/utils_bsr/utils_image.py:444-460) as closed forms.  The mode's
+// bits are: 1 = transpose (the view is W x H), 2 = flip the source rows, 4 = flip the source columns:
+//   0 identity, 1 transpose, 2 flip(H), 3 rot90 k=3, 4 flip(W), 5 rot90 k=1, 6 rot180, 7 anti-transpose.
+struct Pix {
+  int y, x;
+};
+GRL_HD bool d8_transposes(int mode) { return (mode & 1) != 0; }
+
+// Source pixel in the (H x W) image of position (y, x) of view `mode` (which is H x W, or W x H when it transposes).
+GRL_HD Pix d8_src(int mode, int y, int x, int H, int W) {
+  const int r = (mode & 1) ? x : y, c = (mode & 1) ? y : x;
+  return {(mode & 2) ? H - 1 - r : r, (mode & 4) ? W - 1 - c : c};
+}
+
+// The way back: position in view `mode` of pixel (y, x) of the (H x W) image, i.e. d8_src(mode, .)^-1.  Every mode but 3
+// and 5 is its own inverse; for those two this is view 8 - mode applied to the view.
+GRL_HD Pix d8_inv(int mode, int y, int x, int H, int W) {
+  const int r = (mode & 2) ? H - 1 - y : y, c = (mode & 4) ? W - 1 - x : x;
+  return (mode & 1) ? Pix{c, r} : Pix{r, c};
+}
+
 }  // namespace grl

@@ -65,5 +65,8 @@ int launch_attn(const AttnArgs& a, cudaStream_t st);
 // fused tensor_round + shave + squared-error reduction (RGB and luma) -> per-image PSNR (metric.cu)
 int launch_psnr(const float* restored, const float* target, int B, int C, int H, int W, int border,
                 unsigned long long* workspace, float* psnr_rgb, float* psnr_y, cudaStream_t st);
+// x8 self-ensemble: the 4 views of one group, and the ordered average of the 8 mapped-back outputs (ensemble.cu)
+int launch_ens_gather(const float* x, int B, int C, int H, int W, int group, float* views, cudaStream_t st);
+int launch_ens_merge(const float* ya, const float* yb, int B, int C, int Hs, int Ws, float* y, cudaStream_t st);
 
 }  // namespace grl

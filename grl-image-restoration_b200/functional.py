@@ -153,6 +153,44 @@ def window_attention(qkv, B, grid, heads, logit_scale, bias, use_mask, out=None)
     return out
 
 
+def d8_index(mode, H, W, inverse=False):
+    """Host expansion of the self-ensemble's view maps (CPU, no device needed).  inverse=False: (H', W') int32 flat
+    source index y*W + x of every position of view `mode` = augment_img_tensor4(., mode) of an (H, W) image; inverse=True:
+    (H, W) int32 flat index into the (H', W') view of every image pixel."""
+    Hv, Wv = (W, H) if mode & 1 else (H, W)
+    out = torch.empty((H, W) if inverse else (Hv, Wv), dtype=torch.int32)
+    capi.check(capi.lib().grl_d8_index_host(int(mode), int(H), int(W), int(bool(inverse)),
+                                            ctypes.c_void_p(out.data_ptr())))
+    return out
+
+
+def ens_gather(x, group, out=None):
+    """x (B, C, H, W) fp32 -> the 4 views augment_img_tensor4(x, 2*i + group), i = 0..3, as (4B, C, H', W') view-major
+    (index i*B + b); (H', W') = (W, H) for group 1."""
+    x = _f32c(x, "x")
+    B, C, H, W = x.shape
+    shape = (4 * B, C) + ((W, H) if group else (H, W))
+    if out is None:
+        out = torch.empty(shape, device=x.device, dtype=torch.float32)
+    elif tuple(out.shape) != shape or out.dtype != torch.float32 or not out.is_contiguous():
+        raise RuntimeError(f"grl_b200: ens_gather output must be contiguous float32 {shape}")
+    capi.check(capi.lib().grl_ens_gather_f32(capi.ptr(x), B, C, H, W, int(group), capi.ptr(out), capi.stream()))
+    return out
+
+
+def ens_merge(ya, yb, B):
+    """Self-ensemble average: ya (4B, C, Hs, Ws) outputs of views 0, 2, 4, 6 and yb (4B, C, Ws, Hs) of views 1, 3, 5, 7
+    -> (B, C, Hs, Ws) = 0.125 * (V_0 + ... + V_7) in mode order, V_m = view m's output mapped back."""
+    ya, yb = _f32c(ya, "ya"), _f32c(yb, "yb")
+    n, C, Hs, Ws = ya.shape
+    if n != 4 * B or tuple(yb.shape) != (n, C, Ws, Hs):
+        raise RuntimeError(f"grl_b200: ens_merge needs (4B, C, Hs, Ws) and (4B, C, Ws, Hs) view outputs, got "
+                           f"{tuple(ya.shape)} / {tuple(yb.shape)} for B={B}")
+    y = torch.empty(B, C, Hs, Ws, device=ya.device, dtype=torch.float32)
+    capi.check(capi.lib().grl_ens_merge_f32(capi.ptr(ya), capi.ptr(yb), B, C, Hs, Ws, capi.ptr(y), capi.stream()))
+    return y
+
+
 def stripe_attention(qkv, anchor, B, tok_grid, anc_grid, heads, scale1, bias1, scale2, bias2, use_mask, out=None):
     """qkv (B, L, 3c) view (stripe half), anchor (B, Ha, Wa, c) -> (B, L, c)."""
     qp, ldq = _token_rows(qkv, "qkv")

@@ -552,8 +552,12 @@ class GRL(nn.Module):
                  anchor_one_stage=True, anchor_window_down_factor=1, out_proj_type="linear", local_connection=False,
                  drop_rate=0.0, attn_drop_rate=0.0, drop_path_rate=0.1, norm_layer=nn.LayerNorm,
                  pretrained_window_size=[0, 0], pretrained_stripe_size=[0, 0], conv_type="1conv", init_method="n",
-                 fairscale_checkpoint=False, offload_to_cpu=False, euclidean_dist=False, **kwargs):
+                 fairscale_checkpoint=False, offload_to_cpu=False, euclidean_dist=False, self_ensemble=False, **kwargs):
         super().__init__()
+        # x8 geometric self-ensemble in forward (off: the reference's forward).  Views are forwarded in chunks of at most
+        # ensemble_max_batch images, which bounds the activation memory of the 8x larger batch.
+        self.self_ensemble = bool(self_ensemble)
+        self.ensemble_max_batch = 16
         self._requested_precision = kwargs.pop("precision", None) or os.environ.get("GRL_B200_PRECISION", "fp32")
         out_channels = out_channels or in_channels
         self.in_channels, self.out_channels = in_channels, out_channels
@@ -880,6 +884,34 @@ class GRL(nn.Module):
     @torch.no_grad()
     def forward(self, x):
         K.capi.require_device(x)
+        return self._forward_self_ensemble(x) if self.self_ensemble else self._forward_once(x)
+
+    @torch.no_grad()
+    def _forward_self_ensemble(self, x):
+        """y = 0.125 * (V_0 + ... + V_7), V_m = inverse_m(forward(augment_img_tensor4(x, m))) (utils/utils_bsr/
+        utils_image.py:444-460): 8 independent forwards, each with its own padding, on the views gathered by one kernel
+        per group.  Group A (modes 0, 2, 4, 6) keeps (H, W) and goes first, group B (the transposed modes) follows; when
+        H == W both groups share one view batch.  Each forward takes at most ensemble_max_batch views."""
+        xin = x.float().contiguous()
+        B, C, H, W = xin.shape
+        if H == W:
+            views = torch.empty(8 * B, C, H, W, device=xin.device, dtype=torch.float32)
+            K.ens_gather(xin, 0, out=views[: 4 * B])
+            K.ens_gather(xin, 1, out=views[4 * B:])
+            y = self._forward_chunks(views)
+            ya, yb = y[: 4 * B], y[4 * B:]
+        else:
+            ya = self._forward_chunks(K.ens_gather(xin, 0))
+            yb = self._forward_chunks(K.ens_gather(xin, 1))
+        return K.ens_merge(ya, yb, B).to(x.dtype)
+
+    def _forward_chunks(self, views):
+        n = max(1, int(self.ensemble_max_batch))
+        outs = [self._forward_once(views[i:i + n]) for i in range(0, views.shape[0], n)]
+        return outs[0] if len(outs) == 1 else torch.cat(outs)
+
+    @torch.no_grad()
+    def _forward_once(self, x):
         H, W = x.shape[2:]
         if self.precision != "fp32":
             xin = x.float().contiguous()

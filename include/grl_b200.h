@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define GRL_B200_ABI_VERSION 3
+#define GRL_B200_ABI_VERSION 4
 
 typedef enum {
   GRL_OK = 0,
@@ -261,6 +261,21 @@ int grl_tc_attn_variant(int variant);
  * geometry.  workspace: 16 * B bytes of device memory (zeroed by the call). */
 int grl_psnr_f32(const float* restored, const float* target, int B, int C, int H, int W, int border, void* workspace,
                  size_t workspace_bytes, float* psnr_rgb, float* psnr_y, void* stream);
+
+/* ---- x8 self-ensemble (geometric test-time augmentation) ----------------------------------------
+ * The 8 views are augment_img_tensor4(img, mode) (utils/utils_bsr/utils_image.py:444-460).  Group A = modes 0, 2, 4, 6
+ * (the view keeps (H, W)), group B = modes 1, 3, 5, 7 (the view is (W, H)); inside a group view i is mode 2*i + group. */
+/* Host expansion of the view maps: inverse == 0: out (H', W') int32 = flat index sy*W + sx of the source pixel of every
+ * view position ((H', W') = (W, H) for group B); inverse != 0: out (H, W) int32 = flat index py*W' + px of the view
+ * position that holds each image pixel (the map that undoes the view). */
+int grl_d8_index_host(int mode, int H, int W, int inverse, int32_t* out);
+/* augment_img_tensor4(x, mode) for the 4 modes of one group in one pass: x (B, C, H, W) fp32 -> views (4B, C, H', W'),
+ * view-major (view i of image b is index i*B + b). */
+int grl_ens_gather_f32(const float* x, int B, int C, int H, int W, int group, float* views, void* stream);
+/* The self-ensemble average: y[b] = 0.125 * (V_0 + V_1 + ... + V_7), summed in mode order in fp32, where V_m is view m's
+ * network output mapped back by the inverse of augment_img_tensor4(., m).  ya: group A outputs (4B, C, Hs, Ws); yb: group B
+ * outputs (4B, C, Ws, Hs), both view-major (they may be the two halves of one tensor when Hs == Ws); y (B, C, Hs, Ws). */
+int grl_ens_merge_f32(const float* ya, const float* yb, int B, int C, int Hs, int Ws, float* y, void* stream);
 
 #ifdef __cplusplus
 }
