@@ -514,13 +514,21 @@ def synth_state_dict(cfg, seed=0, style="spread"):
     affine, and logit_scale spread over [ln 5, ln 150] so the clamp at ln 100 is exercised -- a deliberately harsh,
     near-chaotic network.  style "init": the distribution the reference's own constructor produces
     (grl.py:455-462: Linear ~ trunc_normal(std 0.02) with zero bias, LayerNorm identity, logit_scale = ln 10,
-    Conv2d = PyTorch's default kaiming-uniform), i.e. what an untrained reference model computes."""
+    Conv2d = PyTorch's default kaiming-uniform), i.e. what an untrained reference model computes.
+    style "routed": "init" with every parameter that routes per head or per row made distinct, so that a swapped,
+    misordered or dropped one changes the output: per-head logit_scale over [ln 5, ln 150] (a different draw for the
+    window, stripe-1 and stripe-2 transforms), cpb_mlp weights as in "spread" plus a random cpb_mlp.0.bias, Linear
+    biases ~ N(0, 0.02), LayerNorm weight 1 + 0.1 N and bias 0.02 N (cpb_mlp.0.bias: 0.1 N).  The overrides draw from a
+    second per-name generator, so "init" and "spread" are unchanged."""
     import zlib
 
+    if style not in ("spread", "init", "routed"):
+        raise ValueError(f"unknown weight style {style!r}")
     sd = {}
     for name, shape in sorted(param_shapes(cfg).items()):
         g = torch.Generator().manual_seed((zlib.crc32(name.encode()) + 7919 * seed) % (2 ** 31))
-        if style == "init":
+        if style in ("init", "routed"):
+            linear_bias = False
             if name.endswith("logit_scale"):
                 v = torch.full(shape, log(10.0))
             elif ".norm" in name or name.startswith("norm_"):
@@ -532,8 +540,21 @@ def synth_state_dict(cfg, seed=0, style="spread"):
                 v = (torch.rand(shape, generator=g) * 2 - 1) * bound
             elif name.endswith("bias"):
                 v = torch.zeros(shape)
+                linear_bias = True
             else:
                 v = torch.nn.init.trunc_normal_(torch.empty(shape), std=0.02, generator=g)
+            if style == "routed":
+                r = torch.Generator().manual_seed((zlib.crc32(name.encode()) + 7919 * seed + 104729) % (2 ** 31))
+                if name.endswith("logit_scale"):
+                    v = log(5.0) + (log(150.0) - log(5.0)) * torch.rand(shape, generator=r)
+                elif "cpb_mlp" in name:
+                    v = torch.randn(shape, generator=r) * (0.7 if name.endswith("0.weight") else
+                                                           0.15 if name.endswith("2.weight") else 0.1)
+                elif ".norm" in name or name.startswith("norm_"):
+                    v = (1.0 + 0.1 * torch.randn(shape, generator=r)) if name.endswith("weight") else \
+                        0.02 * torch.randn(shape, generator=r)
+                elif linear_bias:
+                    v = 0.02 * torch.randn(shape, generator=r)
             sd[name] = v.float()
             continue
         if name.endswith("logit_scale"):

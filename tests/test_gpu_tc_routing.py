@@ -1,0 +1,199 @@
+"""Parameter routing of the tensor-core path, gated on weights that expose it.
+
+Under the constructor-distributed "init" weights every logit_scale is ln 10, every Linear bias is zero, every LayerNorm is
+the identity and the activated position-bias tables are ~8 everywhere, so a swapped logit scale, a misrouted bias table
+or a dropped bias row leaves the output unchanged.  These gates run on style "routed" (oracle.synth_state_dict: "init"
+with distinct per-head logit scales, "spread"-like cpb_mlp weights and nonzero Linear biases / LayerNorm affine), against
+the fp32 path of the same module, and prove they can see routing errors: each mutation control edits one parameter
+group of a deep copy (Python-side only, never a kernel) in the way a routing bug would misuse it, and the copy's
+tensor-core output must fail the gate against the UNMUTATED fp32 output.
+
+Gates, chosen from one measurement on an H100 80GB HBM3 (400 W power limit; the kernels are deterministic, so a rerun
+gives the same numbers) with the rule: unmutated worst case <= G / 4 (block) or >= G + 6 dB (network), every mutation
+>= 4 G or <= G - 6 dB.
+  block:   e = rms(y_tc - y_fp32) / rms(y_fp32 - x), i.e. relative to the block's update rather than to the residual.
+           fp16: unmutated <= 1.8e-3, mutations >= 5.0e-2  ->  G_BLK = 1e-2.
+  network: PSNR(y_tc, y_fp32) per configuration and operand format (G_NET).  One gate cannot serve every configuration:
+           micro_odd_d's mutations land at 52-66 dB (its blocks contribute little to the output) while small_dn_128's
+           unmutated fp16 output is at 62 dB.  bf16 misses the 6 dB margin on cfg1_tiny_x2_64 (unmutated 44.3 dB, worst
+           mutation 32.5 dB: gate 38.5) and micro_gray (54.5 / 44.1 dB: gate 49.5); every mutation still fails its gate.
+"""
+import copy
+
+import pytest
+import torch
+
+pytestmark = pytest.mark.gpu
+
+G_BLK = 1e-2
+G_NET = {  # case: {format: gate in dB}; measured (unmutated / worst mutation) fp16 | bf16
+    "cfg1_tiny_x2_64": {"fp16": 47.0, "bf16": 38.5},  # 62.7 / 32.6 | 44.3 / 32.5
+    "micro_cab_x2": {"fp16": 66.0, "bf16": 57.5},     # 81.8 / 50.9 | 64.5 / 50.8
+    "micro_pad_dn": {"fp16": 52.0, "bf16": 44.0},     # 67.1 / 37.1 | 50.8 / 36.9
+    "micro_groups": {"fp16": 50.0, "bf16": 42.5},     # 68.4 / 32.9 | 52.3 / 32.7
+    "micro_odd_d": {"fp16": 81.0, "bf16": 71.5},      # 96.3 / 65.5 | 77.8 / 65.2
+    "micro_gray": {"fp16": 60.0, "bf16": 49.5},       # 74.3 / 45.0 | 54.5 / 44.1
+    "small_sr4_64": {"fp16": 63.0, "bf16": 54.0},     # 79.4 / 47.2 | 60.7 / 47.2
+    "small_dn_128": {"fp16": 45.0, "bf16": 34.5},     # 62.1 / 28.5 | 41.0 / 28.2
+}
+
+
+def _swap(a, b):
+    t = a.detach().clone()
+    a.copy_(b)
+    b.copy_(t)
+
+
+def _mut_swap_stripe_scales(blk):
+    sa = blk.attn.stripe_attn
+    _swap(sa.attn_transform1.logit_scale, sa.attn_transform2.logit_scale)
+
+
+def _mut_roll_window_scale(blk):
+    ls = blk.attn.window_attn.attn_transform.logit_scale
+    if ls.shape[0] < 2:
+        return False
+    ls.copy_(torch.roll(ls.detach().clone(), 1, 0))
+
+
+def _mut_swap_stripe_cpb(blk):
+    sa = blk.attn.stripe_attn
+    for p, q in zip(sa.attn_transform1.cpb_mlp.parameters(), sa.attn_transform2.cpb_mlp.parameters()):
+        _swap(p, q)
+
+
+def _mut_mirror_window_dy(blk):
+    blk.attn.window_attn.attn_transform.cpb_mlp[0].weight[:, 0].neg_()
+
+
+def _mut_zero(getter):
+    def f(blk):
+        getter(blk).zero_()
+    return f
+
+
+def _mut_norm1_identity(blk):
+    blk.norm1.weight.fill_(1.0)
+    blk.norm1.bias.zero_()
+
+
+MUTATIONS = {  # name -> in-place edit of one block's parameters (returns False where it cannot change anything)
+    "a_swap_stripe_logit_scale": _mut_swap_stripe_scales,
+    "b_roll_window_logit_scale": _mut_roll_window_scale,
+    "c_swap_stripe_cpb_mlp": _mut_swap_stripe_cpb,
+    "d_mirror_window_cpb_dy": _mut_mirror_window_dy,
+    "e_zero_qkv_bias": _mut_zero(lambda b: b.attn.qkv.body.bias),
+    "f_zero_anchor_bias": _mut_zero(lambda b: b.attn.anchor.body[0].reduction.bias),
+    "g_zero_proj_bias": _mut_zero(lambda b: b.attn.proj.bias),
+    "h_norm1_identity": _mut_norm1_identity,
+}
+
+
+@torch.no_grad()
+def mutate(module, name):
+    """Applies mutation `name` to every transformer block of `module` (a block or a network); False if it changed nothing."""
+    blocks = [module] if hasattr(module, "norm1") else [b for layer in module.layers for b in layer.blocks]
+    return any(MUTATIONS[name](b) is not False for b in blocks)
+
+
+def build(pkg, oracle, cfg, device, style, seed=0):
+    m = pkg.GRL(**cfg)
+    m.load_state_dict(oracle.synth_state_dict(cfg, seed=seed, style=style), strict=False)
+    return m.to(device).eval()
+
+
+# (name, config, block input size): micro_cab_x2 at the size of its stored reference taps; GRL-Small (C 128, head_dim 32)
+# and GRL-Base (C 180, head_dim 30: the ones-column path), blocks 0 and 1 (no shift / shifted, both stripe directions)
+def block_cases(pkg, cases):
+    return [("micro_cab_x2", cases["micro_cab_x2"]["cfg"], (16, 32)),
+            ("small_sr4", pkg.configs.grl_config("small", "sr", 4, 64), (64, 64)),
+            ("base_sr4", pkg.configs.grl_config("base", "sr", 4, 64), (64, 64))]
+
+
+def block_errors(pkg, oracle, cfg, hw, device, style, block_ids, x=None, precision="fp16", mutations=MUTATIONS):
+    """{block: {"unmutated": e, mutation: e}} with e = rms(y_tc - y_fp32) / rms(y_fp32 - x), y_fp32 always unmutated."""
+    m = build(pkg, oracle, cfg, device, style)
+    C = cfg["embed_dim"]
+    if x is None:
+        x = torch.randn(1, hw[0] * hw[1], C, generator=torch.Generator().manual_seed(11))
+    x = x.to(device)
+    tim = m.get_table_index_mask(device, hw)
+    out = {}
+    for bi in block_ids:
+        blk = m.layers[0].blocks[bi]
+        m.set_precision("fp32")
+        y32 = blk(x, hw, tim)
+        upd = (y32 - x).pow(2).mean().sqrt().item()
+        m.set_precision(precision)
+        e = {"unmutated": (blk(x, hw, tim) - y32).pow(2).mean().sqrt().item() / upd}
+        for name in mutations:
+            mb = copy.deepcopy(blk)
+            if mutate(mb, name):
+                e[name] = (mb(x, hw, tim) - y32).pow(2).mean().sqrt().item() / upd
+        out[bi] = (e, y32)
+    return out
+
+
+def net_cases(pkg, cases):
+    out = [(n, c["cfg"], c["batch"], tuple(c["hw"]), c["sigma"]) for n, c in cases.items()]
+    out.append(("small_sr4_64", pkg.configs.grl_config("small", "sr", 4, 64), 1, (64, 64), 0.0))
+    out.append(("small_dn_128", pkg.configs.grl_config("small", "dn", 1, 128), 1, (100, 120), 50.0))
+    return out
+
+
+def psnr(a, b):
+    return (-10 * torch.log10(((a - b) ** 2).mean())).item()
+
+
+def net_psnrs(pkg, oracle, cfg, batch, hw, sigma, device, style, precision, mutations=MUTATIONS):
+    m = build(pkg, oracle, cfg, device, style)
+    x = oracle.synth_input((batch, cfg["in_channels"], *hw), seed=1234, noise_sigma=sigma).to(device)
+    m.set_precision("fp32")
+    y32 = m(x)
+    m.set_precision(precision)
+    p = {"unmutated": psnr(m(x), y32)}
+    for name in mutations:
+        mc = copy.deepcopy(m)
+        if mutate(mc, name):
+            mc.set_precision(precision)
+            p[name] = psnr(mc(x), y32)
+    return p
+
+
+@pytest.mark.parametrize("name", ["micro_cab_x2", "small_sr4", "base_sr4"])
+def test_block_gate_routed(pkg, oracle, cases, golden_loader, device, name):
+    """Block gate on "routed" weights; on micro_cab_x2 the fp32 reference is first anchored to the oracle (<= 1e-3)."""
+    (_, cfg, hw), = [c for c in block_cases(pkg, cases) if c[0] == name]
+    x = golden_loader("model_micro_cab_x2.npz")["block_input"] if name == "micro_cab_x2" else None
+    ids = range(4) if name == "micro_cab_x2" else range(2)
+    res = block_errors(pkg, oracle, cfg, hw, device, "routed", ids, x)
+    if name == "micro_cab_x2":
+        sd = oracle.synth_state_dict(cfg, seed=0, style="routed")
+        tim = oracle.table_index_mask(cfg, hw)
+        for bi in ids:
+            with torch.no_grad():
+                ref = oracle.transformer_block(sd, f"layers.0.blocks.{bi}.", x, hw, oracle.block_settings(cfg, 0, bi), tim)
+            assert (res[bi][1].cpu() - ref).abs().max().item() <= 1e-3, bi
+    for bi, (e, _) in res.items():
+        print(f"{name} block {bi}: " + "  ".join(f"{k} {v:.2e}" for k, v in e.items()))
+        assert e["unmutated"] <= G_BLK, (bi, e["unmutated"])
+        for k, v in e.items():
+            if k != "unmutated":
+                assert v > G_BLK, f"block {bi}: mutation {k} passes the gate (e = {v:.2e})"
+        assert len(e) == len(MUTATIONS) + 1  # every mutation applies to these blocks (all have >= 2 window heads)
+
+
+@pytest.mark.parametrize("precision", ["fp16", "bf16"])
+@pytest.mark.parametrize("case", list(G_NET))
+def test_network_gate_routed(pkg, oracle, cases, device, case, precision):
+    """Network gate on "routed" weights: PSNR(tensor-core path, fp32 path) >= G_NET; every mutation (applied to every
+    block) falls below it."""
+    (_, cfg, batch, hw, sigma), = [c for c in net_cases(pkg, cases) if c[0] == case]
+    p = net_psnrs(pkg, oracle, cfg, batch, hw, sigma, device, "routed", precision)
+    print(f"{case} [{precision}]: " + "  ".join(f"{k} {v:.1f}" for k, v in p.items()))
+    gate = G_NET[case][precision]
+    assert p["unmutated"] >= gate
+    for k, v in p.items():
+        if k != "unmutated":
+            assert v < gate, f"mutation {k} passes the gate (PSNR {v:.1f} dB)"
+    assert len(p) == len(MUTATIONS) + 1 - (case == "micro_gray")  # its single window head cannot be rolled

@@ -89,3 +89,17 @@ def test_param_counts(oracle, pkg, geometry_golden):
     for key, (v, t, s, sz) in {"tiny_sr_x2": ("tiny", "sr", 2, 64), "base_dn_x1": ("base", "dn", 1, 128)}.items():
         shapes = oracle.param_shapes(pkg.configs.grl_config(v, t, s, sz))
         assert sum(int(np.prod(x)) for x in shapes.values()) == counts[key]
+
+
+def test_routed_style_keeps_init_elsewhere(oracle, cases):
+    """"routed" differs from "init" exactly in the routed parameter groups, and those are distinct per head / row."""
+    cfg = cases["micro_odd_d"]["cfg"]
+    a, r = oracle.synth_state_dict(cfg, style="init"), oracle.synth_state_dict(cfg, style="routed")
+    routed = lambda n: ("logit_scale" in n or "cpb_mlp" in n or ".norm" in n or n.startswith("norm_")  # noqa: E731
+                        or n.endswith(("qkv.body.bias", "reduction.bias", "proj.bias", "fc1.bias", "fc2.bias")))
+    for n in a:
+        assert torch.equal(a[n], r[n]) != routed(n), n
+        if n.endswith("logit_scale"):
+            assert r[n].unique().numel() == r[n].numel() and (r[n].min() >= 1.6) and (r[n].max() <= 5.02)
+    p = "layers.0.blocks.0.attn."
+    assert not torch.equal(r[p + "stripe_attn.attn_transform1.logit_scale"], r[p + "stripe_attn.attn_transform2.logit_scale"])
