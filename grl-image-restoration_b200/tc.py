@@ -8,6 +8,7 @@ statistics and every accumulator are fp32.
 Reference semantics: mixed_attn_block_efficient.py:351-381,:539-556; mixed_attn_block.py:948-983; grl.py:164-170,:506-551.
 """
 import ctypes
+from typing import NamedTuple
 
 import torch
 
@@ -169,6 +170,54 @@ def attention(gq, gk, q, q_off, k, k_off, v, v_off, out, o_off, B, heads, bias, 
     K._timed(tag, lambda: capi.check(capi.lib().grl_tc_attn(ctypes.byref(p), capi.stream())))
 
 
+class AttnLaunch(NamedTuple):
+    """One grl_tc_attn launch of a block.  q / k / v / out name an operand buffer and its first column: "qkv" (B*L,
+    nslots*32) and "anchor" (B*La, hs*32) from the projections, "x1" the dense (B*nW*hs*Na, 32) stripe intermediate,
+    "merged" (B*L, k_proj) the input of the output projection."""
+    role: str  # "window", "stripe1" (anchors attend to the stripe's tokens), "stripe2" (tokens attend to the anchors)
+    gq: object
+    gk: object
+    heads: int
+    q: tuple
+    k: tuple
+    v: tuple
+    out: tuple
+    ones_col: bool
+    use_mask: bool
+    v_dense: bool
+    o_dense: bool
+
+
+def attention_launch(role, gq, gk, hw, hs, c, use_mask):
+    """Descriptor of one of the three attention launches of a block with hw window heads, hs stripe heads and c = C / 2
+    channels per half.  Host only: the QKV slot order is [window q|k|v][stripe q|k|v] x head (BlockPlan)."""
+    if role == "window":
+        return AttnLaunch(role, gq, gk, hw, ("qkv", 0), ("qkv", hw * SLOT), ("qkv", 2 * hw * SLOT), ("merged", 0),
+                          c // hw < SLOT, use_mask, False, False)
+    ones = c // hs < SLOT
+    if role == "stripe1":  # writes X1 dense; with the ones column, X1[:, 31] == 1 is pass 2's denominator column
+        return AttnLaunch(role, gq, gk, hs, ("anchor", 0), ("qkv", (3 * hw + hs) * SLOT), ("qkv", (3 * hw + 2 * hs) * SLOT),
+                          ("x1", 0), ones, use_mask, False, True)
+    if role == "stripe2":
+        return AttnLaunch(role, gq, gk, hs, ("qkv", 3 * hw * SLOT), ("anchor", 0), ("x1", 0), ("merged", hw * SLOT), ones,
+                          use_mask, True, False)
+    raise ValueError(role)
+
+
+def attention_launches(blk, x_size):
+    """The three attention launches BlockPlan.run issues for block `blk` at resolution x_size: window attention, then
+    stripe pass 1 and pass 2 through X1."""
+    wa, sa = blk.attn.window_attn, blk.attn.stripe_attn
+    hw, hs, c = wa.num_heads, sa.num_heads, blk.dim // 2
+    s = wa.shift_size
+    gw = G.token_grid(x_size, wa.window_size, (s, s))
+    tok, anc = sa.grids(x_size)
+    # the shift masks exist exactly for the shifted blocks (EfficientMixAttnTransformerBlock._get_table_index_mask)
+    return (attention_launch("window", gw, gw, hw, hs, c, bool(blk.window_shift)),
+            attention_launch("stripe1", anc, tok, hw, hs, c, bool(blk.stripe_shift)),
+            attention_launch("stripe2", tok, anc, hw, hs, c, bool(blk.stripe_shift)))
+
+
 def bias_rows_pad(rows):
     return round_up(rows + 16, 4)  # slack for the aligned over-reads of the shifted copies (16: staged rows, variant 4)
 
@@ -316,18 +365,16 @@ class BlockPlan:
              slot_scale=self.anc_scale)
         # attention
         merged = _h16(B * L, self.k_proj, device=dev, fmt=fmt, zero=self.k_proj != (hw + hs) * SLOT)
-        s = wa.shift_size
-        gw = G.token_grid(x_size, wa.window_size, (s, s))
-        attention(gw, gw, qkv, 0, qkv, hw * SLOT, qkv, 2 * hw * SLOT, merged, 0, B, hw, bias_w, t["mask_w"] is not None,
-                  tag="window_attn", ones_col=self.ones_w)
-        tok, anc = sa.grids(x_size)
-        nW = (tok.H // tok.wh) * (tok.W // tok.ww)
+        launches = attention_launches(blk, x_size)
+        anc = launches[1].gq
+        nW = (anc.H // anc.wh) * (anc.W // anc.ww)
         x1 = _h16(B * nW * hs * anc.wh * anc.ww, SLOT, device=dev, fmt=fmt)
-        use_mask = t["mask_a2w"] is not None
-        attention(anc, tok, anchor, 0, qkv, (3 * hw + hs) * SLOT, qkv, (3 * hw + 2 * hs) * SLOT, x1, 0, B, hs, bias_1,
-                  use_mask, o_dense=True, tag="stripe_attn", ones_col=self.ones_s)
-        attention(tok, anc, qkv, 3 * hw * SLOT, anchor, 0, x1, 0, merged, hw * SLOT, B, hs, bias_2, use_mask,
-                  v_dense=True, tag="stripe_attn", ones_col=self.ones_s)
+        buf = {"qkv": qkv, "anchor": anchor, "x1": x1, "merged": merged}
+        bias = {"window": bias_w, "stripe1": bias_1, "stripe2": bias_2}
+        for ln in launches:
+            attention(ln.gq, ln.gk, buf[ln.q[0]], ln.q[1], buf[ln.k[0]], ln.k[1], buf[ln.v[0]], ln.v[1], buf[ln.out[0]],
+                      ln.out[1], B, ln.heads, bias[ln.role], ln.use_mask, v_dense=ln.v_dense, o_dense=ln.o_dense,
+                      tag="window_attn" if ln.role == "window" else "stripe_attn", ones_col=ln.ones_col)
         # CAB
         cab_y = gate = None
         if self.cab:

@@ -220,6 +220,121 @@ def cosine_attention(sd, pre, q, k, v, table, index, mask, merge_heads=True):
     return x
 
 
+# --------------------------------------------------------------------------------------
+# the tensor-core attention kernel's algorithm (csrc/attn_tc.cu), in float64
+# --------------------------------------------------------------------------------------
+
+ATTN_KEY_TILE = 64   # keys per tile (attn_tc.cu: KT)
+ATTN_Q_TILE = 128    # query rows per CTA (kQT); a partial last tile is padded
+ATTN_WARP_ROWS = 32  # rows that share one lazy-rescale decision
+ATTN_TAU = 8.0       # attn_tc.cuh: kTau
+LOG2E = 1.4426950408889634
+
+
+def lazy_softmax_emulate(x, v, dtype, mutation=None):
+    """The attention kernel's softmax on log2-domain scores x (..., R, N), R a multiple of 32, and values v (..., N, d).
+
+    Keys go in tiles of 64, in order.  Each row keeps a reference m_ref: the first tile sets it to the tile maximum; after
+    that it moves only when the tile maximum of some row of its warp (32 consecutive rows) exceeds it by more than
+    ATTN_TAU, and then every row of that warp moves by delta = max(mx - m_ref, 0) and scales O and l by 2^-delta.
+    P = exp2(x - m_ref) is rounded to `dtype`, O += P V and l += sum of the ROUNDED P (what the ones-column of V yields).
+    Everything else is float64.  Returns (O / l, info) with info["rescales"] the warp rescales after the first tile and
+    info["p_max"] the largest P.
+
+    mutation imitates a kernel bug: "rescale_o_only" (l misses the rescale), "unrounded_denominator" (l sums the
+    unrounded P)."""
+    *lead, R, N = x.shape
+    o = x.new_zeros(*lead, R, v.shape[-1])
+    l = x.new_zeros(*lead, R)
+    m_ref = None
+    rescales, p_max = 0, 0.0
+    for t, k0 in enumerate(range(0, N, ATTN_KEY_TILE)):
+        xt = x[..., k0:k0 + ATTN_KEY_TILE]
+        mx = xt.amax(-1)
+        if t == 0:
+            m_ref = mx.clone()
+        else:
+            warp = (mx - m_ref > ATTN_TAU).unflatten(-1, (R // ATTN_WARP_ROWS, ATTN_WARP_ROWS)).any(-1, keepdim=True)
+            grow = warp.expand(*warp.shape[:-1], ATTN_WARP_ROWS).flatten(-2)
+            n = int(warp.sum())
+            if n:
+                delta = torch.where(grow, (mx - m_ref).clamp_min(0.0), torch.zeros_like(mx))
+                m_ref = m_ref + delta
+                sc = torch.exp2(-delta)
+                o = o * sc[..., None]
+                if mutation != "rescale_o_only":
+                    l = l * sc
+                rescales += n
+        p = torch.exp2(xt - m_ref[..., None])
+        p16 = p.to(dtype).to(x.dtype)
+        o = o + p16 @ v[..., k0:k0 + ATTN_KEY_TILE, :].to(x.dtype)
+        l = l + (p if mutation == "unrounded_denominator" else p16).sum(-1)
+        p_max = max(p_max, float(p.max()))
+    return o / l[..., None], {"rescales": rescales, "p_max": p_max}
+
+
+def attn_windows(tokens, grid, heads):
+    """(B, H, W, heads * 32) token slots -> (B * nW, heads, wh * ww, 32) in the order the kernel walks a window:
+    torch.roll by (-sh, -sw), then partition.  grid = (H, W, wh, ww, sh, sw)."""
+    _, _, wh, ww, sh, sw = grid
+    t = torch.roll(tokens, (-sh, -sw), (1, 2)) if sh or sw else tokens
+    return partition(t, (wh, ww)).reshape(-1, wh * ww, heads, 32).transpose(1, 2)
+
+
+def attn_pair_geometry(gq, gk, use_mask):
+    """(index (Nq, Nk), mask (nW, Nq, Nk) of 0 / -100, or None) of one launch of the attention kernel.  Equal windows are
+    window attention; otherwise the smaller window is the anchor window of a stripe pass (df = token / anchor window)."""
+    if gq[2:4] == gk[2:4]:
+        res, ws, sh, df, w2a = gq[:2], list(gq[2:4]), list(gq[4:6]), 1, True
+    else:
+        w2a = gq[2] > gk[2]  # the queries are the tokens: pass 2
+        tg, ag = (gq, gk) if w2a else (gk, gq)
+        df = tg[2] // ag[2]
+        assert tg[3] // ag[3] == df and tg[0] // ag[0] == df
+        res, ws, sh = tg[:2], list(tg[2:4]), list(tg[4:6])
+    index = position_index(ws, df, w2a)
+    mask = shift_mask(list(res), ws, sh, df, w2a) if use_mask else None
+    return index, mask
+
+
+def attn_launch_reference(q, k, v, table, index, mask, dtype, mutation=None, max_elems=1 << 25):
+    """One launch of the attention kernel on gathered operands, in float64 on q's device.
+
+    q (Bw, h, Nq, 32), k and v (Bw, h, Nk, 32): the 16-bit operand values (q carries exp(min(s, ln 100)) * log2 e);
+    table (h, rows) bias in log2 units; index (Nq, Nk) into it; mask (nW, Nq, Nk) of 0 / -100 (window w uses mask[w % nW])
+    or None.  Returns (exact, emulated, info), each output (Bw, h, Nq, 32) float64:
+      exact:    softmax over the keys of 2^(S + bias + mask log2 e), times V;
+      emulated: lazy_softmax_emulate of the same scores, rounded to `dtype`.  The query tile is padded to 128 rows the
+                way the kernel pads it (zero Q, the bias and mask row of query 0): those rows share warp decisions.
+    Windows are processed in chunks of at most max_elems scores."""
+    f = torch.float64
+    dev = q.device
+    Bw, h, Nq, _ = q.shape
+    Nk = k.shape[2]
+    qp = -(-Nq // ATTN_Q_TILE) * ATTN_Q_TILE
+    r = torch.arange(qp, device=dev)
+    rows = torch.where(r < Nq, r, 0)
+    bias = table.to(dev, f)[:, index.to(dev)[rows]]  # (h, qp, Nk)
+    mlog = None if mask is None else mask.to(dev, f)[:, rows] * LOG2E
+    exact, emul = torch.empty(Bw, h, Nq, 32, dtype=f, device=dev), torch.empty(Bw, h, Nq, 32, dtype=f, device=dev)
+    info = {"rescales": 0, "p_max": 0.0}
+    step = max(1, max_elems // (h * qp * Nk))
+    for w0 in range(0, Bw, step):
+        w1 = min(Bw, w0 + step)
+        qq = torch.zeros(w1 - w0, h, qp, 32, dtype=f, device=dev)
+        qq[:, :, :Nq] = q[w0:w1].to(f)
+        vv = v[w0:w1].to(f)
+        x = qq @ k[w0:w1].to(f).transpose(-1, -2) + bias
+        if mlog is not None:
+            x = x + mlog[torch.arange(w0, w1, device=dev) % mlog.shape[0]].unsqueeze(1)
+        exact[w0:w1] = torch.softmax(x[:, :, :Nq] * log(2.0), dim=-1) @ vv
+        o, inf = lazy_softmax_emulate(x, vv, dtype, mutation)
+        emul[w0:w1] = o[:, :, :Nq].to(dtype).to(f)
+        info["rescales"] += inf["rescales"]
+        info["p_max"] = max(info["p_max"], inf["p_max"])
+    return exact, emul, info
+
+
 def window_attention(sd, pre, qkv, x_size, ws, heads, shifted, table, index, mask):
     """mixed_attn_block_efficient.py:128-165."""
     H, W = x_size

@@ -1,8 +1,7 @@
-"""bf16 tensor-core operators (wgmma GEMM / implicit-GEMM conv / fused attention) vs fp32 references evaluated on
+"""bf16 tensor-core operators (wgmma GEMM / implicit-GEMM conv) vs fp32 references evaluated on
 the same bf16-rounded operands.  Tolerances are bf16-sized: these tests prove descriptor / layout / addressing
 correctness (a wrong swizzle or index gives O(1) errors), the PSNR gate of the whole network is in
 test_gpu_model_bf16.py."""
-import math
 import os
 
 import pytest
@@ -130,160 +129,3 @@ def test_gemm_layernorm_epilogue(tc, device, C, cab, fmt):
     assert (o16.cpu().float()[:, :C] - ref).abs().max().item() <= tol16
     if cpad > C:
         assert o16.cpu().float()[:, C:].abs().max().item() == 0
-
-
-def _attn_ref(q, k, v, bias_idx, table, mask, fmt=0):
-    """q (Bw, h, Nq, d) pre-normalised+scaled (log2 domain), k (Bw,h,Nk,d), v; table (h, rows) log2 domain."""
-    s = bf(q, fmt) @ bf(k, fmt).transpose(-1, -2)
-    s = s + table[:, bias_idx.reshape(-1)].view(table.shape[0], *bias_idx.shape).unsqueeze(0)
-    if mask is not None:
-        s = (s.view(-1, mask.shape[0], *s.shape[1:]) + (mask * 1.4426950408889634).unsqueeze(1).unsqueeze(0)).view(s.shape)
-    p = torch.softmax(s * math.log(2.0), dim=-1)
-    return p @ bf(v, fmt)
-
-
-ATT = [  # B, H, W, (wh, ww), heads, shifted
-    (1, 16, 16, (8, 8), 2, False), (2, 32, 64, (32, 32), 3, True), (1, 24, 36, (12, 12), 2, True),
-    (1, 16, 32, (16, 16), 1, True), (1, 8, 16, (4, 8), 2, False),
-]
-
-
-def _run_window(tc, oracle, device, B, H, W, ws, heads, shifted, fmt, table_fn=None):
-    from grl_image_restoration_b200 import geometry as G
-
-    d, nsl = 30, 3 * heads
-    L = H * W
-    g = torch.Generator().manual_seed(31)
-    qkv = torch.zeros(B, L, nsl, 32)
-    qkv[..., :d] = torch.randn(B, L, nsl, d, generator=g)
-    qkv[:, :, : 2 * heads, :d] = F.normalize(qkv[:, :, : 2 * heads, :d], dim=-1)
-    qkv[:, :, :heads] *= 9.0  # scaled queries (log2 domain logits up to ~9)
-    table = torch.rand(heads, (2 * ws[0] - 1) * (2 * ws[1] - 1), generator=g) * 16 * tc.LOG2E
-    if table_fn is not None:
-        table = table_fn(table)
-    s = ws[0] // 2 if shifted else 0
-    # reference through the oracle's partition / roll helpers
-    t = qkv.view(B, H, W, nsl * 32)
-    if s:
-        t = torch.roll(t, (-s, -s), (1, 2))
-    win = oracle.partition(t, ws).reshape(-1, ws[0] * ws[1], 3, heads, 32).permute(2, 0, 3, 1, 4)
-    mask = oracle.shift_mask([H, W], list(ws), [s, s]) if shifted else None
-    o = _attn_ref(win[0], win[1], win[2], oracle.position_index(list(ws)), table, mask, fmt)
-    o = o.transpose(1, 2).reshape(-1, ws[0], ws[1], heads * 32)
-    ref = oracle.unpartition(o, ws, (H, W))
-    if s:
-        ref = torch.roll(ref, (s, s), (1, 2))
-    ref = ref.reshape(B, L, heads * 32)
-    q16 = qkv.view(B * L, nsl * 32).to(device).to(tc.DTYPE[fmt])
-    out = torch.zeros(B * L, heads * 32, device=device, dtype=tc.DTYPE[fmt])
-    grid = G.token_grid((H, W), ws, (s, s))
-    tc.attention(grid, grid, q16, 0, q16, heads * 32, q16, 2 * heads * 32, out, 0, B, heads, tc.shifted_copies(table.to(device)), shifted)
-    got = out.cpu().float().view(B, L, heads * 32)
-    err = (got - ref).abs().max().item()
-    assert err <= 4e-2 * max(1.0, ref.abs().max().item()), err
-    assert (got - ref).abs().mean().item() <= 6e-3
-
-
-@pytest.mark.parametrize("fmt", [0, 1])
-@pytest.mark.parametrize("B,H,W,ws,heads,shifted", ATT)
-def test_attention_tc_window(tc, oracle, device, B, H, W, ws, heads, shifted, fmt):
-    _run_window(tc, oracle, device, B, H, W, ws, heads, shifted, fmt)
-
-
-@pytest.mark.parametrize("slope", [0.6, 6.0])
-@pytest.mark.parametrize("shifted", [False, True])
-def test_attention_tc_lazy_rescale_path(tc, oracle, device, slope, shifted):
-    """A bias that GROWS with the key row (by `slope` log2 units per row, 2 rows per 64-key tile) makes every row's running
-    maximum outgrow its reference by more than 2^8 repeatedly (slope 6: on every tile; 0.6: every ~7 tiles), i.e. the
-    kernel's reference moves and O and the row sums are rescaled -- the path the random
-    tables of the other tests almost never take after the first tile."""
-    ws = (32, 32)
-
-    def grow(table):
-        rows = torch.arange(table.shape[1])
-        dh = rows // (2 * ws[1] - 1) - (ws[0] - 1)  # query row - key row of this relative position
-        return table * 0.25 + (-slope * dh.float()).unsqueeze(0)
-
-    _run_window(tc, oracle, device, 2, 32, 64, ws, 3, shifted, 0, table_fn=grow)
-
-
-@pytest.mark.parametrize("fmt", [0, 1])
-@pytest.mark.parametrize("B,H,W,stripe,df,heads,shifted", [(1, 16, 32, (8, 16), 2, 2, True), (1, 64, 64, (64, 64), 2, 3, True),
-                                                          (2, 32, 32, (32, 16), 4, 2, False), (1, 48, 96, (48, 96), 4, 1, True)])
-def test_attention_tc_stripe_chain(tc, oracle, device, B, H, W, stripe, df, heads, shifted, fmt):
-    """Both passes of the anchored stripe attention through the dense X1 intermediate."""
-    from grl_image_restoration_b200 import geometry as G
-
-    d, L = 30, H * W
-    g = torch.Generator().manual_seed(41)
-    qkv = torch.zeros(B, L, 3 * heads, 32)
-    qkv[..., :d] = torch.randn(B, L, 3 * heads, d, generator=g)
-    qkv[:, :, : 2 * heads, :d] = F.normalize(qkv[:, :, : 2 * heads, :d], dim=-1) * 7.0
-    Ha, Wa = H // df, W // df
-    anc = torch.zeros(B, Ha * Wa, heads, 32)
-    anc[..., :d] = F.normalize(torch.randn(B, Ha * Wa, heads, d, generator=g), dim=-1)
-    ss = list(stripe)
-    sh = [x // 2 for x in ss] if shifted else [0, 0]
-    ass, ash = [x // df for x in ss], [x // df for x in sh]
-    rows = (ss[0] + ass[0] - 1) * (ss[1] + ass[1] - 1)
-    t1 = torch.rand(heads, rows, generator=g) * 16 * tc.LOG2E
-    t2 = torch.rand(heads, rows, generator=g) * 16 * tc.LOG2E
-    t = qkv.view(B, H, W, -1)
-    a = anc.view(B, Ha, Wa, -1)
-    if shifted:
-        t = torch.roll(t, (-sh[0], -sh[1]), (1, 2))
-        a = torch.roll(a, (-ash[0], -ash[1]), (1, 2))
-    tw = oracle.partition(t, ss).reshape(-1, ss[0] * ss[1], 3, heads, 32).permute(2, 0, 3, 1, 4)
-    aw = oracle.partition(a, ass).reshape(-1, ass[0] * ass[1], heads, 32).permute(0, 2, 1, 3)
-    ma = oracle.shift_mask([H, W], ss, sh, df, False) if shifted else None
-    mw = oracle.shift_mask([H, W], ss, sh, df, True) if shifted else None
-    x1 = _attn_ref(aw, tw[1], tw[2], oracle.position_index(ss, df, False), t1, ma, fmt)
-    y = _attn_ref(tw[0], aw, bf(x1, fmt), oracle.position_index(ss, df, True), t2, mw, fmt)
-    y = y.transpose(1, 2).reshape(-1, ss[0], ss[1], heads * 32)
-    ref = oracle.unpartition(y, ss, (H, W))
-    if shifted:
-        ref = torch.roll(ref, (sh[0], sh[1]), (1, 2))
-    ref = ref.reshape(B, L, heads * 32)
-    q16 = qkv.view(B * L, -1).to(device).to(tc.DTYPE[fmt])
-    a16 = anc.view(B * Ha * Wa, -1).to(device).to(tc.DTYPE[fmt])
-    tok, ag = G.token_grid((H, W), ss, sh), G.anchor_grid((H, W), ss, sh, df)
-    nW = (H // ss[0]) * (W // ss[1])
-    x1d = torch.empty(B * nW * heads * ass[0] * ass[1], 32, device=device, dtype=tc.DTYPE[fmt])
-    out = torch.zeros(B * L, heads * 32, device=device, dtype=tc.DTYPE[fmt])
-    tc.attention(ag, tok, a16, 0, q16, heads * 32, q16, 2 * heads * 32, x1d, 0, B, heads, tc.shifted_copies(t1.to(device)), shifted, o_dense=True)
-    tc.attention(tok, ag, q16, 0, a16, 0, x1d, 0, out, 0, B, heads, tc.shifted_copies(t2.to(device)), shifted, v_dense=True)
-    got = out.cpu().float().view(B, L, heads * 32)
-    assert (x1d.cpu().float().view(x1.shape) - x1).abs().max().item() <= 4e-2 * max(1.0, x1.abs().max().item())
-    err = (got - ref).abs().max().item()
-    assert err <= 5e-2 * max(1.0, ref.abs().max().item()), err
-
-
-@pytest.mark.parametrize("fmt", [0, 1])
-def test_attention_tc_ones_column_denominator(tc, oracle, device, fmt):
-    """head_dim < 32: V[:, 31] == 1 makes the P V MMA produce the softmax denominator (ones_col=True)."""
-    from grl_image_restoration_b200 import geometry as G
-
-    B, H, W, ws, heads, d = 1, 32, 64, (32, 32), 3, 30
-    nsl, L = 3 * heads, H * W
-    g = torch.Generator().manual_seed(77)
-    qkv = torch.zeros(B, L, nsl, 32)
-    qkv[..., :d] = torch.randn(B, L, nsl, d, generator=g)
-    qkv[:, :, : 2 * heads, :d] = F.normalize(qkv[:, :, : 2 * heads, :d], dim=-1)
-    qkv[:, :, :heads] *= 9.0
-    table = torch.rand(heads, (2 * ws[0] - 1) * (2 * ws[1] - 1), generator=g) * 16 * tc.LOG2E
-    s = ws[0] // 2
-    t = torch.roll(qkv.view(B, H, W, nsl * 32), (-s, -s), (1, 2))
-    win = oracle.partition(t, ws).reshape(-1, ws[0] * ws[1], 3, heads, 32).permute(2, 0, 3, 1, 4)
-    o = _attn_ref(win[0], win[1], win[2], oracle.position_index(list(ws)), table, oracle.shift_mask([H, W], list(ws), [s, s]),
-                  fmt)
-    ref = torch.roll(oracle.unpartition(o.transpose(1, 2).reshape(-1, ws[0], ws[1], heads * 32), ws, (H, W)), (s, s), (1, 2))
-    ref = ref.reshape(B, L, heads, 32)
-    qkv[:, :, 2 * heads:, 31] = 1.0  # what the QKV epilogue writes through the bias when head_dim < 32
-    q16 = qkv.view(B * L, nsl * 32).to(device).to(tc.DTYPE[fmt])
-    out = torch.zeros(B * L, heads * 32, device=device, dtype=tc.DTYPE[fmt])
-    grid = G.token_grid((H, W), ws, (s, s))
-    tc.attention(grid, grid, q16, 0, q16, heads * 32, q16, 2 * heads * 32, out, 0, B, heads,
-                 tc.shifted_copies(table.to(device)), True, ones_col=True)
-    got = out.cpu().float().view(B, L, heads, 32)
-    assert (got[..., :d] - ref[..., :d]).abs().max().item() <= 4e-2 * max(1.0, ref.abs().max().item())
-    assert (got[..., 31] - 1.0).abs().max().item() <= 2e-3 and got[..., 30].abs().max().item() == 0

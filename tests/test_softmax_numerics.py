@@ -7,47 +7,26 @@ What the kernel does per query row, in the log2 domain (x = S + bias + mask, eve
     when head_dim < 32);
   * LAZY rescale (kTau = 8): the reference moves only when the maximum of a row of the warp (32 rows) outgrew its reference by
     more than 2^8 (always on the first tile); then every row of the warp takes delta = max(mx - m_ref, 0), scales O by 2^-delta.
-The emulation below is that algorithm, not the kernel; it guards the design constants (kTau vs the fp16 range, 16-bit P with an
-fp32 denominator built from the same rounded values) independently of any GPU."""
+The emulation (grl_oracle.lazy_softmax_emulate, also the reference of tests/test_gpu_tc_attn.py) is that algorithm, not
+the kernel; it guards the design constants (kTau vs the fp16 range, 16-bit P with an fp32 denominator built from the same
+rounded values) independently of any GPU."""
 import pytest
 import torch
 
-K_TAU = 8.0  # csrc/attn_tc.cuh: kTau
-KT = 64      # keys per tile
+from grl_oracle import ATTN_KEY_TILE as KT, ATTN_TAU as K_TAU, lazy_softmax_emulate
+
 MASK_LOG2 = 100.0 * 1.4426950408889634  # the shift mask (-100) in the log2 domain
 
 
 def emulate(x, v, fmt):
     """x (R, N) log2-domain scores, v (N, d) values (already in the operand format) -> (out (R, d), rescales per warp)."""
-    R, N = x.shape
-    dt = torch.float16 if fmt == "fp16" else torch.bfloat16
-    o = torch.zeros(R, v.shape[1], dtype=torch.float32)
-    l = torch.zeros(R, dtype=torch.float32)
-    m_ref = torch.zeros(R, dtype=torch.float32)
-    rescales = 0
-    for t, k0 in enumerate(range(0, N, KT)):
-        xt = x[:, k0:k0 + KT].float()
-        mx = xt.max(dim=1).values
-        for w in range(0, R, 32):  # the decision is warp-wide, the amount is per row
-            rows = slice(w, min(w + 32, R))
-            if t == 0 or bool((mx[rows] - m_ref[rows] > K_TAU).any()):
-                delta = mx[rows].clone() if t == 0 else (mx[rows] - m_ref[rows]).clamp_min(0.0)
-                m_ref[rows] += delta
-                if t > 0:
-                    sc = torch.exp2(-delta)
-                    o[rows] *= sc[:, None]
-                    l[rows] *= sc
-                    rescales += 1
-        p = torch.exp2(xt - m_ref[:, None])
-        assert float(p.max()) <= 2.0 ** K_TAU * (1 + 1e-6)  # the bound that keeps P inside the fp16 range
-        p16 = p.to(dt).float()
-        o += p16 @ v[k0:k0 + KT].float()
-        l += p16.sum(dim=1)
-    return o / l[:, None], rescales
+    out, info = lazy_softmax_emulate(x.double(), v.double(), torch.float16 if fmt == "fp16" else torch.bfloat16)
+    assert info["p_max"] <= 2.0 ** K_TAU * (1 + 1e-6)  # the bound that keeps P inside the fp16 range
+    return out, info["rescales"]
 
 
 def exact(x, v):
-    return (torch.softmax(x.double() * 0.6931471805599453, dim=1) @ v.double()).float()  # softmax of 2^x
+    return torch.softmax(x.double() * 0.6931471805599453, dim=1) @ v.double()  # softmax of 2^x
 
 
 def _case(name, R=128, N=1024, d=30):
