@@ -262,11 +262,12 @@ int grl_tc_channel_gate(const void* y, int64_t ld, int fmt, int B, int64_t L, in
   return launch_channel_gate_from_partial((const float*)ws, chunks, B, L, C, w1, b1, w2, b2, R, gate, (cudaStream_t)stream);
 }
 
-int grl_tc_gemm(const GrlTcGemm* p, void* stream) {
+}  // extern "C"
+
+// GrlTcGemm -> the launcher's problem and arguments, with the argument checks of grl_tc_gemm and grl_tc_gemm_path
+static int tc_gemm_problem(const GrlTcGemm* p, tc::GemmTcProblem& q, tc::GemmTcArgs& a) {
   GRL_REQUIRE(p != nullptr, "tc_gemm: null problem");
-  if (!grl_device_ok()) return fail(GRL_ERR_ARCH, "tc_gemm: wgmma kernels need an sm_90 device");
-  tc::GemmTcProblem q = {p->x, p->w, p->M, p->B, p->H, p->W, p->kpad, p->npad, p->taps, p->epi};
-  tc::GemmTcArgs a;
+  q = {p->x, p->w, p->M, p->B, p->H, p->W, p->kpad, p->npad, p->taps, p->epi};
   memset(&a, 0, sizeof(a));
   if (check_fmt(p->fmt)) return GRL_ERR_INVALID;
   a.fmt = p->fmt;
@@ -290,7 +291,31 @@ int grl_tc_gemm(const GrlTcGemm* p, void* stream) {
                     p->L > 0 && (p->ldo_f32 % 4) == 0 && (p->ldo_bf16 % 8) == 0,
                 "tc_gemm: LN epilogue arguments");
   if (p->out_bf16) GRL_REQUIRE((p->ldo_bf16 % 8) == 0, "tc_gemm: bf16 output pitch must be a multiple of 8");
+  return GRL_OK;
+}
+
+extern "C" {
+
+int grl_tc_gemm(const GrlTcGemm* p, void* stream) {
+  GRL_REQUIRE(p != nullptr, "tc_gemm: null problem");
+  if (!grl_device_ok()) return fail(GRL_ERR_ARCH, "tc_gemm: wgmma kernels need an sm_90 device");
+  tc::GemmTcProblem q;
+  tc::GemmTcArgs a;
+  int rc = tc_gemm_problem(p, q, a);
+  if (rc != GRL_OK) return rc;
   return tc::launch_gemm_tc(q, a, (cudaStream_t)stream);
+}
+
+int grl_tc_gemm_path(const GrlTcGemm* p, GrlTcGemmPath* out) {
+  GRL_REQUIRE(out != nullptr, "tc_gemm_path: null output");
+  tc::GemmTcProblem q;
+  tc::GemmTcArgs a;
+  int bn = 0, rc;
+  if ((rc = tc_gemm_problem(p, q, a)) != GRL_OK) return rc;
+  if ((rc = tc::plan_gemm_tc(q, a, &bn)) != GRL_OK) return rc;
+  out->bn = bn, out->epi_mode = a.epi_mode, out->conv = q.taps == 9, out->n_tiles = a.n_tiles;
+  out->nk_total = a.taps * a.nk, out->grid = a.total_tiles;
+  return GRL_OK;
 }
 
 int grl_tc_attn_variant(int variant) { return tc::attn_variant(variant); }

@@ -58,6 +58,7 @@ struct GemmTcProblem {
   int kpad, npad, taps, epi;
 };
 
+int plan_gemm_tc(const GemmTcProblem& p, GemmTcArgs& a, int* bn);  // host only: the launch path (gemm_tc.cu)
 int launch_gemm_tc(const GemmTcProblem& p, GemmTcArgs a, cudaStream_t st);
 
 // Fused attention on packed bf16 head slots (32 wide).  See attn_tc.cu.

@@ -8,6 +8,7 @@ statistics and every accumulator are fp32.
 Reference semantics: mixed_attn_block_efficient.py:351-381,:539-556; mixed_attn_block.py:948-983; grl.py:164-170,:506-551.
 """
 import ctypes
+import inspect
 from typing import NamedTuple
 
 import torch
@@ -115,9 +116,30 @@ def pack_conv(conv, cin_pad, npad, fmt=0, ps_r=0):
     return out.reshape(npad, 9 * cin_pad).to(DTYPE[fmt]).contiguous(), bias
 
 
-def gemm(x16, w16, bias, *, M=0, image=None, kpad, npad, taps=1, epi=EPI_BIAS_ACT, n_store=0, n_real=0, out_bf16=None,
-         out_f32=None, res_f32=None, act=K.ACT_NONE, slope=0.0, slot_scale=None, C=0, gamma=None, beta=None, eps=1e-5,
-         res_scale=1.0, cab_y=None, cab_gate=None, L=1, ps_r=0, out_nchw=None, nchw_r=1, post_scale=1.0, post_shift=None):
+class Spec(NamedTuple):
+    """Shape and dtype of a tensor argument in a launch descriptor (GemmLaunch).  data_ptr() is a non-null stand-in:
+    grl_tc_gemm_path only tests pointers for NULL."""
+    shape: tuple
+    dtype: torch.dtype
+
+    def data_ptr(self):
+        return 256
+
+
+def _pitch(t):
+    """Elements from one row of t's last dimension to the next: a view of a wider buffer keeps the buffer's pitch."""
+    if isinstance(t, Spec) or t.dim() < 2:
+        return t.shape[-1]
+    if t.stride(-1) != 1 or any(t.shape[i] > 1 and t.stride(i) != t.stride(i + 1) * t.shape[i + 1] for i in range(t.dim() - 2)):
+        raise RuntimeError("grl_b200: gemm outputs / residuals need unit-stride rows at one pitch")
+    return t.stride(-2)
+
+
+def gemm_problem(x16, w16, bias, *, M=0, image=None, kpad, npad, taps=1, epi=EPI_BIAS_ACT, n_store=0, n_real=0,
+                 out_bf16=None, out_f32=None, res_f32=None, act=K.ACT_NONE, slope=0.0, slot_scale=None, C=0, gamma=None,
+                 beta=None, eps=1e-5, res_scale=1.0, cab_y=None, cab_gate=None, L=1, ps_r=0, out_nchw=None, nchw_r=1,
+                 post_scale=1.0, post_shift=None):
+    """The GrlTcGemm of one launch (arguments: gemm)."""
     p = capi.GrlTcGemm()
     if x16.dtype != w16.dtype:
         raise RuntimeError("grl_b200: activation / weight operand formats differ")
@@ -129,11 +151,11 @@ def gemm(x16, w16, bias, *, M=0, image=None, kpad, npad, taps=1, epi=EPI_BIAS_AC
     p.kpad, p.npad, p.taps, p.epi = kpad, npad, taps, epi
     p.n_store, p.n_real = n_store, n_real
     if out_bf16 is not None:
-        p.out_bf16, p.ldo_bf16 = out_bf16.data_ptr(), out_bf16.shape[-1]
+        p.out_bf16, p.ldo_bf16 = out_bf16.data_ptr(), _pitch(out_bf16)
     if out_f32 is not None:
-        p.out_f32, p.ldo_f32 = out_f32.data_ptr(), out_f32.shape[-1]
+        p.out_f32, p.ldo_f32 = out_f32.data_ptr(), _pitch(out_f32)
     if res_f32 is not None:
-        p.res_f32, p.ldr = res_f32.data_ptr(), res_f32.shape[-1]
+        p.res_f32, p.ldr = res_f32.data_ptr(), _pitch(res_f32)
     p.act, p.slope = act, slope
     if slot_scale is not None:
         p.slot_scale = slot_scale.data_ptr()
@@ -142,7 +164,7 @@ def gemm(x16, w16, bias, *, M=0, image=None, kpad, npad, taps=1, epi=EPI_BIAS_AC
         p.gamma, p.beta = gamma.data_ptr(), beta.data_ptr()
     p.eps, p.res_scale = eps, res_scale
     if cab_y is not None:
-        p.cab_y, p.ld_caby, p.cab_gate = cab_y.data_ptr(), cab_y.shape[-1], cab_gate.data_ptr()
+        p.cab_y, p.ld_caby, p.cab_gate = cab_y.data_ptr(), _pitch(cab_y), cab_gate.data_ptr()
     p.L = L
     p.ps_r = ps_r
     if out_nchw is not None:  # (B, C_out, Hc, Wc) fp32 planes: denormalise + crop + bhwc -> bchw folded into the store
@@ -150,7 +172,39 @@ def gemm(x16, w16, bias, *, M=0, image=None, kpad, npad, taps=1, epi=EPI_BIAS_AC
         p.post_scale = post_scale
         for i in range(4):
             p.post_shift[i] = float(post_shift[i]) if post_shift is not None and i < len(post_shift) else 0.0
+    return p
+
+
+def gemm(x16, w16, bias, **kw):
+    """One grl_tc_gemm launch (keyword arguments: gemm_problem)."""
+    p = gemm_problem(x16, w16, bias, **kw)
     capi.check(capi.lib().grl_tc_gemm(ctypes.byref(p), capi.stream()))
+
+
+class GemmLaunch(NamedTuple):
+    """One tc.gemm call of a forward: `name` (e.g. "stage0.block1.fc1", "conv_last") and gemm_problem's arguments with
+    their defaults applied and a Spec in place of every tensor."""
+    name: str
+    args: dict
+
+
+def _spec(v):
+    return Spec(tuple(v.shape), v.dtype) if isinstance(v, (torch.Tensor, Spec)) else v
+
+
+def gemm_launch(name, x16, w16, bias, **kw):
+    """The descriptor of gemm(x16, w16, bias, **kw)."""
+    b = inspect.signature(gemm_problem).bind(x16, w16, bias, **kw)
+    b.apply_defaults()
+    return GemmLaunch(name, {k: _spec(v) for k, v in b.arguments.items()})
+
+
+def gemm_path(launch):
+    """grl_tc_gemm_path of a descriptor: the tile width, epilogue mode, tiling and grid the library picks for it."""
+    out = capi.GrlTcGemmPath()
+    p = gemm_problem(**launch.args)
+    capi.check(capi.lib().grl_tc_gemm_path(ctypes.byref(p), ctypes.byref(out)))
+    return out
 
 
 def attention(gq, gk, q, q_off, k, k_off, v, v_off, out, o_off, B, heads, bias, use_mask, v_dense=False,
@@ -434,3 +488,115 @@ def conv_plan(owner, name, conv, cin_pad, fmt, ps_r=0):
         plan = ConvPlan(conv, cin_pad, fmt, ps_r)
         cache[name] = plan
     return plan
+
+
+def gemm_launches(model, x_shape):
+    """Descriptors of every tc.gemm / tc.conv3x3 launch of one tensor-core forward of GRL `model` on a (B, Cin, H, W)
+    input, in launch order, with the arguments GRL._forward_bf16, TransformerStage.forward_tc and BlockPlan.run pass
+    (operand format: model.precision).  Host only: shapes come from the modules, nothing is packed or launched."""
+    from torch import nn
+
+    fmt = FMT[model.precision]
+    B, Cin, H, W = x_shape
+    ps = model.pad_size
+    Hp, Wp = round_up(H, ps), round_up(W, ps)
+    L = Hp * Wp
+    C = model.embed_dim
+    cpad = round_up(C, 64)
+    s = model.upscale
+    out = []
+
+    def h16(*shape):
+        return Spec(shape, DTYPE[fmt])
+
+    def f32(*shape):
+        return Spec(shape, torch.float32)
+
+    def conv(name, module, x16, *, n_store=None, act=K.ACT_NONE, slope=0.0, out_bf16=None, out_f32=None, res_f32=None,
+             **tail):
+        cin_pad, cout = x16.shape[-1], module.weight.shape[0]
+        npad = round_up(cout, 64)  # ConvPlan
+        b, h, w = x16.shape[:3]
+        out.append(gemm_launch(name, x16, h16(npad, 9 * cin_pad), f32(npad), image=(b, h, w), kpad=cin_pad, npad=npad,
+                               taps=9, epi=EPI_BIAS_ACT, n_store=npad if n_store is None else n_store, n_real=cout,
+                               out_bf16=out_bf16, out_f32=out_f32, res_f32=res_f32, act=act, slope=slope, **tail))
+
+    def block(name, blk):  # BlockPlan.__init__ / run
+        hw, hs = blk.attn.window_attn.num_heads, blk.attn.stripe_attn.num_heads
+        n_qkv = (3 * hw + 3 * hs) * SLOT
+        out.append(gemm_launch(f"{name}.qkv", h16(B, L, cpad), h16(n_qkv, cpad), f32(n_qkv), M=B * L, kpad=cpad,
+                               npad=n_qkv, epi=EPI_QKV, n_store=n_qkv, out_bf16=h16(B * L, n_qkv),
+                               slot_scale=f32(n_qkv // SLOT)))
+        df = blk.attn.anchor.body[0].down_factor
+        La, n_anc = (Hp // df) * (Wp // df), round_up(hs * SLOT, 32)
+        out.append(gemm_launch(f"{name}.anchor", h16(B, Hp // df, Wp // df, cpad), h16(n_anc, cpad), f32(n_anc),
+                               M=B * La, kpad=cpad, npad=n_anc, epi=EPI_QKV, n_store=n_anc, out_bf16=h16(B * La, n_anc),
+                               slot_scale=f32(hs)))
+        cab = {}
+        if blk.args.local_connection:
+            cmid_pad = round_up(blk.conv.cab[0].weight.shape[0], 64)
+            out.append(gemm_launch(f"{name}.cab1", h16(B, Hp, Wp, cpad), h16(cmid_pad, 9 * cpad), f32(cmid_pad),
+                                   image=(B, Hp, Wp), kpad=cpad, npad=cmid_pad, taps=9, epi=EPI_BIAS_ACT,
+                                   n_store=cmid_pad, out_bf16=h16(B, Hp, Wp, cmid_pad), act=K.ACT_GELU))
+            out.append(gemm_launch(f"{name}.cab2", h16(B, Hp, Wp, cmid_pad), h16(cpad, 9 * cmid_pad), f32(cpad),
+                                   image=(B, Hp, Wp), kpad=cmid_pad, npad=cpad, taps=9, epi=EPI_BIAS_ACT, n_store=cpad,
+                                   out_bf16=h16(B * L, cpad)))
+            cab = dict(cab_y=h16(B * L, cpad), cab_gate=f32(B, C))
+        n_ln = 64 if C <= 64 else 128 if C <= 128 else 192 if C <= 192 else 256
+        k_proj = round_up((hw + hs) * SLOT, 64)
+        hpad = round_up(blk.mlp.fc1.weight.shape[0], 64)
+        def ln(nm, kpad, norm, **kw):
+            out.append(gemm_launch(f"{name}.{nm}", h16(B * L, kpad), h16(n_ln, kpad), f32(n_ln), M=B * L, kpad=kpad,
+                                   npad=n_ln, epi=EPI_LN, n_store=n_ln, n_real=C, out_bf16=h16(B, L, cpad),
+                                   out_f32=f32(B, L, C), res_f32=f32(B, L, C), C=C, gamma=_spec(norm.weight),
+                                   beta=_spec(norm.bias), eps=norm.eps, res_scale=blk.res_scale, L=L, **kw))
+
+        ln("proj", k_proj, blk.norm1, **cab)
+        out.append(gemm_launch(f"{name}.fc1", h16(B, L, cpad), h16(hpad, cpad), f32(hpad), M=B * L, kpad=cpad, npad=hpad,
+                               epi=EPI_BIAS_ACT, n_store=hpad, act=K.ACT_GELU, out_bf16=h16(B * L, hpad)))
+        ln("fc2", hpad, blk.norm2)
+
+    # GRL._forward_bf16
+    need_res = model.upsampler not in ("pixelshuffle", "pixelshuffledirect", "nearest+conv") and model.in_channels == model.out_channels
+    mean = model._mean_list
+    shift = mean if len(mean) > 1 else mean * 4
+    cf = round_up(model.conv_first.weight.shape[0], 64)
+    conv("conv_first", model.conv_first, h16(B, Hp, Wp, 64), out_bf16=h16(B, Hp, Wp, cf), out_f32=f32(B, Hp, Wp, C))
+    for si, layer in enumerate(model.layers):  # TransformerStage.forward_tc
+        for bi, blk in enumerate(layer.blocks):
+            block(f"stage{si}.block{bi}", blk)
+        conv(f"stage{si}.conv", layer.conv, h16(B, Hp, Wp, cpad), n_store=cpad, out_bf16=h16(B, L, cpad),
+             out_f32=f32(B, L, C), res_f32=f32(B, L, C))
+    body = h16(B, Hp, Wp, round_up(model.conv_after_body.weight.shape[0], 64))
+    conv("conv_after_body", model.conv_after_body, h16(B, Hp, Wp, cpad), out_bf16=body, res_f32=f32(B, Hp, Wp, C))
+
+    def final(name, module, x16, r, res=None):
+        conv(name, module, x16, out_nchw=f32(B, model.out_channels, H * s, W * s), nchw_r=r, post_scale=1.0 / model.img_range,
+             post_shift=shift, res_f32=res)
+
+    def lrelu(name, module, x16, slope):
+        o = h16(*x16.shape[:3], round_up(module.weight.shape[0], 64))
+        conv(name, module, x16, act=K.ACT_LEAKY, slope=slope, out_bf16=o)
+        return o
+
+    if model.upsampler == "pixelshuffle":
+        u = lrelu("conv_before_upsample", model.conv_before_upsample[0], body, 0.01)
+        mods = list(model.upsample.up)
+        for i, m in enumerate(mods):
+            if isinstance(m, nn.Conv2d):
+                r, cout = mods[i + 1].upscale_factor, m.weight.shape[0]
+                o = h16(u.shape[0], u.shape[1] * r, u.shape[2] * r, cout // (r * r))
+                conv(f"upsample.up.{i}", m, u, n_store=cout, out_bf16=o, ps_r=r)
+                u = o
+        final("conv_last", model.conv_last, u, 1)
+    elif model.upsampler == "pixelshuffledirect":
+        final("upsample.up.0", model.upsample.up[0], body, model.upsample.up[1].upscale_factor)
+    elif model.upsampler == "nearest+conv":
+        u = lrelu("conv_before_upsample", model.conv_before_upsample[0], body, 0.01)
+        u = lrelu("conv_up1", model.conv_up1, h16(B, 2 * u.shape[1], 2 * u.shape[2], u.shape[3]), 0.2)
+        u = lrelu("conv_up2", model.conv_up2, h16(B, 2 * u.shape[1], 2 * u.shape[2], u.shape[3]), 0.2)
+        u = lrelu("conv_hr", model.conv_hr, u, 0.2)
+        final("conv_last", model.conv_last, u, 1)
+    else:
+        final("conv_last", model.conv_last, body, 1, f32(B, Hp, Wp, Cin) if need_res else None)
+    return out

@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define GRL_B200_ABI_VERSION 4
+#define GRL_B200_ABI_VERSION 5
 
 typedef enum {
   GRL_OK = 0,
@@ -214,6 +214,18 @@ typedef struct {
   float post_shift[4];
 } GrlTcGemm;
 int grl_tc_gemm(const GrlTcGemm* p, void* stream);
+
+/* The launch path grl_tc_gemm takes for problem p, from the same host-side selection, without a device: validates p
+ * like grl_tc_gemm (pointers are only tested for NULL, never dereferenced) and fills *out. */
+typedef struct {
+  int32_t bn;       /* N tile width: 64, 128, 192 or 256 */
+  int32_t epi_mode; /* 0 = 16-bit outputs only, 1 = fp32 staging (whole row in one tile), 2 = direct per-row stores */
+  int32_t conv;     /* 1 = implicit-GEMM 3x3 conv (taps == 9) */
+  int32_t n_tiles;  /* N tiles of one row tile */
+  int32_t nk_total; /* 64-wide k chunks through the 4-stage operand ring: taps * kpad / 64 */
+  int64_t grid;     /* CTAs: row tiles (conv: 8 x 16 pixel patches of every image) x n_tiles */
+} GrlTcGemmPath;
+int grl_tc_gemm_path(const GrlTcGemm* p, GrlTcGemmPath* out);
 
 /* Fused cosine attention over packed bf16 head slots: out = softmax2(q k^T + bias + mask) v, one call per
  * WindowAttention.forward and two per AnchorStripeAttention.forward (efficient.py:128-165,:215-270).

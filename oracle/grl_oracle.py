@@ -335,6 +335,140 @@ def attn_launch_reference(q, k, v, table, index, mask, dtype, mutation=None, max
     return exact, emul, info
 
 
+GEMM_TILE_M = 128       # accumulator rows per CTA of gemm_tc_kernel (kBM)
+GEMM_CONV_PATCH = (8, 16)  # conv row tile: an 8 x 16 pixel patch (kTH, kTW)
+GEMM_K_CHUNK = 64       # k per stage of the operand ring (kBK)
+GELU_AS_ABS_ERR = 5e-7  # max |gelu_as - erf GELU| over fp32 inputs (tests/test_gpu_tc_gemm.py::test_gelu_as_bound)
+
+
+def gelu_as_emulate(x):
+    """gemm_tc.cu's gelu_as in numpy float32 with a correctly rounded reciprocal and exp2 (the hardware's .approx
+    errors are not modelled) and fmaf as one rounding of the float64 result.  x: float32 ndarray."""
+    import numpy as np
+
+    f = np.float32
+
+    def fma(a, b, c):
+        return (a.astype(np.float64) * b + c).astype(f)
+
+    z = np.abs(x) * f(0.70710678118654752440)
+    t = (1.0 / fma(f(0.3275911), z, f(1.0)).astype(np.float64)).astype(f)
+    e = np.exp2(((-z * z) * f(1.4426950408889634)).astype(np.float64)).astype(f)
+    p = fma(f(1.061405429), t, f(-1.453152027))
+    p = fma(p, t, f(1.421413741))
+    p = fma(p, t, f(-0.284496736))
+    p = fma(p, t, f(0.254829592))
+    erf_abs = fma(-p * t, e, f(1.0))
+    half_x = f(0.5) * x
+    return fma(half_x, np.copysign(erf_abs, x), half_x)
+
+
+def _gelu(v, tanh=False):
+    if tanh:
+        return 0.5 * v * (1 + torch.tanh((2 / torch.pi) ** 0.5 * (v + 0.044715 * v ** 3)))
+    return 0.5 * v * (1 + torch.special.erf(v * 0.5 ** 0.5))
+
+
+def gemm_launch_reference(x, w, bias, *, taps=1, epi=0, act=0, slope=0.0, n_res=0, res=None, slot_scale=None, gamma=None,
+                          beta=None, eps=1e-5, res_scale=1.0, cab_y=None, cab_gate=None, L=1, ps_r=0, nchw_r=0, crop=None,
+                          post_scale=1.0, post_shift=None, bn=None, mutation=None):
+    """One grl_tc_gemm launch in float64 on x's device, from the 16-bit operand values (gemm_tc.cu; include/grl_b200.h).
+
+    x: (M, K) rows, or (B, H, W, K) channels-last when taps == 9 (3 x 3 conv, zero padding); w (N, taps K) with
+    k = tap K + c, tap = 3 dy + dx; bias (N,).  epi 0: act(acc + b) (act 1 = erf GELU, 2 = LeakyReLU(slope)) + res on the
+    first n_res columns; epi 1: every 32-wide slot with slot_scale > 0 becomes (acc + b) scale / max(||acc + b||, 1e-12);
+    epi 2: res + res_scale LayerNorm(acc + b) over the first C = len(gamma) columns (two-pass moments, biased variance)
+    + cab_y cab_gate[row // L].  Returns {"y": (rows, N or C) in token order}, plus "ps" (B, H r, W r, N / r^2) for the
+    PixelShuffle store (column n = q N / r^2 + c) and "nchw" (B, N / r^2, Hc, Wc) = y post_scale + post_shift[c] for the
+    NCHW tail (torch channel order n = c r^2 + q), cropped to crop = (Hc, Wc).
+
+    mutation imitates a kernel bug: "bias_tile_local" / "slot_scale_per_tile" (index by the column inside the bn-wide N
+    tile), "drop_kchunk" (k chunk 4 of 64, the first that reuses a ring stage, is skipped), "taps_transposed" (dy <-> dx),
+    "ln_unbiased" (variance over n - 1), "ln_no_eps", "ln_naive_fp32" (E[x^2] - E[x]^2 in float32),
+    "cab_gate_per_tile" (every row takes the gate of its row tile's first row), "no_residual_last_tile" (the last row tile
+    / pixel patch adds no residual), "gelu_tanh", "ps_swapped" (PixelShuffle store with q and c swapped)."""
+    f = torch.float64
+    dev = x.device
+    x, w, bias = x.to(f), w.to(f).clone(), bias.to(f).clone()
+    conv = taps == 9
+    K = x.shape[-1]
+    N = w.shape[0]
+    if mutation == "drop_kchunk":
+        w[:, 4 * GEMM_K_CHUNK:5 * GEMM_K_CHUNK] = 0
+    if conv:
+        B, H, W, _ = x.shape
+        xp = F.pad(x, (0, 0, 1, 1, 1, 1))
+        acc = torch.zeros(B, H, W, N, dtype=f, device=dev)
+        for t in range(9):
+            dy, dx = divmod(t, 3)
+            if mutation == "taps_transposed":
+                dy, dx = dx, dy
+            acc += xp[:, dy:dy + H, dx:dx + W] @ w[:, t * K:(t + 1) * K].T
+        acc = acc.reshape(-1, N)
+        py, px = GEMM_CONV_PATCH
+        yy, xx = torch.meshgrid(torch.arange(H, device=dev), torch.arange(W, device=dev), indexing="ij")
+        tile = ((torch.arange(B, device=dev)[:, None, None] * -(-H // py) + yy // py) * -(-W // px) + xx // px).reshape(-1)
+    else:
+        acc = x @ w.T
+        tile = torch.arange(acc.shape[0], device=dev) // GEMM_TILE_M
+    cols = torch.arange(N, device=dev)
+    if mutation == "bias_tile_local":
+        bias = bias[cols % bn]
+    v = acc + bias
+    last = tile == tile.max()
+    if res is not None:
+        res = res.to(f).reshape(v.shape[0], -1).clone()
+        if mutation == "no_residual_last_tile":
+            res[last] = 0
+    if epi == 0:
+        if act == 1:
+            v = _gelu(v, mutation == "gelu_tanh")
+        elif act == 2:
+            v = torch.where(v > 0, v, v * slope)
+        if res is not None:
+            v[:, :n_res] += res[:, :n_res]
+    elif epi == 1:
+        s = v.reshape(v.shape[0], -1, 32)
+        sc = slot_scale.to(dev, f)
+        if mutation == "slot_scale_per_tile":
+            sc = sc[(cols[::32] % bn) // 32]
+        nrm = s.pow(2).sum(-1, keepdim=True).sqrt().clamp_min(1e-12)
+        v = torch.where(sc[None, :, None] > 0, s * sc[None, :, None] / nrm, s).reshape(v.shape)
+    else:
+        C = gamma.numel()
+        u = v[:, :C]
+        if mutation == "ln_naive_fp32":
+            u32 = u.float()
+            mean = u32.mean(-1, keepdim=True)
+            var = (u32 * u32).mean(-1, keepdim=True) - mean * mean
+            mean, var = mean.to(f), var.to(f)
+        else:
+            mean = u.mean(-1, keepdim=True)
+            var = (u - mean).pow(2).sum(-1, keepdim=True) / (C - 1 if mutation == "ln_unbiased" else C)
+        e = 0.0 if mutation == "ln_no_eps" else eps
+        v = (u - mean) / torch.sqrt(var + e) * gamma.to(dev, f) + beta.to(dev, f)
+        v = res[:, :C] + res_scale * v
+        if cab_y is not None:
+            rows = torch.arange(v.shape[0], device=dev)
+            if mutation == "cab_gate_per_tile":
+                rows = rows // GEMM_TILE_M * GEMM_TILE_M
+            v = v + cab_y.to(f).reshape(v.shape[0], -1)[:, :C] * cab_gate.to(dev, f)[rows // L]
+    out = {"y": v}
+    if ps_r:
+        r, Bi, Hi, Wi = ps_r, *x.shape[:3]
+        if mutation == "ps_swapped":  # column n read as torch's c r^2 + q
+            t = v.reshape(Bi, Hi, Wi, -1, r, r).permute(0, 1, 4, 2, 5, 3)
+        else:
+            t = v.reshape(Bi, Hi, Wi, r, r, -1).permute(0, 1, 3, 2, 4, 5)
+        out["ps"] = t.reshape(Bi, Hi * r, Wi * r, -1)
+    if nchw_r:
+        r, Bi, Hi, Wi = nchw_r, *x.shape[:3]
+        t = v[:, :n_res].reshape(Bi, Hi, Wi, -1, r, r).permute(0, 3, 1, 4, 2, 5).reshape(Bi, -1, Hi * r, Wi * r)
+        t = t[:, :, :crop[0], :crop[1]] * post_scale
+        out["nchw"] = t + torch.tensor(list(post_shift)[:t.shape[1]], dtype=f, device=dev)[None, :, None, None]
+    return out
+
+
 def window_attention(sd, pre, qkv, x_size, ws, heads, shifted, table, index, mask):
     """mixed_attn_block_efficient.py:128-165."""
     H, W = x_size
