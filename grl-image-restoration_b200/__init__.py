@@ -6,8 +6,9 @@ from .modules import (  # noqa: F401
     EfficientMixAttnTransformerBlock, MixedAttention, Mlp, QKVProjection, TransformerStage, Upsample, UpsampleOneStep,
     WindowAttention, build_last_conv,
 )
+from .functional import demosaic  # noqa: F401
 
 __all__ = ["GRL", "TransformerStage", "EfficientMixAttnTransformerBlock", "MixedAttention", "WindowAttention",
            "AnchorStripeAttention", "AffineTransform", "CAB", "ChannelAttention", "Mlp", "QKVProjection",
            "AnchorProjection", "AnchorLinear", "CPB_MLP", "Upsample", "UpsampleOneStep", "build_last_conv",
-           "configs", "geometry"]
+           "configs", "geometry", "demosaic"]

@@ -11,7 +11,7 @@ _PKG = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_PKG, "libgrl_b200.so")
 HEADER_PATH = os.path.join(os.path.dirname(_PKG), "include", "grl_b200.h")
 
-ABI_VERSION = 5
+ABI_VERSION = 6
 c_int, c_i64, c_f32, c_vp, c_sz = ctypes.c_int, ctypes.c_int64, ctypes.c_float, ctypes.c_void_p, ctypes.c_size_t
 
 
@@ -65,6 +65,7 @@ _SIGNATURES = {
     "grl_tc_pack16": (c_int, [c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_vp]),
     "grl_tc_unpack16": (c_int, [c_vp, c_i64, c_int, c_vp, c_i64, c_i64, c_int, c_int, c_vp]),
     "grl_tc_head_pack": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(c_f32), c_f32, c_vp, c_int, c_vp, c_int, c_vp]),
+    "grl_tc_head_pack_rggb": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(c_f32), c_f32, c_vp, c_int, c_vp, c_int, c_vp]),
     "grl_tc_avgpool16": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp]),
     "grl_tc_slot_scale": (c_int, [c_vp, c_vp, c_vp, c_int, c_int, c_vp, c_vp]),
     "grl_tc_channel_gate_workspace": (c_sz, [c_int, c_i64, c_int]),
@@ -88,6 +89,8 @@ _SIGNATURES = {
     "grl_d8_index_host": (c_int, [c_int, c_int, c_int, c_int, c_vp]),
     "grl_ens_gather_f32": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp]),
     "grl_ens_merge_f32": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp]),
+    "grl_demosaic_host": (c_int, [c_vp, c_int, c_int, c_int, c_vp]),
+    "grl_demosaic_f32": (c_int, [c_vp, c_int, c_int, c_int, c_vp, c_vp]),
 }
 
 _lib = None

@@ -3,6 +3,7 @@
 #include <string.h>
 
 #include "grl_common.cuh"
+#include "grl_demosaic.h"
 #include "ops_f32.h"
 #include "ops_tc.h"
 
@@ -242,6 +243,12 @@ int grl_tc_head_pack(const float* x, int B, int Cin, int H, int W, int Hp, int W
   GRL_REQUIRE(x && y16, "head_pack: null argument");
   return tc::launch_head_pack(x, B, Cin, H, W, Hp, Wp, mean4, range, y16, Cpad, y32, fmt, (cudaStream_t)stream);
 }
+int grl_tc_head_pack_rggb(const float* cfa4, int B, int h, int w, int Hp, int Wp, const float* mean4, float range, void* y16,
+                          int Cpad, float* y32, int fmt, void* stream) {
+  if (check_fmt(fmt)) return GRL_ERR_INVALID;
+  GRL_REQUIRE(cfa4 && y16, "head_pack_rggb: null argument");
+  return tc::launch_head_pack_rggb(cfa4, B, h, w, Hp, Wp, mean4, range, y16, Cpad, y32, fmt, (cudaStream_t)stream);
+}
 int grl_tc_avgpool16(const void* x, void* y, int B, int H, int W, int Cpad, int df, int fmt, void* stream) {
   if (check_fmt(fmt)) return GRL_ERR_INVALID;
   return tc::launch_avgpool_bf16(x, y, B, H, W, Cpad, df, fmt, (cudaStream_t)stream);
@@ -380,6 +387,22 @@ int grl_ens_gather_f32(const float* x, int B, int C, int H, int W, int group, fl
 
 int grl_ens_merge_f32(const float* ya, const float* yb, int B, int C, int Hs, int Ws, float* y, void* stream) {
   return launch_ens_merge(ya, yb, B, C, Hs, Ws, y, (cudaStream_t)stream);
+}
+
+// ---------------------------------------------------------------- demosaicking
+int grl_demosaic_host(const float* cfa4, int B, int h, int w, float* out) {
+  GRL_REQUIRE(cfa4 && out && B >= 0 && h >= 2 && w >= 2, "demosaic_host: bad arguments B=%d h=%d w=%d", B, h, w);
+  const int H = 2 * h, W = 2 * w;
+  for (int b = 0; b < B; ++b)
+    for (int c = 0; c < 3; ++c)
+      for (int y = 0; y < H; ++y)
+        for (int x = 0; x < W; ++x)
+          out[(((size_t)b * 3 + c) * H + y) * W + x] = dm_pixel(cfa4 + (size_t)b * 4 * h * w, h, w, c, y, x);
+  return GRL_OK;
+}
+
+int grl_demosaic_f32(const float* cfa4, int B, int h, int w, float* out, void* stream) {
+  return launch_demosaic(cfa4, B, h, w, out, (cudaStream_t)stream);
 }
 
 }  // extern "C"

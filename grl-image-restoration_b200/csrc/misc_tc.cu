@@ -1,6 +1,8 @@
-// misc_tc.cu -- small memory-bound kernels around the tensor-core path: fp32 -> padded bf16 packing, bf16 average
-// pooling (anchors), channel means of the CAB features, per-block preparation of the attention constants.
+// misc_tc.cu -- small memory-bound kernels around the tensor-core path: the network head (from RGB planes or from packed
+// Bayer planes), fp32 -> padded bf16 packing, bf16 average pooling (anchors), channel means of the CAB features, per-block
+// preparation of the attention constants.
 #include "grl_common.cuh"
+#include "grl_demosaic.h"
 #include "ops_tc.h"
 #include "tc_common.cuh"
 
@@ -63,13 +65,28 @@ __global__ void avgpool_bf16_kernel(const uint16_t* __restrict__ x, uint16_t* __
 }
 
 // Network input: check_image_size (reflect pad to a multiple of pad_size, grl.py:479-489) + (x - mean) * img_range
-// (grl.py:510-511) + bchw -> channels-last + 16-bit operand pack, one pass.  One thread per padded pixel.
+// (grl.py:510-511) + bchw -> channels-last + 16-bit operand pack, one pass.  One thread per padded pixel; Src reads raw
+// channel c of image b at the source pixel (ys, xs) the padding maps the padded pixel to.
 struct HeadMean {
   float m[4];
 };
-__global__ void head_pack_kernel(const float* __restrict__ x, int B, int Cin, int H, int W, int Hp, int Wp, HeadMean mean,
-                                 float range, int reflect, uint16_t* __restrict__ y16, int Cpad, float* __restrict__ y32,
-                                 int fmt) {
+struct PlanarSrc {  // (B, Cin, H, W) planes
+  const float* x;
+  int Cin, H, W;
+  __device__ __forceinline__ float operator()(int b, int c, int ys, int xs) const {
+    return x[(((long long)b * Cin + c) * H + ys) * W + xs];
+  }
+};
+struct RggbSrc {  // packed RGGB planes (B, 4, h, w), demosaiced on the fly (dm_matlab, grl_demosaic.h)
+  const float* cfa4;
+  int h, w;
+  __device__ __forceinline__ float operator()(int b, int c, int ys, int xs) const {
+    return dm_pixel(cfa4 + (long long)b * 4 * h * w, h, w, c, ys, xs);
+  }
+};
+template <class Src>
+__global__ void head_pack_kernel(Src src, int B, int Cin, int H, int W, int Hp, int Wp, HeadMean mean, float range,
+                                 int reflect, uint16_t* __restrict__ y16, int Cpad, float* __restrict__ y32, int fmt) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (long long)B * Hp * Wp) return;
   const int xp = (int)(i % Wp);
@@ -85,7 +102,7 @@ __global__ void head_pack_kernel(const float* __restrict__ x, int B, int Cin, in
   }
   float v[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
   for (int c = 0; c < Cin; ++c) {
-    const float raw = inside ? x[(((long long)b * Cin + c) * H + ys) * W + xs] : 0.f;
+    const float raw = inside ? src(b, c, ys, xs) : 0.f;
     v[c] = (raw - mean.m[c]) * range;
     if (y32) y32[i * Cin + c] = v[c];
   }
@@ -127,8 +144,9 @@ __global__ void slot_scale_kernel(const float* __restrict__ ls_w, const float* _
   }
 }
 
-int launch_head_pack(const float* x, int B, int Cin, int H, int W, int Hp, int Wp, const float* mean4, float range, void* y16,
-                     int Cpad, float* y32, int fmt, cudaStream_t st) {
+template <class Src>
+static int launch_head(Src src, int B, int Cin, int H, int W, int Hp, int Wp, const float* mean4, float range, void* y16,
+                       int Cpad, float* y32, int fmt, cudaStream_t st) {
   GRL_REQUIRE(Cin >= 1 && Cin <= 4 && Cpad % 8 == 0 && Cpad >= 8 && Hp >= H && Wp >= W && H > 0 && W > 0,
               "head_pack: bad shape (Cin %d, %dx%d -> %dx%d, Cpad %d)", Cin, H, W, Hp, Wp, Cpad);
   const long long total = (long long)B * Hp * Wp;
@@ -136,9 +154,18 @@ int launch_head_pack(const float* x, int B, int Cin, int H, int W, int Hp, int W
   HeadMean m;
   for (int c = 0; c < 4; ++c) m.m[c] = mean4 ? mean4[c] : 0.f;
   const int reflect = (Hp - H < H && Wp - W < W) ? 1 : 0;  // torch raises otherwise and the reference pads with zeros
-  head_pack_kernel<<<ceil_div(total, 256), 256, 0, st>>>(x, B, Cin, H, W, Hp, Wp, m, range, reflect, (uint16_t*)y16, Cpad, y32, fmt);
+  head_pack_kernel<<<ceil_div(total, 256), 256, 0, st>>>(src, B, Cin, H, W, Hp, Wp, m, range, reflect, (uint16_t*)y16, Cpad, y32, fmt);
   GRL_LAUNCH_CHECK("head_pack_kernel");
   return GRL_OK;
+}
+int launch_head_pack(const float* x, int B, int Cin, int H, int W, int Hp, int Wp, const float* mean4, float range, void* y16,
+                     int Cpad, float* y32, int fmt, cudaStream_t st) {
+  return launch_head(PlanarSrc{x, Cin, H, W}, B, Cin, H, W, Hp, Wp, mean4, range, y16, Cpad, y32, fmt, st);
+}
+int launch_head_pack_rggb(const float* cfa4, int B, int h, int w, int Hp, int Wp, const float* mean4, float range, void* y16,
+                          int Cpad, float* y32, int fmt, cudaStream_t st) {
+  GRL_REQUIRE(h >= 2 && w >= 2, "head_pack_rggb: packed RGGB planes need h, w >= 2, got %dx%d", h, w);
+  return launch_head(RggbSrc{cfa4, h, w}, B, 3, 2 * h, 2 * w, Hp, Wp, mean4, range, y16, Cpad, y32, fmt, st);
 }
 int launch_pack_bf16(const float* x, long long ldx, void* y, long long M, int C, int Cpad, int fmt, cudaStream_t st) {
   GRL_REQUIRE(Cpad % 8 == 0 && Cpad >= C, "pack_bf16: bad padding %d for %d channels", Cpad, C);

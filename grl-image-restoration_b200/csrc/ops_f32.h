@@ -68,5 +68,7 @@ int launch_psnr(const float* restored, const float* target, int B, int C, int H,
 // x8 self-ensemble: the 4 views of one group, and the ordered average of the 8 mapped-back outputs (ensemble.cu)
 int launch_ens_gather(const float* x, int B, int C, int H, int W, int group, float* views, cudaStream_t st);
 int launch_ens_merge(const float* ya, const float* yb, int B, int C, int Hs, int Ws, float* y, cudaStream_t st);
+// dm_matlab: packed RGGB planes (B, 4, h, w) -> RGB (B, 3, 2h, 2w) (demosaic.cu)
+int launch_demosaic(const float* cfa4, int B, int h, int w, float* out, cudaStream_t st);
 
 }  // namespace grl

@@ -100,6 +100,9 @@ namespace tc {
 // 16-bit pack of the network input: x (B, Cin, H, W) fp32 -> y16 (B, Hp, Wp, Cpad) and, optionally, y32 (B, Hp, Wp, Cin)
 int launch_head_pack(const float* x, int B, int Cin, int H, int W, int Hp, int Wp, const float* mean4, float range, void* y16,
                      int Cpad, float* y32, int fmt, cudaStream_t st);
+// the same from packed RGGB planes (B, 4, h, w): the input pixel is dm_matlab of the planes at the source pixel, Cin = 3
+int launch_head_pack_rggb(const float* cfa4, int B, int h, int w, int Hp, int Wp, const float* mean4, float range, void* y16,
+                          int Cpad, float* y32, int fmt, cudaStream_t st);
 int launch_pack_bf16(const float* x, long long ldx, void* y, long long M, int C, int Cpad, int fmt, cudaStream_t st);
 int launch_unpack_bf16(const void* x, long long ldx, int x_off, float* y, long long ldy, long long M, int C, int fmt,
                        cudaStream_t st);

@@ -191,6 +191,33 @@ def ens_merge(ya, yb, B):
     return y
 
 
+def _cfa4(x):
+    x = _f32c(x, "cfa4")
+    if x.dim() != 4 or x.shape[1] != 4 or x.shape[2] < 2 or x.shape[3] < 2:
+        raise ValueError(f"grl_b200: packed RGGB Bayer planes must be (B, 4, h, w) with h, w >= 2, got {tuple(x.shape)}")
+    return x
+
+
+def demosaic(x):
+    """The reference's dm_matlab (utils/utils_mosaic.py:36-111), the dm task's input transform (engines/base.py:127-128):
+    packed RGGB planes x (B, 4, h, w) float32 on the GPU (R, G of the even rows, G of the odd rows, B) -> RGB
+    (B, 3, 2h, 2w) float32.  One sm_90a kernel; GRL(input_format="rggb") fuses the same arithmetic into its head."""
+    x = _cfa4(x)
+    B, _, h, w = x.shape
+    y = torch.empty(B, 3, 2 * h, 2 * w, device=x.device, dtype=torch.float32)
+    capi.check(capi.lib().grl_demosaic_f32(capi.ptr(x), B, h, w, capi.ptr(y), capi.stream()))
+    return y
+
+
+def demosaic_host(x):
+    """demosaic evaluated on the CPU by the library's host copy of the same closed form (tests)."""
+    x = x.float().contiguous()
+    B, _, h, w = x.shape
+    y = torch.empty(B, 3, 2 * h, 2 * w, dtype=torch.float32)
+    capi.check(capi.lib().grl_demosaic_host(ctypes.c_void_p(x.data_ptr()), B, h, w, ctypes.c_void_p(y.data_ptr())))
+    return y
+
+
 def stripe_attention(qkv, anchor, B, tok_grid, anc_grid, heads, scale1, bias1, scale2, bias2, use_mask, out=None):
     """qkv (B, L, 3c) view (stripe half), anchor (B, Ha, Wa, c) -> (B, L, c)."""
     qp, ldq = _token_rows(qkv, "qkv")

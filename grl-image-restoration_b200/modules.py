@@ -552,12 +552,21 @@ class GRL(nn.Module):
                  anchor_one_stage=True, anchor_window_down_factor=1, out_proj_type="linear", local_connection=False,
                  drop_rate=0.0, attn_drop_rate=0.0, drop_path_rate=0.1, norm_layer=nn.LayerNorm,
                  pretrained_window_size=[0, 0], pretrained_stripe_size=[0, 0], conv_type="1conv", init_method="n",
-                 fairscale_checkpoint=False, offload_to_cpu=False, euclidean_dist=False, self_ensemble=False, **kwargs):
+                 fairscale_checkpoint=False, offload_to_cpu=False, euclidean_dist=False, self_ensemble=False,
+                 input_format="rgb", **kwargs):
         super().__init__()
         # x8 geometric self-ensemble in forward (off: the reference's forward).  Views are forwarded in chunks of at most
         # ensemble_max_batch images, which bounds the activation memory of the 8x larger batch.
         self.self_ensemble = bool(self_ensemble)
         self.ensemble_max_batch = 16
+        # "rggb": forward takes the dm task's packed RGGB Bayer planes (B, 4, h, w) and demosaics them on the device with
+        # the reference engine's dm_matlab (engines/base.py:127-128) before the network; "rgb" (default): the reference's
+        # forward.  Feed "rggb" only data that the caller has not demosaiced already.
+        if input_format not in ("rgb", "rggb"):
+            raise ValueError(f"input_format must be 'rgb' or 'rggb', got {input_format!r}")
+        if input_format == "rggb" and in_channels != 3:
+            raise ValueError(f"input_format='rggb' demosaics to 3 channels, but in_channels={in_channels}")
+        self.input_format = input_format
         self._requested_precision = kwargs.pop("precision", None) or os.environ.get("GRL_B200_PRECISION", "fp32")
         out_channels = out_channels or in_channels
         self.in_channels, self.out_channels = in_channels, out_channels
@@ -771,15 +780,18 @@ class GRL(nn.Module):
         return t.view(B, H, W, C)
 
     @torch.no_grad()
-    def _forward_bf16(self, x):
-        """grl.py:506-551 on the tensor-core kernels; x is the RAW (B, Cin, H, W) fp32 input.  Head: one kernel does
-        check_image_size + (x - mean) * img_range + bchw -> bhwc + operand pack; tail: the last conv's epilogue writes
-        x / img_range + mean, cropped, as bchw planes; PixelShuffle is a store-address pattern of the conv before it."""
+    def _forward_bf16(self, x, rggb=False):
+        """grl.py:506-551 on the tensor-core kernels; x is the RAW (B, Cin, H, W) fp32 input, or with rggb its packed
+        (B, 4, H/2, W/2) Bayer planes.  Head: one kernel does [dm_matlab +] check_image_size + (x - mean) * img_range +
+        bchw -> bhwc + operand pack; tail: the last conv's epilogue writes x / img_range + mean, cropped, as bchw planes;
+        PixelShuffle is a store-address pattern of the conv before it."""
         from . import tc
 
         dev = x.device
         fmt = tc.FMT[self.precision]
         B, Cin, H, W = x.shape
+        if rggb:
+            Cin, H, W = 3, 2 * H, 2 * W
         Hp = (H + self.pad_size - 1) // self.pad_size * self.pad_size
         Wp = (W + self.pad_size - 1) // self.pad_size * self.pad_size
         C = self.embed_dim
@@ -787,7 +799,8 @@ class GRL(nn.Module):
         s = self.upscale
         need_res = self.upsampler not in ("pixelshuffle", "pixelshuffledirect", "nearest+conv") and self.in_channels == self.out_channels
         mean = self._mean_list
-        x16, xc32 = tc.head_pack(x, Hp, Wp, mean, self.img_range, 64, fmt, want_f32=need_res)
+        head = tc.head_pack_rggb if rggb else tc.head_pack
+        x16, xc32 = head(x, Hp, Wp, mean, self.img_range, 64, fmt, want_f32=need_res)
         shift = mean if len(mean) > 1 else mean * 4
 
         def conv(name, module, inp16, cin_pad, *, act=K.ACT_NONE, slope=0.0, res=None, want_f32=False, want16=True, ps_r=0,
@@ -852,11 +865,11 @@ class GRL(nn.Module):
         return super().load_state_dict(*args, **kwargs)
 
     @torch.no_grad()
-    def _forward_graphed(self, x):
-        """Replays a captured graph of _forward_bf16 for this input shape (captures it on first use, after two eager
-        warm-up forwards that build the packed weights / bias tables / kernel attributes).  The result is a fresh tensor
-        (the caller may mutate it in place, engines/base.py:113)."""
-        key = (tuple(x.shape), x.device.index, self.precision)
+    def _forward_graphed(self, x, rggb=False):
+        """Replays a captured graph of _forward_bf16 for this input shape and format (captures it on first use, after two
+        eager warm-up forwards that build the packed weights / bias tables / kernel attributes).  The result is a fresh
+        tensor (the caller may mutate it in place, engines/base.py:113)."""
+        key = (tuple(x.shape), x.device.index, self.precision, "rggb" if rggb else "rgb")
         ent = self._graphs.get(key)
         if ent is None:
             static_in = x.clone()
@@ -864,11 +877,11 @@ class GRL(nn.Module):
             side.wait_stream(torch.cuda.current_stream())
             with torch.cuda.stream(side):
                 for _ in range(2):
-                    self._forward_bf16(static_in)
+                    self._forward_bf16(static_in, rggb)
             torch.cuda.current_stream().wait_stream(side)
             graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(graph):
-                static_out = self._forward_bf16(static_in)
+                static_out = self._forward_bf16(static_in, rggb)
             ent = (graph, static_in, static_out)
             self._graphs[key] = ent
         graph, static_in, static_out = ent
@@ -883,6 +896,23 @@ class GRL(nn.Module):
 
     @torch.no_grad()
     def forward(self, x):
+        K.capi.require_device(x)
+        if self.input_format == "rgb":
+            return self.forward_rgb(x)
+        if self.input_format != "rggb":
+            raise ValueError(f"input_format must be 'rgb' or 'rggb', got {self.input_format!r}")
+        if self.in_channels != 3 or x.dim() != 4 or x.shape[1] != 4 or x.shape[2] < 2 or x.shape[3] < 2:
+            raise ValueError(f"input_format='rggb' takes packed RGGB Bayer planes (B, 4, h, w) with h, w >= 2 and a "
+                             f"3-channel network; got input {tuple(x.shape)}, in_channels={self.in_channels}")
+        cfa = x.float().contiguous()
+        if self.precision == "fp32" or self.self_ensemble:
+            # demosaic once, then the RGB forward (the engine's order: the ensemble's views are views of the RGB image)
+            return self.forward_rgb(K.demosaic(cfa)).to(x.dtype)
+        return self._forward_once(cfa, rggb=True).to(x.dtype)
+
+    @torch.no_grad()
+    def forward_rgb(self, x):
+        """The forward on a (B, in_channels, H, W) image whatever input_format says (self_ensemble applies)."""
         K.capi.require_device(x)
         return self._forward_self_ensemble(x) if self.self_ensemble else self._forward_once(x)
 
@@ -911,12 +941,15 @@ class GRL(nn.Module):
         return outs[0] if len(outs) == 1 else torch.cat(outs)
 
     @torch.no_grad()
-    def _forward_once(self, x):
+    def _forward_once(self, x, rggb=False):
+        """One forward on the tensor-core or fp32 kernels; rggb (tensor-core path only): x is packed Bayer planes and the
+        demosaic runs inside the head kernel."""
         H, W = x.shape[2:]
         if self.precision != "fp32":
             xin = x.float().contiguous()
-            y = self._forward_graphed(xin) if self.use_cuda_graph else self._forward_bf16(xin)
+            y = self._forward_graphed(xin, rggb) if self.use_cuda_graph else self._forward_bf16(xin, rggb)
             return y.to(x.dtype)
+        assert not rggb, "the fp32 path demosaics in forward"
         x = self.check_image_size(x)
         self.mean = self.mean.type_as(x)
         x = ((x - self.mean) * self.img_range).float()

@@ -48,17 +48,31 @@ def _h16(*shape, device, fmt, zero=False):
     return (torch.zeros if zero else torch.empty)(*shape, device=device, dtype=DTYPE[fmt])
 
 
+def _mean4(mean):
+    m = [float(v) for v in (mean if isinstance(mean, (list, tuple)) else mean.flatten().tolist())]
+    m = (m * 4)[:4] if len(m) == 1 else (m + [0.0] * 4)[:4]
+    return (ctypes.c_float * 4)(*m)
+
+
 def head_pack(x, hp, wp, mean, img_range, cpad=64, fmt=0, want_f32=False):
     """Network input (B, Cin, H, W) fp32 -> 16-bit channels-last (B, hp, wp, cpad) [+ fp32 (B, hp, wp, Cin)]: reflect pad,
     (x - mean) * img_range, layout change and operand pack in one kernel (grl_tc_head_pack)."""
     B, Cin, H, W = x.shape
     y16 = _h16(B, hp, wp, cpad, device=x.device, fmt=fmt)
     y32 = torch.empty(B, hp, wp, Cin, device=x.device, dtype=torch.float32) if want_f32 else None
-    m = [float(v) for v in (mean if isinstance(mean, (list, tuple)) else mean.flatten().tolist())]
-    m = (m * 4)[:4] if len(m) == 1 else (m + [0.0] * 4)[:4]
-    arr = (ctypes.c_float * 4)(*m)
-    capi.check(capi.lib().grl_tc_head_pack(capi.ptr(x), B, Cin, H, W, hp, wp, arr, float(img_range), capi.ptr(y16), cpad,
-                                           capi.ptr(y32), fmt, capi.stream()))
+    capi.check(capi.lib().grl_tc_head_pack(capi.ptr(x), B, Cin, H, W, hp, wp, _mean4(mean), float(img_range), capi.ptr(y16),
+                                           cpad, capi.ptr(y32), fmt, capi.stream()))
+    return y16, y32
+
+
+def head_pack_rggb(cfa4, hp, wp, mean, img_range, cpad=64, fmt=0, want_f32=False):
+    """head_pack of K.demosaic(cfa4) in one kernel (grl_tc_head_pack_rggb): packed RGGB planes (B, 4, h, w) fp32 ->
+    (B, hp, wp, cpad) [+ fp32 (B, hp, wp, 3)] for the (2h, 2w) image, without writing the RGB image."""
+    B, _, h, w = cfa4.shape
+    y16 = _h16(B, hp, wp, cpad, device=cfa4.device, fmt=fmt)
+    y32 = torch.empty(B, hp, wp, 3, device=cfa4.device, dtype=torch.float32) if want_f32 else None
+    capi.check(capi.lib().grl_tc_head_pack_rggb(capi.ptr(cfa4), B, h, w, hp, wp, _mean4(mean), float(img_range),
+                                                capi.ptr(y16), cpad, capi.ptr(y32), fmt, capi.stream()))
     return y16, y32
 
 
@@ -493,11 +507,14 @@ def conv_plan(owner, name, conv, cin_pad, fmt, ps_r=0):
 def gemm_launches(model, x_shape):
     """Descriptors of every tc.gemm / tc.conv3x3 launch of one tensor-core forward of GRL `model` on a (B, Cin, H, W)
     input, in launch order, with the arguments GRL._forward_bf16, TransformerStage.forward_tc and BlockPlan.run pass
-    (operand format: model.precision).  Host only: shapes come from the modules, nothing is packed or launched."""
+    (operand format: model.precision).  With model.input_format == "rggb", x_shape is the packed (B, 4, h, w) Bayer input
+    and the network runs on the (2h, 2w) image.  Host only: shapes come from the modules, nothing is packed or launched."""
     from torch import nn
 
     fmt = FMT[model.precision]
     B, Cin, H, W = x_shape
+    if getattr(model, "input_format", "rgb") == "rggb":
+        Cin, H, W = 3, 2 * H, 2 * W
     ps = model.pad_size
     Hp, Wp = round_up(H, ps), round_up(W, ps)
     L = Hp * Wp

@@ -9,6 +9,17 @@ global pool see the same data as in the reference), outputs are summed into E, a
 """
 import torch
 
+from . import functional as K
+
+
+def _rgb_frame(model, x):
+    """A model that takes packed Bayer planes (GRL input_format="rggb") is tiled on the demosaiced frame, the engine's
+    order (engines/base.py:127-128 before :90-116): demosaicing each tile on its own would reflect at the tile edges and
+    change the pixels there.  Returns the per-tile callable and the frame to cut."""
+    if getattr(model, "input_format", "rgb") == "rggb":
+        return model.forward_rgb, K.demosaic(x.float().contiguous()).to(x.dtype)
+    return model, x
+
 
 def tile_origins(size, tile, overlap):
     stride = tile - overlap
@@ -28,16 +39,18 @@ def _accumulate(E, W, origins, outs, tile, scale):
 
 @torch.no_grad()
 def forward_tile(model, x, tile, tile_overlap, scale=None, max_batch=16):
-    """x (B, C, H, W) on the GPU -> (B, C_out, H*scale, W*scale)."""
-    b, _, h, w = x.shape
+    """x (B, C, H, W) on the GPU -> (B, C_out, H*scale, W*scale); for an input_format="rggb" model x is (B, 4, H/2, W/2)
+    and the result is that of the demosaiced (H, W) frame."""
     scale = model.upscale if scale is None else scale
+    fn, x = _rgb_frame(model, x)
+    b, _, h, w = x.shape
     tile = min(tile, h, w)
     origins = _origins(b, h, w, tile, tile_overlap)
     E = W = None
     for i in range(0, len(origins), max_batch):
         chunk = origins[i:i + max_batch]
         patches = torch.stack([x[bi, :, hi:hi + tile, wi:wi + tile] for bi, hi, wi in chunk])
-        out = model(patches)
+        out = fn(patches)
         if E is None:
             E = torch.zeros(b, out.shape[1], h * scale, w * scale, device=x.device, dtype=out.dtype)
             W = torch.zeros_like(E)
@@ -62,8 +75,10 @@ def forward_tile_sharded(model, x, tile, tile_overlap, scale=None, max_batch=16,
     if not (dist.is_available() and dist.is_initialized()) or dist.get_world_size(group) == 1:
         return forward_tile(model, x, tile, tile_overlap, scale=scale, max_batch=max_batch)
     rank, world = dist.get_rank(group), dist.get_world_size(group)
-    b, _, h, w = x.shape
     scale = model.upscale if scale is None else scale
+    c_model = getattr(model, "out_channels", None)
+    fn, x = _rgb_frame(model, x)
+    b, _, h, w = x.shape
     tile = min(tile, h, w)
     origins = _origins(b, h, w, tile, tile_overlap)
     mine = shard_tiles(len(origins), rank, world)
@@ -72,12 +87,12 @@ def forward_tile_sharded(model, x, tile, tile_overlap, scale=None, max_batch=16,
     for i in range(0, len(mine), max_batch):
         chunk = [origins[j] for j in mine[i:i + max_batch]]
         patches = torch.stack([x[bi, :, hi:hi + tile, wi:wi + tile] for bi, hi, wi in chunk])
-        outs.append(model(patches))
+        outs.append(fn(patches))
     if outs:
         local = torch.cat(outs)
         c_out, dtype = local.shape[1], local.dtype
     else:  # more ranks than tiles: this rank only takes part in the exchange
-        c_out, dtype = getattr(model, "out_channels", x.shape[1]), x.dtype
+        c_out, dtype = c_model if c_model is not None else x.shape[1], x.dtype
         local = torch.zeros(0, c_out, tile * scale, tile * scale, device=x.device, dtype=dtype)
     send = torch.zeros(per_rank, c_out, tile * scale, tile * scale, device=x.device, dtype=dtype)
     send[: local.shape[0]] = local

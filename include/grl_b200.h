@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define GRL_B200_ABI_VERSION 5
+#define GRL_B200_ABI_VERSION 6
 
 typedef enum {
   GRL_OK = 0,
@@ -154,6 +154,12 @@ int grl_tc_unpack16(const void* x16, int64_t ldx, int x_off, float* y, int64_t l
  * channels-last copy (B, Hp, Wp, Cin) the no-upsampler heads add back (grl.py:540-547).  mean4: 4 HOST floats. */
 int grl_tc_head_pack(const float* x, int B, int Cin, int H, int W, int Hp, int Wp, const float* mean4, float range, void* y16,
                      int Cpad, float* y32, int fmt, void* stream);
+/* grl_tc_head_pack of the demosaiced image, with the demosaic fused in: cfa4 (B, 4, h, w) fp32 packed RGGB planes are the
+ * network input dm_matlab(cfa4) (utils/utils_mosaic.py:36-111; engines/base.py:127-128) of size (H, W) = (2h, 2w), Cin = 3.
+ * Each padded pixel is the demosaic at the source pixel check_image_size maps it to (zero pad as in grl_tc_head_pack), so
+ * the full-resolution RGB image is never written.  y32 as in grl_tc_head_pack.  h, w >= 2. */
+int grl_tc_head_pack_rggb(const float* cfa4, int B, int h, int w, int Hp, int Wp, const float* mean4, float range, void* y16,
+                          int Cpad, float* y32, int fmt, void* stream);
 /* AvgPool2d(df) on 16-bit channels-last data (AnchorLinear.pooling, mixed_attn_block.py:725). */
 int grl_tc_avgpool16(const void* x16, void* y16, int B, int H, int W, int Cpad, int df, int fmt, void* stream);
 /* Per-slot multipliers of the packed qkv layout [win q|k|v][stripe q|k|v] x heads: exp(min(logit_scale, ln100))*log2(e)
@@ -288,6 +294,16 @@ int grl_ens_gather_f32(const float* x, int B, int C, int H, int W, int group, fl
  * network output mapped back by the inverse of augment_img_tensor4(., m).  ya: group A outputs (4B, C, Hs, Ws); yb: group B
  * outputs (4B, C, Ws, Hs), both view-major (they may be the two halves of one tensor when Hs == Ws); y (B, C, Hs, Ws). */
 int grl_ens_merge_f32(const float* ya, const float* yb, int B, int C, int Hs, int Ws, float* y, void* stream);
+
+/* ---- demosaicking (the dm task's input, engines/base.py:127-128) ----------------------------------
+ * dm_matlab (utils/utils_mosaic.py:36-111): packed RGGB planes cfa4 (B, 4, h, w) fp32 (R, G at (even, odd), G at (odd,
+ * even), B; data/datasets/restoration_dm.py:33) -> RGB (B, 3, 2h, 2w) fp32.  The mosaic is reflect-padded by 2 and
+ * correlated with the four 5 x 5 filters; each channel keeps the raw mosaic value at its native sites and takes one
+ * filter's response at the others (utils_mosaic.py:97-109).  Every response is summed in the fixed tap order of
+ * csrc/grl_demosaic.h, so the host expansion and both kernels agree bit for bit.  h, w >= 2. */
+/* Host evaluation (tests): cfa4 and out are HOST pointers. */
+int grl_demosaic_host(const float* cfa4, int B, int h, int w, float* out);
+int grl_demosaic_f32(const float* cfa4, int B, int h, int w, float* out, void* stream);
 
 #ifdef __cplusplus
 }
