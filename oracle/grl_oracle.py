@@ -335,6 +335,52 @@ def attn_launch_reference(q, k, v, table, index, mask, dtype, mutation=None, max
     return exact, emul, info
 
 
+ATTN_F32_KEY_TILE = 32  # keys per online-softmax step of attn_f32_kernel (ops_f32.cu: kKT)
+
+
+def attn_f32_reference(q, k, v, logit_scale, table, index, mask, mutation=None, max_elems=1 << 25):
+    """One launch of the fp32 attention kernel (ops_f32.cu attn_f32_kernel) on gathered operands, in float64 on q's device.
+
+    q (Bw, h, Nq, d), k and v (Bw, h, Nk, d) as stored (q and k un-normalised: the kernel normalises them with the
+    F.normalize eps); logit_scale (h,) natural log, clamped at ln 100; table (h, rows) bias in natural units; index
+    (Nq, Nk) into it; mask (nW, Nq, Nk) of 0 / -100 (window w uses mask[w % nW]) or None.  Returns (Bw, h, Nq, d).
+
+    mutation imitates a kernel bug: "k_unnormalised", "scale_unclamped", "rescale_missing_l" (the running denominator
+    is not rescaled when a later key tile of ATTN_F32_KEY_TILE keys raises the row maximum)."""
+    f = torch.float64
+    dev = q.device
+    qn = F.normalize(q.to(f), dim=-1, eps=1e-12)
+    kn = k.to(f) if mutation == "k_unnormalised" else F.normalize(k.to(f), dim=-1, eps=1e-12)
+    ls = logit_scale.to(dev, f).reshape(-1)
+    sc = torch.exp(ls if mutation == "scale_unclamped" else ls.clamp(max=log(100.0)))[:, None, None]
+    bias = table.to(dev, f)[:, index.to(dev)]
+    mk = None if mask is None else mask.to(dev, f)
+    Bw, h, Nq, d = q.shape
+    Nk = k.shape[2]
+    out = torch.empty(Bw, h, Nq, d, dtype=f, device=dev)
+    step = max(1, max_elems // (h * Nq * Nk))
+    for w0 in range(0, Bw, step):
+        w1 = min(Bw, w0 + step)
+        x = qn[w0:w1] @ kn[w0:w1].transpose(-1, -2) * sc + bias
+        if mk is not None:
+            x = x + mk[torch.arange(w0, w1, device=dev) % mk.shape[0]].unsqueeze(1)
+        vv = v[w0:w1].to(f)
+        if mutation != "rescale_missing_l":
+            out[w0:w1] = torch.softmax(x, dim=-1) @ vv
+            continue
+        m = torch.full(x.shape[:-1], -float("inf"), dtype=f, device=dev)
+        l, o = torch.zeros_like(m), torch.zeros(*x.shape[:-1], d, dtype=f, device=dev)
+        for k0 in range(0, Nk, ATTN_F32_KEY_TILE):
+            xt = x[..., k0:k0 + ATTN_F32_KEY_TILE]
+            mn = torch.maximum(m, xt.amax(-1))
+            p = torch.exp(xt - mn[..., None])
+            o = o * torch.exp(m - mn)[..., None] + p @ vv[..., k0:k0 + ATTN_F32_KEY_TILE, :]
+            l = l + p.sum(-1)
+            m = mn
+        out[w0:w1] = o / l[..., None]
+    return out
+
+
 GEMM_TILE_M = 128       # accumulator rows per CTA of gemm_tc_kernel (kBM)
 GEMM_CONV_PATCH = (8, 16)  # conv row tile: an 8 x 16 pixel patch (kTH, kTW)
 GEMM_K_CHUNK = 64       # k per stage of the operand ring (kBK)

@@ -1,0 +1,1050 @@
+"""The fp32 parity path's kernels (csrc/ops_f32.cu) on every launch path the released configs take, against float64.
+
+Launch paths.  An attention launch's signature (`attn_path`) is the kernel specialisation plus its tile edges: the role
+(window, stripe pass 1, stripe pass 2: this fixes dense V and dense output), the head_dim template D, d < D, a partial
+and a second 128-query tile, a partial and a second 32-key tile, the shift mask and a non-zero roll.  A GEMM's
+(`gemm_path`) is conv or linear, a partial last 16-wide k tile, the number of k tiles, a partial and a second 64-wide N
+tile, the activation, bias and residual.  The CPU tests walk every block of the released configs (tiny / small / base x
+SR x2 x3 x4, dn, deblur, jpeg, dm at their smallest padded size) through tc.attention_launches, the grids that
+grl_window_attn_f32 / grl_stripe_attn_f32 launch, and through `gemm_calls`, the K.linear / K.conv3x3 calls of the fp32
+forward, and fail naming any path without a case.  test_recorded_launches_match_lists checks both lists one for one
+against the C-ABI calls of real fp32 forwards.
+
+Cases call the C ABI directly and write into NaN-filled buffers with guard rows (and guard columns where a pitch
+allows): every owned element must be written and nothing else.  Attention: 2 x 2 windows of the pass's grid, B = 2, the
+config's heads and head_dim, the production 6c-wide qkv pitch; q and k un-normalised with one all-zero token, per-head
+logit scales across the ln 100 clamp, a CPB-like bias table.  Stripe pass 2 is checked on the kernel's own X1, and the
+whole chain against the float64 chain.  GEMM: B = 2, M = 200 linear rows (an image boundary inside a 64-row tile), conv
+images of 13 x 21, spread row and column scales, GELU inputs below -8, and rows (linear) or pixels (conv, every tap)
+of zero input, whose accumulators are exact, so the gate there sees the epilogue alone.
+
+Gates: |got - ref64| <= bound per element, with bounds derived from the kernels' fixed summation orders (u = 2^-24,
+gamma_n = n u / (1 - n u), erff / expf errors from the CUDA Programming Guide):
+  GEMM / conv: gamma_K sum |a_k w_k| for the FMA chain, one rounding each for bias, activation and residual; the erf
+    term of GELU counts as absolute, 0.5 |x| (erff error + 3 u), since 1 + erf cancels below about -3;
+  ln_residual: two-pass moments over C with the warp's lane-strided order (ceil(C / 32) + 5 additions per sum);
+  channel gate: 256-row chunk sums, a sequential sum over the chunks, the MLP (lane-strided + warp tree, then a
+    sequential chain), expf;
+  bias table: the 2-FMA hidden unit, ReLU, a 512-long FMA chain, expf;
+  avgpool: bit-exact (a sequential fp32 sum in (dy, dx) order times an exact power-of-two division).
+Attention is gated as measured: |got - ref64| in fp32 ulps at max(|ref|, the row's rms) <= GATE_ATTN (pass 2 on the
+whole chain: GATE_CHAIN), 2 x the worst case of one run on an H100 80GB HBM3 at a 400 W power limit.  Every case
+prints its worst error / bound ratio.  Mutation controls are derived from the float64 reference (a kernel bug's
+effect, never an edited kernel); each must fail its gate on every case where it applies, and each case prints which
+of them the old operator tests' 2e-4 max-abs bound would have missed.
+"""
+import ctypes
+import math
+from functools import lru_cache
+from typing import NamedTuple
+
+import pytest
+import torch
+import torch.nn.functional as F
+
+import grl_oracle as O
+
+B = 2
+GUARD = 3          # NaN guard rows before and after every output buffer
+U = 2.0 ** -24     # fp32 unit roundoff
+ERFF_ULP = 2       # CUDA C++ Programming Guide, maximum ulp error of erff / expf (no fast math)
+EXPF_ULP = 2
+OLD_TOL = 2e-4     # the max-abs bound of the operator tests this file replaces
+GATE_ATTN = 1695.0   # fp32 ulps at max(|ref|, row rms): 2 x the worst case, 847.2 (small/sr window; H100 80GB HBM3, 400 W)
+GATE_CHAIN = 2165.0  # both stripe passes against the float64 chain: 2 x the worst case, 1082.3 (same card)
+TASKS = (("sr", 2), ("sr", 3), ("sr", 4), ("dn", 1), ("deblur", 1), ("jpeg", 1), ("dm", 1))
+ACT_NONE, ACT_GELU, ACT_LEAKY = 0, 1, 2
+
+
+def gamma(n):
+    return n * U / (1 - n * U)
+
+
+@lru_cache(maxsize=None)
+def released_model(pkg, variant, task, scale):
+    """A released config at its smallest padded size, on the CPU (host-side walks only)."""
+    cfg = pkg.configs.grl_config(variant, task, scale)
+    return pkg.GRL(**dict(cfg, img_size=math.lcm(cfg["window_size"], *cfg["stripe_size"])))
+
+
+def released_models(pkg):
+    for variant in ("tiny", "small", "base"):
+        for task, s in TASKS:
+            yield f"{variant}/{task}x{s}", released_model(pkg, variant, task, s)
+
+
+# ------------------------------------------------------------------------------------------------------- attention
+
+
+def attn_path(ln, d):
+    """(role, D, d < D, Nq % 128 != 0, Nq > 128, Nk % 32 != 0, Nk > 32, use_mask, non-zero roll)."""
+    D = 16 if d <= 16 else 32 if d <= 32 else 64
+    nq, nk = ln.gq.wh * ln.gq.ww, ln.gk.wh * ln.gk.ww
+    roll = any((g.sh, g.sw) != (0, 0) for g in (ln.gq, ln.gk))
+    return (ln.role, D, d < D, nq % 128 != 0, nq > 128, nk % 32 != 0, nk > 32, bool(ln.use_mask), roll)
+
+
+def block_attention(blk, x_size):
+    """(launch descriptor, head_dim) of the three attention launches of a block."""
+    from grl_image_restoration_b200 import tc
+
+    return [(ln, blk.dim // 2 // ln.heads) for ln in tc.attention_launches(blk, x_size)]
+
+
+class AttnCase(NamedTuple):
+    src: str      # the first released config / block that launches this path (or why an extra case exists)
+    role: str     # "window", "stripe1" (anchors attend to the stripe's tokens), "stripe2" (tokens attend to anchors)
+    win: tuple    # the token window of the pass: the attention window or the (oriented) stripe
+    df: int       # anchor down factor (1 for window attention)
+    shifted: bool
+    heads: int
+    d: int
+    shift: tuple = None  # the roll when shifted; None: half the window
+
+
+# one case per released path, from its first launcher (stage 0: block 0 or 1 unshifted, block 2 shifted stripes)
+ATTN_CASES = [
+    AttnCase("tiny/sr", "window", (32, 32), 1, True, 2, 16),
+    AttnCase("tiny/sr", "stripe1", (64, 64), 4, True, 2, 16),
+    AttnCase("tiny/sr", "stripe2", (64, 64), 4, True, 2, 16),
+    AttnCase("tiny/deblur", "window", (12, 12), 1, True, 2, 16),
+    AttnCase("tiny/deblur", "stripe1", (48, 96), 4, True, 2, 16),
+    AttnCase("tiny/jpeg", "stripe2", (72, 144), 4, True, 2, 16),
+    AttnCase("tiny/dm", "window", (8, 8), 1, True, 2, 16),
+    AttnCase("tiny/dm", "stripe1", (32, 32), 4, True, 2, 16),
+    AttnCase("tiny/sr", "window", (32, 32), 1, False, 2, 16),
+    AttnCase("tiny/sr", "stripe1", (64, 64), 4, False, 2, 16),
+    AttnCase("tiny/sr", "stripe2", (64, 64), 4, False, 2, 16),
+    AttnCase("tiny/deblur", "window", (12, 12), 1, False, 2, 16),
+    AttnCase("tiny/deblur", "stripe1", (48, 96), 4, False, 2, 16),
+    AttnCase("tiny/jpeg", "stripe2", (72, 144), 4, False, 2, 16),
+    AttnCase("tiny/dm", "window", (8, 8), 1, False, 2, 16),
+    AttnCase("tiny/dm", "stripe1", (32, 32), 4, False, 2, 16),
+    AttnCase("small/sr", "window", (32, 32), 1, True, 2, 32),
+    AttnCase("small/sr", "stripe1", (64, 64), 4, True, 2, 32),
+    AttnCase("small/sr", "stripe2", (64, 64), 4, True, 2, 32),
+    AttnCase("small/deblur", "window", (12, 12), 1, True, 2, 32),
+    AttnCase("small/deblur", "stripe1", (48, 96), 4, True, 2, 32),
+    AttnCase("small/jpeg", "stripe2", (72, 144), 4, True, 2, 32),
+    AttnCase("small/dm", "window", (8, 8), 1, True, 2, 32),
+    AttnCase("small/dm", "stripe1", (32, 32), 4, True, 2, 32),
+    AttnCase("small/sr", "window", (32, 32), 1, False, 2, 32),
+    AttnCase("small/sr", "stripe1", (64, 64), 4, False, 2, 32),
+    AttnCase("small/sr", "stripe2", (64, 64), 4, False, 2, 32),
+    AttnCase("small/deblur", "window", (12, 12), 1, False, 2, 32),
+    AttnCase("small/deblur", "stripe1", (48, 96), 4, False, 2, 32),
+    AttnCase("small/jpeg", "stripe2", (72, 144), 4, False, 2, 32),
+    AttnCase("small/dm", "window", (8, 8), 1, False, 2, 32),
+    AttnCase("small/dm", "stripe1", (32, 32), 4, False, 2, 32),
+    AttnCase("base/sr", "window", (32, 32), 1, True, 3, 30),
+    AttnCase("base/sr", "stripe1", (64, 64), 2, True, 3, 30),
+    AttnCase("base/sr", "stripe2", (64, 64), 2, True, 3, 30),
+    AttnCase("base/deblur", "window", (12, 12), 1, True, 3, 30),
+    AttnCase("base/deblur", "stripe1", (48, 96), 4, True, 3, 30),
+    AttnCase("base/jpeg", "stripe2", (72, 144), 4, True, 3, 30),
+    AttnCase("base/dm", "window", (8, 8), 1, True, 3, 30),
+    AttnCase("base/dm", "stripe1", (32, 32), 4, True, 3, 30),
+    AttnCase("base/sr", "window", (32, 32), 1, False, 3, 30),
+    AttnCase("base/sr", "stripe1", (64, 64), 2, False, 3, 30),
+    AttnCase("base/sr", "stripe2", (64, 64), 2, False, 3, 30),
+    AttnCase("base/deblur", "window", (12, 12), 1, False, 3, 30),
+    AttnCase("base/deblur", "stripe1", (48, 96), 4, False, 3, 30),
+    AttnCase("base/jpeg", "stripe2", (72, 144), 4, False, 3, 30),
+    AttnCase("base/dm", "window", (8, 8), 1, False, 3, 30),
+    AttnCase("base/dm", "stripe1", (32, 32), 4, False, 3, 30),
+]
+ATTN_EXTRAS = [  # limits no released config uses, and the earlier operator tests' geometries
+    AttnCase("extra: head_dim 64 (D = 64)", "window", (16, 16), 1, True, 2, 64),
+    AttnCase("extra: head_dim 64 (D = 64)", "stripe2", (32, 32), 4, True, 2, 64),
+    AttnCase("extra: 8 heads, the kernel's limit", "window", (8, 8), 1, True, 8, 8),
+    AttnCase("extra: 8 heads, the kernel's limit", "stripe2", (16, 32), 2, False, 8, 12),
+    AttnCase("extra: released jpeg window, 1296 keys", "window", (36, 36), 1, True, 2, 16),
+    AttnCase("extra: 8x8 window, head_dim 9", "window", (8, 8), 1, True, 2, 9),
+    AttnCase("extra: 8x8 window, head_dim 9", "window", (8, 8), 1, False, 2, 9),
+    AttnCase("extra: 4x4 window, 16 keys", "window", (4, 4), 1, False, 3, 10),
+    AttnCase("extra: 6x6 window, head_dim 40", "window", (6, 6), 1, True, 2, 40),
+    AttnCase("extra: 8x16 stripes, head_dim 9", "stripe2", (8, 16), 2, True, 2, 9),
+    AttnCase("extra: 16x8 stripes, head_dim 9", "stripe2", (16, 8), 2, False, 2, 9),
+    AttnCase("extra: stripe groups, 4x16 stripes", "stripe2", (4, 16), 2, True, 2, 8),
+    AttnCase("extra: stripe groups, 4x8 stripes", "stripe2", (4, 8), 2, False, 2, 8),
+    AttnCase("extra: stripe groups, 32x8 stripes shifted by (0, 4)", "stripe2", (32, 8), 2, True, 2, 8, (0, 4)),
+    AttnCase("extra: df 3, 1 head", "stripe2", (6, 12), 3, True, 1, 32),
+]
+
+
+def attn_case_launch(case):
+    """(x_size, launch descriptor) of a case: an image of 2 x 2 windows of the pass's grid."""
+    from grl_image_restoration_b200 import geometry as G, tc
+
+    wh, ww = case.win
+    x_size = (2 * wh, 2 * ww)
+    sh = (case.shift or (wh // 2, ww // 2)) if case.shifted else (0, 0)
+    tok = G.token_grid(x_size, case.win, sh)
+    gq = gk = tok
+    if case.role != "window":
+        anc = G.anchor_grid(x_size, case.win, sh, case.df)
+        gq, gk = (anc, tok) if case.role == "stripe1" else (tok, anc)
+    return x_size, tc.attention_launch(case.role, gq, gk, case.heads, case.heads, case.heads * case.d, case.shifted)
+
+
+def test_released_attention_paths_have_cases(pkg):
+    """Every attention path of every block of every released config has a case, and every case of ATTN_CASES is a
+    released path."""
+    have = {attn_path(attn_case_launch(c)[1], c.d): c for c in ATTN_CASES}
+    assert len(have) == len(ATTN_CASES), "two cases share a path"
+    released, missing = set(), {}
+    for name, model in released_models(pkg):
+        for si, layer in enumerate(model.layers):
+            for bi, blk in enumerate(layer.blocks):
+                for ln, d in block_attention(blk, model.input_resolution):
+                    s = attn_path(ln, d)
+                    released.add(s)
+                    if s not in have:
+                        missing.setdefault(s, f"{name} stage {si} block {bi} {ln.role}")
+    for s, name in missing.items():
+        print(f"fp32 attention path without a case: {s}, first launched by {name}")
+    assert not missing, f"{len(missing)} released fp32 attention paths have no case: " + "; ".join(
+        f"{s} ({name})" for s, name in missing.items())
+    stale = [c for c in ATTN_CASES if attn_path(attn_case_launch(c)[1], c.d) not in released]
+    assert not stale, f"cases that no released config launches: {stale}"
+    print(f"{len(released)} released fp32 attention paths")
+
+
+# ------------------------------------------------------------------------------------------------------------ GEMM
+
+
+class GemmCall(NamedTuple):
+    name: str
+    conv: bool
+    K: int        # 9 Cin for a conv
+    N: int
+    act: int
+    slope: float
+    bias: bool
+    res: bool
+
+
+def gemm_calls(model):
+    """The K.linear / K.conv3x3 calls of one fp32 forward of `model`, in order (modules.py)."""
+    out = []
+
+    def lin(name, m, act=ACT_NONE):
+        out.append(GemmCall(name, False, m.weight.shape[1], m.weight.shape[0], act, 0.0, m.bias is not None, False))
+
+    def conv(name, m, act=ACT_NONE, slope=0.0, res=False):
+        out.append(GemmCall(name, True, 9 * m.weight.shape[1], m.weight.shape[0], act, slope, m.bias is not None, res))
+
+    conv("conv_first", model.conv_first)
+    for si, layer in enumerate(model.layers):
+        for bi, blk in enumerate(layer.blocks):
+            p = f"stage{si}.block{bi}."
+            lin(p + "qkv", blk.attn.qkv.body)
+            lin(p + "anchor", blk.attn.anchor.body[0].reduction)
+            lin(p + "proj", blk.attn.proj)
+            if blk.args.local_connection:
+                conv(p + "cab1", blk.conv.cab[0], ACT_GELU)
+                conv(p + "cab2", blk.conv.cab[2])
+            lin(p + "fc1", blk.mlp.fc1, ACT_GELU)
+            lin(p + "fc2", blk.mlp.fc2)
+        conv(f"stage{si}.conv", layer.conv, res=True)
+    conv("conv_after_body", model.conv_after_body, res=True)
+    if model.upsampler == "pixelshuffle":
+        conv("conv_before_upsample", model.conv_before_upsample[0], ACT_LEAKY, 0.01)
+        for i, m in enumerate(model.upsample.up):
+            if isinstance(m, torch.nn.Conv2d):
+                conv(f"upsample.up.{i}", m)
+        conv("conv_last", model.conv_last)
+    elif model.upsampler == "pixelshuffledirect":
+        conv("upsample.up.0", model.upsample.up[0])
+    elif model.upsampler == "nearest+conv":
+        conv("conv_before_upsample", model.conv_before_upsample[0], ACT_LEAKY, 0.01)
+        for n in ("conv_up1", "conv_up2", "conv_hr"):
+            conv(n, getattr(model, n), ACT_LEAKY, 0.2)
+        conv("conv_last", model.conv_last)
+    else:
+        conv("conv_last", model.conv_last, res=model.in_channels == model.out_channels)
+    return out
+
+
+def gemm_path(g):
+    """(conv, K % 16 != 0, k tiles, N % 64 != 0, N > 64, act, bias, residual)."""
+    return (g.conv, g.K % 16 != 0, -(-g.K // 16), g.N % 64 != 0, g.N > 64, g.act, g.bias, g.res)
+
+
+class GemmCase(NamedTuple):
+    src: str
+    conv: bool
+    K: int
+    N: int
+    act: int = ACT_NONE
+    res: bool = False
+    slope: float = 0.01  # LeakyReLU only
+
+    def call(self):
+        return GemmCall(self.src, self.conv, self.K, self.N, self.act, self.slope if self.act == ACT_LEAKY else 0.0,
+                        True, self.res)
+
+
+GEMM_CASES = [  # one case per released path, from its first launcher
+    GemmCase("tiny/srx2 conv_first", True, 27, 64),
+    GemmCase("tiny/srx2 qkv", False, 64, 192),
+    GemmCase("tiny/srx2 anchor", False, 64, 32),
+    GemmCase("tiny/srx2 proj", False, 64, 64),
+    GemmCase("tiny/srx2 fc1", False, 64, 128, ACT_GELU),
+    GemmCase("tiny/srx2 fc2", False, 128, 64),
+    GemmCase("tiny/srx2 stage0.conv", True, 576, 64, res=True),
+    GemmCase("tiny/srx2 upsample.up.0", True, 576, 12),
+    GemmCase("tiny/dnx1 conv_last", True, 576, 3, res=True),
+    GemmCase("small/srx2 conv_first", True, 27, 128),
+    GemmCase("small/srx2 qkv", False, 128, 384),
+    GemmCase("small/srx2 fc1", False, 128, 256, ACT_GELU),
+    GemmCase("small/srx2 fc2", False, 256, 128),
+    GemmCase("small/srx2 stage0.conv", True, 1152, 128, res=True),
+    GemmCase("small/srx2 conv_before_upsample", True, 1152, 64, ACT_LEAKY),
+    GemmCase("small/srx2 upsample.up.0", True, 576, 256),
+    GemmCase("small/dnx1 conv_last", True, 1152, 3, res=True),
+    GemmCase("base/srx2 conv_first", True, 27, 180),
+    GemmCase("base/srx2 qkv", False, 180, 540),
+    GemmCase("base/srx2 cab1", True, 1620, 45, ACT_GELU),
+    GemmCase("base/srx2 cab2", True, 405, 180),
+    GemmCase("base/srx2 fc1", False, 180, 360, ACT_GELU),
+    GemmCase("base/srx2 fc2", False, 360, 180),
+    GemmCase("base/srx2 stage0.conv", True, 1620, 180, res=True),
+    GemmCase("base/srx2 conv_before_upsample", True, 1620, 64, ACT_LEAKY),
+    GemmCase("base/dnx1 conv_last", True, 1620, 3, res=True),
+]
+GEMM_EXTRAS = [  # the earlier operator tests' shapes whose paths no released forward takes (all with a residual)
+    GemmCase("extra: linear K 180 N 90 + residual", False, 180, 90, res=True),
+    GemmCase("extra: linear K 180 N 360 GELU + residual", False, 180, 360, ACT_GELU, True),
+    GemmCase("extra: linear K 360 N 180 + residual", False, 360, 180, res=True),
+    GemmCase("extra: linear K 5 N 3 LeakyReLU 0.2 + residual", False, 5, 3, ACT_LEAKY, True, 0.2),
+    GemmCase("extra: linear K 64 N 64 + residual", False, 64, 64, res=True),
+    GemmCase("extra: conv Cin 36 N 9 GELU + residual", True, 324, 9, ACT_GELU, True),
+    GemmCase("extra: conv Cin 3 N 64 + residual", True, 27, 64, res=True),
+    GemmCase("extra: conv Cin 45 N 180 + residual", True, 405, 180, res=True),
+    GemmCase("extra: conv Cin 64 N 12 LeakyReLU + residual", True, 576, 12, ACT_LEAKY, True),
+    GemmCase("extra: conv Cin 180 N 45 GELU + residual", True, 1620, 45, ACT_GELU, True),
+]
+
+
+def test_released_gemm_paths_have_cases(pkg):
+    """Every GEMM path of every released fp32 forward has a case, and every case of GEMM_CASES is a released path."""
+    have = {gemm_path(c.call()): c for c in GEMM_CASES + GEMM_EXTRAS}
+    assert len(have) == len(GEMM_CASES + GEMM_EXTRAS), "two cases share a path"
+    released, missing = set(), {}
+    for name, model in released_models(pkg):
+        for g in gemm_calls(model):
+            s = gemm_path(g)
+            released.add(s)
+            if s not in have:
+                missing.setdefault(s, f"{name} {g.name}")
+    for s, name in missing.items():
+        print(f"fp32 gemm path without a case: {s}, first launched by {name}")
+    assert not missing, f"{len(missing)} released fp32 gemm paths have no case: " + "; ".join(
+        f"{s} ({name})" for s, name in missing.items())
+    stale = [c for c in GEMM_CASES if gemm_path(c.call()) not in released]
+    assert not stale, f"cases that no released config launches: {stale}"
+    print(f"{len(released)} released fp32 gemm paths")
+
+
+# ----------------------------------------------------------------------------------------------------------------- GPU
+
+
+@pytest.fixture(scope="module")
+def lib(pkg, device):
+    from grl_image_restoration_b200 import capi
+
+    if capi.lib().grl_device_ok() != 1:
+        pytest.skip("the library is built for sm_90a")
+    return capi.lib()
+
+
+def ptr(t, offset=0):
+    return ctypes.c_void_p(t.data_ptr() + 4 * offset)
+
+
+def stream():
+    from grl_image_restoration_b200 import capi
+
+    return capi.stream()
+
+
+def nan_rows(rows, cols, device, guard_cols=0):
+    """A NaN-filled (rows, cols + guard_cols) fp32 buffer with GUARD rows before and after: (inner rows, whole)."""
+    buf = torch.full((rows + 2 * GUARD, cols + guard_cols), float("nan"), device=device)
+    return buf[GUARD:GUARD + rows], buf
+
+
+def check_written(buf, cols, what, guard_cols=0):
+    """The inner rows' first `cols` columns are all written (finite); guard rows and columns are untouched."""
+    assert bool(buf[:GUARD].isnan().all() and buf[-GUARD:].isnan().all()), f"{what}: wrote into a guard row"
+    inner = buf[GUARD:-GUARD]
+    assert bool(inner[:, :cols].isfinite().all()), f"{what}: an owned element was not written"
+    if guard_cols:
+        assert bool(inner[:, cols:].isnan().all()), f"{what}: wrote into the guard columns"
+
+
+def ulp32(x):
+    return torch.clamp(torch.finfo(torch.float32).eps * torch.exp2((torch.frexp(x.abs())[1] - 1).double()),
+                       min=2.0 ** -149)
+
+
+def ulp_stats(got, ref):
+    """max |got - ref| in fp32 ulps at max(|ref|, the row's rms) (rows: the last dimension)."""
+    scale = torch.maximum(ref.abs(), ref.pow(2).mean(-1, keepdim=True).sqrt())
+    return float(((got.double() - ref).abs() / ulp32(scale)).nan_to_num(float("inf")).max())
+
+
+def bound_ratio(got, ref, bound):
+    """max |got - ref| / bound (inf where either side is NaN)."""
+    return float(((got.double() - ref).abs() / bound).nan_to_num(float("inf")).max())
+
+
+def old_misses(mut, ref):
+    """The old operator tests' bound would pass a kernel that computes `mut` instead of `ref`."""
+    return float((mut - ref).abs().nan_to_num(float("inf")).max()) <= OLD_TOL
+
+
+def report(name, ratio, gate, kind="bound"):
+    caught = not ratio <= gate
+    print(f"  mutation '{name}': {ratio:.3g} x {kind} -> {'FAILS the gate' if caught else 'passes the gate'}")
+    return caught
+
+
+# --------------------------------------------------------------------------------------------------- GPU: attention
+
+
+def grid_t(g):
+    return (g.H, g.W, g.wh, g.ww, g.sh, g.sw)
+
+
+def windows(t, g, heads):
+    """(B, H, W, c) tokens -> (B nW, heads, wh ww, c / heads) in the kernel's window order (roll by -shift, then
+    partition); g = (H, W, wh, ww, sh, sw)."""
+    _, _, wh, ww, sh, sw = g
+    t = torch.roll(t, (-sh, -sw), (1, 2)) if sh or sw else t
+    return O.partition(t, (wh, ww)).reshape(-1, wh * ww, heads, t.shape[-1] // heads).transpose(1, 2)
+
+
+def cpb_like(rows_hw, df, heads, seed, device):
+    """(heads, rows) 16 sigmoid(MLP(coords)) of a random CPB-like MLP over a launch's relative coordinates."""
+    coords = O.coords_table(list(rows_hw), df).reshape(-1, 2).double()
+    g = torch.Generator().manual_seed(seed)
+    w1, b1 = torch.randn(512, 2, generator=g).double() * 0.7, torch.randn(512, generator=g).double() * 0.1
+    w2 = torch.randn(heads, 512, generator=g).double() * 0.15
+    return (16 * torch.sigmoid(torch.relu(coords @ w1.T + b1) @ w2.T)).T.float().contiguous().to(device)
+
+
+def logit_scales(heads, reverse, device):
+    """Per-head logit scales (natural log) from ln 5 to ln 150: they cross the clamp at ln 100."""
+    s = torch.linspace(math.log(5.0), math.log(150.0), heads) if heads > 1 else torch.tensor([math.log(150.0)])
+    return (s.flip(0) if reverse else s).float().to(device)
+
+
+def unwindows(o, g, nb):
+    """Inverse of `windows`: (B nW, heads, wh ww, d) -> (B, H, W, heads d)."""
+    H, W, wh, ww, sh, sw = g
+    t = O.unpartition(o.transpose(1, 2).reshape(-1, wh, ww, o.shape[1] * o.shape[3]), (wh, ww), (H, W))
+    assert t.shape[0] == nb
+    return torch.roll(t, (sh, sw), (1, 2)) if sh or sw else t
+
+
+class Pass(NamedTuple):
+    """One attention launch on float64 operands: q, k (B, H, W, c) tokens; v tokens or, for stripe pass 2, the dense
+    X1 (B nW, heads, Nk, d); o_dense: the launch writes dense X1 (stripe pass 1) instead of tokens."""
+    gq: tuple
+    gk: tuple
+    q: torch.Tensor
+    k: torch.Tensor
+    v: torch.Tensor
+    v_dense: bool
+    o_dense: bool
+    scale: torch.Tensor
+    table: torch.Tensor
+    use_mask: bool
+
+
+def attn_ref(p, heads, mutation=None, index=None, mask=None, v=None, roll=True, drop_last_key=False):
+    """float64 reference of one pass in the kernel's window layout (B nW, heads, Nq, d).  roll=False: the kernel read
+    and wrote the un-rolled grids."""
+    gq, gk = (p.gq, p.gk) if roll else (p.gq[:4] + (0, 0), p.gk[:4] + (0, 0))
+    i0, m0 = O.attn_pair_geometry(p.gq, p.gk, p.use_mask)
+    index = i0 if index is None else index
+    mask = (m0 if mask is None else mask) if p.use_mask else None
+    v = p.v if v is None else v
+    q, k, vw = windows(p.q, gq, heads), windows(p.k, gk, heads), v if p.v_dense else windows(v, gk, heads)
+    if drop_last_key:
+        k, vw, index, mask = k[:, :, :-1], vw[:, :, :-1], index[:, :-1], None if mask is None else mask[..., :-1]
+    o = O.attn_f32_reference(q, k, vw, p.scale, p.table, index, mask, mutation)
+    if not roll and not p.o_dense:  # written to the un-rolled token positions
+        o = windows(unwindows(o, gq, B), p.gq, heads)
+    return o
+
+
+def attn_mutations(p, heads, x1_kernel=None):
+    """Mutation name -> the float64 reference of a kernel with that bug, for the mutations that apply to this pass."""
+    out = {}
+    index, mask = O.attn_pair_geometry(p.gq, p.gk, p.use_mask)
+    nk = index.shape[1]
+    # the relative position whose neighbour's entry moves the softmax most, on the last window: max p (1 - p) |e^delta - 1|
+    q, k = windows(p.q, p.gq, heads)[-1:], windows(p.k, p.gk, heads)[-1:]
+    tab = p.table.double()
+    idx = index.to(tab.device)
+    x = F.normalize(q, dim=-1) @ F.normalize(k, dim=-1).transpose(-1, -2)
+    x = x * torch.exp(p.scale.double().clamp(max=math.log(100.0)))[:, None, None] + tab[:, idx]
+    if mask is not None:
+        x = x + mask[-1].to(x)
+    pr = torch.softmax(x, -1)
+    nb = (idx + 1).clamp(max=tab.shape[1] - 1)
+    hit = (pr * (1 - pr) * (torch.exp(tab[:, nb] - tab[:, idx]) - 1).abs()).reshape(-1, idx.numel()).amax(0).argmax()
+    r = int(idx.flatten()[hit])
+    out["bias entry read from its neighbour"] = attn_ref(p, heads, index=torch.where(index == r, r + 1, index))
+    if mask is not None and bool((mask[-1] != 0).any()):
+        w = mask.shape[0] - 1  # the bottom-right window: masked and wrapped
+        rq = O.region_ids(p.gq[:2], p.gq[2:4], p.gq[4:6])[w]
+        rk = O.region_ids(p.gk[:2], p.gk[2:4], p.gk[4:6])[w]
+        i, j = (mask[w] != 0).nonzero()[0].tolist()
+        m2 = mask.clone()
+        m2[w] = torch.where((rq[:, None] == rq[i]) & (rk[None, :] == rk[j]), 0.0, mask[w])
+        out["shift-mask region pair unmasked"] = attn_ref(p, heads, mask=m2)
+    if any(p.gq[4:6]) or any(p.gk[4:6]):
+        out["roll missing"] = attn_ref(p, heads, roll=False)
+    if nk % 32:
+        out["last key of the partial key tile dropped"] = attn_ref(p, heads, drop_last_key=True)
+    if bool((p.scale > math.log(100.0)).any()):
+        out["logit scale not clamped at ln 100"] = attn_ref(p, heads, "scale_unclamped")
+    out["k not normalised"] = attn_ref(p, heads, "k_unnormalised")
+    if nk > 32:
+        out["rescale missing from the denominator"] = attn_ref(p, heads, "rescale_missing_l")
+    if x1_kernel is not None and heads > 1:
+        out["pass 2 reads X1 of the neighbouring head"] = attn_ref(p, heads, v=x1_kernel.roll(-1, 1))
+    return out
+
+
+def attn_inputs(case, x_size, device, seed):
+    """qkv (B L, 6c) with per-token-head scales 2^U(-2, 2) and one all-zero token; anchors (B, Ha, Wa, c) likewise."""
+    h, d = case.heads, case.d
+    c = h * d
+    H, W = x_size
+    g = torch.Generator().manual_seed(seed)
+    qkv = torch.randn(B * H * W, 6 * h, d, generator=g) * torch.exp2(4 * torch.rand(B * H * W, 6 * h, 1, generator=g) - 2)
+    qkv[H * W + 5] = 0.0  # batch 1: q = k = v = 0 takes the F.normalize eps path
+    Ha, Wa = H // case.df, W // case.df
+    anc = torch.randn(B * Ha * Wa, h, d, generator=g) * torch.exp2(4 * torch.rand(B * Ha * Wa, h, 1, generator=g) - 2)
+    anc[Ha * Wa + 1] = 0.0
+    return qkv.view(B * H * W, 6 * c).to(device), anc.view(B, Ha, Wa, c).to(device)
+
+
+def attn_id(c):
+    return (f"{c.src.split(':')[0].replace('/', '-')}-{c.role}-{c.win[0]}x{c.win[1]}-df{c.df}-"
+            f"{'s' if c.shifted else 'u'}-h{c.heads}d{c.d}")
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("case", ATTN_CASES + ATTN_EXTRAS, ids=attn_id)
+def test_attention_path(lib, device, case):
+    from grl_image_restoration_b200 import capi
+
+    x_size, ln = attn_case_launch(case)
+    sig = attn_path(ln, case.d)
+    h, d = case.heads, case.d
+    c = h * d
+    H, W = x_size
+    L = H * W
+    seed = (ATTN_CASES + ATTN_EXTRAS).index(case)
+    qkv, anc = attn_inputs(case, x_size, device, seed)
+    merged, mbuf = nan_rows(B * L, 2 * c, device)
+    if case.role == "window":
+        gq = ln.gq
+        scale = logit_scales(h, False, device)
+        table = cpb_like(case.win, 1, h, seed + 100, device)
+        capi.check(lib.grl_window_attn_f32(ptr(qkv), 6 * c, ptr(merged), 2 * c, B, gq, h, d, ptr(scale), ptr(table),
+                                           int(ln.use_mask), stream()))
+        torch.cuda.synchronize()
+        check_written(mbuf[:, :c], c, "output")
+        assert bool(mbuf[:, c:].isnan().all()), "wrote outside its half of the merged buffer"
+        tok = qkv.double().view(B, H, W, 6 * c)
+        p = Pass(grid_t(gq), grid_t(gq), tok[..., :c], tok[..., c:2 * c], tok[..., 2 * c:3 * c], False, False, scale,
+                 table, ln.use_mask)
+        got = windows(merged.view(B, H, W, 2 * c)[..., :c], p.gq, h)
+        x1 = None
+    else:
+        tokg, ancg = (ln.gk, ln.gq) if case.role == "stripe1" else (ln.gq, ln.gk)
+        s1, s2 = logit_scales(h, False, device), logit_scales(h, True, device)
+        t1, t2 = cpb_like(case.win, case.df, h, seed + 100, device), cpb_like(case.win, case.df, h, seed + 200, device)
+        nbytes = lib.grl_stripe_attn_workspace(B, tokg, ancg, h, d)
+        ws, wbuf = nan_rows(nbytes // 4 // d, d, device)
+        capi.check(lib.grl_stripe_attn_f32(ptr(qkv, 3 * c), 6 * c, ptr(anc), c, ptr(merged, c), 2 * c, B, tokg, ancg,
+                                           h, d, ptr(s1), ptr(t1), ptr(s2), ptr(t2), int(ln.use_mask), ptr(ws),
+                                           nbytes, stream()))
+        torch.cuda.synchronize()
+        check_written(wbuf, d, "X1")
+        check_written(mbuf[:, c:], c, "output")
+        assert bool(mbuf[:, :c].isnan().all()), "wrote outside its half of the merged buffer"
+        tok = qkv.double().view(B, H, W, 6 * c)[..., 3 * c:]
+        Na = ancg.wh * ancg.ww
+        x1 = ws.view(-1, h, Na, d)
+        p1 = Pass(grid_t(ancg), grid_t(tokg), anc.double(), tok[..., c:2 * c], tok[..., 2 * c:], False, True, s1, t1,
+                  ln.use_mask)
+        p2 = Pass(grid_t(tokg), grid_t(ancg), tok[..., :c], anc.double(), x1.double(), True, False, s2, t2,
+                  ln.use_mask)
+        p, got = (p1, x1) if case.role == "stripe1" else (p2, windows(merged.view(B, H, W, 2 * c)[..., c:], p2.gq, h))
+    ref = attn_ref(p, h)
+    stats = ulp_stats(got, ref)
+    print(f"\n[fp32 attention] {case.src} {case.role} {case.win} df{case.df} shifted={case.shifted} h{h} d{d} path={sig}: "
+          f"{stats:.1f} ulp ({stats / GATE_ATTN:.3f} x gate)")
+    ok = stats <= GATE_ATTN
+    if case.role == "stripe2":
+        chain = attn_ref(p2, h, v=attn_ref(p1, h))
+        sc = ulp_stats(got, chain)
+        print(f"  chain vs float64 chain: {sc:.1f} ulp ({sc / GATE_CHAIN:.3f} x gate)")
+        ok = ok and sc <= GATE_CHAIN
+    missed, old = [], []
+    for name, m in attn_mutations(p, h, x1.double() if case.role == "stripe2" else None).items():
+        if not report(name, ulp_stats(got, m), GATE_ATTN, "ulp"):
+            missed.append(name)
+        if old_misses(m, ref):
+            old.append(name)
+    print(f"  the old {OLD_TOL} bound misses {len(old)}: {old}")
+    assert ok, (case, stats)
+    assert not missed, f"mutations the gate does not catch: {missed}"
+
+
+# -------------------------------------------------------------------------------------------------------- GPU: GEMM
+
+
+HT, WT, M_LIN = 13, 21, 200
+ZERO_ROWS = (7, 150)  # linear rows of zero input: the accumulator is exactly 0
+
+
+def im2col(x, transposed=False, wrap=False):
+    """(B, H, W, Cin) -> (B H W, 9 Cin) with k = tap Cin + c, tap = 3 (dy + 1) + (dx + 1) (pack_conv_weight's order).
+    Padding reads zero; wrap=True reads the flat neighbour m + dy W + dx instead (the previous row or image)."""
+    Bn, H, W, C = x.shape
+    flat = x.reshape(-1, C)
+    M = flat.shape[0]
+    m = torch.arange(M, device=x.device)
+    yy, xx = (m // W) % H, m % W
+    cols = []
+    for t in range(9):
+        dy, dx = divmod(t, 3)
+        if transposed:
+            dy, dx = dx, dy
+        dy, dx = dy - 1, dx - 1
+        src = m + dy * W + dx
+        ok = (src >= 0) & (src < M) if wrap else (yy + dy >= 0) & (yy + dy < H) & (xx + dx >= 0) & (xx + dx < W)
+        cols.append(torch.where(ok[:, None], flat[src.clamp(0, M - 1)], 0.0))
+    return torch.cat(cols, 1)
+
+
+def gemm_bound(A, w, b, act, slope, res):
+    """Per-element bound on |kernel - float64| of act(A w^T + b) (+ res), for a sequential FMA chain over k."""
+    K = A.shape[1]
+    v = A @ w.T + b
+    e = gamma(K) * (A.abs() @ w.abs().T)
+    e = e + U * (v.abs() + e)                                              # + bias
+    if act == ACT_GELU:
+        y = O._gelu(v)
+        e = 1.13 * e + 0.5 * v.abs() * (ERFF_ULP * U + 3 * U) + U * y.abs()  # |GELU'| <= 1.13; erf term absolute
+    elif act == ACT_LEAKY:
+        y = torch.where(v > 0, v, v * slope)
+        e = max(1.0, slope) * e + U * y.abs()
+    else:
+        y = v
+    if res is not None:
+        e = e + U * ((y + res).abs() + e)
+    return e, v
+
+
+def gemm_operands(case, device, seed):
+    g = torch.Generator().manual_seed(seed)
+    K, N = case.K, case.N
+    cin = K // 9 if case.conv else K
+    rows = B * HT * WT if case.conv else M_LIN
+
+    def spread(n, lo, hi):
+        return torch.exp2(lo + (hi - lo) * torch.rand(n, generator=g))
+
+    x = torch.randn(rows, cin, generator=g) * spread(rows, -2, 1)[:, None] * spread(cin, -1, 1)[None, :]
+    w = torch.randn(N, K, generator=g) * K ** -0.5 * spread(N, -1, 1)[:, None]
+    b = torch.randn(N, generator=g) * (3.0 if case.act == ACT_GELU else 0.5)
+    if case.act == ACT_GELU:
+        b[::5] = -12.0  # GELU inputs below -8, where 1 + erf cancels
+    res = (torch.randn(rows, N, generator=g) * spread(rows, -1, 1)[:, None]) if case.res else None
+    if case.conv:  # pixel (5, 9) of both images sees zeros on every tap
+        x = x.view(B, HT, WT, cin)
+        x[:, 4:7, 8:11] = 0.0
+    else:
+        x[list(ZERO_ROWS)] = 0.0
+    return [t if t is None else t.float().to(device) for t in (x, w, b, res)]
+
+
+def gemm_id(c):
+    return c.src.replace("extra: ", "extra-").replace(" ", "_").replace(",", "").replace("/", "-")
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("case", GEMM_CASES + GEMM_EXTRAS, ids=gemm_id)
+def test_gemm_path(lib, device, case):
+    from grl_image_restoration_b200 import capi
+
+    x, w, b, res = gemm_operands(case, device, (GEMM_CASES + GEMM_EXTRAS).index(case))
+    slope = case.call().slope
+    K, N = case.K, case.N
+    if case.conv:
+        M = B * HT * WT
+        y, buf = nan_rows(M, N, device)
+        capi.check(lib.grl_conv3x3_f32(ptr(x), ptr(w), ptr(b), ptr(res) if res is not None else None, ptr(y), B, HT,
+                                       WT, K // 9, N, case.act, slope, stream()))
+        guard_cols = 0
+    else:
+        M, guard_cols = M_LIN, 4
+        y, buf = nan_rows(M, N, device, guard_cols)
+        capi.check(lib.grl_linear_f32(ptr(x), K, ptr(w), ptr(b), ptr(res) if res is not None else None, N, ptr(y),
+                                      N + guard_cols, M, N, K, case.act, slope, stream()))
+    torch.cuda.synchronize()
+    check_written(buf, N, "output", guard_cols)
+    got = y[:, :N]
+    x64, w64, b64 = x.double(), w.double(), b.double()
+    r64 = None if res is None else res.double()
+    A = im2col(x64) if case.conv else x64
+
+    def ref(A=A, w=w64, b=b64, r=r64, mutation=None):
+        return O.gemm_launch_reference(A, w, b, act=case.act, slope=slope, n_res=N, res=r, mutation=mutation)["y"]
+
+    y64 = ref()
+    bound, v = gemm_bound(A, w64, b64, case.act, slope, r64)
+    if case.act == ACT_GELU:
+        assert bool((v < -8).any()), "no GELU input below -8"
+    ratio = bound_ratio(got, y64, bound)
+    print(f"\n[fp32 gemm] {case.src} path={gemm_path(case.call())}: worst error / bound {ratio:.3f}, "
+          f"max |err| {float((got.double() - y64).abs().max()):.2e}")
+    muts = {}
+    if K % 16:
+        w2 = w64.clone()
+        w2[:, K // 16 * 16:] = 0
+        muts["partial last k tile dropped"] = ref(w=w2)
+    if case.conv:
+        muts["taps transposed"] = ref(A=im2col(x64, transposed=True))
+        muts["padding taps wrap into the previous row / image"] = ref(A=im2col(x64, wrap=True))
+    if N > 1:
+        nb = torch.arange(N, device=device) + 1
+        nb[-1] = N - 2
+        muts["bias of the neighbouring column"] = ref(b=b64[nb])
+    if r64 is not None:
+        r2 = r64.clone()
+        r2[(M - 1) // 64 * 64:] = 0
+        muts["no residual on the last row tile"] = ref(r=r2)
+    if case.act == ACT_GELU:
+        muts["tanh-GELU"] = ref(mutation="gelu_tanh")
+    missed, old = [], []
+    for name, m in muts.items():
+        if not report(name, bound_ratio(got, m, bound), 1.0):
+            missed.append(name)
+        if old_misses(m, y64):
+            old.append(name)
+    print(f"  the old {OLD_TOL} bound misses {len(old)}: {old}")
+    assert ratio <= 1.0, (case, ratio)
+    assert not missed, f"mutations the gate does not catch: {missed}"
+
+
+# ------------------------------------------------------------------------------------------- GPU: LayerNorm residual
+
+
+L_LN = 100  # 8-row blocks: the image boundary at row 100 lies inside the block of rows 96..103
+HIGH_MEAN_ROWS, LOW_STD_ROWS = (5, 133), (7, 150)
+
+
+def ln_reference(u, gamma_, beta, eps, rs, x, cy, gate, mutation=None):
+    C = u.shape[1]
+    if mutation == "naive fp32 E[x^2] - E[x]^2":
+        u32 = u.float()
+        mean32 = u32.mean(1, keepdim=True)
+        mean, var = mean32.double(), ((u32 * u32).mean(1, keepdim=True) - mean32 * mean32).double()
+    else:
+        mean = u.mean(1, keepdim=True)
+        var = (u - mean).pow(2).sum(1, keepdim=True) / (C - 1 if mutation == "n - 1 variance" else C)
+    e = 0.0 if mutation == "no eps" else eps
+    r = (u - mean) / torch.sqrt(var + e) * gamma_ + beta
+    r = r * (1.0 if mutation == "res_scale dropped" else rs)
+    if x is not None:
+        r = r + x
+    if cy is not None:
+        rows = torch.arange(u.shape[0], device=u.device)
+        if mutation == "CAB gate of the wrong image at the boundary":
+            rows = rows // 8 * 8  # every row of an 8-row block takes the image of the block's first row
+        r = r + cy * gate[rows // L_LN]
+    return r
+
+
+def ln_bound(u, gamma_, beta, eps, rs, x, cy, gate):
+    """Per-element bound: two-pass moments over C, each a lane-strided sequential sum plus a 5-level warp tree."""
+    C = u.shape[1]
+    ns = -(-C // 32) + 5
+    mean = u.mean(1, keepdim=True)
+    e_mean = gamma(ns) * u.abs().sum(1, keepdim=True) / C + U * mean.abs()
+    d = u - mean
+    var = d.pow(2).mean(1, keepdim=True)
+    # the deviations carry the common mean error (its cross term sums to zero) and one rounding each
+    e_var = e_mean ** 2 + (var + e_mean ** 2) * (gamma(ns) + 4 * U)
+    rel_v = (e_var + U * (var + eps)) / (var + eps)
+    rel_r = 0.5 * rel_v * (1 + rel_v) + 2.5 * U  # sqrt, reciprocal
+    rstd = 1 / torch.sqrt(var + eps)
+    n = d * rstd
+    e_n = (e_mean + U * (d.abs() + e_mean)) * rstd + n.abs() * (rel_r + U)
+    t = n * gamma_ + beta
+    e = gamma_.abs() * e_n + U * ((n * gamma_).abs() + t.abs())
+    r = t * rs
+    e = abs(rs) * e + U * r.abs()
+    if x is not None:
+        r = r + x
+        e = e + U * r.abs()
+    if cy is not None:
+        cg = cy * gate[torch.arange(u.shape[0], device=u.device) // L_LN]
+        e = e + U * (cg.abs() + (r + cg).abs())
+    return e * (1 + 1e-6)
+
+
+LN_CASES = [(C, with_x, cab) for C in (64, 128, 180) for with_x, cab in ((False, False), (True, False), (True, True))]
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("C,with_x,cab", LN_CASES, ids=lambda v: str(v))
+def test_ln_residual(lib, device, C, with_x, cab):
+    from grl_image_restoration_b200 import capi
+
+    g = torch.Generator().manual_seed(C * 4 + 2 * with_x + cab)
+    M = B * L_LN
+    u = torch.randn(M, C, generator=g) * torch.exp2(3 * torch.rand(M, 1, generator=g) - 1) + torch.randn(M, 1, generator=g)
+    for r in HIGH_MEAN_ROWS:
+        u[r] = 100.0 + torch.randn(C, generator=g)
+    for r in LOW_STD_ROWS:
+        u[r] = 0.3 + 1e-2 * torch.randn(C, generator=g)
+    gamma_, beta = 1 + 0.3 * torch.randn(C, generator=g), 0.2 * torch.randn(C, generator=g)
+    x = torch.randn(M, C, generator=g) if with_x else None
+    cy = torch.randn(M, C, generator=g) * torch.exp2(2 * torch.rand(M, 1, generator=g) - 1) if cab else None
+    gate = torch.sigmoid(torch.randn(B, C, generator=g)) if cab else None
+    rs, eps = 0.5, 1e-5
+    dv = [t if t is None else t.float().to(device) for t in (u, gamma_, beta, x, cy, gate)]
+    out, buf = nan_rows(M, C, device)
+    capi.check(lib.grl_ln_residual_f32(ptr(dv[3]) if with_x else None, ptr(dv[0]), ptr(dv[1]), ptr(dv[2]), eps, rs,
+                                       ptr(dv[4]) if cab else None, ptr(dv[5]) if cab else None, L_LN, ptr(out), M, C,
+                                       stream()))
+    torch.cuda.synchronize()
+    check_written(buf, C, "output")
+    d64 = [t if t is None else t.double() for t in dv]
+    ref = ln_reference(d64[0], d64[1], d64[2], eps, rs, d64[3], d64[4], d64[5])
+    bound = ln_bound(d64[0], d64[1], d64[2], eps, rs, d64[3], d64[4], d64[5])
+    ratio = bound_ratio(out, ref, bound)
+    hm = list(HIGH_MEAN_ROWS)
+    print(f"\n[fp32 ln_residual] C={C} x={with_x} cab={cab}: worst error / bound {ratio:.3f} "
+          f"(high-mean rows {bound_ratio(out[hm], ref[hm], bound[hm]):.3f})")
+    names = ["n - 1 variance", "no eps", "naive fp32 E[x^2] - E[x]^2", "res_scale dropped"]
+    if cab:
+        names.append("CAB gate of the wrong image at the boundary")
+    missed, old = [], []
+    for name in names:
+        m = ln_reference(d64[0], d64[1], d64[2], eps, rs, d64[3], d64[4], d64[5], mutation=name)
+        if not report(name, bound_ratio(out, m, bound), 1.0):
+            missed.append(name)
+        if old_misses(m, ref):
+            old.append(name)
+    print(f"  the old {OLD_TOL} bound misses {len(old)}: {old}")
+    assert ratio <= 1.0, ratio
+    assert not missed, f"mutations the gate does not catch: {missed}"
+
+
+# ------------------------------------------------------------------------------------------------ GPU: channel gate
+
+POOL_ROWS = 256  # rows per partial sum (ops_f32.cu: kPoolRows)
+
+
+def gate_reference(y, w1, b1, w2, b2, mutation=None):
+    L = y.shape[1]
+    chunks = -(-L // POOL_ROWS)
+    if mutation == "partial last chunk dropped":
+        mean = y[:, :(chunks - 1) * POOL_ROWS].sum(1) / L
+    elif mutation == "division by chunks x 256":
+        mean = y.sum(1) / (chunks * POOL_ROWS)
+    else:
+        mean = y.mean(1)
+    hpre = mean @ w1.T + b1
+    h = hpre if mutation == "ReLU missing" else torch.relu(hpre)
+    return torch.sigmoid(h @ w2.T + b2)
+
+
+def gate_bound(y, w1, b1, w2, b2):
+    L, C = y.shape[1], y.shape[2]
+    R = w1.shape[0]
+    mean = y.mean(1)
+    e_mean = gamma(POOL_ROWS + -(-L // POOL_ROWS)) * y.abs().sum(1) / L + U * mean.abs()
+    hpre = mean @ w1.T + b1
+    e_h = e_mean @ w1.abs().T + gamma(-(-C // 32) + 5) * (mean.abs() @ w1.abs().T) + U * hpre.abs()
+    h = torch.relu(hpre)
+    s = h @ w2.T + b2
+    e_s = e_h @ w2.abs().T + gamma(R) * (b2.abs() + h @ w2.abs().T)
+    gt = torch.sigmoid(s)
+    return gt * (1 - gt) * e_s + gt * (2 * EXPF_ULP * U * (1 - gt) + 2 * U)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("L", [1, 100, 1000])
+def test_channel_gate(lib, device, L):
+    from grl_image_restoration_b200 import capi
+
+    C, R = 180, 10  # GRL-Base's CAB: ChannelAttention(180, reduction 18)
+    g = torch.Generator().manual_seed(L)
+    y = torch.randn(B, L, C, generator=g) + 0.3
+    w1, b1 = torch.randn(R, C, generator=g) * 0.1, torch.randn(R, generator=g) * 0.5
+    w2, b2 = torch.randn(C, R, generator=g) * 0.3, torch.randn(C, generator=g) * 0.5
+    dv = [t.float().to(device).contiguous() for t in (y, w1, b1, w2, b2)]
+    nbytes = lib.grl_channel_gate_workspace(B, L, C)
+    ws = torch.full((nbytes // 4,), float("nan"), device=device)
+    out, buf = nan_rows(B, C, device)
+    capi.check(lib.grl_channel_gate_f32(ptr(dv[0]), B, L, C, ptr(dv[1]), ptr(dv[2]), ptr(dv[3]), ptr(dv[4]), R,
+                                        ptr(out), ptr(ws), nbytes, stream()))
+    torch.cuda.synchronize()
+    check_written(buf, C, "gate")
+    d64 = [t.double() for t in dv]
+    ref = gate_reference(*d64)
+    bound = gate_bound(*d64)
+    ratio = bound_ratio(out, ref, bound)
+    print(f"\n[fp32 channel gate] B={B} L={L} C={C} R={R}: worst error / bound {ratio:.3f}")
+    missed, old = [], []
+    for name in ("partial last chunk dropped", "division by chunks x 256", "ReLU missing"):
+        if name == "division by chunks x 256" and L % POOL_ROWS == 0:
+            continue
+        m = gate_reference(*d64, mutation=name)
+        if not report(name, bound_ratio(out, m, bound), 1.0):
+            missed.append(name)
+        if old_misses(m, ref):
+            old.append(name)
+    print(f"  the old {OLD_TOL} bound misses {len(old)}: {old}")
+    assert ratio <= 1.0, ratio
+    assert not missed, f"mutations the gate does not catch: {missed}"
+
+
+# ------------------------------------------------------------------------------------ GPU: avgpool, bias table
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("df", [1, 2, 4])
+def test_avgpool_bit_exact(lib, device, df):
+    """The kernel sums the df x df pixels in (dy, dx) order in fp32 and divides by df^2 (exact): bit for bit."""
+    from grl_image_restoration_b200 import capi
+
+    H, W, C = 16, 24, 36
+    x = (torch.randn(B, H, W, C, generator=torch.Generator().manual_seed(df)) * 3).to(device)
+    Ho, Wo = H // df, W // df
+    out, buf = nan_rows(B * Ho * Wo, C, device)
+    capi.check(lib.grl_avgpool_f32(ptr(x), ptr(out), B, H, W, C, df, stream()))
+    torch.cuda.synchronize()
+    check_written(buf, C, "output")
+    xc = x.cpu().view(B, Ho, df, Wo, df, C)
+    s = torch.zeros(B, Ho, Wo, C)
+    for dy in range(df):
+        for dx in range(df):
+            s = s + xc[:, :, dy, :, dx]
+    ref = (s / float(df * df)).reshape(-1, C)
+    assert torch.equal(out.cpu(), ref), float((out.cpu() - ref).abs().max())
+
+
+def bias_table_bound(t, w1, b1, w2):
+    """16 sigmoid(W2 relu(W1 t + b1)): two FMAs per hidden unit, a sequential FMA chain over them, expf."""
+    hpre = t @ w1.T + b1
+    e_h = gamma(2) * (t.abs() @ w1.abs().T + b1.abs())
+    h = torch.relu(hpre)
+    acc = h @ w2.T
+    e_acc = e_h @ w2.abs().T + gamma(w1.shape[0]) * (h @ w2.abs().T)
+    sg = torch.sigmoid(acc)
+    return (16 * (sg * (1 - sg) * e_acc + sg * (2 * EXPF_ULP * U * (1 - sg) + 2 * U))).T, (16 * sg).T
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("heads", range(1, 9))
+def test_bias_table(lib, device, heads):
+    from grl_image_restoration_b200 import capi
+
+    hidden = 512
+    table = O.coords_table([32, 64], 2).reshape(-1, 2)  # 47 x 95 = 4465 rows: a partial last 128-row block
+    rows = table.shape[0]
+    g = torch.Generator().manual_seed(heads)
+    w1, b1 = torch.randn(hidden, 2, generator=g) * 0.7, torch.randn(hidden, generator=g) * 0.1
+    w2 = torch.randn(heads, hidden, generator=g) * 0.15
+    dv = [t.float().to(device).contiguous() for t in (table, w1, b1, w2)]
+    out, buf = nan_rows(heads, rows, device)
+    capi.check(lib.grl_bias_table_f32(ptr(dv[0]), rows, ptr(dv[1]), ptr(dv[2]), ptr(dv[3]), hidden, heads, ptr(out),
+                                      stream()))
+    torch.cuda.synchronize()
+    check_written(buf, rows, "table")
+    bound, ref = bias_table_bound(*[t.double() for t in dv])
+    ratio = bound_ratio(out, ref, bound)
+    print(f"\n[fp32 bias table] heads={heads} hidden={hidden} rows={rows}: worst error / bound {ratio:.3f}")
+    assert ratio <= 1.0, ratio
+
+
+# --------------------------------------------------------------------------------------------- GPU: recorded launches
+
+
+class Recorder:
+    """Stands in for capi.lib(): records the fp32 GEMM and attention calls, forwards every call to the library."""
+
+    def __init__(self, lib):
+        self._lib, self.gemm, self.attn = lib, [], []
+
+    def __getattr__(self, name):
+        return getattr(self._lib, name)
+
+    def grl_linear_f32(self, x, ldx, w, b, res, ldr, y, ldy, M, N, K, act, slope, st):
+        self.gemm.append((False, K, N, act, slope, b is not None, res is not None))
+        return self._lib.grl_linear_f32(x, ldx, w, b, res, ldr, y, ldy, M, N, K, act, slope, st)
+
+    def grl_conv3x3_f32(self, x, w, b, res, y, Bn, H, W, Cin, Cout, act, slope, st):
+        self.gemm.append((True, 9 * Cin, Cout, act, slope, b is not None, res is not None))
+        return self._lib.grl_conv3x3_f32(x, w, b, res, y, Bn, H, W, Cin, Cout, act, slope, st)
+
+    def grl_window_attn_f32(self, qkv, ldq, out, ldo, Bn, grid, heads, d, ls, bias, use_mask, st):
+        self.attn.append(("window", grid_t(grid), grid_t(grid), heads, d, bool(use_mask)))
+        return self._lib.grl_window_attn_f32(qkv, ldq, out, ldo, Bn, grid, heads, d, ls, bias, use_mask, st)
+
+    def grl_stripe_attn_f32(self, qkv, ldq, anc, lda, out, ldo, Bn, tok, ancg, heads, d, s1, b1, s2, b2, use_mask, ws,
+                            nbytes, st):
+        self.attn.append(("stripe1", grid_t(ancg), grid_t(tok), heads, d, bool(use_mask)))
+        self.attn.append(("stripe2", grid_t(tok), grid_t(ancg), heads, d, bool(use_mask)))
+        return self._lib.grl_stripe_attn_f32(qkv, ldq, anc, lda, out, ldo, Bn, tok, ancg, heads, d, s1, b1, s2, b2,
+                                             use_mask, ws, nbytes, st)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("variant,task,scale", [("tiny", "sr", 2), ("small", "jpeg", 1), ("base", "sr", 4),
+                                                ("base", "dm", 1)])
+def test_recorded_launches_match_lists(pkg, lib, device, monkeypatch, variant, task, scale):
+    """The C-ABI calls of a real fp32 forward (smallest padded size, an input that needs padding) are, one for one and
+    in order, gemm_calls and the blocks' tc.attention_launches, and each one's path has a case."""
+    from grl_image_restoration_b200 import capi
+
+    cfg = pkg.configs.grl_config(variant, task, scale)
+    model = pkg.GRL(**dict(cfg, img_size=math.lcm(cfg["window_size"], *cfg["stripe_size"])))
+    model.set_precision("fp32")
+    model = model.to(device).eval()
+    S = model.pad_size
+    x = torch.rand(1, 3, S - 5, S - 3, generator=torch.Generator().manual_seed(0)).to(device)
+    rec = Recorder(lib)
+    monkeypatch.setattr(capi, "lib", lambda: rec)
+    y = model(x)
+    torch.cuda.synchronize()
+    monkeypatch.undo()
+    assert y.shape == (1, 3, (S - 5) * cfg["upscale"], (S - 3) * cfg["upscale"])
+    want_g = gemm_calls(model)
+    assert len(rec.gemm) == len(want_g), (len(rec.gemm), len(want_g))
+    for got, g in zip(rec.gemm, want_g):
+        assert got == (g.conv, g.K, g.N, g.act, g.slope, g.bias, g.res), (g.name, got)
+    gemm_have = {gemm_path(c.call()) for c in GEMM_CASES}
+    assert all(gemm_path(g) in gemm_have for g in want_g)
+    want_a = [(ln, d) for layer in model.layers for blk in layer.blocks for ln, d in block_attention(blk, (S, S))]
+    assert len(rec.attn) == len(want_a), (len(rec.attn), len(want_a))
+    attn_have = {attn_path(attn_case_launch(c)[1], c.d) for c in ATTN_CASES}
+    for got, (ln, d) in zip(rec.attn, want_a):
+        assert got == (ln.role, grid_t(ln.gq), grid_t(ln.gk), ln.heads, d, bool(ln.use_mask)), got
+        assert attn_path(ln, d) in attn_have, (got, attn_path(ln, d))
+    print(f"\n{variant}/{task}x{scale}: {len(rec.gemm)} GEMM and {len(rec.attn)} attention launches match the lists")

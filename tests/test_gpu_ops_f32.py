@@ -1,5 +1,6 @@
-"""fp32 CUDA operators vs the CPU oracle on identical seeded inputs (parity tests proper; run with -m gpu).
-Tolerance: BASELINE.json's fp32 gate is 1e-3 max-abs; these operator-level checks use 2e-4 (observed ~1e-5)."""
+"""fp32 CUDA operators and modules vs the CPU oracle and tensors of the unmodified reference (run with -m gpu).
+Tolerance: BASELINE.json's fp32 gate is 1e-3 max-abs; these checks use 2e-4.  The kernels themselves are tested on
+every released launch path against float64 with derived bounds in test_gpu_f32_paths.py."""
 import pytest
 import torch
 import torch.nn.functional as F
@@ -18,56 +19,6 @@ def test_native_library_loaded(pkg, device):
     assert capi.lib().grl_device_ok() == 1, "not an sm_90 device"
     with open("/proc/self/maps") as f:
         assert "libgrl_b200.so" in f.read()
-
-
-@pytest.mark.parametrize("M,N,K,act", [(257, 540, 180, 0), (1000, 90, 180, 0), (64, 360, 180, 1), (513, 180, 360, 0),
-                                       (7, 3, 5, 2), (128, 64, 64, 0)])
-def test_linear(pkg, device, M, N, K, act):
-    from grl_image_restoration_b200 import functional as Kf
-
-    x, w, b, r = rnd((M, K), 1), rnd((N, K), 2, K ** -0.5), rnd((N,), 3), rnd((M, N), 4)
-    ref = F.linear(x, w, b)
-    ref = F.gelu(ref) if act == 1 else (F.leaky_relu(ref, 0.2) if act == 2 else ref)
-    ref = ref + r
-    y = Kf.linear(x.to(device), w.to(device), b.to(device), act, 0.2, r.to(device)).cpu()
-    assert (y - ref).abs().max().item() <= TOL
-
-
-@pytest.mark.parametrize("B,H,W,Cin,Cout,act", [(2, 16, 24, 36, 9, 1), (1, 32, 32, 3, 64, 0), (1, 8, 8, 45, 180, 0),
-                                                (2, 9, 7, 64, 12, 2), (1, 64, 64, 180, 45, 1)])
-def test_conv3x3(pkg, device, B, H, W, Cin, Cout, act):
-    from grl_image_restoration_b200 import functional as Kf
-
-    x, w, b = rnd((B, Cin, H, W), 5), rnd((Cout, Cin, 3, 3), 6, (9 * Cin) ** -0.5), rnd((Cout,), 7)
-    r = rnd((B, Cout, H, W), 8)
-    ref = F.conv2d(x, w, b, padding=1)
-    ref = F.gelu(ref) if act == 1 else (F.leaky_relu(ref, 0.01) if act == 2 else ref)
-    ref = ref + r
-    y = Kf.conv3x3(x.permute(0, 2, 3, 1).contiguous().to(device), Kf.pack_conv_weight(w).to(device), b.to(device), act,
-                   0.01, r.permute(0, 2, 3, 1).contiguous().to(device))
-    assert (y.cpu().permute(0, 3, 1, 2) - ref).abs().max().item() <= TOL
-
-
-def test_avgpool_ln_gate(pkg, device):
-    from grl_image_restoration_b200 import functional as Kf
-
-    x = rnd((2, 16, 24, 36), 9)
-    for df in (1, 2, 4):
-        ref = F.avg_pool2d(x.permute(0, 3, 1, 2), df, df).permute(0, 2, 3, 1)
-        assert (Kf.avgpool(x.to(device), df).cpu() - ref).abs().max().item() <= 1e-6
-    B, L, C = 2, 384, 180
-    xx, u, g, be = rnd((B, L, C), 10), rnd((B, L, C), 11, 3.0) + 0.7, rnd((C,), 12) + 1, rnd((C,), 13)
-    cy, gate = rnd((B, L, C), 14), torch.sigmoid(rnd((B, C), 15))
-    ref = xx + 0.1 * F.layer_norm(u, (C,), g, be, 1e-5) + cy * gate.unsqueeze(1)
-    y = Kf.ln_residual(xx.to(device), u.to(device), g.to(device), be.to(device), 1e-5, 0.1, cy.to(device), gate.to(device))
-    assert (y.cpu() - ref).abs().max().item() <= 2e-5
-    y = Kf.ln_residual(None, u.to(device), g.to(device), be.to(device))
-    assert (y.cpu() - F.layer_norm(u, (C,), g, be, 1e-5)).abs().max().item() <= 2e-5
-    w1, b1, w2, b2 = rnd((10, C), 16, 0.1), rnd((10,), 17), rnd((C, 10), 18, 0.3), rnd((C,), 19)
-    yy = rnd((B, 1000, C), 20) + 0.3
-    refg = torch.sigmoid(F.linear(torch.relu(F.linear(yy.mean(1), w1, b1)), w2, b2))
-    gg = Kf.channel_gate(yy.to(device), w1.to(device), b1.to(device), w2.to(device), b2.to(device))
-    assert (gg.cpu() - refg).abs().max().item() <= 1e-5
 
 
 def _affine_sd(heads, seed):
@@ -95,63 +46,6 @@ def test_bias_table_and_affine(pkg, oracle, device):
     t = F.linear(torch.relu(F.linear(table, sd["cpb_mlp.0.weight"], sd["cpb_mlp.0.bias"])), sd["cpb_mlp.2.weight"])
     refb = (16 * torch.sigmoid(t)).view(-1, heads).t()
     assert (mod.bias_table(table.to(device)).cpu() - refb).abs().max().item() <= 1e-5
-
-
-WIN_CASES = [  # (B, H, W, window, heads, d, shifted)
-    (2, 16, 32, (8, 8), 2, 9, True), (1, 16, 32, (8, 8), 2, 9, False), (1, 64, 64, (32, 32), 2, 16, True),
-    (1, 24, 36, (12, 12), 3, 30, True), (2, 32, 32, (16, 16), 1, 32, True), (1, 16, 16, (4, 4), 3, 10, False),
-    (1, 12, 12, (6, 6), 2, 40, True),
-]
-
-
-@pytest.mark.parametrize("B,H,W,ws,heads,d,shifted", WIN_CASES)
-def test_window_attention(pkg, oracle, device, B, H, W, ws, heads, d, shifted):
-    c = heads * d
-    sd = _affine_sd(heads, 40)
-    qkv_full = rnd((B, H * W, 6 * c), 41, 2.0)  # both halves: the kernel must honour the row stride of the view
-    qkv = qkv_full[..., : 3 * c]
-    table, index = oracle.coords_table(list(ws)), oracle.position_index(list(ws))
-    mask = oracle.shift_mask([H, W], list(ws), [ws[0] // 2] * 2) if shifted else None
-    ref = oracle.window_attention({"w.attn_transform." + k: v for k, v in sd.items()}, "w.", qkv, (H, W), ws, heads,
-                                  shifted, table, index, mask)
-    mod = pkg.WindowAttention((H, W), ws, heads, window_shift=shifted)
-    mod.attn_transform.load_state_dict(sd)
-    mod = mod.to(device)
-    q = qkv_full.to(device)[..., : 3 * c]
-    out = mod(q, (H, W), table.to(device), None, None if mask is None else torch.empty(0))
-    assert (out.cpu() - ref).abs().max().item() <= TOL
-
-
-STRIPE_CASES = [  # (B, H, W, stripe, groups, df, heads, d, shifted)
-    (2, 16, 32, [8, 16], [None, None], 2, 2, 9, True), (1, 16, 32, [16, 8], [None, None], 2, 2, 9, False),
-    (1, 64, 64, [64, 64], [None, None], 4, 2, 16, True), (1, 32, 32, [4, None], [None, 2], 2, 2, 8, True),
-    (1, 32, 32, [None, 8], [1, None], 2, 2, 8, True), (1, 16, 16, [4, None], [None, 2], 2, 2, 8, False), (1, 24, 24, [6, 12], [None, None], 3, 1, 32, True),
-    (1, 64, 128, [64, 128], [None, None], 2, 3, 30, True), (1, 48, 96, [48, 96], [None, None], 4, 3, 30, True),
-]
-
-
-@pytest.mark.parametrize("B,H,W,stripe,groups,df,heads,d,shifted", STRIPE_CASES)
-def test_stripe_attention(pkg, oracle, device, B, H, W, stripe, groups, df, heads, d, shifted):
-    c = heads * d
-    sd1, sd2 = _affine_sd(heads, 50), _affine_sd(heads, 60)
-    qkv_full = rnd((B, H * W, 6 * c), 51, 2.0)
-    qkv = qkv_full[..., 3 * c:]
-    anchor = rnd((B, H // df, W // df, c), 52, 2.0)
-    ss, sss = oracle.stripe_info(stripe, groups, True, (H, W))
-    table = oracle.coords_table(ss, df)
-    ia, iw = oracle.position_index(ss, df, False), oracle.position_index(ss, df, True)
-    ma = oracle.shift_mask([H, W], ss, sss, df, False) if shifted else None
-    mw = oracle.shift_mask([H, W], ss, sss, df, True) if shifted else None
-    sd = {"s.attn_transform1." + k: v for k, v in sd1.items()}
-    sd.update({"s.attn_transform2." + k: v for k, v in sd2.items()})
-    ref = oracle.stripe_attention(sd, "s.", qkv, anchor, (H, W), stripe, groups, shifted, df, heads, table, ia, iw, ma, mw)
-    mod = pkg.AnchorStripeAttention((H, W), stripe, groups, shifted, heads, anchor_window_down_factor=df)
-    mod.attn_transform1.load_state_dict(sd1)
-    mod.attn_transform2.load_state_dict(sd2)
-    mod = mod.to(device)
-    mk = torch.empty(0) if shifted else None
-    out = mod(qkv_full.to(device)[..., 3 * c:], anchor.to(device), (H, W), table.to(device), None, None, mk, mk)
-    assert (out.cpu() - ref).abs().max().item() <= TOL
 
 
 def test_block_and_stage_against_reference_taps(pkg, oracle, cases, golden_loader, device):
