@@ -9,14 +9,13 @@
 //
 // One CTA = one (window|stripe, head, 128-query tile).  Keys stream through shared memory in tiles of KT (TMA boxes where
 // the rolled window rows have contiguous runs, else cp.async gathers with the roll / partition address arithmetic of
-// grl_geometry.h folded in; 64-byte swizzle either way, so the tiles are valid wgmma operands as they land).  Warpgroup 0 (one query row per thread in the softmax) issues both products, two
-// m64 halves each:
-//   S  = Q K^T        A = Q [128 x 32] K-major SW64,  B = K tile [KT x 32] K-major SW64
-//   P                 softmax numerators exp2(x - m_ref) (lazily rescaled reference, kTau), 16-bit, written to smem as [128 x KT] K-major SW128
-//   Oj = P V          A = P,  B = V tile [KT keys x 32] MN-major SW64
-// The accumulator fragments pass through an fp32 tile in shared memory so that every thread then owns one whole row;
-// the running output lives in registers (o = o * corr + Oj).  Two CTAs are co-resident per SM, which is what overlaps
-// one CTA's MMAs with another's softmax.
+// grl_geometry.h folded in; 64-byte swizzle either way, so the tiles are valid wgmma operands as they land).  Two
+// consumer warpgroups own 64 query rows each and keep everything of their rows in registers:
+//   S  = Q K^T        m64n64k16, A = Q rows [64 x 32] K-major SW64 (smem), B = K tile [KT x 32] K-major SW64
+//   P                 exp2(S + bias + mask - m_ref) on the accumulator fragment (lazily rescaled reference, kTau), 16-bit
+//   O += P V          m64n32k16, A = P from registers (the S fragment is the A fragment), B = V tile [KT x 32] MN-major SW64
+// O stays in the wgmma accumulator across tiles and is rescaled in place on the rare tiles whose reference moves.  The
+// tensor core overlaps one warpgroup's products with the softmax of the other three warpgroups on the SM (two CTAs).
 #include <stdlib.h>
 #include <string.h>
 
@@ -35,17 +34,27 @@ namespace tc {
     _Pragma("unroll") for (int c_ = 0; c_ < 4; ++c_) cp_async_16((base) + sw64((r), c_), (src) + c_ * 8, (ok)); \
   } while (0)
 
-constexpr int kAttnThreads = kQT + 32;  // warpgroup 0 (MMA + softmax, one query row per thread) + 1 producer warp
+constexpr int kAttnStages = 4;                 // K / V ring depth
+constexpr int kAttnThreads = 2 * 128 + 32;     // two consumer warpgroups (64 query rows each) + 1 producer warp
 
-__device__ __forceinline__ void wg_barrier() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
+// OR of `pred` over the 64 threads of named barrier `id` (one warp pair = 32 consecutive query rows)
+__device__ __forceinline__ bool pair_any(bool pred, int id) {
+  uint32_t r;
+  asm volatile(
+      "{\n\t.reg .pred p, q;\n\tsetp.ne.u32 q, %1, 0;\n\tbar.red.or.pred p, %2, 64, q;\n\tselp.u32 %0, 1, 0, p;\n\t}"
+      : "=r"(r)
+      : "r"((uint32_t)pred), "r"(id)
+      : "memory");
+  return r != 0;
+}
 
-// Warp-specialised pipeline (tiles t = 0..nt-1 of KT keys, double-buffered K / V / key metadata):
-//   warp 4 (producer): TMA boxes or cp.async gathers of Q / K_t / V_t (roll + partition addressing), the key offsets / region ids
-//       of tile t, into buffer t & 1 once the consumers have released it (kv_empty); publishes them on kv_full.
-//   warps 0-3 (warpgroup 0): wait kv_full(t) -> S_t = Q K_t^T -> smem -> row t: S + bias -> exp2 / running max ->
-//       16-bit P_t -> smem -> O_t = P_t V_t -> release buffer -> smem -> o = o * corr + O_t.
-// KW: key-window width when it is a power of two >= 8 (bias rows read as aligned float4 from the 4-way shifted table
-// copies), 0 = generic scalar path.
+// Warp-specialised pipeline (tiles t = 0..nt-1 of KT keys, a ring of kAttnStages buffers of K / V / key metadata):
+//   warp 8 (producer): TMA boxes or cp.async gathers of Q / K_t / V_t (roll + partition addressing), the key offsets / region ids
+//       of tile t, into stage t % NS once the consumers have released it (kv_empty); publishes them on kv_full.
+//   warpgroups 0, 1 (query rows 64g..64g+63): wait kv_full(t) -> bias into the accumulator -> S_t = bias + Q K_t^T
+//       (fragment) -> mask -> lazy rescale -> 16-bit P_t in registers -> O += P_t V_t -> release stage t.
+// KW: key-window width when it is a power of two >= 8 (each column pair's bias read as one aligned float2 from the
+// shifted table copies), 0 = generic scalar path.
 // VAR: bit 0 = bf16 operands (else fp16), bit 1 = ones-column denominators -- compile-time so the exp / pack loop has no
 // uniform branches.
 // TMA boxes of the token tensors for geometries whose window rows split into aligned runs of box tokens that are
@@ -57,20 +66,18 @@ struct AttnMaps {
 
 template <int KT, int KW, int VAR>
 __global__ void __launch_bounds__(kAttnThreads, 2) attn_tc_kernel(const __grid_constant__ AttnMaps tm, const AttnTcArgs a) {
-  static_assert(KT == 64, "P tiles: 128-byte rows (SWIZZLE_128B)");
+  static_assert(KT == 64, "S fragments of m64n64 products: one key tile per product");
+  constexpr int NS = kAttnStages;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  using S = AttnSmem<KT>;
+  using S = AttnSmem<KT, NS>;
   uint8_t* Qs = smem;
   uint8_t* Ks = smem + S::OFF_K;
   uint8_t* Vs = smem + S::OFF_V;
-  uint8_t* Ps = smem + S::OFF_P;
-  float* Fs = reinterpret_cast<float*>(smem + S::OFF_F);      // S_t [kQT][SP], then O_t [kQT][OP]
-  int* koff_s = reinterpret_cast<int*>(smem + S::OFF_META);  // [2][KT]
-  int* krid_s = koff_s + 2 * KT;                              // [2][KT]
-  uint64_t* kv_full = reinterpret_cast<uint64_t*>(smem + S::OFF_BAR);  // [2] tile landed (32 producer arrivals)
-  uint64_t* kv_empty = kv_full + 2;                                    // [2] tile consumed (1 arrival)
-  constexpr int SP = S::SP, OP = S::OP;
+  int* koff_s = reinterpret_cast<int*>(smem + S::OFF_META);  // [NS][KT]
+  int* krid_s = koff_s + NS * KT;                             // [NS][KT]
+  uint64_t* kv_full = reinterpret_cast<uint64_t*>(smem + S::OFF_BAR);  // [NS] tile landed (32 producer arrivals)
+  uint64_t* kv_empty = kv_full + NS;                                   // [NS] tile consumed (1 arrival per warpgroup)
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int Nq = a.gq.wh * a.gq.ww, Nk = a.gk.wh * a.gk.ww;
@@ -87,22 +94,24 @@ __global__ void __launch_bounds__(kAttnThreads, 2) attn_tc_kernel(const __grid_c
   const int wr = w / nww, wc = w - wr * nww;
   const int Wt = a.gq.ww + a.gk.ww - 1;
   const int ntiles = (Nk + KT - 1) / KT;
+  // a warpgroup whose 64 rows all lie beyond Nq has nothing to compute (its rows form rescale groups of their own)
+  const int nwg = Nq - qt * kQT > 64 ? 2 : 1;
 
   if (tid == 0) {
-    for (int i = 0; i < 2; ++i) {
+    for (int i = 0; i < NS; ++i) {
       mbar_init(&kv_full[i], 32);
-      mbar_init(&kv_empty[i], 1);
+      mbar_init(&kv_empty[i], nwg);
     }
     mbar_init_fence();
   }
   __syncthreads();
   constexpr int fmt = (VAR & 1) ? FMT_BF16 : FMT_F16;
 
-  if (warp == 4) {
+  if (warp == 8) {
     // =============================================================== producer
     for (int t = 0; t < ntiles; ++t) {
-      const int buf = t & 1, k0 = t * KT;
-      if (t >= 2) mbar_wait(&kv_empty[buf], ((t >> 1) - 1) & 1);  // tile t - 2 is consumed
+      const int buf = t % NS, k0 = t * KT;
+      if (t >= NS) mbar_wait(&kv_empty[buf], (t / NS - 1) & 1);  // tile t - NS is consumed
       // Q (first tile) and K / V of full tiles come as TMA boxes where the geometry has them; tails and dense V are gathered
       const bool tma_q = t == 0 && tm.box_q > 0 && (qt + 1) * kQT <= Nq;
       const bool tma_k = tm.box_k > 0 && k0 + KT <= Nk;
@@ -156,192 +165,194 @@ __global__ void __launch_bounds__(kAttnThreads, 2) attn_tc_kernel(const __grid_c
       }
     }
   } else {
-    // =============================================================== warpgroup 0: MMAs + softmax (thread = query row)
-    const int qi = qt * kQT + tid;
-    const bool q_ok = qi < Nq;
-    const Tok tq = locate(a.gq, wr, wc, q_ok ? qi : 0);
-    const long long q_tok = (long long)(b * a.gq.H + tq.y) * a.gq.W + tq.x;
+    // =============================================================== warpgroups 0, 1: MMAs + softmax on the fragments
+    const int wg = warp >> 2, wq = warp & 3, tig = tid & 127;
+    if (wg >= nwg) return;
+    // accumulator fragment coordinates: rows fr and fr + 8 of the warpgroup's 64, columns 8i + fc, 8i + fc + 1
+    const int fr = 16 * wq + (lane >> 2), fc = 2 * (lane & 3);
     // bias:  idx(i, j) = base_i - koff_j  (grl_geometry.h rel_index); table copy c holds T shifted right by c entries
     const float* bias_h = a.bias + (size_t)h * 4 * a.rows_pad;
-    const int base_i = (tq.ih + a.gk.wh - 1) * Wt + tq.iw + a.gk.ww - 1;
-    const int q_rid = region_id(a.gq, tq.r, tq.c);
+    // What the thread's two rows need per tile (bias base, mask region) and at the end (output element offset) is kept
+    // in shared memory and read back when used: registers are the budget of two CTAs per SM.
+    int4* row_s = reinterpret_cast<int4*>(smem + S::OFF_ROWS) + tid;                 // base_i[2], q_rid[2]
+    long long* dst_s = reinterpret_cast<long long*>(smem + S::OFF_DST) + 2 * tid;  // output offsets, -1: row >= Nq
+    {
+      int v[4];
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {  // rows past Nq take query 0's bias and mask row (their Q rows are zero)
+        const int qi = qt * kQT + 64 * wg + fr + 8 * j;
+        const Tok tq = locate(a.gq, wr, wc, qi < Nq ? qi : 0);
+        v[j] = (tq.ih + a.gk.wh - 1) * Wt + tq.iw + a.gk.ww - 1;
+        v[2 + j] = region_id(a.gq, tq.r, tq.c);
+        dst_s[j] = qi >= Nq ? -1ll
+                   : a.o_dense ? (((long long)bw * a.heads + h) * Nq + qi) * kDP
+                               : ((long long)(b * a.gq.H + tq.y) * a.gq.W + tq.x) * a.ldo + a.o_off + h * kDP;
+      }
+      *row_s = make_int4(v[0], v[1], v[2], v[3]);
+    }
     const bool need_mask = a.use_mask && (wr == nwh - 1 || wc == nww - 1);
     // ones-column: when head_dim < 32 the projection epilogue sets column 31 of every V row to 1, so O[:, 31] =
     // sum_j P_ij is the softmax denominator -- accumulated by the tensor core from the very P it multiplies with V,
-    // and rescaled together with the other columns; the 64 FADDs per tile of the explicit row sum disappear.
+    // and rescaled together with the other columns.
     constexpr bool ones = (VAR & 2) != 0;
-    // accumulator fragment coordinates of this thread (row within each 64-row half, first column of each 8-column block)
-    const int fr = 16 * warp + (lane >> 2), fc = 2 * (lane & 3);
-    const uint32_t q_sa = smem_u32(Qs), p_sa = smem_u32(Ps);
+    // the lazy-rescale decision is shared by 32 consecutive rows: warps 0-1 and 2-3 of the warpgroup (named barriers 1-4)
+    const int pair_bar = 1 + 2 * wg + (wq >> 1);
+    const uint32_t q_sa = smem_u32(Qs) + wg * (64 * 64);
 
-    float o[kDP];
+    float oacc[16];
 #pragma unroll
-    for (int e = 0; e < kDP; ++e) o[e] = 0.f;
-    float m_ref = 0.f, l_run = 0.f;
+    for (int e = 0; e < 16; ++e) oacc[e] = 0.f;
+    float m_ref[2] = {0.f, 0.f}, l_run[2] = {0.f, 0.f};
 
     for (int t = 0; t < ntiles; ++t) {
-      const int buf = t & 1, k0 = t * KT;
-      mbar_wait(&kv_full[buf], (t >> 1) & 1);
-      {  // ---- S_t = Q K_t^T
-        float sacc[2][32];
+      const int buf = t % NS, k0 = t * KT;
+      mbar_wait(&kv_full[buf], (t / NS) & 1);
+      float s[32];
+      const int4 rw = *row_s;
+      const int base_i[2] = {rw.x, rw.y}, q_rid[2] = {rw.z, rw.w};
+      // ---- the bias of this tile (log2 domain) is the accumulator's initial value, so that S_t = bias + Q K_t^T comes
+      // out of the MMA without a second set of registers; s[4i + 2j + e] = row fr + 8j, column 8i + fc + e
+      if ((KW > 0) && (k0 + KT <= Nk)) {
+        // keys kj = k0 + 8i + fc, kj + 1 (kj even) are adjacent in one key row: table entries e0 = base - koff(kj), e0 - 1.
+        // k0 % 64 == 0 and KW % 8 == 0, so koff(kj) = koff(k0 + fc) + R(i) Wt + C(i) with compile-time R, C: one pointer
+        // per row and key row, constant offsets inside it.
+        constexpr int KWS = KW > 0 ? KW : 8;
+        const int e00 = (k0 / KWS) * Wt + (k0 % KWS) + fc;
+#pragma unroll
+        for (int i = 0; i < KT / 8; ++i) {
+          // KWS >= 64: the tile lies inside one key row (k0 % KWS + 63 < KWS); else k0 % KWS == 0
+          const int R = KWS >= 64 ? 0 : 8 * i / KWS, C = KWS >= 64 ? 8 * i : 8 * i % KWS;
+#pragma unroll
+          for (int j = 0; j < 2; ++j) {
+            const int er = base_i[j] - e00 - R * Wt;  // e0 of the key row's first pair in this tile
+            const int cpy = (er + 1) & 1;  // copy in which T[e0 - 1], T[e0] start at an even (8-byte aligned) position
+            const float2 bb = __ldg(reinterpret_cast<const float2*>(bias_h + (cpy * (a.rows_pad + 1) + er - 1 - C)));
+            s[4 * i + 2 * j] = bb.y;
+            s[4 * i + 2 * j + 1] = bb.x;
+          }
+        }
+      } else {
+#pragma unroll
+        for (int i = 0; i < KT / 8; ++i) {
+          const int2 ko = *reinterpret_cast<const int2*>(koff_s + buf * KT + 8 * i + fc);
+#pragma unroll
+          for (int j = 0; j < 2; ++j) {
+            s[4 * i + 2 * j] = __ldg(bias_h + base_i[j] - ko.x);
+            s[4 * i + 2 * j + 1] = __ldg(bias_h + base_i[j] - ko.y);
+          }
+        }
+      }
+      {  // ---- S_t = bias + Q K_t^T
         const uint32_t k_sa = smem_u32(Ks + buf * S::KV_BYTES);
+        wgmma_fence_regs(s);
         wgmma_fence();
 #pragma unroll
-        for (int hh = 0; hh < 2; ++hh)
-#pragma unroll
-          for (int k = 0; k < kDP / 16; ++k) {
-            const uint64_t ad = gmma_desc(q_sa + hh * (64 * 64) + k * 32, 16, 512, SWZ_64B);
-            const uint64_t bd = gmma_desc(k_sa + k * 32, 16, 512, SWZ_64B);
-            if (fmt == FMT_BF16) wgmma_n64_bf16(sacc[hh], ad, bd, k != 0);
-            else wgmma_n64_f16(sacc[hh], ad, bd, k != 0);
-          }
+        for (int k = 0; k < kDP / 16; ++k) {
+          const uint64_t ad = gmma_desc(q_sa + k * 32, 16, 512, SWZ_64B);
+          const uint64_t bd = gmma_desc(k_sa + k * 32, 16, 512, SWZ_64B);
+          if (fmt == FMT_BF16) wgmma_n64_bf16(s, ad, bd, true);
+          else wgmma_n64_f16(s, ad, bd, true);
+        }
         wgmma_commit();
         wgmma_wait<0>();
-        wg_barrier();  // every row has read O_{t-1} out of the fp32 tile
-#pragma unroll
-        for (int hh = 0; hh < 2; ++hh)
-#pragma unroll
-          for (int i = 0; i < KT / 8; ++i) {
-            float* d = Fs + (hh * 64 + fr) * SP + 8 * i + fc;
-            *reinterpret_cast<float2*>(d) = make_float2(sacc[hh][4 * i], sacc[hh][4 * i + 1]);
-            *reinterpret_cast<float2*>(d + 8 * SP) = make_float2(sacc[hh][4 * i + 2], sacc[hh][4 * i + 3]);
-          }
-        wg_barrier();
-      }
-      const bool full_tile = (KW > 0) && (k0 + KT <= Nk);
-
-      // ---- logits of this tile (log2 domain): S + bias
-      float lg[KT];
-#pragma unroll
-      for (int c0 = 0; c0 < KT; c0 += 32) {
-        uint32_t v[32];
-#pragma unroll
-        for (int j = 0; j < 32; j += 4) {
-          const uint4 x = *reinterpret_cast<const uint4*>(Fs + tid * SP + c0 + j);
-          v[j] = x.x, v[j + 1] = x.y, v[j + 2] = x.z, v[j + 3] = x.w;
-        }
-        if (full_tile) {
-          constexpr int KWS = KW > 0 ? KW : 4;
-          constexpr int RW = (KWS >= 32) ? 32 : KWS;  // consecutive keys of one key row inside this chunk
-#pragma unroll
-          for (int r0 = 0; r0 < 32; r0 += RW) {
-            const int kj = k0 + c0 + r0;  // first key of the run (CTA-uniform, multiple of 4)
-            const int s0 = base_i - ((kj / KWS) * Wt + (kj % KWS)) - 3;  // table index of key kj + 3
-            const int cpy = (-s0) & 3;
-            const float4* bp = reinterpret_cast<const float4*>(bias_h + (size_t)cpy * a.rows_pad + (s0 + cpy));
-#pragma unroll
-            for (int qd = 0; qd < RW / 4; ++qd) {
-              const float4 bb = __ldg(bp - qd);
-              const int j = c0 + r0 + 4 * qd;
-              lg[j + 0] = __uint_as_float(v[r0 + 4 * qd + 0]) + bb.w;
-              lg[j + 1] = __uint_as_float(v[r0 + 4 * qd + 1]) + bb.z;
-              lg[j + 2] = __uint_as_float(v[r0 + 4 * qd + 2]) + bb.y;
-              lg[j + 3] = __uint_as_float(v[r0 + 4 * qd + 3]) + bb.x;
-            }
-          }
-        } else {
-#pragma unroll
-          for (int j = 0; j < 32; ++j)
-            lg[c0 + j] = __uint_as_float(v[j]) + __ldg(bias_h + base_i - koff_s[buf * KT + c0 + j]);
-        }
+        wgmma_fence_regs(s);
       }
 
       if (need_mask) {
 #pragma unroll
-        for (int j = 0; j < KT; ++j)
-          if (krid_s[buf * KT + j] != q_rid) lg[j] += kMaskLog2;
+        for (int i = 0; i < KT / 8; ++i) {
+          const int2 rr = *reinterpret_cast<const int2*>(krid_s + buf * KT + 8 * i + fc);
+#pragma unroll
+          for (int j = 0; j < 2; ++j) {
+            if (rr.x != q_rid[j]) s[4 * i + 2 * j] += kMaskLog2;
+            if (rr.y != q_rid[j]) s[4 * i + 2 * j + 1] += kMaskLog2;
+          }
+        }
       }
       if (k0 + KT > Nk) {
 #pragma unroll
-        for (int j = 0; j < KT; ++j)
-          if (k0 + j >= Nk) lg[j] = -INFINITY;
-      }
-      float mx[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
+        for (int i = 0; i < KT / 8; ++i)
 #pragma unroll
-      for (int j = 0; j < KT; j += 4) {
-        mx[0] = fmaxf(mx[0], lg[j]), mx[1] = fmaxf(mx[1], lg[j + 1]);
-        mx[2] = fmaxf(mx[2], lg[j + 2]), mx[3] = fmaxf(mx[3], lg[j + 3]);
+          for (int e = 0; e < 4; ++e)
+            if (k0 + 8 * i + fc + (e & 1) >= Nk) s[4 * i + e] = -INFINITY;
       }
-      // Lazy rescale: the reference m_ref moves only when the tile maximum of some row of the warp outgrew it by more than
-      // 2^kTau (and on the first tile); P = exp2(x - m_ref) <= 2^kTau stays far inside the fp16 range.
-      const float mxt = fmaxf(fmaxf(mx[0], mx[1]), fmaxf(mx[2], mx[3]));
-      float corr = 1.f;
+      float mx[2];
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        float m0 = s[2 * j], m1 = s[2 * j + 1];
+#pragma unroll
+        for (int i = 1; i < KT / 8; ++i) m0 = fmaxf(m0, s[4 * i + 2 * j]), m1 = fmaxf(m1, s[4 * i + 2 * j + 1]);
+        m0 = fmaxf(m0, m1);
+        m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, 1));
+        mx[j] = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, 2));
+      }
+      // Lazy rescale: the reference m_ref moves only when the tile maximum of some row of the 32-row group outgrew it by
+      // more than 2^kTau (and on the first tile); P = exp2(x - m_ref) <= 2^kTau stays far inside the fp16 range.
       if (t == 0) {
-        m_ref = mxt;
-      } else if (__any_sync(0xffffffffu, mxt - m_ref > kTau)) {
-        const float delta = fmaxf(mxt - m_ref, 0.f);
-        m_ref += delta;
-        corr = ex2(-delta);
+        m_ref[0] = mx[0], m_ref[1] = mx[1];
+      } else if (pair_any(mx[0] - m_ref[0] > kTau || mx[1] - m_ref[1] > kTau, pair_bar)) {
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+          const float delta = fmaxf(mx[j] - m_ref[j], 0.f);
+          m_ref[j] += delta;
+          const float corr = ex2(-delta);
+          l_run[j] *= corr;
+#pragma unroll
+          for (int i = 0; i < kDP / 8; ++i) oacc[4 * i + 2 * j] *= corr, oacc[4 * i + 2 * j + 1] *= corr;
+        }
       }
-      float ps[4] = {0.f, 0.f, 0.f, 0.f};  // independent partial sums (no 64-long dependent FADD chain)
+      // ---- P_t, rounded to the operand format, packed straight into the A fragments of the P V product (k-step kk:
+      // column blocks 2kk and 2kk + 1)
+      uint32_t pa[KT / 16][4];
 #pragma unroll
-      for (int c = 0; c < KT / 8; ++c) {
-        float p[8];
+      for (int i = 0; i < KT / 8; ++i)
 #pragma unroll
-        for (int e = 0; e < 8; ++e) p[e] = ex2(lg[c * 8 + e] - m_ref);
-        uint4 pk;
-        if (fmt == FMT_BF16)
-          pk = make_uint4(pack_bf16(p[0], p[1]), pack_bf16(p[2], p[3]), pack_bf16(p[4], p[5]), pack_bf16(p[6], p[7]));
-        else
-          pk = make_uint4(pack_f16(p[0], p[1]), pack_f16(p[2], p[3]), pack_f16(p[4], p[5]), pack_f16(p[6], p[7]));
-        if (!ones) {  // the denominator is the sum of the ROUNDED P that the MMA multiplies with V
-          const uint32_t w[4] = {pk.x, pk.y, pk.z, pk.w};
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const float2 f = unpack16(w[e], fmt);
-            ps[e] += f.x + f.y;
+        for (int j = 0; j < 2; ++j) {
+          const uint32_t u = pack16(ex2(s[4 * i + 2 * j] - m_ref[j]), ex2(s[4 * i + 2 * j + 1] - m_ref[j]), fmt);
+          pa[i >> 1][2 * (i & 1) + j] = u;
+          if (!ones) {  // the denominator is the sum of the ROUNDED P that the MMA multiplies with V
+            const float2 f = unpack16(u, fmt);
+            l_run[j] += f.x + f.y;
           }
         }
-        // [128 x 64] K-major, SWIZZLE_128B
-        *reinterpret_cast<uint4*>(Ps + tid * 128 + ((c ^ (tid & 7)) << 4)) = pk;
-      }
-      l_run = l_run * corr + ((ps[0] + ps[1]) + (ps[2] + ps[3]));
-      fence_proxy_async_smem();  // P_t (generic-proxy stores) -> visible to the tensor core
-      wg_barrier();              // ... from every row; and every row is done reading S_t
-
-      {  // ---- O_t = P_t V_t
-        float oacc[2][16];
+      {  // ---- O += P_t V_t
         const uint32_t v_sa = smem_u32(Vs + buf * S::KV_BYTES);
+        wgmma_fence_regs(oacc);
         wgmma_fence();
 #pragma unroll
-        for (int hh = 0; hh < 2; ++hh)
-#pragma unroll
-          for (int k = 0; k < KT / 16; ++k) {
-            const uint64_t ad = gmma_desc(p_sa + hh * (64 * 128) + k * 32, 16, 1024, SWZ_128B);
-            const uint64_t bd = gmma_desc(v_sa + k * 1024, 16, 512, SWZ_64B);
-            if (fmt == FMT_BF16) wgmma_n32t_bf16(oacc[hh], ad, bd, k != 0);
-            else wgmma_n32t_f16(oacc[hh], ad, bd, k != 0);
-          }
+        for (int kk = 0; kk < KT / 16; ++kk) {
+          const uint64_t bd = gmma_desc(v_sa + kk * 1024, 16, 512, SWZ_64B);
+          if (fmt == FMT_BF16) wgmma_rs_n32t_bf16(oacc, pa[kk], bd);
+          else wgmma_rs_n32t_f16(oacc, pa[kk], bd);
+        }
         wgmma_commit();
         wgmma_wait<0>();
-        if (tid == 0) mbar_arrive(&kv_empty[buf]);  // K_t / V_t / metadata of buffer `buf` are no longer read
-#pragma unroll
-        for (int hh = 0; hh < 2; ++hh)
-#pragma unroll
-          for (int i = 0; i < kDP / 8; ++i) {
-            float* d = Fs + (hh * 64 + fr) * OP + 8 * i + fc;
-            *reinterpret_cast<float2*>(d) = make_float2(oacc[hh][4 * i], oacc[hh][4 * i + 1]);
-            *reinterpret_cast<float2*>(d + 8 * OP) = make_float2(oacc[hh][4 * i + 2], oacc[hh][4 * i + 3]);
-          }
-        wg_barrier();
+        wgmma_fence_regs(oacc);
       }
-      // o is kept relative to m_ref: one FFMA per element, o <- o * corr_t + O_t
-#pragma unroll
-      for (int e = 0; e < kDP; e += 4) {
-        const float4 x = *reinterpret_cast<const float4*>(Fs + tid * OP + e);
-        o[e] = fmaf(o[e], corr, x.x), o[e + 1] = fmaf(o[e + 1], corr, x.y);
-        o[e + 2] = fmaf(o[e + 2], corr, x.z), o[e + 3] = fmaf(o[e + 3], corr, x.w);
-      }
+      // stage t (K / V / metadata) is no longer read: its P V has completed, and that product needed every warp's P
+      // fragment, so every warp is past its metadata reads.  (Keeping P_t V_t in flight under S_{t+1} would hold P and
+      // the next bias live together, beyond the 96 registers of two CTAs per SM.)
+      if (tig == 0) mbar_arrive(&kv_empty[buf]);
     }
-    if (q_ok) {
-      const float inv = 1.0f / (ones ? o[kDP - 1] : l_run);
-      __nv_bfloat16* dst = a.o_dense ? a.out + (((long long)bw * a.heads + h) * Nq + qi) * kDP
-                                     : a.out + q_tok * a.ldo + a.o_off + h * kDP;
 #pragma unroll
-      for (int e = 0; e < kDP; e += 8)
-        *reinterpret_cast<uint4*>(dst + e) =
-            make_uint4(pack16(o[e] * inv, o[e + 1] * inv, fmt), pack16(o[e + 2] * inv, o[e + 3] * inv, fmt),
-                       pack16(o[e + 4] * inv, o[e + 5] * inv, fmt), pack16(o[e + 6] * inv, o[e + 7] * inv, fmt));
+    for (int j = 0; j < 2; ++j) {
+      float den;
+      if (ones) {
+        den = __shfl_sync(0xffffffffu, oacc[13 + 2 * j], lane | 3);  // O[:, 31]: block 3, column 6 + 1 of lane 4r + 3
+      } else {
+        den = l_run[j];
+        den += __shfl_xor_sync(0xffffffffu, den, 1);
+        den += __shfl_xor_sync(0xffffffffu, den, 2);
+      }
+      const float inv = 1.0f / den;
+      const long long off = dst_s[j];
+      if (off >= 0) {
+        __nv_bfloat16* dst = a.out + off;
+#pragma unroll
+        for (int i = 0; i < kDP / 8; ++i)
+          *reinterpret_cast<uint32_t*>(dst + 8 * i + fc) =
+              pack16(oacc[4 * i + 2 * j] * inv, oacc[4 * i + 2 * j + 1] * inv, fmt);
+      }
     }
   }
 }
@@ -354,10 +365,10 @@ static int launch_attn_var(const AttnMaps& tm, const AttnTcArgs& a, unsigned nbl
   int dev = 0;
   GRL_CUDA(cudaGetDevice(&dev));
   if (dev < 0 || dev >= kMaxDevices || !configured[dev]) {
-    GRL_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnSmem<KT>::TOTAL));
+    GRL_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnSmem<KT, kAttnStages>::TOTAL));
     if (dev >= 0 && dev < kMaxDevices) configured[dev] = true;
   }
-  kern<<<nblk, kAttnThreads, AttnSmem<KT>::TOTAL, st>>>(tm, a);
+  kern<<<nblk, kAttnThreads, AttnSmem<KT, kAttnStages>::TOTAL, st>>>(tm, a);
   GRL_LAUNCH_CHECK("attn_tc_kernel");
   return GRL_OK;
 }
@@ -438,7 +449,7 @@ int launch_attn_tc(const AttnTcArgs& a, cudaStream_t st) {
         (!a.v_dense && !token_map(&tm.v, a.v, a.ldv, nk, tm.box_k, a.fmt)))
       tm.box_k = 0;
   }
-  // 64 keys per tile: one 128-byte row of P per query (SWIZZLE_128B), 2 CTAs / SM
+  // 64 keys per tile: one m64n64 S fragment per warpgroup, 2 CTAs / SM
   switch (a.gk.ww) {
     case 8: return launch_attn_one<64, 8>(tm, a, (unsigned)nblk, st);
     case 16: return launch_attn_one<64, 16>(tm, a, (unsigned)nblk, st);

@@ -22,20 +22,20 @@ __device__ __forceinline__ float ex2(float x) {
 // byte offset of 16-byte chunk c of row r in a 64-byte-row SWIZZLE_64B tile
 __device__ __forceinline__ uint32_t sw64(int r, int c) { return (uint32_t)(r * 64 + ((c ^ ((r >> 1) & 3)) << 4)); }
 
-template <int KT>
+// Q, then a ring of NS stages of K / V tiles and their key metadata (stage = tile % NS), the consumer threads' row
+// records, then the ring's mbarriers.
+template <int KT, int NS>
 struct AttnSmem {
   static constexpr int Q_BYTES = kQT * 64;
   static constexpr int KV_BYTES = KT * 64;
-  static constexpr int P_BYTES = kQT * KT * 2;
-  static constexpr int SP = KT + 4, OP = kDP + 4;  // fp32 row pitches of S and O: % 8 == 4, conflict-free 16-byte rows
   static constexpr int OFF_K = Q_BYTES;
-  static constexpr int OFF_V = OFF_K + 2 * KV_BYTES;
-  static constexpr int OFF_P = (OFF_V + 2 * KV_BYTES + 1023) / 1024 * 1024;
-  static constexpr int OFF_F = OFF_P + P_BYTES;                              // fp32 S tile, later the O tile
-  static constexpr int OFF_META = OFF_F + kQT * (SP > OP ? SP : OP) * 4;    // int koff[2][KT], rid[2][KT] (tile % 2)
-  static constexpr int OFF_BAR = OFF_META + 4 * KT * 4;
-  static constexpr int TOTAL = OFF_BAR + 64 + 1024;
-  static_assert(P_BYTES % 1024 == 0, "P tiles must be 1024-byte aligned");
+  static constexpr int OFF_V = OFF_K + NS * KV_BYTES;
+  static constexpr int OFF_META = OFF_V + NS * KV_BYTES;  // int koff[NS][KT], rid[NS][KT]
+  static constexpr int OFF_ROWS = OFF_META + 2 * NS * KT * 4;  // int4 per consumer thread: bias bases, region ids
+  static constexpr int OFF_DST = OFF_ROWS + 2 * kQT * 16;       // 2 x int64 per consumer thread: output offsets
+  static constexpr int OFF_BAR = OFF_DST + 2 * kQT * 16;
+  static constexpr int TOTAL = OFF_BAR + 2 * NS * 8 + 1024;
+  static_assert(KV_BYTES % 512 == 0, "K / V tiles must stay aligned to the 64-byte swizzle repeat");
 };
 
 }  // namespace tc

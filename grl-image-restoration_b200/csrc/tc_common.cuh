@@ -110,6 +110,13 @@ template <int N>
 __device__ __forceinline__ void wgmma_wait() {
   asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
+// Pins accumulator registers in program order, so that the compiler moves no arithmetic on them across an in-flight
+// wgmma's issue or wait (it does not know that the MMA writes them asynchronously).
+template <int N>
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
 // Accumulator fragment of one m64nN warpgroup MMA: thread t (warp w = t / 32, lane l) holds, for every 8-column block i,
 // d[4i + {0,1}] = D[16w + l/4][8i + 2(l%4) + {0,1}] and d[4i + {2,3}] = the same columns of row 16w + l/4 + 8.
 // D[64 x N] (+)= A[64 x 16] * B[16 x N]; A K-major, B K-major (n64) or MN-major (n32, transposed B).  All 128 threads of
@@ -132,6 +139,20 @@ GRL_WGMMA(wgmma_n64_bf16, 64, 32, GRL_R32, GRL_D32, 32, 33, 34, "bf16", 0)
 GRL_WGMMA(wgmma_n64_f16, 64, 32, GRL_R32, GRL_D32, 32, 33, 34, "f16", 0)
 GRL_WGMMA(wgmma_n32t_bf16, 32, 16, GRL_R16, GRL_D16, 16, 17, 18, "bf16", 1)
 GRL_WGMMA(wgmma_n32t_f16, 32, 16, GRL_R16, GRL_D16, 16, 17, 18, "f16", 1)
+// Register-A form: m64n32k16, D += A B with A[64 x 16] from registers and B MN-major in shared memory.  Thread t (warp w,
+// lane l) supplies a[0] = A[16w + l/4][2(l%4) + {0,1}], a[1] = the same columns of row 16w + l/4 + 8, a[2] / a[3] = columns
+// 8 + 2(l%4) + {0,1} of those two rows (low half = lower column) -- for k = 16j..16j+15 that is exactly the accumulator
+// fragment of an m64nN product over those columns (blocks 2j and 2j + 1 above), packed to 16 bits.
+#define GRL_WGMMA_RS(NAME, TY)                                                                                        \
+  __device__ __forceinline__ void NAME(float (&d)[16], const uint32_t (&a)[4], uint64_t bdesc) {                     \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"                                                    \
+                 "wgmma.mma_async.sync.aligned.m64n32k16.f32." TY "." TY " {" GRL_R16 "}, {%16, %17, %18, %19}, %20, " \
+                 "p, 1, 1, 1;\n\t}"                                                                                 \
+                 : GRL_D16                                                                                          \
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc));                                         \
+  }
+GRL_WGMMA_RS(wgmma_rs_n32t_bf16, "bf16")
+GRL_WGMMA_RS(wgmma_rs_n32t_f16, "f16")
 
 __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
   __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
