@@ -86,11 +86,11 @@ def avgpool(x, df):
     return y
 
 
-def ln_residual(x, u, gamma, beta, eps=1e-5, res_scale=1.0, cab_y=None, cab_gate=None):
+def ln_residual(x, u, gamma, beta, eps=1e-5, res_scale=1.0, cab_y=None, cab_gate=None, out=None):
     """(x or 0) + res_scale * LN(u) (+ cab_y * gate[b]); x, u (B, L, C)."""
     u = _f32c(u, "u")
     B, L, C = u.shape
-    out = torch.empty_like(u)
+    out = torch.empty_like(u) if out is None else out
     capi.check(capi.lib().grl_ln_residual_f32(
         capi.ptr(_f32c(x, "x")) if x is not None else None, capi.ptr(u), capi.ptr(gamma), capi.ptr(beta), eps,
         res_scale, capi.ptr(_f32c(cab_y, "cab_y")) if cab_y is not None else None,

@@ -21,6 +21,7 @@ import torch.nn.functional as F
 
 from . import functional as K
 from . import geometry as G
+from . import tc
 from .geometry import to_2tuple, _get_stripe_info
 
 _LN_MAX = math.log(1.0 / 0.01)
@@ -381,12 +382,8 @@ class EfficientMixAttnTransformerBlock(nn.Module):
         """Tensor-core path with the residual stream as an explicit PAIR: x32 fp32 (B, L, C) and its 16-bit operand copy
         x16 (B, L, Cpad) (None: packed here).  Returns the pair of the block's output, so a stage / network chains
         blocks without re-packing and without hiding state on tensors."""
-        from . import tc
-
         K.capi.require_device(x32)
-        t = self._get_table_index_mask(all_table_index_mask)
-        x32 = x32 if x32.is_contiguous() else x32.contiguous()
-        return tc.block_plan(self, tc.FMT[self.precision]).run(self, x32, x16, x_size, t)
+        return tc.block_plan(self, tc.FMT[self.precision]).run(self, x32, x16, x_size, all_table_index_mask)
 
     @torch.no_grad()
     def forward(self, x, x_size, all_table_index_mask):
@@ -511,23 +508,8 @@ class TransformerStage(nn.Module):
     @torch.no_grad()
     def forward_tc(self, x32, x16, x_size, table_index_mask):
         """Tensor-core path of the stage on the explicit (fp32 stream, 16-bit operand copy) pair; returns the pair."""
-        from . import tc
-
-        B, L, C = x32.shape
-        H, W = x_size
-        fmt = tc.FMT[self.blocks[0].precision]
-        cpad = tc.round_up(C, 64)
-        r32, r16 = x32, x16
-        for blk in self.blocks:
-            r32, r16 = blk.forward_tc(r32, r16, x_size, table_index_mask)
-        if r16 is None or r16.dtype != tc.DTYPE[fmt]:
-            r16 = tc.pack_rows(r32.contiguous(), cpad, fmt)
-        plan = tc.conv_plan(self, "conv", self.conv, cpad, fmt)
-        out32 = torch.empty(B, L, C, device=x32.device, dtype=torch.float32)
-        out16 = torch.empty(B, L, cpad, device=x32.device, dtype=tc.DTYPE[fmt])
-        tc.conv3x3(r16.view(B, H, W, cpad), plan.w, plan.b, cpad, plan.npad, n_store=cpad, n_real=C, out_bf16=out16,
-                   out_f32=out32, res_f32=x32.contiguous())
-        return out32, out16
+        K.capi.require_device(x32)
+        return tc.stage_forward(self, x32, x16, x_size, table_index_mask)
 
     @torch.no_grad()
     def forward(self, x, x_size, table_index_mask):
@@ -665,8 +647,6 @@ class GRL(nn.Module):
         that MMA operand format (fp32 accumulation, residual stream, LayerNorm and softmax statistics); fp16 operands
         (11-bit mantissa) are what meets the 0.01 dB PSNR gate, bf16 is provided for range-critical checkpoints.
         "auto": fp16 when the architecture fits the tensor-core kernels (head_dim <= 32, C % 4 == 0), else fp32."""
-        from . import tc
-
         if precision not in ("fp32", "fp16", "bf16", "auto"):
             raise ValueError(f"precision must be fp32 / fp16 / bf16 / auto, got {precision!r}")
         ok = all(tc.supported(self.embed_dim, b.num_heads_w, b.num_heads_s) for l in self.layers for b in l.blocks)
@@ -779,78 +759,6 @@ class GRL(nn.Module):
         t = K.ln_residual(None, t, self.norm_end.weight, self.norm_end.bias, self.norm_end.eps)
         return t.view(B, H, W, C)
 
-    @torch.no_grad()
-    def _forward_bf16(self, x, rggb=False):
-        """grl.py:506-551 on the tensor-core kernels; x is the RAW (B, Cin, H, W) fp32 input, or with rggb its packed
-        (B, 4, H/2, W/2) Bayer planes.  Head: one kernel does [dm_matlab +] check_image_size + (x - mean) * img_range +
-        bchw -> bhwc + operand pack; tail: the last conv's epilogue writes x / img_range + mean, cropped, as bchw planes;
-        PixelShuffle is a store-address pattern of the conv before it."""
-        from . import tc
-
-        dev = x.device
-        fmt = tc.FMT[self.precision]
-        B, Cin, H, W = x.shape
-        if rggb:
-            Cin, H, W = 3, 2 * H, 2 * W
-        Hp = (H + self.pad_size - 1) // self.pad_size * self.pad_size
-        Wp = (W + self.pad_size - 1) // self.pad_size * self.pad_size
-        C = self.embed_dim
-        cpad = tc.round_up(C, 64)
-        s = self.upscale
-        need_res = self.upsampler not in ("pixelshuffle", "pixelshuffledirect", "nearest+conv") and self.in_channels == self.out_channels
-        mean = self._mean_list
-        head = tc.head_pack_rggb if rggb else tc.head_pack
-        x16, xc32 = head(x, Hp, Wp, mean, self.img_range, 64, fmt, want_f32=need_res)
-        shift = mean if len(mean) > 1 else mean * 4
-
-        def conv(name, module, inp16, cin_pad, *, act=K.ACT_NONE, slope=0.0, res=None, want_f32=False, want16=True, ps_r=0,
-                 final_r=0):
-            plan = tc.conv_plan(self, name, module, cin_pad, fmt, ps_r)
-            b, h, w, _ = inp16.shape
-            tail, o16, o32 = {}, None, None
-            if final_r:  # network output: (B, C_out, H s, W s) planes straight from the epilogue
-                tail = dict(out_nchw=torch.empty(B, self.out_channels, H * s, W * s, device=dev, dtype=torch.float32),
-                            nchw_r=final_r, post_scale=1.0 / self.img_range, post_shift=shift)
-            elif ps_r:
-                o16 = torch.empty(b, h * ps_r, w * ps_r, plan.cout // (ps_r * ps_r), device=dev, dtype=tc.DTYPE[fmt])
-                tail = dict(ps_r=ps_r)
-            else:
-                o16 = torch.empty(b, h, w, plan.npad, device=dev, dtype=tc.DTYPE[fmt]) if want16 else None
-                o32 = torch.empty(b, h, w, plan.cout, device=dev, dtype=torch.float32) if want_f32 else None
-            tc.conv3x3(inp16, plan.w, plan.b, cin_pad, plan.npad, n_store=plan.cout if ps_r else plan.npad, n_real=plan.cout,
-                       act=act, slope=slope, out_bf16=o16, out_f32=o32, res_f32=res, **tail)
-            return (tail["out_nchw"], None) if final_r else (o16, o32)
-
-        f16, f32 = conv("conv_first", self.conv_first, x16, 64, want_f32=True)
-        feat = f32.view(B, Hp * Wp, C)
-        t = K.ln_residual(None, feat, self.norm_start.weight, self.norm_start.bias, self.norm_start.eps)
-        tim = self.get_table_index_mask(dev, (Hp, Wp))
-        t16 = None  # 16-bit operand copy of the residual stream, carried explicitly from block to block
-        for layer in self.layers:
-            t, t16 = layer.forward_tc(t, t16, (Hp, Wp), tim)
-        t = K.ln_residual(None, t, self.norm_end.weight, self.norm_end.bias, self.norm_end.eps)
-        t16 = tc.pack_rows(t, cpad, fmt).view(B, Hp, Wp, cpad)
-        body16, _ = conv("conv_after_body", self.conv_after_body, t16, cpad, res=f32)
-        if self.upsampler == "pixelshuffle":
-            u16, _ = conv("conv_before_upsample", self.conv_before_upsample[0], body16, cpad, act=K.ACT_LEAKY, slope=0.01)
-            mods = list(self.upsample.up)
-            for i, m in enumerate(mods):
-                if isinstance(m, nn.Conv2d):  # always followed by its PixelShuffle (upsample.py:6-30)
-                    u16, _ = conv(f"upsample.up.{i}", m, u16, u16.shape[-1], ps_r=mods[i + 1].upscale_factor)
-            y, _ = conv("conv_last", self.conv_last, u16, u16.shape[-1], final_r=1)
-        elif self.upsampler == "pixelshuffledirect":
-            y, _ = conv("upsample.up.0", self.upsample.up[0], body16, cpad, final_r=self.upsample.up[1].upscale_factor)
-        elif self.upsampler == "nearest+conv":
-            u16, _ = conv("conv_before_upsample", self.conv_before_upsample[0], body16, cpad, act=K.ACT_LEAKY, slope=0.01)
-            up = lambda v: v.repeat_interleave(2, dim=1).repeat_interleave(2, dim=2).contiguous()
-            u16, _ = conv("conv_up1", self.conv_up1, up(u16), u16.shape[-1], act=K.ACT_LEAKY, slope=0.2)
-            u16, _ = conv("conv_up2", self.conv_up2, up(u16), u16.shape[-1], act=K.ACT_LEAKY, slope=0.2)
-            u16, _ = conv("conv_hr", self.conv_hr, u16, u16.shape[-1], act=K.ACT_LEAKY, slope=0.2)
-            y, _ = conv("conv_last", self.conv_last, u16, u16.shape[-1], final_r=1)
-        else:
-            y, _ = conv("conv_last", self.conv_last, body16, cpad, res=xc32, final_r=1)
-        return y
-
     # ---- CUDA graphs ----------------------------------------------------------------------------
     def reset_cuda_graphs(self):
         """Drops every captured graph (they bake in the addresses of the packed weights and of their static buffers)."""
@@ -866,7 +774,7 @@ class GRL(nn.Module):
 
     @torch.no_grad()
     def _forward_graphed(self, x, rggb=False):
-        """Replays a captured graph of _forward_bf16 for this input shape and format (captures it on first use, after two
+        """Replays a captured graph of tc.forward for this input shape and format (captures it on first use, after two
         eager warm-up forwards that build the packed weights / bias tables / kernel attributes).  The result is a fresh
         tensor (the caller may mutate it in place, engines/base.py:113)."""
         key = (tuple(x.shape), x.device.index, self.precision, "rggb" if rggb else "rgb")
@@ -877,11 +785,11 @@ class GRL(nn.Module):
             side.wait_stream(torch.cuda.current_stream())
             with torch.cuda.stream(side):
                 for _ in range(2):
-                    self._forward_bf16(static_in, rggb)
+                    tc.forward(self, static_in, rggb)
             torch.cuda.current_stream().wait_stream(side)
             graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(graph):
-                static_out = self._forward_bf16(static_in, rggb)
+                static_out = tc.forward(self, static_in, rggb)
             ent = (graph, static_in, static_out)
             self._graphs[key] = ent
         graph, static_in, static_out = ent
@@ -947,7 +855,7 @@ class GRL(nn.Module):
         H, W = x.shape[2:]
         if self.precision != "fp32":
             xin = x.float().contiguous()
-            y = self._forward_graphed(xin, rggb) if self.use_cuda_graph else self._forward_bf16(xin, rggb)
+            y = self._forward_graphed(xin, rggb) if self.use_cuda_graph else tc.forward(self, xin, rggb)
             return y.to(x.dtype)
         assert not rggb, "the fp32 path demosaics in forward"
         x = self.check_image_size(x)

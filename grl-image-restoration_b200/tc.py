@@ -2,7 +2,9 @@
 
 Host-side orchestration only: one-time weight packing (pad head_dim to 32-wide slots, pad channel pitches to
 multiples of 64, permute the QKV rows into [window q|k|v][stripe q|k|v] x head order, im2col-order the 3x3 kernels)
-and the launch sequence of the wgmma kernels behind the C ABI (grl_tc_gemm / grl_tc_attn, include/grl_b200.h).
+and the launch sequence of the wgmma kernels behind the C ABI (grl_tc_gemm / grl_tc_attn, include/grl_b200.h).  That
+sequence is written once (forward / stage_forward / BlockPlan.run) and issued through a launcher: Device runs it,
+Listing records its GEMMs without a device (gemm_launches).
 Numerics contract (DESIGN.md): bf16 only for MMA operands; residual stream, LayerNorm, L2-normalisation, softmax
 statistics and every accumulator are fp32.
 Reference semantics: mixed_attn_block_efficient.py:351-381,:539-556; mixed_attn_block.py:948-983; grl.py:164-170,:506-551.
@@ -12,6 +14,7 @@ import inspect
 from typing import NamedTuple
 
 import torch
+from torch import nn
 
 from . import capi
 from . import functional as K
@@ -54,33 +57,33 @@ def _mean4(mean):
     return (ctypes.c_float * 4)(*m)
 
 
-def head_pack(x, hp, wp, mean, img_range, cpad=64, fmt=0, want_f32=False):
+def head_pack(x, hp, wp, mean, img_range, cpad=64, fmt=0, want_f32=False, out=None):
     """Network input (B, Cin, H, W) fp32 -> 16-bit channels-last (B, hp, wp, cpad) [+ fp32 (B, hp, wp, Cin)]: reflect pad,
-    (x - mean) * img_range, layout change and operand pack in one kernel (grl_tc_head_pack)."""
+    (x - mean) * img_range, layout change and operand pack in one kernel (grl_tc_head_pack).  out: that pair, preallocated."""
     B, Cin, H, W = x.shape
-    y16 = _h16(B, hp, wp, cpad, device=x.device, fmt=fmt)
-    y32 = torch.empty(B, hp, wp, Cin, device=x.device, dtype=torch.float32) if want_f32 else None
+    y16, y32 = out or (_h16(B, hp, wp, cpad, device=x.device, fmt=fmt),
+                       torch.empty(B, hp, wp, Cin, device=x.device, dtype=torch.float32) if want_f32 else None)
     capi.check(capi.lib().grl_tc_head_pack(capi.ptr(x), B, Cin, H, W, hp, wp, _mean4(mean), float(img_range), capi.ptr(y16),
                                            cpad, capi.ptr(y32), fmt, capi.stream()))
     return y16, y32
 
 
-def head_pack_rggb(cfa4, hp, wp, mean, img_range, cpad=64, fmt=0, want_f32=False):
+def head_pack_rggb(cfa4, hp, wp, mean, img_range, cpad=64, fmt=0, want_f32=False, out=None):
     """head_pack of K.demosaic(cfa4) in one kernel (grl_tc_head_pack_rggb): packed RGGB planes (B, 4, h, w) fp32 ->
     (B, hp, wp, cpad) [+ fp32 (B, hp, wp, 3)] for the (2h, 2w) image, without writing the RGB image."""
     B, _, h, w = cfa4.shape
-    y16 = _h16(B, hp, wp, cpad, device=cfa4.device, fmt=fmt)
-    y32 = torch.empty(B, hp, wp, 3, device=cfa4.device, dtype=torch.float32) if want_f32 else None
+    y16, y32 = out or (_h16(B, hp, wp, cpad, device=cfa4.device, fmt=fmt),
+                       torch.empty(B, hp, wp, 3, device=cfa4.device, dtype=torch.float32) if want_f32 else None)
     capi.check(capi.lib().grl_tc_head_pack_rggb(capi.ptr(cfa4), B, h, w, hp, wp, _mean4(mean), float(img_range),
                                                 capi.ptr(y16), cpad, capi.ptr(y32), fmt, capi.stream()))
     return y16, y32
 
 
-def pack_rows(x, cpad, fmt=0):
+def pack_rows(x, cpad, fmt=0, out=None):
     """fp32 (..., C) contiguous -> 16-bit (..., cpad), zero padded."""
     C = x.shape[-1]
     M = x.numel() // C
-    y = _h16(*x.shape[:-1], cpad, device=x.device, fmt=fmt)
+    y = _h16(*x.shape[:-1], cpad, device=x.device, fmt=fmt) if out is None else out
     capi.check(capi.lib().grl_tc_pack16(capi.ptr(x), C, capi.ptr(y), M, C, cpad, fmt, capi.stream()))
     return y
 
@@ -221,6 +224,36 @@ def gemm_path(launch):
     return out
 
 
+class Device:
+    """Launcher of a tensor-core forward on the GPU: every kernel runs.  The forward hands it each GEMM (`gemm`) and
+    every other kernel (`run`, a wrapper and its arguments)."""
+    caches = True  # attention constants computed through it are real, so BlockPlan may keep them
+
+    def gemm(self, name, x16, w16, bias, **kw):
+        gemm(x16, w16, bias, **kw)  # the module's gemm at call time (tests record launches by replacing it)
+
+    def run(self, fn, *args, **kw):
+        fn(*args, **kw)
+
+
+class Listing:
+    """Launcher of a listing run: activations are meta tensors, every GEMM is recorded as a GemmLaunch and nothing is
+    launched."""
+    caches = False
+
+    def __init__(self):
+        self.launches = []
+
+    def gemm(self, name, x16, w16, bias, **kw):
+        self.launches.append(gemm_launch(name, x16, w16, bias, **kw))
+
+    def run(self, fn, *args, **kw):
+        pass
+
+
+DEVICE = Device()
+
+
 def attention(gq, gk, q, q_off, k, k_off, v, v_off, out, o_off, B, heads, bias, use_mask, v_dense=False,
               o_dense=False, tag="attn", ones_col=False):
     p = capi.GrlTcAttn()
@@ -299,24 +332,31 @@ def shifted_copies(table_hr):
     return out
 
 
-def bias_table_log2(transform, table):
-    """16*sigmoid(cpb_mlp(table))*log2(e) as the 4-copy table of the attention kernel."""
+def bias_table_log2(transform, table, out):
+    """16*sigmoid(cpb_mlp(table))*log2(e) as the 4-copy table of the attention kernel, written into `out`: zero-filled
+    (heads, 4, bias_rows_pad(rows)) fp32."""
     t = table.reshape(-1, 2)
     w1, b1, w2 = transform.cpb_mlp[0].weight, transform.cpb_mlp[0].bias, transform.cpb_mlp[2].weight
     heads, hidden = w2.shape
-    rows_pad = bias_rows_pad(t.shape[0])
-    out = torch.zeros(heads, 4, rows_pad, device=t.device, dtype=torch.float32)
     capi.check(capi.lib().grl_tc_bias_table4(capi.ptr(t), t.shape[0], capi.ptr(w1), capi.ptr(b1), capi.ptr(w2), hidden,
-                                             heads, LOG2E, rows_pad, capi.ptr(out), capi.stream()))
-    return out
+                                             heads, LOG2E, out.shape[2], capi.ptr(out), capi.stream()))
 
 
-def conv3x3(x16, wpack, bias, cin_pad, npad, *, n_store, n_real=0, act=K.ACT_NONE, slope=0.0, out_bf16=None,
-            out_f32=None, res_f32=None, **tail):
-    """x16 bf16 (B, H, W, cin_pad) channels-last.  tail: ps_r / out_nchw / nchw_r / post_scale / post_shift (head-tail fusion)."""
+def channel_gate(y16, ld, B, L, C, ca, gate):
+    """CAB gate (B, C) fp32 into `gate` from the 16-bit features y16 (B*L, ld); ca: the packed ChannelAttention weights."""
+    lib = capi.lib()
+    nbytes = lib.grl_tc_channel_gate_workspace(B, L, C)
+    ws = torch.empty(max(nbytes, 4) // 4, device=y16.device, dtype=torch.float32)
+    w1, b1, w2, b2 = ca
+    capi.check(lib.grl_tc_channel_gate(capi.ptr(y16), ld, fmt_of(y16), B, L, C, capi.ptr(w1), capi.ptr(b1), capi.ptr(w2),
+                                       capi.ptr(b2), w1.shape[0], capi.ptr(gate), capi.ptr(ws), nbytes, capi.stream()))
+
+
+def conv3x3(x16, wpack, bias, cin_pad, npad, *, n_store, launch=DEVICE, name="", **kw):
+    """x16 16-bit (B, H, W, cin_pad) channels-last; kw: gemm's outputs, residual, activation and head-tail fusion."""
     B, H, W, _ = x16.shape
-    gemm(x16, wpack, bias, image=(B, H, W), kpad=cin_pad, npad=npad, taps=9, epi=EPI_BIAS_ACT, n_store=n_store,
-         n_real=n_real, out_bf16=out_bf16, out_f32=out_f32, res_f32=res_f32, act=act, slope=slope, **tail)
+    launch.gemm(name, x16, wpack, bias, image=(B, H, W), kpad=cin_pad, npad=npad, taps=9, epi=EPI_BIAS_ACT,
+                n_store=n_store, **kw)
 
 
 def _version_key(module):
@@ -393,8 +433,11 @@ class BlockPlan:
                        a3.weight.detach().reshape(a3.weight.shape[0], -1).contiguous(), a3.bias.detach())
 
     @torch.no_grad()
-    def run(self, blk, x32, x16, x_size, t):
-        """x32 fp32 (B, L, C), x16 bf16 (B, L, cpad) or None -> (x32', x16')."""
+    def run(self, blk, x32, x16, x_size, all_table_index_mask, launch=DEVICE, name=""):
+        """x32 fp32 (B, L, C), x16 16-bit (B, L, cpad) or None -> (x32', x16').  Launches through `launch`; GEMMs are
+        named "{name}.qkv" etc."""
+        t = blk._get_table_index_mask(all_table_index_mask)
+        x32 = x32 if x32.is_contiguous() else x32.contiguous()
         B, L, C = x32.shape
         H, W = x_size
         dev = x32.device
@@ -402,35 +445,40 @@ class BlockPlan:
         hw, hs, cpad = self.hw, self.hs, self.cpad
         fmt = self.fmt
         if x16 is None or x16.dtype != DTYPE[fmt]:
-            x16 = pack_rows(x32, cpad, fmt)
-        lib = capi.lib()
+            x16 = _h16(B, L, cpad, device=dev, fmt=fmt)
+            launch.run(pack_rows, x32, cpad, fmt, out=x16)
         wa, sa = at.window_attn, at.stripe_attn
         # attention constants of this block (slot scales + activated bias tables): functions of the parameters and
         # the coordinate tables only, so they are cached until a parameter or the resolution changes
         ckey = (self.key, t["table_w"].data_ptr(), t["table_s"].data_ptr(), t["table_s"].shape)
-        if self._const_key != ckey:
+        if self._const_key == ckey:
+            slot_scale, bias_w, bias_1, bias_2 = self._consts
+        else:
             slot_scale = torch.empty(self.nslots, device=dev, dtype=torch.float32)
-            capi.check(lib.grl_tc_slot_scale(capi.ptr(wa.attn_transform.logit_scale),
-                                             capi.ptr(sa.attn_transform1.logit_scale),
-                                             capi.ptr(sa.attn_transform2.logit_scale), hw, hs, capi.ptr(slot_scale),
-                                             capi.stream()))
-            self._consts = (slot_scale, bias_table_log2(wa.attn_transform, t["table_w"]),
-                            bias_table_log2(sa.attn_transform1, t["table_s"]),
-                            bias_table_log2(sa.attn_transform2, t["table_s"]))
-            self._const_key = ckey
-        slot_scale, bias_w, bias_1, bias_2 = self._consts
+            launch.run(lambda: capi.check(capi.lib().grl_tc_slot_scale(
+                capi.ptr(wa.attn_transform.logit_scale), capi.ptr(sa.attn_transform1.logit_scale),
+                capi.ptr(sa.attn_transform2.logit_scale), hw, hs, capi.ptr(slot_scale), capi.stream())))
+            tables = ((wa.attn_transform, t["table_w"]), (sa.attn_transform1, t["table_s"]),
+                      (sa.attn_transform2, t["table_s"]))
+            bias_w, bias_1, bias_2 = [torch.zeros(tr.cpb_mlp[2].weight.shape[0], 4, bias_rows_pad(tb.numel() // 2),
+                                                  device=dev, dtype=torch.float32) for tr, tb in tables]
+            for (tr, tb), out in zip(tables, (bias_w, bias_1, bias_2)):
+                launch.run(bias_table_log2, tr, tb, out)
+            if launch.caches:  # never keep a listing run's meta constants: a later forward would launch with them
+                self._const_key, self._consts = ckey, (slot_scale, bias_w, bias_1, bias_2)
         # projections
         qkv = _h16(B * L, self.n_qkv, device=dev, fmt=fmt)
-        gemm(x16, self.w_qkv, self.b_qkv, M=B * L, kpad=cpad, npad=self.n_qkv, epi=EPI_QKV, n_store=self.n_qkv,
-             out_bf16=qkv, slot_scale=slot_scale)
+        launch.gemm(f"{name}.qkv", x16, self.w_qkv, self.b_qkv, M=B * L, kpad=cpad, npad=self.n_qkv, epi=EPI_QKV,
+                    n_store=self.n_qkv, out_bf16=qkv, slot_scale=slot_scale)
         df = self.df
         pooled = _h16(B, H // df, W // df, cpad, device=dev, fmt=fmt)
-        capi.check(lib.grl_tc_avgpool16(capi.ptr(x16), capi.ptr(pooled), B, H, W, cpad, df, fmt, capi.stream()))
+        launch.run(lambda: capi.check(capi.lib().grl_tc_avgpool16(capi.ptr(x16), capi.ptr(pooled), B, H, W, cpad, df, fmt,
+                                                                  capi.stream())))
         La = (H // df) * (W // df)
         n_anc = self.w_anc.shape[0]
         anchor = _h16(B * La, n_anc, device=dev, fmt=fmt)
-        gemm(pooled, self.w_anc, self.b_anc, M=B * La, kpad=cpad, npad=n_anc, epi=EPI_QKV, n_store=n_anc, out_bf16=anchor,
-             slot_scale=self.anc_scale)
+        launch.gemm(f"{name}.anchor", pooled, self.w_anc, self.b_anc, M=B * La, kpad=cpad, npad=n_anc, epi=EPI_QKV,
+                    n_store=n_anc, out_bf16=anchor, slot_scale=self.anc_scale)
         # attention
         merged = _h16(B * L, self.k_proj, device=dev, fmt=fmt, zero=self.k_proj != (hw + hs) * SLOT)
         launches = attention_launches(blk, x_size)
@@ -440,39 +488,35 @@ class BlockPlan:
         buf = {"qkv": qkv, "anchor": anchor, "x1": x1, "merged": merged}
         bias = {"window": bias_w, "stripe1": bias_1, "stripe2": bias_2}
         for ln in launches:
-            attention(ln.gq, ln.gk, buf[ln.q[0]], ln.q[1], buf[ln.k[0]], ln.k[1], buf[ln.v[0]], ln.v[1], buf[ln.out[0]],
-                      ln.out[1], B, ln.heads, bias[ln.role], ln.use_mask, v_dense=ln.v_dense, o_dense=ln.o_dense,
-                      tag="window_attn" if ln.role == "window" else "stripe_attn", ones_col=ln.ones_col)
+            launch.run(attention, ln.gq, ln.gk, buf[ln.q[0]], ln.q[1], buf[ln.k[0]], ln.k[1], buf[ln.v[0]], ln.v[1],
+                       buf[ln.out[0]], ln.out[1], B, ln.heads, bias[ln.role], ln.use_mask, v_dense=ln.v_dense,
+                       o_dense=ln.o_dense, tag="window_attn" if ln.role == "window" else "stripe_attn", ones_col=ln.ones_col)
         # CAB
         cab_y = gate = None
         if self.cab:
             t1 = _h16(B, H, W, self.cmid_pad, device=dev, fmt=fmt)
             conv3x3(x16.view(B, H, W, cpad), self.w_cab1, self.b_cab1, cpad, self.cmid_pad, n_store=self.cmid_pad,
-                    act=K.ACT_GELU, out_bf16=t1)
+                    act=K.ACT_GELU, out_bf16=t1, launch=launch, name=f"{name}.cab1")
             cab_y = _h16(B * L, cpad, device=dev, fmt=fmt)
-            conv3x3(t1, self.w_cab2, self.b_cab2, self.cmid_pad, cpad, n_store=cpad, out_bf16=cab_y)
-            nbytes = lib.grl_tc_channel_gate_workspace(B, L, C)
-            ws = torch.empty(max(nbytes, 4) // 4, device=dev, dtype=torch.float32)
+            conv3x3(t1, self.w_cab2, self.b_cab2, self.cmid_pad, cpad, n_store=cpad, out_bf16=cab_y, launch=launch,
+                    name=f"{name}.cab2")
             gate = torch.empty(B, C, device=dev, dtype=torch.float32)
-            w1, b1, w2, b2 = self.ca
-            capi.check(lib.grl_tc_channel_gate(capi.ptr(cab_y), cpad, fmt, B, L, C, capi.ptr(w1), capi.ptr(b1), capi.ptr(w2),
-                                               capi.ptr(b2), w1.shape[0], capi.ptr(gate), capi.ptr(ws), nbytes,
-                                               capi.stream()))
+            launch.run(channel_gate, cab_y, cpad, B, L, C, self.ca, gate)
         # proj + LN1 + residual (+ CAB)
         y32 = torch.empty(B, L, C, device=dev, dtype=torch.float32)
         y16 = _h16(B, L, cpad, device=dev, fmt=fmt)
-        gemm(merged, self.w_proj, self.b_proj, M=B * L, kpad=self.k_proj, npad=self.n_ln, epi=EPI_LN, n_store=self.n_ln,
-             n_real=C, out_bf16=y16, out_f32=y32, res_f32=x32, C=C, gamma=blk.norm1.weight, beta=blk.norm1.bias,
-             eps=blk.norm1.eps, res_scale=blk.res_scale, cab_y=cab_y, cab_gate=gate, L=L)
+        launch.gemm(f"{name}.proj", merged, self.w_proj, self.b_proj, M=B * L, kpad=self.k_proj, npad=self.n_ln, epi=EPI_LN,
+                    n_store=self.n_ln, n_real=C, out_bf16=y16, out_f32=y32, res_f32=x32, C=C, gamma=blk.norm1.weight,
+                    beta=blk.norm1.bias, eps=blk.norm1.eps, res_scale=blk.res_scale, cab_y=cab_y, cab_gate=gate, L=L)
         # MLP + LN2 + residual
         hid = _h16(B * L, self.hpad, device=dev, fmt=fmt)
-        gemm(y16, self.w_fc1, self.b_fc1, M=B * L, kpad=cpad, npad=self.hpad, epi=EPI_BIAS_ACT, n_store=self.hpad,
-             act=K.ACT_GELU, out_bf16=hid)
+        launch.gemm(f"{name}.fc1", y16, self.w_fc1, self.b_fc1, M=B * L, kpad=cpad, npad=self.hpad, epi=EPI_BIAS_ACT,
+                    n_store=self.hpad, act=K.ACT_GELU, out_bf16=hid)
         z32 = torch.empty(B, L, C, device=dev, dtype=torch.float32)
         z16 = _h16(B, L, cpad, device=dev, fmt=fmt)
-        gemm(hid, self.w_fc2, self.b_fc2, M=B * L, kpad=self.hpad, npad=self.n_ln, epi=EPI_LN, n_store=self.n_ln, n_real=C,
-             out_bf16=z16, out_f32=z32, res_f32=y32, C=C, gamma=blk.norm2.weight, beta=blk.norm2.bias, eps=blk.norm2.eps,
-             res_scale=blk.res_scale, L=L)
+        launch.gemm(f"{name}.fc2", hid, self.w_fc2, self.b_fc2, M=B * L, kpad=self.hpad, npad=self.n_ln, epi=EPI_LN,
+                    n_store=self.n_ln, n_real=C, out_bf16=z16, out_f32=z32, res_f32=y32, C=C, gamma=blk.norm2.weight,
+                    beta=blk.norm2.bias, eps=blk.norm2.eps, res_scale=blk.res_scale, L=L)
         return z32, z16
 
 
@@ -490,9 +534,27 @@ class ConvPlan:
     def __init__(self, conv, cin_pad, fmt, ps_r=0):
         self.key = (_version_key(conv), fmt, ps_r)
         self.cout = conv.weight.shape[0]
-        self.cin_pad = cin_pad
+        self.cin_pad, self.ps_r = cin_pad, ps_r
         self.npad = round_up(self.cout, 64)
         self.w, self.b = pack_conv(conv, cin_pad, self.npad, fmt, ps_r)
+
+    def run(self, launch, name, x16, *, want16=True, want_f32=False, rows=False, **kw):
+        """One launch on x16 (B, H, W, cin_pad) channels-last -> (16-bit out, fp32 out), each None unless asked for:
+        (B, H, W, npad) and (B, H, W, cout), or (B, H*W, .) with rows; with ps_r the 16-bit output is the shuffled
+        (B, H r, W r, cout / r^2).  kw: residual, activation and the NCHW tail (conv3x3)."""
+        B, H, W, _ = x16.shape
+        r, dev = self.ps_r, x16.device
+        px = (B, H * W) if rows else (B, H, W)
+        o16 = o32 = None
+        if r:
+            o16 = torch.empty(B, H * r, W * r, self.cout // (r * r), device=dev, dtype=self.w.dtype)
+        elif want16:
+            o16 = torch.empty(*px, self.npad, device=dev, dtype=self.w.dtype)
+        if want_f32:
+            o32 = torch.empty(*px, self.cout, device=dev, dtype=torch.float32)
+        conv3x3(x16, self.w, self.b, self.cin_pad, self.npad, n_store=self.cout if r else self.npad, n_real=self.cout,
+                out_bf16=o16, out_f32=o32, ps_r=r, launch=launch, name=name, **kw)
+        return o16, o32
 
 
 def conv_plan(owner, name, conv, cin_pad, fmt, ps_r=0):
@@ -504,116 +566,96 @@ def conv_plan(owner, name, conv, cin_pad, fmt, ps_r=0):
     return plan
 
 
-def gemm_launches(model, x_shape):
-    """Descriptors of every tc.gemm / tc.conv3x3 launch of one tensor-core forward of GRL `model` on a (B, Cin, H, W)
-    input, in launch order, with the arguments GRL._forward_bf16, TransformerStage.forward_tc and BlockPlan.run pass
-    (operand format: model.precision).  With model.input_format == "rggb", x_shape is the packed (B, 4, h, w) Bayer input
-    and the network runs on the (2h, 2w) image.  Host only: shapes come from the modules, nothing is packed or launched."""
-    from torch import nn
+@torch.no_grad()
+def stage_forward(stage, x32, x16, x_size, table_index_mask, launch=DEVICE, name=""):
+    """TransformerStage on the explicit (fp32 stream (B, L, C), 16-bit operand copy or None) pair: its blocks, then
+    conv3x3 + residual; returns the pair.  GEMMs are named "{name}.block{i}.qkv", ..., "{name}.conv"."""
+    B, L, C = x32.shape
+    H, W = x_size
+    fmt = FMT[stage.blocks[0].precision]
+    cpad = round_up(C, 64)
+    r32, r16 = x32, x16
+    for bi, blk in enumerate(stage.blocks):
+        r32, r16 = block_plan(blk, FMT[blk.precision]).run(blk, r32, r16, x_size, table_index_mask, launch,
+                                                           f"{name}.block{bi}")
+    if r16 is None or r16.dtype != DTYPE[fmt]:
+        r16 = _h16(B, L, cpad, device=x32.device, fmt=fmt)
+        launch.run(pack_rows, r32.contiguous(), cpad, fmt, out=r16)
+    o16, o32 = conv_plan(stage, "conv", stage.conv, cpad, fmt).run(launch, f"{name}.conv", r16.view(B, H, W, cpad),
+                                                                   want_f32=True, rows=True, res_f32=x32.contiguous())
+    return o32, o16
 
+
+@torch.no_grad()
+def forward(model, x, rggb=False, launch=DEVICE):
+    """GRL `model` on the tensor-core kernels (grl.py:506-551); x is the RAW (B, Cin, H, W) fp32 input, or with rggb its
+    packed (B, 4, H/2, W/2) Bayer planes.  Head: one kernel does [dm_matlab +] check_image_size + (x - mean) * img_range +
+    bchw -> bhwc + operand pack; tail: the last conv's epilogue writes x / img_range + mean, cropped, as bchw planes;
+    PixelShuffle is a store-address pattern of the conv before it.  Buffers are allocated on x's device."""
+    dev = x.device
     fmt = FMT[model.precision]
-    B, Cin, H, W = x_shape
-    if getattr(model, "input_format", "rgb") == "rggb":
+    B, Cin, H, W = x.shape
+    if rggb:
         Cin, H, W = 3, 2 * H, 2 * W
-    ps = model.pad_size
-    Hp, Wp = round_up(H, ps), round_up(W, ps)
-    L = Hp * Wp
+    Hp, Wp = round_up(H, model.pad_size), round_up(W, model.pad_size)
     C = model.embed_dim
     cpad = round_up(C, 64)
     s = model.upscale
-    out = []
-
-    def h16(*shape):
-        return Spec(shape, DTYPE[fmt])
-
-    def f32(*shape):
-        return Spec(shape, torch.float32)
-
-    def conv(name, module, x16, *, n_store=None, act=K.ACT_NONE, slope=0.0, out_bf16=None, out_f32=None, res_f32=None,
-             **tail):
-        cin_pad, cout = x16.shape[-1], module.weight.shape[0]
-        npad = round_up(cout, 64)  # ConvPlan
-        b, h, w = x16.shape[:3]
-        out.append(gemm_launch(name, x16, h16(npad, 9 * cin_pad), f32(npad), image=(b, h, w), kpad=cin_pad, npad=npad,
-                               taps=9, epi=EPI_BIAS_ACT, n_store=npad if n_store is None else n_store, n_real=cout,
-                               out_bf16=out_bf16, out_f32=out_f32, res_f32=res_f32, act=act, slope=slope, **tail))
-
-    def block(name, blk):  # BlockPlan.__init__ / run
-        hw, hs = blk.attn.window_attn.num_heads, blk.attn.stripe_attn.num_heads
-        n_qkv = (3 * hw + 3 * hs) * SLOT
-        out.append(gemm_launch(f"{name}.qkv", h16(B, L, cpad), h16(n_qkv, cpad), f32(n_qkv), M=B * L, kpad=cpad,
-                               npad=n_qkv, epi=EPI_QKV, n_store=n_qkv, out_bf16=h16(B * L, n_qkv),
-                               slot_scale=f32(n_qkv // SLOT)))
-        df = blk.attn.anchor.body[0].down_factor
-        La, n_anc = (Hp // df) * (Wp // df), round_up(hs * SLOT, 32)
-        out.append(gemm_launch(f"{name}.anchor", h16(B, Hp // df, Wp // df, cpad), h16(n_anc, cpad), f32(n_anc),
-                               M=B * La, kpad=cpad, npad=n_anc, epi=EPI_QKV, n_store=n_anc, out_bf16=h16(B * La, n_anc),
-                               slot_scale=f32(hs)))
-        cab = {}
-        if blk.args.local_connection:
-            cmid_pad = round_up(blk.conv.cab[0].weight.shape[0], 64)
-            out.append(gemm_launch(f"{name}.cab1", h16(B, Hp, Wp, cpad), h16(cmid_pad, 9 * cpad), f32(cmid_pad),
-                                   image=(B, Hp, Wp), kpad=cpad, npad=cmid_pad, taps=9, epi=EPI_BIAS_ACT,
-                                   n_store=cmid_pad, out_bf16=h16(B, Hp, Wp, cmid_pad), act=K.ACT_GELU))
-            out.append(gemm_launch(f"{name}.cab2", h16(B, Hp, Wp, cmid_pad), h16(cpad, 9 * cmid_pad), f32(cpad),
-                                   image=(B, Hp, Wp), kpad=cmid_pad, npad=cpad, taps=9, epi=EPI_BIAS_ACT, n_store=cpad,
-                                   out_bf16=h16(B * L, cpad)))
-            cab = dict(cab_y=h16(B * L, cpad), cab_gate=f32(B, C))
-        n_ln = 64 if C <= 64 else 128 if C <= 128 else 192 if C <= 192 else 256
-        k_proj = round_up((hw + hs) * SLOT, 64)
-        hpad = round_up(blk.mlp.fc1.weight.shape[0], 64)
-        def ln(nm, kpad, norm, **kw):
-            out.append(gemm_launch(f"{name}.{nm}", h16(B * L, kpad), h16(n_ln, kpad), f32(n_ln), M=B * L, kpad=kpad,
-                                   npad=n_ln, epi=EPI_LN, n_store=n_ln, n_real=C, out_bf16=h16(B, L, cpad),
-                                   out_f32=f32(B, L, C), res_f32=f32(B, L, C), C=C, gamma=_spec(norm.weight),
-                                   beta=_spec(norm.bias), eps=norm.eps, res_scale=blk.res_scale, L=L, **kw))
-
-        ln("proj", k_proj, blk.norm1, **cab)
-        out.append(gemm_launch(f"{name}.fc1", h16(B, L, cpad), h16(hpad, cpad), f32(hpad), M=B * L, kpad=cpad, npad=hpad,
-                               epi=EPI_BIAS_ACT, n_store=hpad, act=K.ACT_GELU, out_bf16=h16(B * L, hpad)))
-        ln("fc2", hpad, blk.norm2)
-
-    # GRL._forward_bf16
     need_res = model.upsampler not in ("pixelshuffle", "pixelshuffledirect", "nearest+conv") and model.in_channels == model.out_channels
     mean = model._mean_list
+    x16 = _h16(B, Hp, Wp, 64, device=dev, fmt=fmt)
+    xc32 = torch.empty(B, Hp, Wp, Cin, device=dev, dtype=torch.float32) if need_res else None
+    launch.run(head_pack_rggb if rggb else head_pack, x, Hp, Wp, mean, model.img_range, 64, fmt, out=(x16, xc32))
     shift = mean if len(mean) > 1 else mean * 4
-    cf = round_up(model.conv_first.weight.shape[0], 64)
-    conv("conv_first", model.conv_first, h16(B, Hp, Wp, 64), out_bf16=h16(B, Hp, Wp, cf), out_f32=f32(B, Hp, Wp, C))
-    for si, layer in enumerate(model.layers):  # TransformerStage.forward_tc
-        for bi, blk in enumerate(layer.blocks):
-            block(f"stage{si}.block{bi}", blk)
-        conv(f"stage{si}.conv", layer.conv, h16(B, Hp, Wp, cpad), n_store=cpad, out_bf16=h16(B, L, cpad),
-             out_f32=f32(B, L, C), res_f32=f32(B, L, C))
-    body = h16(B, Hp, Wp, round_up(model.conv_after_body.weight.shape[0], 64))
-    conv("conv_after_body", model.conv_after_body, h16(B, Hp, Wp, cpad), out_bf16=body, res_f32=f32(B, Hp, Wp, C))
 
-    def final(name, module, x16, r, res=None):
-        conv(name, module, x16, out_nchw=f32(B, model.out_channels, H * s, W * s), nchw_r=r, post_scale=1.0 / model.img_range,
-             post_shift=shift, res_f32=res)
+    def conv(name, module, inp16, ps_r=0, **kw):
+        return conv_plan(model, name, module, inp16.shape[-1], fmt, ps_r).run(launch, name, inp16, **kw)
 
-    def lrelu(name, module, x16, slope):
-        o = h16(*x16.shape[:3], round_up(module.weight.shape[0], 64))
-        conv(name, module, x16, act=K.ACT_LEAKY, slope=slope, out_bf16=o)
-        return o
+    def last(name, module, inp16, r=1, res=None):  # network output: (B, C_out, H s, W s) planes straight from the epilogue
+        y = torch.empty(B, model.out_channels, H * s, W * s, device=dev, dtype=torch.float32)
+        conv(name, module, inp16, want16=False, res_f32=res, out_nchw=y, nchw_r=r, post_scale=1.0 / model.img_range,
+             post_shift=shift)
+        return y
 
+    def ln(norm, u):
+        out = torch.empty(u.shape, device=dev, dtype=torch.float32)  # not empty_like: on meta, its first call imports sympy
+        launch.run(K.ln_residual, None, u, norm.weight, norm.bias, norm.eps, out=out)
+        return out
+
+    _, f32 = conv("conv_first", model.conv_first, x16, want_f32=True)
+    t = ln(model.norm_start, f32.view(B, Hp * Wp, C))
+    tim = model.get_table_index_mask(dev, (Hp, Wp))
+    t16 = None  # 16-bit operand copy of the residual stream, carried explicitly from block to block
+    for si, layer in enumerate(model.layers):
+        t, t16 = stage_forward(layer, t, t16, (Hp, Wp), tim, launch, f"stage{si}")
+    t = ln(model.norm_end, t)
+    t16 = _h16(B, Hp, Wp, cpad, device=dev, fmt=fmt)
+    launch.run(pack_rows, t, cpad, fmt, out=t16)
+    body16, _ = conv("conv_after_body", model.conv_after_body, t16, res_f32=f32)
     if model.upsampler == "pixelshuffle":
-        u = lrelu("conv_before_upsample", model.conv_before_upsample[0], body, 0.01)
+        u16, _ = conv("conv_before_upsample", model.conv_before_upsample[0], body16, act=K.ACT_LEAKY, slope=0.01)
         mods = list(model.upsample.up)
         for i, m in enumerate(mods):
-            if isinstance(m, nn.Conv2d):
-                r, cout = mods[i + 1].upscale_factor, m.weight.shape[0]
-                o = h16(u.shape[0], u.shape[1] * r, u.shape[2] * r, cout // (r * r))
-                conv(f"upsample.up.{i}", m, u, n_store=cout, out_bf16=o, ps_r=r)
-                u = o
-        final("conv_last", model.conv_last, u, 1)
-    elif model.upsampler == "pixelshuffledirect":
-        final("upsample.up.0", model.upsample.up[0], body, model.upsample.up[1].upscale_factor)
-    elif model.upsampler == "nearest+conv":
-        u = lrelu("conv_before_upsample", model.conv_before_upsample[0], body, 0.01)
-        u = lrelu("conv_up1", model.conv_up1, h16(B, 2 * u.shape[1], 2 * u.shape[2], u.shape[3]), 0.2)
-        u = lrelu("conv_up2", model.conv_up2, h16(B, 2 * u.shape[1], 2 * u.shape[2], u.shape[3]), 0.2)
-        u = lrelu("conv_hr", model.conv_hr, u, 0.2)
-        final("conv_last", model.conv_last, u, 1)
-    else:
-        final("conv_last", model.conv_last, body, 1, f32(B, Hp, Wp, Cin) if need_res else None)
-    return out
+            if isinstance(m, nn.Conv2d):  # always followed by its PixelShuffle (upsample.py:6-30)
+                u16, _ = conv(f"upsample.up.{i}", m, u16, ps_r=mods[i + 1].upscale_factor)
+        return last("conv_last", model.conv_last, u16)
+    if model.upsampler == "pixelshuffledirect":
+        return last("upsample.up.0", model.upsample.up[0], body16, model.upsample.up[1].upscale_factor)
+    if model.upsampler == "nearest+conv":
+        u16, _ = conv("conv_before_upsample", model.conv_before_upsample[0], body16, act=K.ACT_LEAKY, slope=0.01)
+        up = lambda v: v.repeat_interleave(2, dim=1).repeat_interleave(2, dim=2).contiguous()
+        u16, _ = conv("conv_up1", model.conv_up1, up(u16), act=K.ACT_LEAKY, slope=0.2)
+        u16, _ = conv("conv_up2", model.conv_up2, up(u16), act=K.ACT_LEAKY, slope=0.2)
+        u16, _ = conv("conv_hr", model.conv_hr, u16, act=K.ACT_LEAKY, slope=0.2)
+        return last("conv_last", model.conv_last, u16)
+    return last("conv_last", model.conv_last, body16, res=xc32)
+
+
+def gemm_launches(model, x_shape):
+    """Descriptors of every GEMM launch of one tensor-core forward of GRL `model` on a (B, Cin, H, W) input, in launch
+    order (operand format: model.precision): `forward` run with the Listing launcher on a meta input.  With
+    model.input_format == "rggb", x_shape is the packed (B, 4, h, w) Bayer input and the network runs on the (2h, 2w)
+    image.  Needs no device: weights are packed on the model's device and nothing is launched."""
+    listing = Listing()
+    forward(model, torch.empty(x_shape, device="meta"), model.input_format == "rggb", listing)
+    return listing.launches

@@ -27,6 +27,7 @@ Gates (measured on an H100 80GB HBM3 at a 400 W power limit, set to 2 x the wors
 Mutation controls are derived from the reference (a kernel bug's effect, never an edited kernel) and must fail the
 gate on every case where they apply.
 """
+import copy
 import math
 from functools import lru_cache
 from typing import NamedTuple
@@ -504,3 +505,27 @@ def test_recorded_launches_match_descriptors(pkg, tc, device, monkeypatch, varia
     for got, ln in zip(recorded, want):
         diff = {k: (got[k], v) for k, v in ln.args.items() if got[k] != v}
         assert not diff, f"{ln.name}: {diff}"
+
+
+@pytest.mark.gpu
+def test_listing_first_leaves_the_forward_unchanged(pkg, tc, device):
+    """gemm_launches on a fresh model, then its forward at the model's own resolution (where both read the registered
+    coordinate tables): bitwise the forward of an identical model that was never listed.  A listing run packs weights
+    on the device, but its attention constants are meta tensors and must not be kept for the forward."""
+    cfg = pkg.configs.grl_config("tiny", "sr", 2)
+    cfg = dict(cfg, img_size=math.lcm(cfg["window_size"], *cfg["stripe_size"]))
+    torch.manual_seed(0)
+    listed = pkg.GRL(**cfg)
+    fresh = copy.deepcopy(listed)
+    S = listed.pad_size
+    x = torch.rand(1, 3, S, S, generator=torch.Generator().manual_seed(0)).to(device)
+    ys = []
+    for model, list_first in ((fresh, False), (listed, True)):
+        model.use_cuda_graph = False
+        model = model.to(device).eval()
+        model.set_precision("fp16")
+        if list_first:
+            assert len(tc.gemm_launches(model, tuple(x.shape))) > 0
+        ys.append(model(x))
+    torch.cuda.synchronize()
+    assert torch.equal(ys[0], ys[1])

@@ -403,7 +403,7 @@ TAILS = [(r, oc, False) for r in (1, 2, 3, 4) for oc in (1, 3)] + [(1, 1, True),
 def test_nchw_tail_store(tc, device, r, oc, with_res, fmt):
     """The network's last conv writes (B, oc, Hc, Wc) fp32 planes from its epilogue: PixelShuffle(r) when r > 1, the crop
     to Hc x Wc, x * post_scale + post_shift[c] as one fmaf, and with the input residual (the no-upsampler tail,
-    modules.py _forward_bf16) the fp32 residual added before it.  Reference: the same conv with a plain fp32 store,
+    tc.forward) the fp32 residual added before it.  Reference: the same conv with a plain fp32 store,
     rearranged and cropped in torch, then scale and shift in float64 rounded to fp32 -- within 1 fp32 ulp (the fmaf's
     single rounding).  The output is a view into a NaN-filled buffer with a guard region after it: no in-crop value may
     stay NaN, and no tile past the crop may write outside it."""
