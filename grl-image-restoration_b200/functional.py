@@ -65,12 +65,12 @@ def pack_conv_weight(weight):
     return weight.detach().permute(0, 2, 3, 1).reshape(co, 9 * ci).contiguous()
 
 
-def conv3x3(x, wpacked, bias=None, act=ACT_NONE, slope=0.0, res=None):
+def conv3x3(x, wpacked, bias=None, act=ACT_NONE, slope=0.0, res=None, out=None):
     """x (B, H, W, Cin) channels-last -> (B, H, W, Cout); stride 1, zero pad 1."""
     x = _f32c(x, "x")
     B, H, W, Cin = x.shape
     Cout = wpacked.shape[0]
-    y = torch.empty(B, H, W, Cout, device=x.device, dtype=torch.float32)
+    y = out if out is not None else torch.empty(B, H, W, Cout, device=x.device, dtype=torch.float32)
     if res is not None:
         res = _f32c(res, "res")
     capi.check(capi.lib().grl_conv3x3_f32(capi.ptr(x), capi.ptr(wpacked), capi.ptr(bias), capi.ptr(res), capi.ptr(y),
@@ -78,10 +78,10 @@ def conv3x3(x, wpacked, bias=None, act=ACT_NONE, slope=0.0, res=None):
     return y
 
 
-def avgpool(x, df):
+def avgpool(x, df, out=None):
     x = _f32c(x, "x")
     B, H, W, C = x.shape
-    y = torch.empty(B, H // df, W // df, C, device=x.device, dtype=torch.float32)
+    y = out if out is not None else torch.empty(B, H // df, W // df, C, device=x.device, dtype=torch.float32)
     capi.check(capi.lib().grl_avgpool_f32(capi.ptr(x), capi.ptr(y), B, H, W, C, df, capi.stream()))
     return y
 
@@ -98,24 +98,24 @@ def ln_residual(x, u, gamma, beta, eps=1e-5, res_scale=1.0, cab_y=None, cab_gate
     return out
 
 
-def channel_gate(y, w1, b1, w2, b2):
+def channel_gate(y, w1, b1, w2, b2, out=None):
     """y (B, L, C) -> gate (B, C) = sigmoid(W2 relu(W1 mean_L(y) + b1) + b2)."""
     y = _f32c(y, "y")
     B, L, C = y.shape
     R = w1.shape[0]
     nbytes = capi.lib().grl_channel_gate_workspace(B, L, C)
     ws = torch.empty(max(nbytes, 4) // 4, device=y.device, dtype=torch.float32)
-    gate = torch.empty(B, C, device=y.device, dtype=torch.float32)
+    gate = out if out is not None else torch.empty(B, C, device=y.device, dtype=torch.float32)
     capi.check(capi.lib().grl_channel_gate_f32(capi.ptr(y), B, L, C, capi.ptr(w1), capi.ptr(b1), capi.ptr(w2),
                                                capi.ptr(b2), R, capi.ptr(gate), capi.ptr(ws), nbytes, capi.stream()))
     return gate
 
 
-def bias_table(table, w1, b1, w2):
+def bias_table(table, w1, b1, w2, out=None):
     """table (..., 2) -> activated bias (heads, rows) = 16*sigmoid(cpb_mlp(table))."""
     t = _f32c(table, "table").reshape(-1, 2)
     heads, hidden = w2.shape
-    out = torch.empty(heads, t.shape[0], device=t.device, dtype=torch.float32)
+    out = out if out is not None else torch.empty(heads, t.shape[0], device=t.device, dtype=torch.float32)
     capi.check(capi.lib().grl_bias_table_f32(capi.ptr(t), t.shape[0], capi.ptr(_f32c(w1, "w1")), capi.ptr(b1),
                                              capi.ptr(_f32c(w2, "w2")), hidden, heads, capi.ptr(out), capi.stream()))
     return out
@@ -198,13 +198,13 @@ def _cfa4(x):
     return x
 
 
-def demosaic(x):
+def demosaic(x, out=None):
     """The reference's dm_matlab (utils/utils_mosaic.py:36-111), the dm task's input transform (engines/base.py:127-128):
     packed RGGB planes x (B, 4, h, w) float32 on the GPU (R, G of the even rows, G of the odd rows, B) -> RGB
     (B, 3, 2h, 2w) float32.  One sm_90a kernel; GRL(input_format="rggb") fuses the same arithmetic into its head."""
     x = _cfa4(x)
     B, _, h, w = x.shape
-    y = torch.empty(B, 3, 2 * h, 2 * w, device=x.device, dtype=torch.float32)
+    y = out if out is not None else torch.empty(B, 3, 2 * h, 2 * w, device=x.device, dtype=torch.float32)
     capi.check(capi.lib().grl_demosaic_f32(capi.ptr(x), B, h, w, capi.ptr(y), capi.stream()))
     return y
 

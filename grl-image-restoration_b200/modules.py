@@ -11,9 +11,11 @@ tools/trainer.py:93-115).  Differences, all deliberate:
 Reference files: models/networks/grl.py, models/common/mixed_attn_block_efficient.py,
 models/common/mixed_attn_block.py, models/common/swin_v1_block.py, models/common/upsample.py.
 """
+import inspect
 import math
 import os
 from types import SimpleNamespace
+from typing import NamedTuple
 
 import torch
 import torch.nn as nn
@@ -32,23 +34,36 @@ def _closed_form_marker(device=None):
     return torch.empty(0, device=device)
 
 
-class _PackedConv:
-    """Caches the (Cout, 9*Cin) im2col-ordered copy of an nn.Conv2d weight (re-packed when the weight changes)."""
-
-    def __init__(self):
-        self._key, self._w = None, None
-
-    def get(self, conv):
-        w = conv.weight
-        key = (w.data_ptr(), w._version, w.device)
-        if key != self._key:
-            self._w, self._key = K.pack_conv_weight(w), key
-        return self._w
+# The fp32 forward is written once, in the module forwards below, and issues every kernel through a launcher (tc.Device
+# runs them, tc.Listing records the GEMMs and attention calls without a device: f32_launches).  Callers allocate every
+# output, so a listing run on a meta input allocates meta tensors and launches nothing.  Modules that issue one listed
+# launch take its full name ("stage0.block1.qkv"); the others take the prefix of their launches' names.
+def linear(launch, name, x, lin, act=K.ACT_NONE):
+    """nn.Linear `lin` on x (..., K) -> (..., N), launched as `name`."""
+    y = torch.empty(*x.shape[:-1], lin.weight.shape[0], device=x.device, dtype=torch.float32)
+    launch.listed(name, K.linear, x, lin.weight, lin.bias, act, out=y)
+    return y
 
 
-def conv2d_cl(conv, cache, x, act=K.ACT_NONE, slope=0.0, res=None):
-    """nn.Conv2d(3x3, stride 1, pad 1) applied to channels-last x (B, H, W, Cin)."""
-    return K.conv3x3(x, cache.get(conv), conv.bias, act, slope, res)
+def conv3x3(launch, name, owner, key, x, act=K.ACT_NONE, slope=0.0, res=None):
+    """nn.Conv2d(3x3, stride 1, pad 1) `owner.<key>` on channels-last x (B, H, W, Cin), launched as `name`.  Its
+    (Cout, 9*Cin) im2col-ordered weight is cached on the owner under `key` and re-packed when the weight changes."""
+    conv = owner.get_submodule(key)
+    w = conv.weight
+    version = (w.data_ptr(), w._version, w.device)
+    cache = owner.__dict__.setdefault("_f32_convs", {})
+    if cache.get(key, (None,))[0] != version:
+        cache[key] = (version, K.pack_conv_weight(w))
+    y = torch.empty(*x.shape[:-1], w.shape[0], device=x.device, dtype=torch.float32)
+    launch.listed(name, K.conv3x3, x, cache[key][1], conv.bias, act, slope, res, out=y)
+    return y
+
+
+def ln_residual(launch, norm, u, x=None, res_scale=1.0, cab_y=None, cab_gate=None):
+    """(x or 0) + res_scale * norm(u) (+ cab_y * cab_gate[b]) for u (B, L, C)."""
+    out = torch.empty(u.shape, device=u.device, dtype=torch.float32)
+    launch.run(K.ln_residual, x, u, norm.weight, norm.bias, norm.eps, res_scale, cab_y, cab_gate, out=out)
+    return out
 
 
 def pixel_shuffle_cl(x, r):
@@ -77,9 +92,13 @@ class AffineTransform(nn.Module):
         self.logit_scale = nn.Parameter(torch.log(10 * torch.ones((num_heads, 1, 1))), requires_grad=True)
         self.cpb_mlp = CPB_MLP(2, num_heads)
 
-    def bias_table(self, relative_coords_table):
+    def bias_table(self, relative_coords_table, launch=tc.DEVICE):
         """(heads, rows) = 16*sigmoid(cpb_mlp(table)) -- what the fused attention kernels consume."""
-        return K.bias_table(relative_coords_table, self.cpb_mlp[0].weight, self.cpb_mlp[0].bias, self.cpb_mlp[2].weight)
+        out = torch.empty(self.cpb_mlp[2].weight.shape[0], relative_coords_table.numel() // 2,
+                          device=relative_coords_table.device, dtype=torch.float32)
+        launch.run(K.bias_table, relative_coords_table, self.cpb_mlp[0].weight, self.cpb_mlp[0].bias,
+                   self.cpb_mlp[2].weight, out=out)
+        return out
 
     @torch.no_grad()
     def forward(self, attn, relative_coords_table, relative_position_index, mask):
@@ -106,14 +125,16 @@ class WindowAttention(nn.Module):
         self.softmax = nn.Softmax(dim=-1)
 
     @torch.no_grad()
-    def forward(self, qkv, x_size, table, index, mask, out=None):
+    def forward(self, qkv, x_size, table, index, mask, out=None, launch=tc.DEVICE, name="window_attn"):
         """qkv (B, L, 3c) -> (B, L, c).  `index` is unused (closed form); `mask is not None` enables the shift mask."""
         B, L, C = qkv.shape
         s = self.shift_size
         grid = G.token_grid(x_size, self.window_size, (s, s))
-        bias = self.attn_transform.bias_table(table)
-        return K.window_attention(qkv, B, grid, self.num_heads, self.attn_transform.logit_scale, bias,
-                                  mask is not None, out)
+        bias = self.attn_transform.bias_table(table, launch)
+        out = torch.empty(B, L, C // 3, device=qkv.device, dtype=torch.float32) if out is None else out
+        launch.listed(name, K.window_attention, qkv, B, grid, self.num_heads, self.attn_transform.logit_scale, bias,
+                      mask is not None, out)
+        return out
 
     def extra_repr(self):
         return (f"window_size={self.window_size}, shift_size={self.shift_size}, "
@@ -149,13 +170,17 @@ class AnchorStripeAttention(nn.Module):
         return G.token_grid(x_size, ss, sh), G.anchor_grid(x_size, ss, sh, df)
 
     @torch.no_grad()
-    def forward(self, qkv, anchor, x_size, table, index_a2w, index_w2a, mask_a2w, mask_w2a, out=None):
+    def forward(self, qkv, anchor, x_size, table, index_a2w, index_w2a, mask_a2w, mask_w2a, out=None, launch=tc.DEVICE,
+                name="stripe_attn"):
         B, L, C = qkv.shape
         tok, anc = self.grids(x_size)
-        b1 = self.attn_transform1.bias_table(table)
-        b2 = self.attn_transform2.bias_table(table)
-        return K.stripe_attention(qkv, anchor, B, tok, anc, self.num_heads, self.attn_transform1.logit_scale, b1,
-                                  self.attn_transform2.logit_scale, b2, mask_a2w is not None, out)
+        b1 = self.attn_transform1.bias_table(table, launch)
+        b2 = self.attn_transform2.bias_table(table, launch)
+        out = torch.empty(B, L, C // 3, device=qkv.device, dtype=torch.float32) if out is None else out
+        launch.listed(name, K.stripe_attention, qkv, anchor, B, tok, anc, self.num_heads,
+                      self.attn_transform1.logit_scale, b1, self.attn_transform2.logit_scale, b2, mask_a2w is not None,
+                      out)
+        return out
 
     def extra_repr(self):
         return (f"stripe_size={self.stripe_size}, stripe_groups={self.stripe_groups}, stripe_shift={self.stripe_shift}, "
@@ -174,8 +199,8 @@ class QKVProjection(nn.Module):
         self.body = nn.Linear(dim, dim * 3, bias=qkv_bias)
 
     @torch.no_grad()
-    def forward(self, x, x_size):
-        return K.linear(x, self.body.weight, self.body.bias)
+    def forward(self, x, x_size, launch=tc.DEVICE, name="qkv"):
+        return linear(launch, name, x, self.body)
 
 
 class AnchorLinear(nn.Module):
@@ -190,10 +215,12 @@ class AnchorLinear(nn.Module):
         self.reduction = nn.Linear(in_channels, out_channels, bias=bias)
 
     @torch.no_grad()
-    def forward(self, x, x_size):
+    def forward(self, x, x_size, launch=tc.DEVICE, name="anchor"):
         B, L, C = x.shape
-        pooled = K.avgpool(x.view(B, x_size[0], x_size[1], C), self.down_factor)
-        return K.linear(pooled, self.reduction.weight, self.reduction.bias)
+        df = self.down_factor
+        pooled = torch.empty(B, x_size[0] // df, x_size[1] // df, C, device=x.device, dtype=torch.float32)
+        launch.run(K.avgpool, x.view(B, x_size[0], x_size[1], C), df, out=pooled)
+        return linear(launch, name, pooled, self.reduction)
 
 
 class AnchorProjection(nn.Module):
@@ -206,9 +233,9 @@ class AnchorProjection(nn.Module):
         self.proj_type = proj_type
         self.body = nn.ModuleList([AnchorLinear(dim, dim // 2, anchor_window_down_factor, proj_type, True)])
 
-    def forward(self, x, x_size):
+    def forward(self, x, x_size, launch=tc.DEVICE, name="anchor"):
         for m in self.body:
-            x = m(x, x_size)
+            x = m(x, x_size, launch, name)
         return x
 
 
@@ -234,17 +261,18 @@ class MixedAttention(nn.Module):
         self.proj_drop = nn.Dropout(proj_drop)
 
     @torch.no_grad()
-    def forward(self, x, x_size, table_index_mask):
+    def forward(self, x, x_size, table_index_mask, launch=tc.DEVICE, name=""):
         B, L, C = x.shape
-        qkv = self.qkv(x, x_size)
+        qkv = self.qkv(x, x_size, launch, f"{name}.qkv")
         qkv_window, qkv_stripe = torch.split(qkv, C * 3 // 2, dim=-1)
-        anchor = self.anchor(x, x_size)
+        anchor = self.anchor(x, x_size, launch, f"{name}.anchor")
         merged = torch.empty(B, L, C, device=x.device, dtype=torch.float32)  # cat([window, stripe]) without the copy
         t = table_index_mask
-        self.window_attn(qkv_window, x_size, t["table_w"], t["index_w"], t["mask_w"], out=merged[..., : C // 2])
+        self.window_attn(qkv_window, x_size, t["table_w"], t["index_w"], t["mask_w"], merged[..., : C // 2], launch,
+                         f"{name}.window_attn")
         self.stripe_attn(qkv_stripe, anchor, x_size, t["table_s"], t["index_a2w"], t["index_w2a"], t["mask_a2w"],
-                         t["mask_w2a"], out=merged[..., C // 2:])
-        return K.linear(merged, self.proj.weight, self.proj.bias)
+                         t["mask_w2a"], merged[..., C // 2:], launch, f"{name}.stripe_attn")
+        return linear(launch, f"{name}.proj", merged, self.proj)
 
     def extra_repr(self):
         return f"dim={self.dim}, input_resolution={self.input_resolution}"
@@ -263,11 +291,13 @@ class ChannelAttention(nn.Module):
                                        nn.Sigmoid())
 
     @torch.no_grad()
-    def gate(self, y):
+    def gate(self, y, launch=tc.DEVICE):
         """y (B, L, C) channels-last -> (B, C) sigmoid gate."""
         a1, a3 = self.attention[1], self.attention[3]
-        return K.channel_gate(y, a1.weight.view(a1.weight.shape[0], -1), a1.bias,
-                              a3.weight.view(a3.weight.shape[0], -1), a3.bias)
+        gate = torch.empty(y.shape[0], y.shape[2], device=y.device, dtype=torch.float32)
+        launch.run(K.channel_gate, y, a1.weight.view(a1.weight.shape[0], -1), a1.bias,
+                   a3.weight.view(a3.weight.shape[0], -1), a3.bias, out=gate)
+        return gate
 
     @torch.no_grad()
     def forward(self, x):
@@ -285,15 +315,14 @@ class CAB(nn.Module):
         self.cab = nn.Sequential(nn.Conv2d(num_feat, num_feat // compress_ratio, 3, 1, 1), nn.GELU(),
                                  nn.Conv2d(num_feat // compress_ratio, num_feat, 3, 1, 1),
                                  ChannelAttention(num_feat, reduction))
-        self._p0, self._p2 = _PackedConv(), _PackedConv()
 
     @torch.no_grad()
-    def features_and_gate(self, x, x_size):
+    def features_and_gate(self, x, x_size, launch=tc.DEVICE, name=""):
         """Returns (y, gate): y (B, L, C) = conv2(gelu(conv1(x))), gate (B, C); CAB(x) = y * gate."""
         B, L, C = x.shape
-        t = conv2d_cl(self.cab[0], self._p0, x.view(B, x_size[0], x_size[1], C), K.ACT_GELU)
-        y = conv2d_cl(self.cab[2], self._p2, t).view(B, L, C)
-        return y, self.cab[3].gate(y)
+        t = conv3x3(launch, f"{name}.cab1", self, "cab.0", x.view(B, x_size[0], x_size[1], C), K.ACT_GELU)
+        y = conv3x3(launch, f"{name}.cab2", self, "cab.2", t).view(B, L, C)
+        return y, self.cab[3].gate(y, launch)
 
     @torch.no_grad()
     def forward(self, x, x_size):
@@ -318,8 +347,8 @@ class Mlp(nn.Module):
         self.drop2 = nn.Dropout(drop_probs[1])
 
     @torch.no_grad()
-    def forward(self, x):
-        return K.linear(K.linear(x, self.fc1.weight, self.fc1.bias, K.ACT_GELU), self.fc2.weight, self.fc2.bias)
+    def forward(self, x, launch=tc.DEVICE, name=""):
+        return linear(launch, f"{name}.fc2", linear(launch, f"{name}.fc1", x, self.fc1, K.ACT_GELU), self.fc2)
 
 
 class EfficientMixAttnTransformerBlock(nn.Module):
@@ -386,17 +415,16 @@ class EfficientMixAttnTransformerBlock(nn.Module):
         return tc.block_plan(self, tc.FMT[self.precision]).run(self, x32, x16, x_size, all_table_index_mask)
 
     @torch.no_grad()
-    def forward(self, x, x_size, all_table_index_mask):
+    def forward(self, x, x_size, all_table_index_mask, launch=tc.DEVICE, name=""):
         if self.precision != "fp32":
             return self.forward_tc(x, None, x_size, all_table_index_mask)[0]
         t = self._get_table_index_mask(all_table_index_mask)
-        u = self.attn(x, x_size, t)
+        u = self.attn(x, x_size, t, launch, name)
+        y = gate = None
         if self.args.local_connection:
-            y, gate = self.conv.features_and_gate(x, x_size)
-            x = K.ln_residual(x, u, self.norm1.weight, self.norm1.bias, self.norm1.eps, self.res_scale, y, gate)
-        else:
-            x = K.ln_residual(x, u, self.norm1.weight, self.norm1.bias, self.norm1.eps, self.res_scale)
-        return K.ln_residual(x, self.mlp(x), self.norm2.weight, self.norm2.bias, self.norm2.eps, self.res_scale)
+            y, gate = self.conv.features_and_gate(x, x_size, launch, name)
+        x = ln_residual(launch, self.norm1, u, x, self.res_scale, y, gate)
+        return ln_residual(launch, self.norm2, self.mlp(x, launch, name), x, self.res_scale)
 
     def extra_repr(self):
         return (f"dim={self.dim}, input_resolution={self.input_resolution}, num_heads=({self.num_heads_w}, "
@@ -426,12 +454,15 @@ class Upsample(nn.Module):
         else:
             raise ValueError(f"scale {scale} is not supported. Supported scales: 2^n and 3.")
         self.up = nn.Sequential(*m)
-        self._packs = [_PackedConv() for _ in m]
 
     @torch.no_grad()
-    def forward_cl(self, x):
+    def forward_cl(self, x, launch=tc.DEVICE, name="upsample"):
+        """Channels-last (B, H, W, C) in and out."""
         for i, m in enumerate(self.up):
-            x = conv2d_cl(m, self._packs[i], x) if isinstance(m, nn.Conv2d) else pixel_shuffle_cl(x, m.upscale_factor)
+            if isinstance(m, nn.Conv2d):
+                x = conv3x3(launch, f"{name}.up.{i}", self, f"up.{i}", x)
+            else:
+                x = pixel_shuffle_cl(x, m.upscale_factor)
         return x
 
     def forward(self, x):
@@ -445,11 +476,11 @@ class UpsampleOneStep(nn.Module):
         super().__init__()
         self.num_feat = num_feat
         self.up = nn.Sequential(nn.Conv2d(num_feat, (scale ** 2) * num_out_ch, 3, 1, 1), nn.PixelShuffle(scale))
-        self._pack = _PackedConv()
 
     @torch.no_grad()
-    def forward_cl(self, x):
-        return pixel_shuffle_cl(conv2d_cl(self.up[0], self._pack, x), self.up[1].upscale_factor)
+    def forward_cl(self, x, launch=tc.DEVICE, name="upsample"):
+        """Channels-last (B, H, W, C) in and out."""
+        return pixel_shuffle_cl(conv3x3(launch, f"{name}.up.0", self, "up.0", x), self.up[1].upscale_factor)
 
     def forward(self, x):
         return self.forward_cl(x.permute(0, 2, 3, 1).contiguous()).permute(0, 3, 1, 2)
@@ -484,7 +515,6 @@ class TransformerStage(nn.Module):
                 pretrained_stripe_size=pretrained_stripe_size, res_scale=0.1 if init_method == "r" else 1.0, args=args))
             # fairscale_checkpoint / offload_to_cpu: activation checkpointing is a no-op for inference (grl.py:133)
         self.conv = build_last_conv(conv_type, dim)
-        self._pack = _PackedConv()
 
     def _init_weights(self):
         """grl.py:138-162."""
@@ -512,15 +542,15 @@ class TransformerStage(nn.Module):
         return tc.stage_forward(self, x32, x16, x_size, table_index_mask)
 
     @torch.no_grad()
-    def forward(self, x, x_size, table_index_mask):
+    def forward(self, x, x_size, table_index_mask, launch=tc.DEVICE, name=""):
         if len(self.blocks) and self.blocks[0].precision != "fp32":
             return self.forward_tc(x, None, x_size, table_index_mask)[0]
         res = x
-        for blk in self.blocks:
-            res = blk(res, x_size, table_index_mask)
+        for bi, blk in enumerate(self.blocks):
+            res = blk(res, x_size, table_index_mask, launch, f"{name}.block{bi}")
         B, L, C = x.shape
         H, W = x_size
-        return conv2d_cl(self.conv, self._pack, res.view(B, H, W, C), res=x.view(B, H, W, C)).view(B, L, C)
+        return conv3x3(launch, f"{name}.conv", self, "conv", res.view(B, H, W, C), res=x.view(B, H, W, C)).view(B, L, C)
 
 
 class GRL(nn.Module):
@@ -625,7 +655,6 @@ class GRL(nn.Module):
             self.lrelu = nn.LeakyReLU(negative_slope=0.2, inplace=True)
         else:
             self.conv_last = nn.Conv2d(embed_dim, out_channels, 3, 1, 1)
-        self._packs = {}
         self._mean_list = [float(v) for v in self.mean.flatten().tolist()]  # host copy (no device sync in forward)
         self._graphs = {}
         # opt-in CUDA-graph replay of the tensor-core forward (one captured graph per input shape): a forward is ~540
@@ -742,23 +771,6 @@ class GRL(nn.Module):
             x = F.pad(x, (0, mod_pad_w, 0, mod_pad_h), "constant")
         return x
 
-    def _conv(self, name, conv, x, act=K.ACT_NONE, slope=0.0, res=None):
-        pack = self._packs.setdefault(name, _PackedConv())
-        return conv2d_cl(conv, pack, x, act, slope, res)
-
-    @torch.no_grad()
-    def _features_cl(self, x):
-        """x (B, H, W, C) channels-last -> same; grl.py:491-504 without the layout round trips."""
-        B, H, W, C = x.shape
-        x_size = (H, W)
-        t = x.view(B, H * W, C)
-        t = K.ln_residual(None, t, self.norm_start.weight, self.norm_start.bias, self.norm_start.eps)
-        tim = self.get_table_index_mask(x.device, x_size)
-        for layer in self.layers:
-            t = layer(t, x_size, tim)
-        t = K.ln_residual(None, t, self.norm_end.weight, self.norm_end.bias, self.norm_end.eps)
-        return t.view(B, H, W, C)
-
     # ---- CUDA graphs ----------------------------------------------------------------------------
     def reset_cuda_graphs(self):
         """Drops every captured graph (they bake in the addresses of the packed weights and of their static buffers)."""
@@ -797,10 +809,16 @@ class GRL(nn.Module):
         graph.replay()
         return static_out.clone()
 
-    def forward_features(self, x):
-        """(B, C, H, W) -> (B, C, H, W) like the reference."""
-        K.capi.require_device(x)
-        return self._features_cl(x.permute(0, 2, 3, 1).contiguous()).permute(0, 3, 1, 2)
+    @torch.no_grad()
+    def forward_features(self, x, launch=tc.DEVICE):
+        """(B, C, H, W) -> (B, C, H, W) like the reference (grl.py:491-504).  Channels-last in between: a permuted
+        channels-last input is read and the result returned as such a view, without layout copies."""
+        B, C, H, W = x.shape
+        t = ln_residual(launch, self.norm_start, x.permute(0, 2, 3, 1).contiguous().view(B, H * W, C))
+        tim = self.get_table_index_mask(x.device, (H, W))
+        for si, layer in enumerate(self.layers):
+            t = layer(t, (H, W), tim, launch, f"stage{si}")
+        return ln_residual(launch, self.norm_end, t).view(B, H, W, C).permute(0, 3, 1, 2)
 
     @torch.no_grad()
     def forward(self, x):
@@ -813,7 +831,7 @@ class GRL(nn.Module):
             raise ValueError(f"input_format='rggb' takes packed RGGB Bayer planes (B, 4, h, w) with h, w >= 2 and a "
                              f"3-channel network; got input {tuple(x.shape)}, in_channels={self.in_channels}")
         cfa = x.float().contiguous()
-        if self.precision == "fp32" or self.self_ensemble:
+        if self.self_ensemble:
             # demosaic once, then the RGB forward (the engine's order: the ensemble's views are views of the RGB image)
             return self.forward_rgb(K.demosaic(cfa)).to(x.dtype)
         return self._forward_once(cfa, rggb=True).to(x.dtype)
@@ -850,37 +868,48 @@ class GRL(nn.Module):
 
     @torch.no_grad()
     def _forward_once(self, x, rggb=False):
-        """One forward on the tensor-core or fp32 kernels; rggb (tensor-core path only): x is packed Bayer planes and the
-        demosaic runs inside the head kernel."""
+        """One forward on the tensor-core or fp32 kernels; rggb: x is packed Bayer planes (the tensor-core path demosaics
+        inside its head kernel)."""
+        if self.precision == "fp32":
+            return self._forward_f32(x, rggb)
+        xin = x.float().contiguous()
+        y = self._forward_graphed(xin, rggb) if self.use_cuda_graph else tc.forward(self, xin, rggb)
+        return y.to(x.dtype)
+
+    @torch.no_grad()
+    def _forward_f32(self, x, rggb=False, launch=tc.DEVICE):
+        """The fp32 forward (grl.py:506-551), channels-last between the head and the tail, every kernel issued through
+        `launch`; rggb: x is packed (B, 4, h, w) Bayer planes, demosaiced first."""
+        if rggb:
+            rgb = torch.empty(x.shape[0], 3, 2 * x.shape[2], 2 * x.shape[3], device=x.device, dtype=torch.float32)
+            launch.run(K.demosaic, x, out=rgb)
+            x = rgb
         H, W = x.shape[2:]
-        if self.precision != "fp32":
-            xin = x.float().contiguous()
-            y = self._forward_graphed(xin, rggb) if self.use_cuda_graph else tc.forward(self, xin, rggb)
-            return y.to(x.dtype)
-        assert not rggb, "the fp32 path demosaics in forward"
         x = self.check_image_size(x)
-        self.mean = self.mean.type_as(x)
-        x = ((x - self.mean) * self.img_range).float()
-        xc = x.permute(0, 2, 3, 1).contiguous()  # channels-last from here on
-        first = self._conv("conv_first", self.conv_first, xc)
-        body = self._conv("conv_after_body", self.conv_after_body, self._features_cl(first), res=first)
+        mean = self.mean.to(x)
+        x = ((x - mean) * self.img_range).float()
+        xc = x.permute(0, 2, 3, 1).contiguous()
+
+        def conv(name, inp, act=K.ACT_NONE, slope=0.0, res=None, key=None):
+            return conv3x3(launch, name, self, key or name, inp, act, slope, res)
+
+        first = conv("conv_first", xc)
+        body = conv("conv_after_body", self.forward_features(first.permute(0, 3, 1, 2), launch).permute(0, 2, 3, 1),
+                    res=first)
         if self.upsampler == "pixelshuffle":
-            t = self._conv("conv_before_upsample", self.conv_before_upsample[0], body, K.ACT_LEAKY, 0.01)
-            y = self._conv("conv_last", self.conv_last, self.upsample.forward_cl(t))
+            t = conv("conv_before_upsample", body, K.ACT_LEAKY, 0.01, key="conv_before_upsample.0")
+            y = conv("conv_last", self.upsample.forward_cl(t, launch))
         elif self.upsampler == "pixelshuffledirect":
-            y = self.upsample.forward_cl(body)
+            y = self.upsample.forward_cl(body, launch)
         elif self.upsampler == "nearest+conv":
-            t = self._conv("conv_before_upsample", self.conv_before_upsample[0], body, K.ACT_LEAKY, 0.01)
+            t = conv("conv_before_upsample", body, K.ACT_LEAKY, 0.01, key="conv_before_upsample.0")
             up = lambda v: v.repeat_interleave(2, dim=1).repeat_interleave(2, dim=2)
-            t = self._conv("conv_up1", self.conv_up1, up(t), K.ACT_LEAKY, 0.2)
-            t = self._conv("conv_up2", self.conv_up2, up(t), K.ACT_LEAKY, 0.2)
-            y = self._conv("conv_last", self.conv_last, self._conv("conv_hr", self.conv_hr, t, K.ACT_LEAKY, 0.2))
+            t = conv("conv_up1", up(t), K.ACT_LEAKY, 0.2)
+            t = conv("conv_up2", up(t), K.ACT_LEAKY, 0.2)
+            y = conv("conv_last", conv("conv_hr", t, K.ACT_LEAKY, 0.2))
         else:
-            if self.in_channels == self.out_channels:
-                y = self._conv("conv_last", self.conv_last, body, res=xc)
-            else:
-                y = self._conv("conv_last", self.conv_last, body)
-        y = y.permute(0, 3, 1, 2) / self.img_range + self.mean
+            y = conv("conv_last", body, res=xc if self.in_channels == self.out_channels else None)
+        y = y.permute(0, 3, 1, 2) / self.img_range + mean
         return y[:, :, : H * self.upscale, : W * self.upscale].contiguous()
 
     def flops(self):
@@ -895,3 +924,57 @@ class GRL(nn.Module):
                 state_dict.pop(k)
                 print(k)
         return state_dict
+
+
+# ----------------------------------------------------------------------------------------------
+# launch listing
+# ----------------------------------------------------------------------------------------------
+class GemmF32(NamedTuple):
+    """One K.linear / K.conv3x3 launch of an fp32 forward (K = 9 Cin for a conv)."""
+    name: str
+    conv: bool
+    K: int
+    N: int
+    act: int
+    slope: float
+    bias: bool
+    res: bool
+
+
+class AttnF32(NamedTuple):
+    """One attention pass of an fp32 forward: a K.window_attention launch ("window"), or pass 1 ("stripe1": anchors
+    attend to the stripe's tokens) / pass 2 ("stripe2": tokens attend to the anchors) of a K.stripe_attention launch."""
+    name: str
+    role: str
+    gq: object
+    gk: object
+    heads: int
+    d: int
+    use_mask: bool
+
+
+def f32_launches(model, x_shape):
+    """GemmF32 / AttnF32 descriptors of one fp32 forward of GRL `model` on a (B, Cin, H, W) input, in launch order:
+    GRL._forward_f32 run with tc.Listing on a meta input (with input_format "rggb", x_shape is the packed (B, 4, h, w)
+    Bayer input of the (2h, 2w) image).  Needs no device: conv weights are packed on the model's device, nothing runs."""
+    if model.precision != "fp32":
+        raise ValueError(f"f32_launches lists the fp32 forward; the model runs {model.precision}")
+    listing = tc.Listing()
+    model._forward_f32(torch.empty(x_shape, device="meta"), model.input_format == "rggb", listing)
+    out = []
+    for name, fn, args, kw in listing.launches:
+        a = inspect.signature(fn).bind(*args, **kw)
+        a.apply_defaults()
+        a = a.arguments
+        if fn in (K.linear, K.conv3x3):
+            w = a["weight"] if fn is K.linear else a["wpacked"]
+            out.append(GemmF32(name, fn is K.conv3x3, w.shape[1], w.shape[0], a["act"], a["slope"], a["bias"] is not None,
+                               a["res"] is not None))
+        else:
+            h, d, mask = a["heads"], a["qkv"].shape[2] // 3 // a["heads"], bool(a["use_mask"])
+            if fn is K.window_attention:
+                out.append(AttnF32(name, "window", a["grid"], a["grid"], h, d, mask))
+            else:
+                tok, anc = a["tok_grid"], a["anc_grid"]
+                out += [AttnF32(name, "stripe1", anc, tok, h, d, mask), AttnF32(name, "stripe2", tok, anc, h, d, mask)]
+    return out

@@ -4,7 +4,7 @@ Host-side orchestration only: one-time weight packing (pad head_dim to 32-wide s
 multiples of 64, permute the QKV rows into [window q|k|v][stripe q|k|v] x head order, im2col-order the 3x3 kernels)
 and the launch sequence of the wgmma kernels behind the C ABI (grl_tc_gemm / grl_tc_attn, include/grl_b200.h).  That
 sequence is written once (forward / stage_forward / BlockPlan.run) and issued through a launcher: Device runs it,
-Listing records its GEMMs without a device (gemm_launches).
+Listing records its GEMMs without a device (gemm_launches).  The fp32 forward (modules.py) uses the same launchers.
 Numerics contract (DESIGN.md): bf16 only for MMA operands; residual stream, LayerNorm, L2-normalisation, softmax
 statistics and every accumulator are fp32.
 Reference semantics: mixed_attn_block_efficient.py:351-381,:539-556; mixed_attn_block.py:948-983; grl.py:164-170,:506-551.
@@ -225,27 +225,28 @@ def gemm_path(launch):
 
 
 class Device:
-    """Launcher of a tensor-core forward on the GPU: every kernel runs.  The forward hands it each GEMM (`gemm`) and
-    every other kernel (`run`, a wrapper and its arguments)."""
+    """Launcher of a forward on the GPU: every kernel runs.  The forward hands it each launch a listing records
+    (`listed`: its name, wrapper and arguments; the GEMMs, and the fp32 attention) and every other kernel (`run`, a
+    wrapper and its arguments).  Outputs are allocated by the caller."""
     caches = True  # attention constants computed through it are real, so BlockPlan may keep them
 
-    def gemm(self, name, x16, w16, bias, **kw):
-        gemm(x16, w16, bias, **kw)  # the module's gemm at call time (tests record launches by replacing it)
+    def listed(self, name, fn, *args, **kw):
+        fn(*args, **kw)
 
     def run(self, fn, *args, **kw):
         fn(*args, **kw)
 
 
 class Listing:
-    """Launcher of a listing run: activations are meta tensors, every GEMM is recorded as a GemmLaunch and nothing is
-    launched."""
+    """Launcher of a listing run: activations are meta tensors, every `listed` launch is recorded as (name, wrapper,
+    args, kwargs) and nothing is launched."""
     caches = False
 
     def __init__(self):
         self.launches = []
 
-    def gemm(self, name, x16, w16, bias, **kw):
-        self.launches.append(gemm_launch(name, x16, w16, bias, **kw))
+    def listed(self, name, fn, *args, **kw):
+        self.launches.append((name, fn, args, kw))
 
     def run(self, fn, *args, **kw):
         pass
@@ -355,8 +356,8 @@ def channel_gate(y16, ld, B, L, C, ca, gate):
 def conv3x3(x16, wpack, bias, cin_pad, npad, *, n_store, launch=DEVICE, name="", **kw):
     """x16 16-bit (B, H, W, cin_pad) channels-last; kw: gemm's outputs, residual, activation and head-tail fusion."""
     B, H, W, _ = x16.shape
-    launch.gemm(name, x16, wpack, bias, image=(B, H, W), kpad=cin_pad, npad=npad, taps=9, epi=EPI_BIAS_ACT,
-                n_store=n_store, **kw)
+    launch.listed(name, gemm, x16, wpack, bias, image=(B, H, W), kpad=cin_pad, npad=npad, taps=9, epi=EPI_BIAS_ACT,
+                  n_store=n_store, **kw)
 
 
 def _version_key(module):
@@ -468,8 +469,8 @@ class BlockPlan:
                 self._const_key, self._consts = ckey, (slot_scale, bias_w, bias_1, bias_2)
         # projections
         qkv = _h16(B * L, self.n_qkv, device=dev, fmt=fmt)
-        launch.gemm(f"{name}.qkv", x16, self.w_qkv, self.b_qkv, M=B * L, kpad=cpad, npad=self.n_qkv, epi=EPI_QKV,
-                    n_store=self.n_qkv, out_bf16=qkv, slot_scale=slot_scale)
+        launch.listed(f"{name}.qkv", gemm, x16, self.w_qkv, self.b_qkv, M=B * L, kpad=cpad, npad=self.n_qkv,
+                      epi=EPI_QKV, n_store=self.n_qkv, out_bf16=qkv, slot_scale=slot_scale)
         df = self.df
         pooled = _h16(B, H // df, W // df, cpad, device=dev, fmt=fmt)
         launch.run(lambda: capi.check(capi.lib().grl_tc_avgpool16(capi.ptr(x16), capi.ptr(pooled), B, H, W, cpad, df, fmt,
@@ -477,8 +478,8 @@ class BlockPlan:
         La = (H // df) * (W // df)
         n_anc = self.w_anc.shape[0]
         anchor = _h16(B * La, n_anc, device=dev, fmt=fmt)
-        launch.gemm(f"{name}.anchor", pooled, self.w_anc, self.b_anc, M=B * La, kpad=cpad, npad=n_anc, epi=EPI_QKV,
-                    n_store=n_anc, out_bf16=anchor, slot_scale=self.anc_scale)
+        launch.listed(f"{name}.anchor", gemm, pooled, self.w_anc, self.b_anc, M=B * La, kpad=cpad, npad=n_anc,
+                      epi=EPI_QKV, n_store=n_anc, out_bf16=anchor, slot_scale=self.anc_scale)
         # attention
         merged = _h16(B * L, self.k_proj, device=dev, fmt=fmt, zero=self.k_proj != (hw + hs) * SLOT)
         launches = attention_launches(blk, x_size)
@@ -505,18 +506,19 @@ class BlockPlan:
         # proj + LN1 + residual (+ CAB)
         y32 = torch.empty(B, L, C, device=dev, dtype=torch.float32)
         y16 = _h16(B, L, cpad, device=dev, fmt=fmt)
-        launch.gemm(f"{name}.proj", merged, self.w_proj, self.b_proj, M=B * L, kpad=self.k_proj, npad=self.n_ln, epi=EPI_LN,
-                    n_store=self.n_ln, n_real=C, out_bf16=y16, out_f32=y32, res_f32=x32, C=C, gamma=blk.norm1.weight,
-                    beta=blk.norm1.bias, eps=blk.norm1.eps, res_scale=blk.res_scale, cab_y=cab_y, cab_gate=gate, L=L)
+        launch.listed(f"{name}.proj", gemm, merged, self.w_proj, self.b_proj, M=B * L, kpad=self.k_proj,
+                      npad=self.n_ln, epi=EPI_LN, n_store=self.n_ln, n_real=C, out_bf16=y16, out_f32=y32, res_f32=x32,
+                      C=C, gamma=blk.norm1.weight, beta=blk.norm1.bias, eps=blk.norm1.eps, res_scale=blk.res_scale,
+                      cab_y=cab_y, cab_gate=gate, L=L)
         # MLP + LN2 + residual
         hid = _h16(B * L, self.hpad, device=dev, fmt=fmt)
-        launch.gemm(f"{name}.fc1", y16, self.w_fc1, self.b_fc1, M=B * L, kpad=cpad, npad=self.hpad, epi=EPI_BIAS_ACT,
-                    n_store=self.hpad, act=K.ACT_GELU, out_bf16=hid)
+        launch.listed(f"{name}.fc1", gemm, y16, self.w_fc1, self.b_fc1, M=B * L, kpad=cpad, npad=self.hpad,
+                      epi=EPI_BIAS_ACT, n_store=self.hpad, act=K.ACT_GELU, out_bf16=hid)
         z32 = torch.empty(B, L, C, device=dev, dtype=torch.float32)
         z16 = _h16(B, L, cpad, device=dev, fmt=fmt)
-        launch.gemm(f"{name}.fc2", hid, self.w_fc2, self.b_fc2, M=B * L, kpad=self.hpad, npad=self.n_ln, epi=EPI_LN,
-                    n_store=self.n_ln, n_real=C, out_bf16=z16, out_f32=z32, res_f32=y32, C=C, gamma=blk.norm2.weight,
-                    beta=blk.norm2.bias, eps=blk.norm2.eps, res_scale=blk.res_scale, L=L)
+        launch.listed(f"{name}.fc2", gemm, hid, self.w_fc2, self.b_fc2, M=B * L, kpad=self.hpad, npad=self.n_ln,
+                      epi=EPI_LN, n_store=self.n_ln, n_real=C, out_bf16=z16, out_f32=z32, res_f32=y32, C=C,
+                      gamma=blk.norm2.weight, beta=blk.norm2.bias, eps=blk.norm2.eps, res_scale=blk.res_scale, L=L)
         return z32, z16
 
 
@@ -658,4 +660,4 @@ def gemm_launches(model, x_shape):
     image.  Needs no device: weights are packed on the model's device and nothing is launched."""
     listing = Listing()
     forward(model, torch.empty(x_shape, device="meta"), model.input_format == "rggb", listing)
-    return listing.launches
+    return [gemm_launch(name, *args, **kw) for name, _, args, kw in listing.launches]

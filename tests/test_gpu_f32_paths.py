@@ -4,11 +4,11 @@ Launch paths.  An attention launch's signature (`attn_path`) is the kernel speci
 (window, stripe pass 1, stripe pass 2: this fixes dense V and dense output), the head_dim template D, d < D, a partial
 and a second 128-query tile, a partial and a second 32-key tile, the shift mask and a non-zero roll.  A GEMM's
 (`gemm_path`) is conv or linear, a partial last 16-wide k tile, the number of k tiles, a partial and a second 64-wide N
-tile, the activation, bias and residual.  The CPU tests walk every block of the released configs (tiny / small / base x
-SR x2 x3 x4, dn, deblur, jpeg, dm at their smallest padded size) through tc.attention_launches, the grids that
-grl_window_attn_f32 / grl_stripe_attn_f32 launch, and through `gemm_calls`, the K.linear / K.conv3x3 calls of the fp32
-forward, and fail naming any path without a case.  test_recorded_launches_match_lists checks both lists one for one
-against the C-ABI calls of real fp32 forwards.
+tile, the activation, bias and residual.  The CPU tests walk the released configs (tiny / small / base x SR x2 x3 x4,
+dn, deblur, jpeg, dm at their smallest padded size) through f32_launches, the fp32 forward run in listing mode: its
+K.linear / K.conv3x3 calls and the passes of its K.window_attention / K.stripe_attention calls, and fail naming any path
+without a case.  test_recorded_launches_match_lists checks that list one for one against the C-ABI calls of real fp32
+forwards.
 
 Cases call the C ABI directly and write into NaN-filled buffers with guard rows (and guard columns where a pitch
 allows): every owned element must be written and nothing else.  Attention: 2 x 2 windows of the pass's grid, B = 2, the
@@ -62,33 +62,36 @@ def gamma(n):
 
 @lru_cache(maxsize=None)
 def released_model(pkg, variant, task, scale):
-    """A released config at its smallest padded size, on the CPU (host-side walks only)."""
+    """(model, fp32 launch descriptors) of a released config at its smallest padded size, on the CPU."""
+    from grl_image_restoration_b200 import modules
+
     cfg = pkg.configs.grl_config(variant, task, scale)
-    return pkg.GRL(**dict(cfg, img_size=math.lcm(cfg["window_size"], *cfg["stripe_size"])))
+    model = pkg.GRL(**dict(cfg, img_size=math.lcm(cfg["window_size"], *cfg["stripe_size"])))
+    return model, modules.f32_launches(model, (1, model.in_channels) + tuple(model.input_resolution))
 
 
 def released_models(pkg):
     for variant in ("tiny", "small", "base"):
         for task, s in TASKS:
-            yield f"{variant}/{task}x{s}", released_model(pkg, variant, task, s)
+            yield f"{variant}/{task}x{s}", *released_model(pkg, variant, task, s)
+
+
+def launches_of(launches, kind):
+    from grl_image_restoration_b200 import modules
+
+    return [ln for ln in launches if isinstance(ln, getattr(modules, kind))]
 
 
 # ------------------------------------------------------------------------------------------------------- attention
 
 
-def attn_path(ln, d):
+def attn_path(ln):
     """(role, D, d < D, Nq % 128 != 0, Nq > 128, Nk % 32 != 0, Nk > 32, use_mask, non-zero roll)."""
+    d = ln.d
     D = 16 if d <= 16 else 32 if d <= 32 else 64
     nq, nk = ln.gq.wh * ln.gq.ww, ln.gk.wh * ln.gk.ww
     roll = any((g.sh, g.sw) != (0, 0) for g in (ln.gq, ln.gk))
     return (ln.role, D, d < D, nq % 128 != 0, nq > 128, nk % 32 != 0, nk > 32, bool(ln.use_mask), roll)
-
-
-def block_attention(blk, x_size):
-    """(launch descriptor, head_dim) of the three attention launches of a block."""
-    from grl_image_restoration_b200 import tc
-
-    return [(ln, blk.dim // 2 // ln.heads) for ln in tc.attention_launches(blk, x_size)]
 
 
 class AttnCase(NamedTuple):
@@ -174,7 +177,7 @@ ATTN_EXTRAS = [  # limits no released config uses, and the earlier operator test
 
 def attn_case_launch(case):
     """(x_size, launch descriptor) of a case: an image of 2 x 2 windows of the pass's grid."""
-    from grl_image_restoration_b200 import geometry as G, tc
+    from grl_image_restoration_b200 import geometry as G, modules
 
     wh, ww = case.win
     x_size = (2 * wh, 2 * ww)
@@ -184,86 +187,31 @@ def attn_case_launch(case):
     if case.role != "window":
         anc = G.anchor_grid(x_size, case.win, sh, case.df)
         gq, gk = (anc, tok) if case.role == "stripe1" else (tok, anc)
-    return x_size, tc.attention_launch(case.role, gq, gk, case.heads, case.heads, case.heads * case.d, case.shifted)
+    return x_size, modules.AttnF32(case.src, case.role, gq, gk, case.heads, case.d, case.shifted)
 
 
 def test_released_attention_paths_have_cases(pkg):
     """Every attention path of every block of every released config has a case, and every case of ATTN_CASES is a
     released path."""
-    have = {attn_path(attn_case_launch(c)[1], c.d): c for c in ATTN_CASES}
+    have = {attn_path(attn_case_launch(c)[1]): c for c in ATTN_CASES}
     assert len(have) == len(ATTN_CASES), "two cases share a path"
     released, missing = set(), {}
-    for name, model in released_models(pkg):
-        for si, layer in enumerate(model.layers):
-            for bi, blk in enumerate(layer.blocks):
-                for ln, d in block_attention(blk, model.input_resolution):
-                    s = attn_path(ln, d)
-                    released.add(s)
-                    if s not in have:
-                        missing.setdefault(s, f"{name} stage {si} block {bi} {ln.role}")
+    for name, _, launches in released_models(pkg):
+        for ln in launches_of(launches, "AttnF32"):
+            s = attn_path(ln)
+            released.add(s)
+            if s not in have:
+                missing.setdefault(s, f"{name} {ln.name} {ln.role}")
     for s, name in missing.items():
         print(f"fp32 attention path without a case: {s}, first launched by {name}")
     assert not missing, f"{len(missing)} released fp32 attention paths have no case: " + "; ".join(
         f"{s} ({name})" for s, name in missing.items())
-    stale = [c for c in ATTN_CASES if attn_path(attn_case_launch(c)[1], c.d) not in released]
+    stale = [c for c in ATTN_CASES if attn_path(attn_case_launch(c)[1]) not in released]
     assert not stale, f"cases that no released config launches: {stale}"
     print(f"{len(released)} released fp32 attention paths")
 
 
 # ------------------------------------------------------------------------------------------------------------ GEMM
-
-
-class GemmCall(NamedTuple):
-    name: str
-    conv: bool
-    K: int        # 9 Cin for a conv
-    N: int
-    act: int
-    slope: float
-    bias: bool
-    res: bool
-
-
-def gemm_calls(model):
-    """The K.linear / K.conv3x3 calls of one fp32 forward of `model`, in order (modules.py)."""
-    out = []
-
-    def lin(name, m, act=ACT_NONE):
-        out.append(GemmCall(name, False, m.weight.shape[1], m.weight.shape[0], act, 0.0, m.bias is not None, False))
-
-    def conv(name, m, act=ACT_NONE, slope=0.0, res=False):
-        out.append(GemmCall(name, True, 9 * m.weight.shape[1], m.weight.shape[0], act, slope, m.bias is not None, res))
-
-    conv("conv_first", model.conv_first)
-    for si, layer in enumerate(model.layers):
-        for bi, blk in enumerate(layer.blocks):
-            p = f"stage{si}.block{bi}."
-            lin(p + "qkv", blk.attn.qkv.body)
-            lin(p + "anchor", blk.attn.anchor.body[0].reduction)
-            lin(p + "proj", blk.attn.proj)
-            if blk.args.local_connection:
-                conv(p + "cab1", blk.conv.cab[0], ACT_GELU)
-                conv(p + "cab2", blk.conv.cab[2])
-            lin(p + "fc1", blk.mlp.fc1, ACT_GELU)
-            lin(p + "fc2", blk.mlp.fc2)
-        conv(f"stage{si}.conv", layer.conv, res=True)
-    conv("conv_after_body", model.conv_after_body, res=True)
-    if model.upsampler == "pixelshuffle":
-        conv("conv_before_upsample", model.conv_before_upsample[0], ACT_LEAKY, 0.01)
-        for i, m in enumerate(model.upsample.up):
-            if isinstance(m, torch.nn.Conv2d):
-                conv(f"upsample.up.{i}", m)
-        conv("conv_last", model.conv_last)
-    elif model.upsampler == "pixelshuffledirect":
-        conv("upsample.up.0", model.upsample.up[0])
-    elif model.upsampler == "nearest+conv":
-        conv("conv_before_upsample", model.conv_before_upsample[0], ACT_LEAKY, 0.01)
-        for n in ("conv_up1", "conv_up2", "conv_hr"):
-            conv(n, getattr(model, n), ACT_LEAKY, 0.2)
-        conv("conv_last", model.conv_last)
-    else:
-        conv("conv_last", model.conv_last, res=model.in_channels == model.out_channels)
-    return out
 
 
 def gemm_path(g):
@@ -281,8 +229,10 @@ class GemmCase(NamedTuple):
     slope: float = 0.01  # LeakyReLU only
 
     def call(self):
-        return GemmCall(self.src, self.conv, self.K, self.N, self.act, self.slope if self.act == ACT_LEAKY else 0.0,
-                        True, self.res)
+        from grl_image_restoration_b200 import modules
+
+        return modules.GemmF32(self.src, self.conv, self.K, self.N, self.act,
+                               self.slope if self.act == ACT_LEAKY else 0.0, True, self.res)
 
 
 GEMM_CASES = [  # one case per released path, from its first launcher
@@ -332,8 +282,8 @@ def test_released_gemm_paths_have_cases(pkg):
     have = {gemm_path(c.call()): c for c in GEMM_CASES + GEMM_EXTRAS}
     assert len(have) == len(GEMM_CASES + GEMM_EXTRAS), "two cases share a path"
     released, missing = set(), {}
-    for name, model in released_models(pkg):
-        for g in gemm_calls(model):
+    for name, _, launches in released_models(pkg):
+        for g in launches_of(launches, "GemmF32"):
             s = gemm_path(g)
             released.add(s)
             if s not in have:
@@ -546,7 +496,7 @@ def test_attention_path(lib, device, case):
     from grl_image_restoration_b200 import capi
 
     x_size, ln = attn_case_launch(case)
-    sig = attn_path(ln, case.d)
+    sig = attn_path(ln)
     h, d = case.heads, case.d
     c = h * d
     H, W = x_size
@@ -1020,8 +970,8 @@ class Recorder:
                                                 ("base", "dm", 1)])
 def test_recorded_launches_match_lists(pkg, lib, device, monkeypatch, variant, task, scale):
     """The C-ABI calls of a real fp32 forward (smallest padded size, an input that needs padding) are, one for one and
-    in order, gemm_calls and the blocks' tc.attention_launches, and each one's path has a case."""
-    from grl_image_restoration_b200 import capi
+    in order, the GEMM and attention launches f32_launches lists, and each one's path has a case."""
+    from grl_image_restoration_b200 import capi, modules
 
     cfg = pkg.configs.grl_config(variant, task, scale)
     model = pkg.GRL(**dict(cfg, img_size=math.lcm(cfg["window_size"], *cfg["stripe_size"])))
@@ -1035,16 +985,106 @@ def test_recorded_launches_match_lists(pkg, lib, device, monkeypatch, variant, t
     torch.cuda.synchronize()
     monkeypatch.undo()
     assert y.shape == (1, 3, (S - 5) * cfg["upscale"], (S - 3) * cfg["upscale"])
-    want_g = gemm_calls(model)
+    launches = modules.f32_launches(model, tuple(x.shape))
+    want_g = launches_of(launches, "GemmF32")
     assert len(rec.gemm) == len(want_g), (len(rec.gemm), len(want_g))
     for got, g in zip(rec.gemm, want_g):
         assert got == (g.conv, g.K, g.N, g.act, g.slope, g.bias, g.res), (g.name, got)
     gemm_have = {gemm_path(c.call()) for c in GEMM_CASES}
     assert all(gemm_path(g) in gemm_have for g in want_g)
-    want_a = [(ln, d) for layer in model.layers for blk in layer.blocks for ln, d in block_attention(blk, (S, S))]
+    want_a = launches_of(launches, "AttnF32")
     assert len(rec.attn) == len(want_a), (len(rec.attn), len(want_a))
-    attn_have = {attn_path(attn_case_launch(c)[1], c.d) for c in ATTN_CASES}
-    for got, (ln, d) in zip(rec.attn, want_a):
-        assert got == (ln.role, grid_t(ln.gq), grid_t(ln.gk), ln.heads, d, bool(ln.use_mask)), got
-        assert attn_path(ln, d) in attn_have, (got, attn_path(ln, d))
-    print(f"\n{variant}/{task}x{scale}: {len(rec.gemm)} GEMM and {len(rec.attn)} attention launches match the lists")
+    attn_have = {attn_path(attn_case_launch(c)[1]) for c in ATTN_CASES}
+    for got, ln in zip(rec.attn, want_a):
+        assert got == (ln.role, grid_t(ln.gq), grid_t(ln.gk), ln.heads, ln.d, bool(ln.use_mask)), (ln.name, got)
+        assert attn_path(ln) in attn_have, (got, attn_path(ln))
+    print(f"\n{variant}/{task}x{scale}: {len(rec.gemm)} GEMM and {len(rec.attn)} attention launches match the list")
+
+
+# ------------------------------------------------------------------------------------------------ listing mode
+
+
+class HostOnly:
+    """Stands in for capi.lib() during a listing run: host helpers (`*_host`) run, any other symbol raises."""
+
+    def __init__(self, lib):
+        self._lib, self.calls = lib, []
+
+    def __getattr__(self, name):
+        if not name.endswith("_host"):
+            raise AssertionError(f"a listing run called {name}")
+        self.calls.append(name)
+        return getattr(self._lib, name)
+
+
+@pytest.mark.parametrize("input_format", ["rgb", "rggb"])
+def test_listing_calls_only_host_helpers(pkg, monkeypatch, input_format):
+    """Listing a released config, at a resolution other than the model's own (so the coordinate tables are computed),
+    makes no library call but the host helpers and never touches a CUDA stream."""
+    from grl_image_restoration_b200 import capi, modules
+
+    cfg = pkg.configs.grl_config("base", "dm", 1)
+    model = pkg.GRL(input_format=input_format, **dict(cfg, img_size=math.lcm(cfg["window_size"], *cfg["stripe_size"])))
+    S = model.pad_size
+    shape = (2, 4, S // 2 + 3, S - 1) if input_format == "rggb" else (2, 3, S + 5, 2 * S - 1)
+    host = HostOnly(capi.lib())
+    monkeypatch.setattr(capi, "lib", lambda: host)
+
+    def no_stream(*args, **kw):
+        raise AssertionError("a listing run asked for a CUDA stream")
+
+    monkeypatch.setattr(torch.cuda, "current_stream", no_stream)
+    launches = modules.f32_launches(model, shape)
+    monkeypatch.undo()
+    assert set(host.calls) == {"grl_coords_table_host"}
+    n_blocks = sum(len(layer.blocks) for layer in model.layers)
+    assert len(launches_of(launches, "AttnF32")) == 3 * n_blocks
+    assert len(launches_of(launches, "GemmF32")) == 7 * n_blocks + len(model.layers) + 3  # CAB: 2 convs per block
+
+
+def test_fp32_and_tensor_core_listings_name_the_same_gemms(pkg):
+    """Both paths run the same network: their listings name the same GEMMs in the same order, except that a tensor-core
+    block runs its CAB convs before the output projection, whose LayerNorm epilogue adds the CAB branch."""
+    from grl_image_restoration_b200 import tc
+
+    def no_cab(names):
+        return [n for n in names if not n.endswith((".cab1", ".cab2"))]
+
+    for name, model, launches in released_models(pkg):
+        shape = (1, model.in_channels) + tuple(model.input_resolution)
+        model.set_precision("fp16")
+        try:
+            names16 = [ln.name for ln in tc.gemm_launches(model, shape)]
+        finally:
+            model.set_precision("fp32")
+        names32 = [g.name for g in launches_of(launches, "GemmF32")]
+        assert sorted(names32) == sorted(names16), name
+        assert no_cab(names32) == no_cab(names16), name
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("task,input_format", [("sr", "rgb"), ("dm", "rggb")])
+def test_listing_first_leaves_the_forward_unchanged(pkg, device, task, input_format):
+    """f32_launches on a fresh fp32 model, then its forward: bitwise the forward of an identical model that was never
+    listed.  A listing run packs conv weights on the device, but keeps no meta tensor a forward would use."""
+    import copy
+
+    from grl_image_restoration_b200 import modules
+
+    cfg = pkg.configs.grl_config("tiny", task, 2 if task == "sr" else 1)
+    cfg = dict(cfg, img_size=math.lcm(cfg["window_size"], *cfg["stripe_size"]), input_format=input_format)
+    torch.manual_seed(0)
+    listed = pkg.GRL(**cfg)
+    fresh = copy.deepcopy(listed)
+    S = listed.pad_size
+    shape = (1, 4, S // 2, S // 2 - 1) if input_format == "rggb" else (1, 3, S, S)
+    x = torch.rand(shape, generator=torch.Generator().manual_seed(0)).to(device)
+    ys = []
+    for model, list_first in ((fresh, False), (listed, True)):
+        model = model.to(device).eval()
+        model.set_precision("fp32")
+        if list_first:
+            assert len(modules.f32_launches(model, tuple(x.shape))) > 0
+        ys.append(model(x))
+    torch.cuda.synchronize()
+    assert torch.equal(ys[0], ys[1])

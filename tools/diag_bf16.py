@@ -27,23 +27,23 @@ for mode in ("synth", "scale10", "scale30"):
     m = m.cuda().eval()
     x = orc.synth_input((1, 3, size, size), seed=5).cuda()
     m.set_precision("fp32")
+    stage_in = {}  # each stage's input in the fp32 forward
+    hooks = [layer.register_forward_pre_hook(lambda mod, args, si=si: stage_in.__setitem__(si, args[0].clone()))
+             for si, layer in enumerate(m.layers)]
     y32 = m(x)
+    for h in hooks:
+        h.remove()
     m.set_precision("bf16")
     y16 = m(x)
     psnr = (-10 * torch.log10(((y16 - y32) ** 2).mean())).item()
     print(f"[{mode}] end-to-end PSNR(bf16, fp32) = {psnr:.1f} dB  max-abs {(y16 - y32).abs().max().item():.3e}  out rms {y32.pow(2).mean().sqrt().item():.3f}")
     # per-block: same fp32 input through both paths
     m.set_precision("fp32")
-    feats = []
-    B, H, W = 1, size, size
-    xc = ((x - m.mean.to(x)) * m.img_range).permute(0, 2, 3, 1).contiguous()
-    from grl_image_restoration_b200 import functional as K, modules as M
-    first = M.conv2d_cl(m.conv_first, M._PackedConv(), xc)
-    t = K.ln_residual(None, first.view(B, H * W, -1), m.norm_start.weight, m.norm_start.bias)
+    H, W = size, size
     tim = m.get_table_index_mask(x.device, (H, W))
     worst = []
     for si, layer in enumerate(m.layers):
-        r = t
+        r = stage_in[si]
         for bi, blk in enumerate(layer.blocks):
             blk.precision = "fp32"
             o32 = blk(r, (H, W), tim)
@@ -54,6 +54,5 @@ for mode in ("synth", "scale10", "scale30"):
             rel = ((o16 - o32).pow(2).mean().sqrt() / upd.pow(2).mean().sqrt()).item()
             worst.append((rel, si, bi))
             r = o32
-        t = layer.conv and M.conv2d_cl(layer.conv, layer._pack, r.view(B, H, W, -1), res=t.view(B, H, W, -1)).view(B, H * W, -1)
     worst.sort(reverse=True)
     print("   per-block rms(err)/rms(update): median %.4f  worst %s" % (sorted(w[0] for w in worst)[len(worst) // 2], [(round(a, 4), s, b) for a, s, b in worst[:4]]))
