@@ -68,7 +68,7 @@ __global__ void avgpool_bf16_kernel(const uint16_t* __restrict__ x, uint16_t* __
 // (grl.py:510-511) + bchw -> channels-last + 16-bit operand pack, one pass.  One thread per padded pixel; Src reads raw
 // channel c of image b at the source pixel (ys, xs) the padding maps the padded pixel to.
 struct HeadMean {
-  float m[4];
+  float m[8];  // Cin <= 8: the channels one 16-byte operand store holds
 };
 struct PlanarSrc {  // (B, Cin, H, W) planes
   const float* x;
@@ -101,7 +101,9 @@ __global__ void head_pack_kernel(Src src, int B, int Cin, int H, int W, int Hp, 
     inside = ys < H && xs < W;  // constant (zero) padding of the RAW image, normalised like every other pixel
   }
   float v[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-  for (int c = 0; c < Cin; ++c) {
+#pragma unroll
+  for (int c = 0; c < 8; ++c) {  // unrolled: v and mean stay in registers / the parameter bank
+    if (c >= Cin) break;
     const float raw = inside ? src(b, c, ys, xs) : 0.f;
     v[c] = (raw - mean.m[c]) * range;
     if (y32) y32[i * Cin + c] = v[c];
@@ -147,12 +149,13 @@ __global__ void slot_scale_kernel(const float* __restrict__ ls_w, const float* _
 template <class Src>
 static int launch_head(Src src, int B, int Cin, int H, int W, int Hp, int Wp, const float* mean4, float range, void* y16,
                        int Cpad, float* y32, int fmt, cudaStream_t st) {
-  GRL_REQUIRE(Cin >= 1 && Cin <= 4 && Cpad % 8 == 0 && Cpad >= 8 && Hp >= H && Wp >= W && H > 0 && W > 0,
+  GRL_REQUIRE(Cin >= 1 && Cin <= 8 && Cpad % 8 == 0 && Cpad >= 8 && Hp >= H && Wp >= W && H > 0 && W > 0,
               "head_pack: bad shape (Cin %d, %dx%d -> %dx%d, Cpad %d)", Cin, H, W, Hp, Wp, Cpad);
   const long long total = (long long)B * Hp * Wp;
   if (total == 0) return GRL_OK;
   HeadMean m;
-  for (int c = 0; c < 4; ++c) m.m[c] = mean4 ? mean4[c] : 0.f;
+  const int n_mean = Cin > 4 ? Cin : 4;  // max(4, Cin) host floats: callers of the Cin <= 4 head pass exactly 4
+  for (int c = 0; c < 8; ++c) m.m[c] = (mean4 && c < n_mean) ? mean4[c] : 0.f;
   const int reflect = (Hp - H < H && Wp - W < W) ? 1 : 0;  // torch raises otherwise and the reference pads with zeros
   head_pack_kernel<<<ceil_div(total, 256), 256, 0, st>>>(src, B, Cin, H, W, Hp, Wp, m, range, reflect, (uint16_t*)y16, Cpad, y32, fmt);
   GRL_LAUNCH_CHECK("head_pack_kernel");

@@ -51,10 +51,12 @@ def _h16(*shape, device, fmt, zero=False):
     return (torch.zeros if zero else torch.empty)(*shape, device=device, dtype=DTYPE[fmt])
 
 
-def _mean4(mean):
+def _mean4(mean, cin=3):
+    """The host mean array grl_tc_head_pack reads: max(4, cin) floats, a single mean broadcast to all of them."""
+    n = max(4, cin)
     m = [float(v) for v in (mean if isinstance(mean, (list, tuple)) else mean.flatten().tolist())]
-    m = (m * 4)[:4] if len(m) == 1 else (m + [0.0] * 4)[:4]
-    return (ctypes.c_float * 4)(*m)
+    m = (m * n)[:n] if len(m) == 1 else (m + [0.0] * n)[:n]
+    return (ctypes.c_float * n)(*m)
 
 
 def head_pack(x, hp, wp, mean, img_range, cpad=64, fmt=0, want_f32=False, out=None):
@@ -63,7 +65,7 @@ def head_pack(x, hp, wp, mean, img_range, cpad=64, fmt=0, want_f32=False, out=No
     B, Cin, H, W = x.shape
     y16, y32 = out or (_h16(B, hp, wp, cpad, device=x.device, fmt=fmt),
                        torch.empty(B, hp, wp, Cin, device=x.device, dtype=torch.float32) if want_f32 else None)
-    capi.check(capi.lib().grl_tc_head_pack(capi.ptr(x), B, Cin, H, W, hp, wp, _mean4(mean), float(img_range), capi.ptr(y16),
+    capi.check(capi.lib().grl_tc_head_pack(capi.ptr(x), B, Cin, H, W, hp, wp, _mean4(mean, Cin), float(img_range), capi.ptr(y16),
                                            cpad, capi.ptr(y32), fmt, capi.stream()))
     return y16, y32
 

@@ -150,8 +150,10 @@ int grl_tc_pack16(const float* x, int64_t ldx, void* y16, int64_t M, int C, int 
 int grl_tc_unpack16(const void* x16, int64_t ldx, int x_off, float* y, int64_t ldy, int64_t M, int C, int fmt, void* stream);
 /* Network input in one pass: check_image_size (reflect pad on the bottom / right up to (Hp, Wp); zero pad when the pad
  * exceeds the image, as grl.py:485-488 falls back) + (x - mean) * img_range (grl.py:510-511) + bchw -> channels-last +
- * 16-bit pack.  x (B, Cin <= 4, H, W) fp32 -> y16 (B, Hp, Wp, Cpad), zero in [Cin, Cpad); y32 (may be NULL): the fp32
- * channels-last copy (B, Hp, Wp, Cin) the no-upsampler heads add back (grl.py:540-547).  mean4: 4 HOST floats. */
+ * 16-bit pack.  x (B, 1 <= Cin <= 8, H, W) fp32 -> y16 (B, Hp, Wp, Cpad), zero in [Cin, Cpad); y32 (may be NULL): the
+ * fp32 channels-last copy (B, Hp, Wp, Cin) the no-upsampler heads add back (grl.py:540-547).  mean4 (may be NULL: zero
+ * mean): max(4, Cin) HOST floats, i.e. exactly 4 for Cin <= 4 and Cin for Cin in 5..8 (the 6-channel dual-pixel input);
+ * entries past Cin are not used. */
 int grl_tc_head_pack(const float* x, int B, int Cin, int H, int W, int Hp, int Wp, const float* mean4, float range, void* y16,
                      int Cpad, float* y32, int fmt, void* stream);
 /* grl_tc_head_pack of the demosaiced image, with the demosaic fused in: cfa4 (B, 4, h, w) fp32 packed RGGB planes are the

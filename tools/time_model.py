@@ -12,7 +12,8 @@ from _pkgload import load_package  # noqa: E402
 
 ap = argparse.ArgumentParser()
 ap.add_argument("--variant", default="base")
-ap.add_argument("--task", default="sr")
+ap.add_argument("--task", default="sr", help="configs.grl_config task: sr, dn, deblur, jpeg, dm, bsr, defocus, defocus_dual")
+ap.add_argument("--in-channels", type=int, default=3, help="dn / jpeg: 1 for the grayscale checkpoints")
 ap.add_argument("--scale", type=int, default=4)
 ap.add_argument("--size", type=int, default=256)
 ap.add_argument("--batch", type=int, default=1)
@@ -25,13 +26,13 @@ a = ap.parse_args()
 pkg = load_package()
 import grl_oracle as orc  # noqa: E402  (weights only)
 
-cfg = pkg.configs.grl_config(a.variant, a.task, a.scale, a.size)
+cfg = pkg.configs.grl_config(a.variant, a.task, a.scale, a.size, in_channels=a.in_channels)
 m = pkg.GRL(**cfg)
 m.load_state_dict(orc.synth_state_dict(cfg, 0, a.style), strict=False)
 m = m.cuda().eval()
 if a.precision is not None and hasattr(m, "set_precision"):
     m.set_precision(a.precision)
-x = torch.rand(a.batch, 3, a.size, a.size, device="cuda")
+x = torch.rand(a.batch, cfg["in_channels"], a.size, a.size, device="cuda")
 from grl_image_restoration_b200 import capi  # noqa: E402
 
 if a.cuda_graph:
