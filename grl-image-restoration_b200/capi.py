@@ -75,6 +75,16 @@ _SIGNATURES = {
     "grl_tc_attn": (c_int, [ctypes.POINTER(GrlTcAttn), c_vp]),
     "grl_tc_attn_variant": (c_int, [c_int]),
     "grl_psnr_f32": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_sz, c_vp, c_vp, c_vp]),
+    "grl_psnrb_workspace": (c_sz, [c_int]),
+    "grl_psnrb_f32": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_sz, c_vp, c_vp, c_vp]),
+    "grl_niqe_workspace": (c_sz, [c_int, c_int, c_int, c_int]),
+    "grl_niqe_features_f32": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_sz, c_vp, c_vp]),
+    "grl_niqe_luma_host": (c_int, [c_vp, c_i64, c_vp]),
+    "grl_niqe_half_taps_host": (c_int, [c_vp]),
+    "grl_niqe_luma_f32": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp]),
+    "grl_niqe_mscn_f32": (c_int, [c_vp, c_int, c_int, c_int, c_vp, c_vp, c_vp]),
+    "grl_niqe_half_f32": (c_int, [c_vp, c_int, c_int, c_int, c_vp, c_vp, c_vp]),
+    "grl_niqe_feat_f32": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_vp, c_vp, c_vp]),
     "grl_affine_f32": (c_int, [c_vp, c_i64, c_int, c_int, c_int, c_vp, c_vp, c_int, c_vp, c_vp, c_int, c_vp]),
     "grl_linear_f32": (c_int, [c_vp, c_i64, c_vp, c_vp, c_vp, c_i64, c_vp, c_i64, c_i64, c_int, c_int, c_int, c_f32, c_vp]),
     "grl_conv3x3_f32": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_f32, c_vp]),

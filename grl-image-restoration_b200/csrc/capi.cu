@@ -4,6 +4,7 @@
 
 #include "grl_common.cuh"
 #include "grl_demosaic.h"
+#include "grl_niqe.h"
 #include "ops_f32.h"
 #include "ops_tc.h"
 
@@ -358,6 +359,59 @@ int grl_psnr_f32(const float* restored, const float* target, int B, int C, int H
               "psnr: workspace %zu bytes < %zu", workspace_bytes, sizeof(unsigned long long) * 2 * (size_t)(B > 0 ? B : 0));
   return launch_psnr(restored, target, B, C, H, W, border, (unsigned long long*)workspace, psnr_rgb, psnr_y,
                      (cudaStream_t)stream);
+}
+
+size_t grl_psnrb_workspace(int B) { return psnrb_workspace(B); }
+
+int grl_psnrb_f32(const float* restored, const float* target, int B, int C, int H, int W, void* workspace,
+                  size_t workspace_bytes, double* psnrb_rgb, double* psnrb_y, void* stream) {
+  GRL_REQUIRE(restored && target && psnrb_rgb, "psnrb: null argument");
+  GRL_REQUIRE(workspace && workspace_bytes >= psnrb_workspace(B), "psnrb: workspace %zu bytes < %zu", workspace_bytes,
+              psnrb_workspace(B));
+  return launch_psnrb(restored, target, B, C, H, W, (unsigned long long*)workspace, psnrb_rgb, psnrb_y, (cudaStream_t)stream);
+}
+
+// ---------------------------------------------------------------- NIQE
+int grl_niqe_luma_host(const uint8_t* rgb, int64_t n, float* y) {
+  GRL_REQUIRE(rgb && y && n >= 0, "niqe_luma_host: bad arguments");
+  for (int64_t i = 0; i < n; ++i) y[i] = niqe_luma(rgb[3 * i], rgb[3 * i + 1], rgb[3 * i + 2]);
+  return GRL_OK;
+}
+
+int grl_niqe_half_taps_host(float* w8) {
+  GRL_REQUIRE(w8, "niqe_half_taps_host: null output");
+  niqe_half_taps(w8);
+  return GRL_OK;
+}
+
+int grl_niqe_luma_f32(const float* restored, int B, int C, int H, int W, int border, float* y, void* stream) {
+  GRL_REQUIRE(restored && y, "niqe_luma: null argument");
+  return launch_niqe_luma(restored, B, C, H, W, border, y, (cudaStream_t)stream);
+}
+
+int grl_niqe_mscn_f32(const float* img, int B, int H, int W, const double* window49, float* out, void* stream) {
+  GRL_REQUIRE(img && out, "niqe_mscn: null argument");
+  return launch_niqe_mscn(img, B, H, W, window49, out, (cudaStream_t)stream);
+}
+
+int grl_niqe_half_f32(const float* img, int B, int H, int W, float* tmp, float* out, void* stream) {
+  GRL_REQUIRE(img && tmp && out, "niqe_half: null argument");
+  return launch_niqe_half(img, B, H, W, tmp, out, (cudaStream_t)stream);
+}
+
+int grl_niqe_feat_f32(const float* mscn1, const float* mscn2, int B, int nbh, int nbw, const double* tables, double* feats,
+                      void* stream) {
+  GRL_REQUIRE(mscn1 && mscn2 && feats, "niqe_feat: null argument");
+  return launch_niqe_feat(mscn1, mscn2, B, nbh, nbw, tables, feats, (cudaStream_t)stream);
+}
+
+size_t grl_niqe_workspace(int B, int H, int W, int border) { return niqe_ws(B, H, W, border); }
+
+int grl_niqe_features_f32(const float* restored, int B, int C, int H, int W, int border, const double* window49,
+                          const double* tables, void* workspace, size_t workspace_bytes, double* feats, void* stream) {
+  GRL_REQUIRE(restored && window49 && tables && feats, "niqe: null argument");
+  return launch_niqe_features(restored, B, C, H, W, border, window49, tables, workspace, workspace_bytes, feats,
+                              (cudaStream_t)stream);
 }
 
 // ---------------------------------------------------------------- x8 self-ensemble

@@ -65,6 +65,20 @@ int launch_attn(const AttnArgs& a, cudaStream_t st);
 // fused tensor_round + shave + squared-error reduction (RGB and luma) -> per-image PSNR (metric.cu)
 int launch_psnr(const float* restored, const float* target, int B, int C, int H, int W, int border,
                 unsigned long long* workspace, float* psnr_rgb, float* psnr_y, cudaStream_t st);
+// PSNR-B: exact integer sums of the error and of the restored image's block-boundary differences -> per image (metric.cu)
+size_t psnrb_workspace(int B);
+int launch_psnrb(const float* restored, const float* target, int B, int C, int H, int W, unsigned long long* workspace,
+                 double* psnrb_rgb, double* psnrb_y, cudaStream_t st);
+// NIQE features: luma, MSCN, x0.5 resize, per-block AGGD features (niqe.cu)
+void niqe_half_taps(float* w8);
+size_t niqe_ws(int B, int H, int W, int border);
+int launch_niqe_luma(const float* x, int B, int C, int H, int W, int border, float* y, cudaStream_t st);
+int launch_niqe_mscn(const float* in, int B, int H, int W, const double* window49, float* out, cudaStream_t st);
+int launch_niqe_half(const float* in, int B, int H, int W, float* tmp, float* out, cudaStream_t st);
+int launch_niqe_feat(const float* m1, const float* m2, int B, int nbh, int nbw, const double* tables, double* feats,
+                     cudaStream_t st);
+int launch_niqe_features(const float* x, int B, int C, int H, int W, int border, const double* window49, const double* tables,
+                         void* ws, size_t ws_bytes, double* feats, cudaStream_t st);
 // x8 self-ensemble: the 4 views of one group, and the ordered average of the 8 mapped-back outputs (ensemble.cu)
 int launch_ens_gather(const float* x, int B, int C, int H, int W, int group, float* views, cudaStream_t st);
 int launch_ens_merge(const float* ya, const float* yb, int B, int C, int Hs, int Ws, float* y, cudaStream_t st);

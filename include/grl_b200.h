@@ -282,6 +282,43 @@ int grl_tc_attn_variant(int variant);
 int grl_psnr_f32(const float* restored, const float* target, int B, int C, int H, int W, int border, void* workspace,
                  size_t workspace_bytes, float* psnr_rgb, float* psnr_y, void* stream);
 
+/* Per-image PSNR-B of the JPEG test commands (PeakSignalNoiseRatioBlock.update, utils/metrics/psnrb.py:141-163) on
+ * tensor_round'ed images, no shave: per channel 10 log10(1 / (mse + bef)) with the blocking-effect factor bef of the
+ * RESTORED image (psnrb.py:22-101, its normalisers H * (W // 8 - 1) etc. as written there, not the counts of the summed
+ * positions), averaged in dB over the channels.  restored / target: (B, C, H, W) fp32, C = 1 or 3, H, W >= 16.
+ * psnrb_y (may be NULL): the same on the luma of grl_psnr_f32 for C == 3, else a copy of psnrb_rgb.  Both outputs are
+ * float64.  The sums are exact integers, so the result does not depend on the launch geometry.
+ * workspace >= grl_psnrb_workspace(B) bytes of device memory (zeroed by the call). */
+size_t grl_psnrb_workspace(int B);
+int grl_psnrb_f32(const float* restored, const float* target, int B, int C, int H, int W, void* workspace,
+                  size_t workspace_bytes, double* psnrb_rgb, double* psnrb_y, void* stream);
+
+/* ---- NIQE features of the blind-SR test command (NaturalImageQualityEvaluator.update, utils/metrics/niqe.py:566-576) --
+ * restored: (B, C = 3, H, W) fp32; the score is the multivariate-Gaussian distance of the features to the caller's
+ * pristine model (metrics.niqe, batched torch float64).  The crop keeps (Hc, Wc) = 96 * floor((H - 2 border, W - 2 border)
+ * / 96) from the top left of the border-cropped image; both need at least 96 pixels.
+ * window49: HOST pointer to the 7 x 7 float64 gaussian_window of niqe_pris_params.npz.  tables: DEVICE (4, 9801) float64:
+ * gam = 0.2 : 0.001 : 10 as np.arange builds it, r_gam = G(2/g)^2 / (G(1/g) G(3/g)) with 1/g computed first,
+ * sqrt(G(1/g) / G(3/g)) and G(2/g) / G(1/g).  feats: (B, nbw * nbh, 36) float64, row iw * nbh + ih, 18 features of the
+ * 96 x 96 block at scale 1 then 18 of the 48 x 48 block at scale 2.  The stage entry points are the pieces
+ * grl_niqe_features_f32 runs, one kernel each (csrc/niqe.cu). */
+size_t grl_niqe_workspace(int B, int H, int W, int border);
+int grl_niqe_features_f32(const float* restored, int B, int C, int H, int W, int border, const double* window49,
+                          const double* tables, void* workspace, size_t workspace_bytes, double* feats, void* stream);
+/* The rounded luma (an integer in [16, 235] as fp32) of n 8-bit RGB triples rgb (n, 3); HOST pointers (csrc/grl_niqe.h). */
+int grl_niqe_luma_host(const uint8_t* rgb, int64_t n, float* y);
+/* The 8 fp32 taps of the x0.5 antialiased bicubic resize (niqe.py:169-238); HOST pointer. */
+int grl_niqe_half_taps_host(float* w8);
+/* luma + crops: y (B, Hc, Wc). */
+int grl_niqe_luma_f32(const float* restored, int B, int C, int H, int W, int border, float* y, void* stream);
+/* MSCN of img (B, H, W) -> out (B, H, W) (niqe.py:447-455). */
+int grl_niqe_mscn_f32(const float* img, int B, int H, int W, const double* window49, float* out, void* stream);
+/* 255 * imresize(img / 255, 0.5) (niqe.py:470-471): img (B, H, W), H and W even; tmp (B, H/2, W); out (B, H/2, W/2). */
+int grl_niqe_half_f32(const float* img, int B, int H, int W, float* tmp, float* out, void* stream);
+/* Features of the MSCN images mscn1 (B, 96 nbh, 96 nbw) and mscn2 (B, 48 nbh, 48 nbw). */
+int grl_niqe_feat_f32(const float* mscn1, const float* mscn2, int B, int nbh, int nbw, const double* tables, double* feats,
+                      void* stream);
+
 /* ---- x8 self-ensemble (geometric test-time augmentation) ----------------------------------------
  * The 8 views are augment_img_tensor4(img, mode) (utils/utils_bsr/utils_image.py:444-460).  Group A = modes 0, 2, 4, 6
  * (the view keeps (H, W)), group B = modes 1, 3, 5, 7 (the view is (W, H)); inside a group view i is mode 2*i + group. */
