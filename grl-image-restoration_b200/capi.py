@@ -77,6 +77,10 @@ _SIGNATURES = {
     "grl_psnr_f32": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_sz, c_vp, c_vp, c_vp]),
     "grl_psnrb_workspace": (c_sz, [c_int]),
     "grl_psnrb_f32": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_sz, c_vp, c_vp, c_vp]),
+    "grl_ssim_workspace": (c_sz, [c_int, c_int, c_int, c_int, c_int]),
+    "grl_ssim_f32": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "grl_ssim_taps_host": (c_int, [c_vp]),
+    "grl_ssim_host": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp]),
     "grl_niqe_workspace": (c_sz, [c_int, c_int, c_int, c_int]),
     "grl_niqe_features_f32": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_sz, c_vp, c_vp]),
     "grl_niqe_luma_host": (c_int, [c_vp, c_i64, c_vp]),

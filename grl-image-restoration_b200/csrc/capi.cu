@@ -371,6 +371,28 @@ int grl_psnrb_f32(const float* restored, const float* target, int B, int C, int 
   return launch_psnrb(restored, target, B, C, H, W, (unsigned long long*)workspace, psnrb_rgb, psnrb_y, (cudaStream_t)stream);
 }
 
+// ---------------------------------------------------------------- SSIM
+size_t grl_ssim_workspace(int B, int C, int H, int W, int border) { return ssim_workspace(B, C, H, W, border); }
+
+int grl_ssim_f32(const float* restored, const float* target, int B, int C, int H, int W, int border, void* workspace,
+                 size_t workspace_bytes, double* ssim_rgb, double* ssim_y, double* map_rgb, double* map_y, void* stream) {
+  GRL_REQUIRE(restored && target && ssim_rgb, "ssim: null argument");
+  return launch_ssim(restored, target, B, C, H, W, border, workspace, workspace_bytes, ssim_rgb, ssim_y, map_rgb, map_y,
+                     (cudaStream_t)stream);
+}
+
+int grl_ssim_taps_host(double* taps11) {
+  GRL_REQUIRE(taps11, "ssim_taps_host: null output");
+  ssim_taps(taps11);
+  return GRL_OK;
+}
+
+int grl_ssim_host(const float* restored, const float* target, int B, int C, int H, int W, int border, double* ssim_rgb,
+                  double* ssim_y, double* map_rgb, double* map_y) {
+  GRL_REQUIRE(restored && target && ssim_rgb, "ssim_host: null argument");
+  return ssim_host(restored, target, B, C, H, W, border, ssim_rgb, ssim_y, map_rgb, map_y);
+}
+
 // ---------------------------------------------------------------- NIQE
 int grl_niqe_luma_host(const uint8_t* rgb, int64_t n, float* y) {
   GRL_REQUIRE(rgb && y && n >= 0, "niqe_luma_host: bad arguments");

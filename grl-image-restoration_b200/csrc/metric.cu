@@ -6,21 +6,24 @@
 // integer (a rounded pixel is k/255; (k1 - k2)^2 <= 65025): the per-image sums are 64-bit integer atomics, so the result
 // is independent of the block schedule.  C == 3 additionally accumulates the error of the luma of MATLAB's rgb2ycbcr
 // (coefficients 65.481, 128.553, 24.966, offset 16, rounded to 8 bit).  HBM-bound: 2 x 4 bytes read per element.
+// PSNR-B and SSIM (RGB and luma, float64 on the same 8-bit integers) follow below.
 #include <algorithm>
+#include <vector>
 
 #include "grl_common.cuh"
+#include "grl_ssim.h"
 #include "ops_f32.h"
 
 namespace grl {
 
-__device__ __forceinline__ float round8(float v) {
+__host__ __device__ __forceinline__ float round8(float v) {
   v = fminf(fmaxf(v, 0.f), 1.f);
   return rintf(v * 255.0f);  // round half to even == torch.round
 }
 
 // y = round(65.481/255 * R + 128.553/255 * G + 24.966/255 * B + 16) with R, G, B on the 0..255 grid
 // (metrics.rgb_to_y: (img * 255) @ (coeff / 255) + 16, rounded)
-__device__ __forceinline__ float luma8(float r, float g, float b) {
+__host__ __device__ __forceinline__ float luma8(float r, float g, float b) {
   float acc = r * (65.481f / 255.0f);
   acc = fmaf(g, 128.553f / 255.0f, acc);
   acc = fmaf(b, 24.966f / 255.0f, acc);
@@ -207,5 +210,263 @@ int launch_psnrb(const float* restored, const float* target, int B, int C, int H
 }
 
 size_t psnrb_workspace(int B) { return sizeof(unsigned long long) * kPsnrbSets * kPsnrbSums * (size_t)(B > 0 ? B : 0); }
+
+// ---- SSIM (utils/metrics/ssim.py:17-85; the closed form is grl_ssim.h) -----------------------------------------------
+// One CTA owns a 32 x 16 tile of output pixels of one image and produces every plane of it: the C channels and, for
+// C == 3, the luma of luma8.  The 8-bit integers of the tile and its 5-pixel halo are staged once (42 x 26 per plane and
+// image, 0 outside the image).  Per plane: the horizontal 11-tap sums of a, b, a^2, b^2, a b go to shared memory (one lane
+// per staged row and four adjacent columns per thread, so a staged value is converted once for four outputs), then each
+// thread takes the vertical sums and the map values of four rows of one column.  The tile's map values are summed in a
+// fixed order into one float64 partial per (image, {channels, luma}, tile); ssim_finalize_kernel sums the partials of an
+// image in a fixed order.  No atomics: the result depends neither on the schedule nor on the batch an image is part of.
+// On paper the kernel is bound by the float64 pipe, not by HBM: about 145 DFMA per plane value against 24 bytes per pixel.
+constexpr int kSsimTW = 32, kSsimTH = 16, kSsimThreads = 128;
+constexpr int kSsimRows = kSsimTH + 2 * kSsimHalo;  // 26 staged rows
+constexpr int kSsimCols = kSsimTW + 2 * kSsimHalo;  // 42 staged columns
+constexpr int kSsimRowBytes = 44;                   // ... in rows of whole 32-bit words (the last two bytes hold 0)
+constexpr int kSsimHStride = kSsimTW + 1;           // row stride of the horizontal sums: the lanes of a warp write one column
+static_assert(kSsimRows <= 32 && kSsimTW == 32 && kSsimThreads == 4 * 32 && kSsimTH == 4 * 4, "thread mapping of ssim_tile_kernel");
+
+// exact double of an integer 0 <= k < 2^32 without the conversion pipe: 2^52 + k is exact, minus 2^52
+__device__ __forceinline__ double ssim_u2d(unsigned k) { return __hiloint2double(0x43300000, (int)k) - 4503599627370496.0; }
+
+__global__ void __launch_bounds__(kSsimThreads)
+ssim_tile_kernel(const float* __restrict__ a, const float* __restrict__ b, int C, int H, int W, int border,
+                 double* __restrict__ partial /* (B, 2, tiles) */, double* __restrict__ map_rgb, double* __restrict__ map_y) {
+  __shared__ __align__(16) unsigned char sk[2][4][kSsimRows][kSsimRowBytes];
+  __shared__ double hs[5][kSsimRows][kSsimHStride];
+  __shared__ double red[2][kSsimThreads / 32];
+  const int img = blockIdx.z, h = H - 2 * border, w = W - 2 * border;
+  const int x0 = blockIdx.x * kSsimTW, y0 = blockIdx.y * kSsimTH;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const long long plane = (long long)H * W, n = (long long)h * w;
+  const float* pa = a + (long long)img * C * plane;
+  const float* pb = b + (long long)img * C * plane;
+
+  // tensor_round + shave + luma, staged as bytes
+  for (int i = threadIdx.x; i < kSsimRows * kSsimRowBytes; i += kSsimThreads) {
+    const int r = i / kSsimRowBytes, c = i - r * kSsimRowBytes;
+    const int y = y0 - kSsimHalo + r, x = x0 - kSsimHalo + c;
+    const bool in = c < kSsimCols && y >= 0 && y < h && x >= 0 && x < w;
+    const long long off = in ? (long long)(y + border) * W + (x + border) : 0;
+    float va[3] = {0.f, 0.f, 0.f}, vb[3] = {0.f, 0.f, 0.f};
+#pragma unroll
+    for (int ch = 0; ch < 3; ++ch)
+      if (ch < C) {
+        if (in) va[ch] = round8(pa[ch * plane + off]), vb[ch] = round8(pb[ch * plane + off]);
+        sk[0][ch][r][c] = (unsigned char)va[ch], sk[1][ch][r][c] = (unsigned char)vb[ch];
+      }
+    if (C == 3) {
+      sk[0][3][r][c] = in ? (unsigned char)luma8(va[0], va[1], va[2]) : 0;
+      sk[1][3][r][c] = in ? (unsigned char)luma8(vb[0], vb[1], vb[2]) : 0;
+    }
+  }
+
+  double sum_rgb = 0.0, sum_y = 0.0;
+  const int planes = C == 3 ? 4 : C;
+  for (int p = 0; p < planes; ++p) {
+    __syncthreads();  // the staged bytes are written (p == 0); the previous plane's vertical pass has read hs
+    if (lane < kSsimRows) {
+      for (int xg = warp; xg < kSsimTW / 4; xg += kSsimThreads / 32) {  // outputs 4 xg .. 4 xg + 3 of staged row `lane`
+        const unsigned* qa = reinterpret_cast<const unsigned*>(&sk[0][p][lane][4 * xg]);
+        const unsigned* qb = reinterpret_cast<const unsigned*>(&sk[1][p][lane][4 * xg]);
+        unsigned ua[4], ub[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) ua[j] = qa[j], ub[j] = qb[j];
+        double va[14], vb[14];
+#pragma unroll
+        for (int j = 0; j < 14; ++j) {
+          va[j] = ssim_u2d((ua[j >> 2] >> (8 * (j & 3))) & 0xffu);
+          vb[j] = ssim_u2d((ub[j >> 2] >> (8 * (j & 3))) & 0xffu);
+        }
+#pragma unroll
+        for (int q = 0; q < 5; ++q) {
+          double v[14];
+#pragma unroll
+          for (int j = 0; j < 14; ++j)  // integers below 2^16: the products are exact
+            v[j] = q == 0 ? va[j] : q == 1 ? vb[j] : q == 2 ? __dmul_rn(va[j], va[j]) : q == 3 ? __dmul_rn(vb[j], vb[j]) : __dmul_rn(va[j], vb[j]);
+          double acc[4] = {0.0, 0.0, 0.0, 0.0};
+#pragma unroll
+          for (int t = 0; t < kSsimTaps; ++t)
+#pragma unroll
+            for (int i = 0; i < 4; ++i) acc[i] = ssim_fma(ssim_tap(t), v[i + t], acc[i]);
+#pragma unroll
+          for (int i = 0; i < 4; ++i) hs[q][lane][4 * xg + i] = acc[i];
+        }
+      }
+    }
+    __syncthreads();
+    double s[5][4];  // column `lane`, rows 4 warp .. 4 warp + 3 of the tile
+#pragma unroll
+    for (int q = 0; q < 5; ++q) {
+      double r[14];
+#pragma unroll
+      for (int j = 0; j < 14; ++j) r[j] = hs[q][4 * warp + j][lane];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        double acc = 0.0;
+#pragma unroll
+        for (int t = 0; t < kSsimTaps; ++t) acc = ssim_fma(ssim_tap(t), r[i + t], acc);
+        s[q][i] = acc;
+      }
+    }
+    const int x = x0 + lane;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int y = y0 + 4 * warp + i;
+      if (x < w && y < h) {
+        const double m = ssim_map_value(s[0][i], s[1][i], s[2][i], s[3][i], s[4][i]);
+        if (p < C) {
+          sum_rgb += m;
+          if (map_rgb) map_rgb[((long long)img * C + p) * n + (long long)y * w + x] = m;
+        } else {
+          sum_y += m;
+          if (map_y) map_y[(long long)img * n + (long long)y * w + x] = m;
+        }
+      }
+    }
+  }
+  // fixed-shape reduction: xor tree in the warp, then the four warps in order
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    sum_rgb += __shfl_xor_sync(0xffffffffu, sum_rgb, o);
+    sum_y += __shfl_xor_sync(0xffffffffu, sum_y, o);
+  }
+  if (lane == 0) red[0][warp] = sum_rgb, red[1][warp] = sum_y;
+  __syncthreads();
+  if (threadIdx.x < 2) {
+    double t = 0.0;
+    for (int k = 0; k < kSsimThreads / 32; ++k) t += red[threadIdx.x][k];
+    const long long tiles = (long long)gridDim.x * gridDim.y, tile = (long long)blockIdx.y * gridDim.x + blockIdx.x;
+    partial[((long long)img * 2 + threadIdx.x) * tiles + tile] = t;
+  }
+}
+
+// Block (g, img): the mean of the map over the channels (g == 0) or over the luma plane (g == 1; for C != 3 the channels
+// again, so ssim_y is a copy of ssim_rgb).  Thread t sums partials t, t + 256, ... in order, then a fixed tree.
+__global__ void __launch_bounds__(256)
+ssim_finalize_kernel(const double* __restrict__ partial, int C, long long tiles, long long n_pix, double* __restrict__ ssim_rgb,
+                     double* __restrict__ ssim_y) {
+  __shared__ double red[8];
+  const int g = blockIdx.x, img = blockIdx.y;
+  double* out = g == 0 ? ssim_rgb : ssim_y;
+  if (!out) return;
+  const bool luma = g == 1 && C == 3;
+  const double* src = partial + ((long long)img * 2 + (luma ? 1 : 0)) * tiles;
+  double t = 0.0;
+  for (long long k = threadIdx.x; k < tiles; k += blockDim.x) t += src[k];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = t;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double v = 0.0;
+    for (int k = 0; k < 8; ++k) v += red[k];
+    out[img] = v / ((double)n_pix * (luma ? 1 : C));
+  }
+}
+
+static long long ssim_tiles(int H, int W, int border) {
+  return (long long)ceil_div(W - 2 * border, kSsimTW) * ceil_div(H - 2 * border, kSsimTH);
+}
+
+static bool ssim_shape_ok(int B, int C, int H, int W, int border) {
+  return B >= 0 && (C == 1 || C == 3) && border >= 0 && H > 0 && W > 0 && 2LL * border < std::min(H, W);
+}
+
+size_t ssim_workspace(int B, int C, int H, int W, int border) {
+  if (!ssim_shape_ok(B, C, H, W, border)) return 0;
+  return sizeof(double) * 2 * (size_t)B * (size_t)ssim_tiles(H, W, border);
+}
+
+#define GRL_SSIM_SHAPE(B, C, H, W, border)                                                                                     \
+  do {                                                                                                                         \
+    GRL_REQUIRE(C == 1 || C == 3, "ssim: needs C == 1 or 3, got %d", C);                                                       \
+    GRL_REQUIRE(B >= 0 && border >= 0 && H > 0 && W > 0, "ssim: bad shape (%d,%d,%d,%d) border %d", B, C, H, W, border);       \
+    GRL_REQUIRE(2LL * border < std::min(H, W), "ssim: border %d leaves no pixel of a %d x %d image", border, H, W);            \
+  } while (0)
+
+int launch_ssim(const float* restored, const float* target, int B, int C, int H, int W, int border, void* workspace,
+                size_t workspace_bytes, double* ssim_rgb, double* ssim_y, double* map_rgb, double* map_y, cudaStream_t st) {
+  GRL_SSIM_SHAPE(B, C, H, W, border);
+  if (B == 0) return GRL_OK;
+  GRL_REQUIRE(workspace && workspace_bytes >= ssim_workspace(B, C, H, W, border), "ssim: workspace %zu bytes < %zu", workspace_bytes,
+              ssim_workspace(B, C, H, W, border));
+  const int h = H - 2 * border, w = W - 2 * border;
+  const int gx = ceil_div(w, kSsimTW), gy = ceil_div(h, kSsimTH);
+  GRL_REQUIRE(gy <= 65535 && B <= 65535, "ssim: %d tile rows / %d images exceed the grid", gy, B);
+  ssim_tile_kernel<<<dim3((unsigned)gx, (unsigned)gy, (unsigned)B), kSsimThreads, 0, st>>>(restored, target, C, H, W, border,
+                                                                                         (double*)workspace, map_rgb, map_y);
+  GRL_LAUNCH_CHECK("ssim_tile_kernel");
+  ssim_finalize_kernel<<<dim3(2, (unsigned)B), 256, 0, st>>>((const double*)workspace, C, (long long)gx * gy, (long long)h * w, ssim_rgb, ssim_y);
+  GRL_LAUNCH_CHECK("ssim_finalize_kernel");
+  return GRL_OK;
+}
+
+void ssim_taps(double* t11) {
+  for (int i = 0; i < kSsimTaps; ++i) t11[i] = ssim_tap(i);
+}
+
+// The same computation on the CPU (HOST pointers): the scores and, when asked for, the maps.  Scratch is host memory.
+int ssim_host(const float* restored, const float* target, int B, int C, int H, int W, int border, double* ssim_rgb,
+              double* ssim_y, double* map_rgb, double* map_y) {
+  GRL_SSIM_SHAPE(B, C, H, W, border);
+  const int h = H - 2 * border, w = W - 2 * border, planes = C == 3 ? 4 : C;
+  const size_t n = (size_t)h * w, plane = (size_t)H * W;
+  std::vector<double> ka(n), kb(n), src(n), hsum(n), sums[5];
+  for (auto& s : sums) s.resize(n);
+  for (int img = 0; img < B; ++img) {
+    const float* pa = restored + (size_t)img * C * plane;
+    const float* pb = target + (size_t)img * C * plane;
+    double tot_rgb = 0.0, tot_y = 0.0;
+    for (int p = 0; p < planes; ++p) {
+      for (int y = 0; y < h; ++y)
+        for (int x = 0; x < w; ++x) {
+          const size_t off = (size_t)(y + border) * W + (x + border);
+          if (p < C) {
+            ka[(size_t)y * w + x] = round8(pa[p * plane + off]), kb[(size_t)y * w + x] = round8(pb[p * plane + off]);
+          } else {
+            ka[(size_t)y * w + x] = luma8(round8(pa[off]), round8(pa[plane + off]), round8(pa[2 * plane + off]));
+            kb[(size_t)y * w + x] = luma8(round8(pb[off]), round8(pb[plane + off]), round8(pb[2 * plane + off]));
+          }
+        }
+      for (int q = 0; q < 5; ++q) {
+        for (size_t i = 0; i < n; ++i)
+          src[i] = q == 0 ? ka[i] : q == 1 ? kb[i] : q == 2 ? ka[i] * ka[i] : q == 3 ? kb[i] * kb[i] : ka[i] * kb[i];
+        for (int y = 0; y < h; ++y)
+          for (int x = 0; x < w; ++x) {
+            double acc = 0.0;
+            for (int t = 0; t < kSsimTaps; ++t) {
+              const int xx = x - kSsimHalo + t;
+              acc = ssim_fma(ssim_tap(t), xx >= 0 && xx < w ? src[(size_t)y * w + xx] : 0.0, acc);
+            }
+            hsum[(size_t)y * w + x] = acc;
+          }
+        for (int y = 0; y < h; ++y)
+          for (int x = 0; x < w; ++x) {
+            double acc = 0.0;
+            for (int t = 0; t < kSsimTaps; ++t) {
+              const int yy = y - kSsimHalo + t;
+              acc = ssim_fma(ssim_tap(t), yy >= 0 && yy < h ? hsum[(size_t)yy * w + x] : 0.0, acc);
+            }
+            sums[q][(size_t)y * w + x] = acc;
+          }
+      }
+      for (size_t i = 0; i < n; ++i) {
+        const double m = ssim_map_value(sums[0][i], sums[1][i], sums[2][i], sums[3][i], sums[4][i]);
+        if (p < C) {
+          tot_rgb += m;
+          if (map_rgb) map_rgb[((size_t)img * C + p) * n + i] = m;
+        } else {
+          tot_y += m;
+          if (map_y) map_y[(size_t)img * n + i] = m;
+        }
+      }
+    }
+    ssim_rgb[img] = tot_rgb / ((double)n * C);
+    if (ssim_y) ssim_y[img] = C == 3 ? tot_y / (double)n : ssim_rgb[img];
+  }
+  return GRL_OK;
+}
 
 }  // namespace grl

@@ -69,6 +69,13 @@ int launch_psnr(const float* restored, const float* target, int B, int C, int H,
 size_t psnrb_workspace(int B);
 int launch_psnrb(const float* restored, const float* target, int B, int C, int H, int W, unsigned long long* workspace,
                  double* psnrb_rgb, double* psnrb_y, cudaStream_t st);
+// SSIM, RGB and luma, one tile kernel + a finalize (metric.cu, grl_ssim.h); ssim_host is the same computation on the CPU
+size_t ssim_workspace(int B, int C, int H, int W, int border);
+int launch_ssim(const float* restored, const float* target, int B, int C, int H, int W, int border, void* workspace,
+                size_t workspace_bytes, double* ssim_rgb, double* ssim_y, double* map_rgb, double* map_y, cudaStream_t st);
+void ssim_taps(double* t11);
+int ssim_host(const float* restored, const float* target, int B, int C, int H, int W, int border, double* ssim_rgb,
+              double* ssim_y, double* map_rgb, double* map_y);
 // NIQE features: luma, MSCN, x0.5 resize, per-block AGGD features (niqe.cu)
 void niqe_half_taps(float* w8);
 size_t niqe_ws(int B, int H, int W, int border);

@@ -3,9 +3,9 @@
 Reference: engines/base.py:255-268 (round -> shave for SR -> metrics), utils/utils_image.py:8-11 (shave), :30-33
 (tensor_round), :43-80 (rgb2ycbcr, MATLAB coefficients, rounded to 8 bit), utils/metrics/psnr.py:44-48 (psnr),
 utils/metrics/ssim.py:17-82 (Gaussian-window SSIM, 11 taps, sigma 1.5, taps rounded to 6 decimals, zero padding).
-psnr_fused() is the hand-written kernel (csrc/metric.cu, grl_psnr_f32) the benchmarked validation step uses for PSNR
-(RGB and luma); the torch-op functions below define the same quantities on any device (SSIM stays torch ops) and are
-what the CPU tests pin against the reference's own functions.
+psnr_fused() and ssim_fused() are the hand-written kernels (csrc/metric.cu, grl_psnr_f32 and grl_ssim_f32) behind
+validation_metrics_fused(), the validation step's four numbers without torch math on the images; the torch-op functions
+below define the same quantities on any device and are what the CPU tests pin against the reference's own functions.
 """
 import math
 
@@ -82,6 +82,27 @@ def ssim(restored, target, border=0, channel="rgb", window_size=11, sigma=1.5):
     c1, c2 = 0.01**2, 0.03**2
     ssim_map = ((2 * mu_a * mu_b + c1) * (2 * cov + c2)) / ((mu_a.pow(2) + mu_b.pow(2) + c1) * (var_a + var_b + c2))
     return ssim_map.mean([-3, -2, -1])
+
+
+def ssim_fused(restored, target, border=0):
+    """(ssim_rgb, ssim_y), each (B,) float64, from one fused kernel over CUDA fp32 (B, C, H, W) images, C = 1 or 3
+    (csrc/metric.cu, grl_ssim_f32): tensor_round + shave + luma + separable float64 window sums on the 8-bit integers;
+    ssim_y is a copy of ssim_rgb for C = 1."""
+    from . import capi
+
+    capi.require_device(restored)
+    capi.require_device(target)
+    if restored.shape != target.shape or restored.dim() != 4:
+        raise RuntimeError(f"grl_b200: ssim_fused needs two (B, C, H, W) tensors of one shape, got {tuple(restored.shape)} / {tuple(target.shape)}")
+    a = restored if (restored.dtype == torch.float32 and restored.is_contiguous()) else restored.float().contiguous()
+    b = target if (target.dtype == torch.float32 and target.is_contiguous()) else target.float().contiguous()
+    B, C, H, W = a.shape
+    nbytes = capi.lib().grl_ssim_workspace(B, C, H, W, int(border))
+    ws = torch.empty(max(nbytes // 8, 1), device=a.device, dtype=torch.float64)
+    out = torch.empty(2, B, device=a.device, dtype=torch.float64)
+    capi.check(capi.lib().grl_ssim_f32(capi.ptr(a), capi.ptr(b), B, C, H, W, int(border), capi.ptr(ws), ws.numel() * 8,
+                                       capi.ptr(out[0]), capi.ptr(out[1]), None, None, capi.stream()))
+    return out[0], out[1]
 
 
 def _grid8(img):
@@ -295,3 +316,12 @@ def validation_metrics(restored, target, scale=1, is_sr=False):
         "ssim": ssim(restored, target, border, "rgb"),
         "ssim_y": ssim(restored, target, border, "y"),
     }
+
+
+def validation_metrics_fused(restored, target, scale=1, is_sr=False):
+    """validation_metrics from the two fused kernels, psnr_fused and ssim_fused, on CUDA images: the same four keys,
+    psnr / psnr_y as float32 and ssim / ssim_y as float64 (B,) tensors."""
+    border = scale if is_sr else 0
+    p, py = psnr_fused(restored, target, border)
+    s, sy = ssim_fused(restored, target, border)
+    return {"psnr": p, "psnr_y": py, "ssim": s, "ssim_y": sy}

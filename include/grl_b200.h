@@ -293,6 +293,26 @@ size_t grl_psnrb_workspace(int B);
 int grl_psnrb_f32(const float* restored, const float* target, int B, int C, int H, int W, void* workspace,
                   size_t workspace_bytes, double* psnrb_rgb, double* psnrb_y, void* stream);
 
+/* Per-image SSIM of the validation step (StructuralSimilarityIndexMeasure.update, utils/metrics/ssim.py:167-193 ->
+ * ssim / _ssim, ssim.py:36-85, after engines/base.py:255-268): both images tensor_round'ed, `border` pixels shaved, local
+ * statistics under the 11-tap Gaussian window of gaussian(11, 1.5) (ssim.py:17-24) with zero padding and no
+ * renormalisation at the border, C1 = 1e-4, C2 = 9e-4, the mean of the map over channels and pixels.  restored / target:
+ * (B, C, H, W) fp32, C == 1 or 3, 2 * border < min(H, W).  ssim_y (may be NULL): the same on the luma of grl_psnr_f32 for
+ * C == 3, else a copy of ssim_rgb.  Both outputs are float64 (B,).  Arithmetic is float64 on the exact 8-bit integers and
+ * separable (csrc/grl_ssim.h); partial sums are combined in a fixed order, so two calls give the same bits and an image
+ * scores the same alone and in a batch.  map_rgb (B, C, H - 2 border, W - 2 border) and map_y (B, 1, ...; written for
+ * C == 3 only) receive the float64 SSIM map when not NULL.  workspace >= grl_ssim_workspace(...) bytes of device memory
+ * (0 for a shape the call refuses). */
+size_t grl_ssim_workspace(int B, int C, int H, int W, int border);
+int grl_ssim_f32(const float* restored, const float* target, int B, int C, int H, int W, int border, void* workspace,
+                 size_t workspace_bytes, double* ssim_rgb, double* ssim_y, double* map_rgb, double* map_y, void* stream);
+/* The 11 normalised float64 window taps (gaussian(11, 1.5), ssim.py:17-24); HOST pointer. */
+int grl_ssim_taps_host(double* taps11);
+/* grl_ssim_f32 on the CPU from the same closed form, HOST pointers; its maps equal the kernel's bit for bit.  Allocates
+ * host scratch of 8 planes of float64. */
+int grl_ssim_host(const float* restored, const float* target, int B, int C, int H, int W, int border, double* ssim_rgb,
+                  double* ssim_y, double* map_rgb, double* map_y);
+
 /* ---- NIQE features of the blind-SR test command (NaturalImageQualityEvaluator.update, utils/metrics/niqe.py:566-576) --
  * restored: (B, C = 3, H, W) fp32; the score is the multivariate-Gaussian distance of the features to the caller's
  * pristine model (metrics.niqe, batched torch float64).  The crop keeps (Hc, Wc) = 96 * floor((H - 2 border, W - 2 border)
