@@ -20,8 +20,6 @@
 #include <string.h>
 
 #include "grl_common.cuh"
-#include "ops_f32.h"
-#include "ops_tc.h"
 #include "attn_tc.cuh"
 #include "tc_common.cuh"
 
@@ -65,7 +63,7 @@ struct AttnMaps {
 };
 
 template <int KT, int KW, int VAR>
-__global__ void __launch_bounds__(kAttnThreads, 2) attn_tc_kernel(const __grid_constant__ AttnMaps tm, const AttnTcArgs a) {
+__global__ void __launch_bounds__(kAttnThreads, 2) attn_tc_kernel(const __grid_constant__ AttnMaps tm, const GrlTcAttn a) {
   static_assert(KT == 64, "S fragments of m64n64 products: one key tile per product");
   constexpr int NS = kAttnStages;
   extern __shared__ uint8_t smem_raw[];
@@ -121,7 +119,7 @@ __global__ void __launch_bounds__(kAttnThreads, 2) attn_tc_kernel(const __grid_c
           const int qi = qt * kQT + r;
           const bool ok = qi < Nq;
           const Tok tq = locate(a.gq, wr, wc, ok ? qi : 0);
-          const __nv_bfloat16* src = a.q + ((long long)(b * a.gq.H + tq.y) * a.gq.W + tq.x) * a.ldq + a.q_off + h * kDP;
+          const __nv_bfloat16* src = static_cast<const __nv_bfloat16*>(a.q) + ((long long)(b * a.gq.H + tq.y) * a.gq.W + tq.x) * a.ldq + a.q_off + h * kDP;
           GRL_ROW_COPY(Qs, r, src, ok);
         }
       }
@@ -129,15 +127,15 @@ __global__ void __launch_bounds__(kAttnThreads, 2) attn_tc_kernel(const __grid_c
         const int kj = k0 + r;
         const bool ok = kj < Nk;
         const Tok tk = locate(a.gk, wr, wc, ok ? kj : 0);
-        const __nv_bfloat16* ksrc = a.k + ((long long)(b * a.gk.H + tk.y) * a.gk.W + tk.x) * a.ldk + a.k_off + h * kDP;
+        const __nv_bfloat16* ksrc = static_cast<const __nv_bfloat16*>(a.k) + ((long long)(b * a.gk.H + tk.y) * a.gk.W + tk.x) * a.ldk + a.k_off + h * kDP;
         if (!tma_k) GRL_ROW_COPY(Ks + buf * S::KV_BYTES, r, ksrc, ok);
         koff_s[buf * KT + r] = tk.ih * Wt + tk.iw;
         krid_s[buf * KT + r] = region_id(a.gk, tk.r, tk.c);
         const __nv_bfloat16* vsrc;
         if (a.v_dense) {
-          vsrc = a.v + (((long long)bw * a.heads + h) * Nk + (ok ? kj : 0)) * kDP;
+          vsrc = static_cast<const __nv_bfloat16*>(a.v) + (((long long)bw * a.heads + h) * Nk + (ok ? kj : 0)) * kDP;
         } else {
-          vsrc = a.v + ((long long)(b * a.gk.H + tk.y) * a.gk.W + tk.x) * a.ldv + a.v_off + h * kDP;
+          vsrc = static_cast<const __nv_bfloat16*>(a.v) + ((long long)(b * a.gk.H + tk.y) * a.gk.W + tk.x) * a.ldv + a.v_off + h * kDP;
         }
         if (!tma_v) GRL_ROW_COPY(Vs + buf * S::KV_BYTES, r, vsrc, ok);
       }
@@ -347,7 +345,7 @@ __global__ void __launch_bounds__(kAttnThreads, 2) attn_tc_kernel(const __grid_c
       const float inv = 1.0f / den;
       const long long off = dst_s[j];
       if (off >= 0) {
-        __nv_bfloat16* dst = a.out + off;
+        __nv_bfloat16* dst = static_cast<__nv_bfloat16*>(a.out) + off;
 #pragma unroll
         for (int i = 0; i < kDP / 8; ++i)
           *reinterpret_cast<uint32_t*>(dst + 8 * i + fc) =
@@ -358,7 +356,7 @@ __global__ void __launch_bounds__(kAttnThreads, 2) attn_tc_kernel(const __grid_c
 }
 
 template <int KT, int KW, int VAR>
-static int launch_attn_var(const AttnMaps& tm, const AttnTcArgs& a, unsigned nblk, cudaStream_t st) {
+static int launch_attn_var(const AttnMaps& tm, const GrlTcAttn& a, unsigned nblk, cudaStream_t st) {
   auto kern = attn_tc_kernel<KT, KW, VAR>;
   // the attribute is per device: a process that drives several GPUs configures each one once
   static bool configured[kMaxDevices] = {false};
@@ -374,7 +372,7 @@ static int launch_attn_var(const AttnMaps& tm, const AttnTcArgs& a, unsigned nbl
 }
 
 template <int KT, int KW>
-static int launch_attn_one(const AttnMaps& tm, const AttnTcArgs& a, unsigned nblk, cudaStream_t st) {
+static int launch_attn_one(const AttnMaps& tm, const GrlTcAttn& a, unsigned nblk, cudaStream_t st) {
   switch ((a.fmt == FMT_BF16 ? 1 : 0) | (a.ones_col ? 2 : 0)) {
     case 0: return launch_attn_var<KT, KW, 0>(tm, a, nblk, st);
     case 1: return launch_attn_var<KT, KW, 1>(tm, a, nblk, st);
@@ -385,7 +383,7 @@ static int launch_attn_one(const AttnMaps& tm, const AttnTcArgs& a, unsigned nbl
 
 // Tokens per TMA box for a window of width ww rolled by sw: the largest power of two <= 64 dividing gcd(ww, sw) (ww if the
 // grid is not rolled horizontally).  0 = no usable box (runs shorter than 8 tokens = 512 bytes, the 64-byte-swizzle repeat).
-int attn_tma_box_tokens(const GrlGrid& g) {
+static int attn_tma_box_tokens(const GrlGrid& g) {
   int d = g.ww;
   if (g.sw > 0) {
     int x = g.ww, y = g.sw;
@@ -398,18 +396,6 @@ int attn_tma_box_tokens(const GrlGrid& g) {
   int bw = 64;
   while (bw > 1 && d % bw) bw >>= 1;
   return bw >= 8 ? bw : 0;
-}
-
-int attn_variant(int set) {
-  static int variant = -1;
-  if (variant < 0) {
-    // default 5: TMA boxes wherever the geometry has them; GRL_ATTN_SPLIT=0 gathers every operand row by row
-    const char* e = getenv("GRL_ATTN_SPLIT");
-    variant = (e && atoi(e) == 0) ? 0 : 5;
-  }
-  const int prev = variant;
-  if (set == 0 || set == 5) variant = set;
-  return prev;
 }
 
 // (B * H * W tokens, ld) 16-bit tensor map with {32 channels, box tokens} boxes; false: no usable map (box 0 then)
@@ -425,7 +411,43 @@ static bool token_map(CUtensorMap* m, const void* base, long long ld, long long 
             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-int launch_attn_tc(const AttnTcArgs& a, cudaStream_t st) {
+}  // namespace tc
+}  // namespace grl
+
+using namespace grl;
+using namespace grl::tc;
+
+extern "C" {
+
+int grl_tc_attn_box_tokens(GrlGrid g) {
+  if (check_grid(g, "attn_box_tokens") != GRL_OK) return 0;
+  return attn_tma_box_tokens(g);
+}
+
+int grl_tc_attn_variant(int set) {
+  static int variant = -1;
+  if (variant < 0) {
+    // default 5: TMA boxes wherever the geometry has them; GRL_ATTN_SPLIT=0 gathers every operand row by row
+    const char* e = getenv("GRL_ATTN_SPLIT");
+    variant = (e && atoi(e) == 0) ? 0 : 5;
+  }
+  const int prev = variant;
+  if (set == 0 || set == 5) variant = set;
+  return prev;
+}
+
+int grl_tc_attn(const GrlTcAttn* p, void* stream) {
+  GRL_REQUIRE(p != nullptr, "tc_attn: null problem");
+  if (!grl_device_ok()) return fail(GRL_ERR_ARCH, "tc_attn: wgmma kernels need an sm_90 device");
+  const GrlTcAttn& a = *p;
+  if (check_fmt(a.fmt)) return GRL_ERR_INVALID;
+  GRL_REQUIRE((a.ldq % 8) == 0 && (a.ldk % 8) == 0 && (a.v_dense || (a.ldv % 8) == 0) &&
+                  (a.o_dense || (a.ldo % 8) == 0) && (a.q_off % 8) == 0 && (a.k_off % 8) == 0 &&
+                  (a.v_off % 8) == 0 && (a.o_off % 8) == 0,
+              "tc_attn: pitches and offsets must be multiples of 8 elements (16 bytes)");
+  GRL_REQUIRE(a.rows == (a.gq.wh + a.gk.wh - 1) * (a.gq.ww + a.gk.ww - 1), "tc_attn: bias table has %d rows, expected %d",
+              a.rows, (a.gq.wh + a.gk.wh - 1) * (a.gq.ww + a.gk.ww - 1));
+  const cudaStream_t st = (cudaStream_t)stream;
   if (a.B == 0) return GRL_OK;
   int rc;
   if ((rc = check_grid(a.gq, "attn_tc(q grid)")) != GRL_OK) return rc;
@@ -440,7 +462,7 @@ int launch_attn_tc(const AttnTcArgs& a, cudaStream_t st) {
   GRL_REQUIRE(nblk < (1ll << 31), "attn_tc: grid too large");
   AttnMaps tm;
   memset(&tm, 0, sizeof(tm));
-  if (attn_variant(-1) == 5) {
+  if (grl_tc_attn_variant(-1) == 5) {
     const long long nq = (long long)a.B * a.gq.H * a.gq.W, nk = (long long)a.B * a.gk.H * a.gk.W;
     tm.box_q = attn_tma_box_tokens(a.gq);
     tm.box_k = attn_tma_box_tokens(a.gk);
@@ -460,5 +482,4 @@ int launch_attn_tc(const AttnTcArgs& a, cudaStream_t st) {
   }
 }
 
-}  // namespace tc
-}  // namespace grl
+}  // extern "C"

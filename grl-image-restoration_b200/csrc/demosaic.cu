@@ -7,7 +7,6 @@
 // 128-byte row segment.
 #include "grl_common.cuh"
 #include "grl_demosaic.h"
-#include "ops_f32.h"
 
 namespace grl {
 
@@ -58,15 +57,32 @@ __global__ void __launch_bounds__(kThreadsX * kThreadsY) demosaic_kernel(const f
 
 }  // namespace
 
-int launch_demosaic(const float* cfa4, int B, int h, int w, float* out, cudaStream_t st) {
+}  // namespace grl
+
+using namespace grl;
+
+extern "C" {
+
+int grl_demosaic_host(const float* cfa4, int B, int h, int w, float* out) {
+  GRL_REQUIRE(cfa4 && out && B >= 0 && h >= 2 && w >= 2, "demosaic_host: bad arguments B=%d h=%d w=%d", B, h, w);
+  const int H = 2 * h, W = 2 * w;
+  for (int b = 0; b < B; ++b)
+    for (int c = 0; c < 3; ++c)
+      for (int y = 0; y < H; ++y)
+        for (int x = 0; x < W; ++x)
+          out[(((size_t)b * 3 + c) * H + y) * W + x] = dm_pixel(cfa4 + (size_t)b * 4 * h * w, h, w, c, y, x);
+  return GRL_OK;
+}
+
+int grl_demosaic_f32(const float* cfa4, int B, int h, int w, float* out, void* stream) {
   GRL_REQUIRE(cfa4 && out, "demosaic: null argument");
   GRL_REQUIRE(B > 0 && h >= 2 && w >= 2, "demosaic: packed RGGB planes must be (B, 4, h, w) with B >= 1 and h, w >= 2, got "
               "B=%d h=%d w=%d", B, h, w);
   GRL_REQUIRE(B <= 65535 && 2LL * h <= 0x7fffffffLL / (2LL * w), "demosaic: shape out of range (B=%d h=%d w=%d)", B, h, w);
   const dim3 grid(ceil_div(2 * w, kTX), ceil_div(2 * h, kTY), B);
-  demosaic_kernel<<<grid, dim3(kThreadsX, kThreadsY), 0, st>>>(cfa4, h, w, out);
+  demosaic_kernel<<<grid, dim3(kThreadsX, kThreadsY), 0, (cudaStream_t)stream>>>(cfa4, h, w, out);
   GRL_LAUNCH_CHECK("demosaic_kernel");
   return GRL_OK;
 }
 
-}  // namespace grl
+}  // extern "C"

@@ -6,7 +6,6 @@
 // the matching global loads walk a column, so those go through a padded shared-memory tile that is loaded row-wise and
 // read column-wise (stride 33 floats: no bank conflicts).  The flips only reverse the order inside a row.
 #include "grl_common.cuh"
-#include "ops_f32.h"
 
 namespace grl {
 
@@ -91,25 +90,51 @@ int check_planes(int B, int C, int H, int W, const char* what) {
 
 }  // namespace
 
-int launch_ens_gather(const float* x, int B, int C, int H, int W, int group, float* views, cudaStream_t st) {
+}  // namespace grl
+
+using namespace grl;
+
+extern "C" {
+
+int grl_d8_index_host(int mode, int H, int W, int inverse, int32_t* out) {
+  GRL_REQUIRE(mode >= 0 && mode < 8 && H > 0 && W > 0 && (long long)H * W <= 0x7fffffffLL && out,
+              "d8_index: bad arguments mode=%d H=%d W=%d", mode, H, W);
+  const int Hv = d8_transposes(mode) ? W : H, Wv = d8_transposes(mode) ? H : W;
+  if (!inverse) {
+    for (int y = 0; y < Hv; ++y)
+      for (int x = 0; x < Wv; ++x) {
+        const Pix p = d8_src(mode, y, x, H, W);
+        out[(size_t)y * Wv + x] = p.y * W + p.x;
+      }
+  } else {
+    for (int y = 0; y < H; ++y)
+      for (int x = 0; x < W; ++x) {
+        const Pix p = d8_inv(mode, y, x, H, W);
+        out[(size_t)y * W + x] = p.y * Wv + p.x;
+      }
+  }
+  return GRL_OK;
+}
+
+int grl_ens_gather_f32(const float* x, int B, int C, int H, int W, int group, float* views, void* stream) {
   GRL_REQUIRE(x && views, "ens_gather: null argument");
   GRL_REQUIRE(group == 0 || group == 1, "ens_gather: group must be 0 (modes 0,2,4,6) or 1 (modes 1,3,5,7), got %d", group);
   int rc = check_planes(B, C, H, W, "ens_gather");
   if (rc != GRL_OK) return rc;
   const dim3 grid(ceil_div(W, kTile), ceil_div(H, kTile), B * C);
-  ens_gather_kernel<<<grid, dim3(kTile, kRows), 0, st>>>(x, B, C, H, W, group, views);
+  ens_gather_kernel<<<grid, dim3(kTile, kRows), 0, (cudaStream_t)stream>>>(x, B, C, H, W, group, views);
   GRL_LAUNCH_CHECK("ens_gather_kernel");
   return GRL_OK;
 }
 
-int launch_ens_merge(const float* ya, const float* yb, int B, int C, int Hs, int Ws, float* y, cudaStream_t st) {
+int grl_ens_merge_f32(const float* ya, const float* yb, int B, int C, int Hs, int Ws, float* y, void* stream) {
   GRL_REQUIRE(ya && yb && y, "ens_merge: null argument");
   int rc = check_planes(B, C, Hs, Ws, "ens_merge");
   if (rc != GRL_OK) return rc;
   const dim3 grid(ceil_div(Ws, kTile), ceil_div(Hs, kTile), B * C);
-  ens_merge_kernel<<<grid, dim3(kTile, kRows), 0, st>>>(ya, yb, B, C, Hs, Ws, y);
+  ens_merge_kernel<<<grid, dim3(kTile, kRows), 0, (cudaStream_t)stream>>>(ya, yb, B, C, Hs, Ws, y);
   GRL_LAUNCH_CHECK("ens_merge_kernel");
   return GRL_OK;
 }
 
-}  // namespace grl
+}  // extern "C"

@@ -24,7 +24,6 @@
 
 #include "grl_common.cuh"
 #include "tc_common.cuh"
-#include "ops_tc.h"
 
 namespace grl {
 namespace tc {
@@ -141,9 +140,20 @@ __device__ __forceinline__ void mma_loop(float (&acc)[BN / 64][32], uint8_t* sme
   wgmma_wait<0>();
 }
 
+// What the host derives from a GrlTcGemm for its launch (plan_gemm_tc); the kernel takes both.
+struct GemmTcPlan {
+  long long M;   // rows: GrlTcGemm::M, or B * H * W for a conv
+  int nk;        // 64-wide k chunks per tap
+  int n_tiles, total_tiles;
+  int tiles_x, tiles_y;  // conv: 8 x 16 pixel patches per image
+  int epi_mode;  // 0 = 16-bit staging, 1 = fp32 staging, 2 = direct
+  int nchw_r;    // GrlTcGemm::nchw_r, at least 1
+};
+
 template <int BN, int EPI, bool CONV>
 __global__ void __launch_bounds__(kThreads, 1)
-gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmTcArgs a) {
+gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GrlTcGemm a,
+              const GemmTcPlan pl) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   using S = GemmSmem<BN>;
@@ -161,17 +171,17 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   // 1-D grid, N tile fastest: the CTAs that share an A tile (same rows, different output columns) are scheduled
   // together, so the tile is read from DRAM once and from L2 afterwards (QKV: 3 column tiles, fc1: 2).
-  const int n_tiles = a.n_tiles;
+  const int n_tiles = pl.n_tiles;
   const int m_idx = blockIdx.x / n_tiles;
   const int n0 = (blockIdx.x - m_idx * n_tiles) * BN;
-  const int nk_total = a.taps * a.nk;
+  const int nk_total = a.taps * pl.nk;
   int m0 = 0, tb = 0, ty0 = 0, tx0 = 0;
   if (CONV) {
     int t = m_idx;
-    const int tx = t % a.tiles_x;
-    t /= a.tiles_x;
-    const int ty = t % a.tiles_y;
-    tb = t / a.tiles_y;
+    const int tx = t % pl.tiles_x;
+    t /= pl.tiles_x;
+    const int ty = t % pl.tiles_y;
+    tb = t / pl.tiles_y;
     ty0 = ty * kTH;
     tx0 = tx * kTW;
   } else {
@@ -199,7 +209,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         uint8_t* sb = sa + S::A_BYTES;
         mbar_expect_tx(&full[s], S::STAGE);
         if (CONV) {
-          const int tap = kc / a.nk, c0 = (kc - tap * a.nk) * kBK;
+          const int tap = kc / pl.nk, c0 = (kc - tap * pl.nk) * kBK;
           tma_load_4d(sa, &tmA, &full[s], c0, tx0 + (tap % 3) - 1, ty0 + (tap / 3) - 1, tb);
         } else {
           tma_load_2d(sa, &tmA, &full[s], kc * kBK, m0);
@@ -226,7 +236,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       tok = (y < a.H && x < a.W) ? ((long long)tb * a.H + y) * a.W + x : -1;
     } else {
       tok = (long long)m0 + row;
-      if (tok >= a.M) tok = -1;
+      if (tok >= pl.M) tok = -1;
     }
     if (half == 0) {
       s_tok[row] = tok;
@@ -234,7 +244,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     }
     for (int c = et; c < BN; c += kEpiThreads) {
       const int n = n0 + c;
-      s_bias[c] = (n < a.N) ? a.bias[n] : 0.f;
+      s_bias[c] = (n < a.n_store) ? a.bias[n] : 0.f;
       if (EPI == EPI_LN) {
         s_gamma[c] = (c < a.C) ? a.gamma[c] : 0.f;
         s_beta[c] = (c < a.C) ? a.beta[c] : 0.f;
@@ -266,10 +276,10 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 
     // epi_mode (chosen on the host): 1 = fp32 staging (LayerNorm / fp32 result / residual, whole row in this tile),
     // 0 = 16-bit staging, 2 = direct per-row stores (odd widths such as the 3-channel image head)
-    if (EPI == EPI_BIAS_ACT && a.epi_mode == 2) {
+    if (EPI == EPI_BIAS_ACT && pl.epi_mode == 2) {
       const long long tok = s_tok[row];
       for (int c0 = 32 * half; c0 < BN; c0 += 64) {
-        if (n0 + c0 >= a.N) break;
+        if (n0 + c0 >= a.n_store) break;
         acc_row32(accs + row * AP + c0, v);
         if (tok < 0) continue;
         float o[32];
@@ -277,17 +287,17 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         for (int j = 0; j < 32; ++j) {
           const int n = n0 + c0 + j;
           float val = tc_act(__uint_as_float(v[j]) + s_bias[c0 + j], a.act, a.slope);
-          if (a.res_f32 && n < a.N_f32) val += __ldg(a.res_f32 + tok * a.ldr + n);
-          o[j] = (n < a.N) ? val : 0.f;
-          if (a.out_f32 && n < a.N_f32) a.out_f32[tok * a.ldo_f32 + n] = o[j];
-          if (CONV && a.out_nchw && n < a.N_f32) {
+          if (a.res_f32 && n < a.n_real) val += __ldg(a.res_f32 + tok * a.ldr + n);
+          o[j] = (n < a.n_store) ? val : 0.f;
+          if (a.out_f32 && n < a.n_real) a.out_f32[tok * a.ldo_f32 + n] = o[j];
+          if (CONV && a.out_nchw && n < a.n_real) {
             // tail fusion: x / img_range + mean (grl.py:549), the crop (:551), channels-last -> bchw and, for the one-step
             // head, PixelShuffle (upsample.py:33-50; torch order n = c r^2 + dy r + dx) folded into the store
-            const int r = a.nchw_r, rr = r * r;
+            const int r = pl.nchw_r, rr = r * r;
             const int c = n / rr, q = n - c * rr;
             const int yy = (ty0 + row / kTW) * r + q / r, xx = (tx0 + row % kTW) * r + q % r;
             if (yy < a.Hc && xx < a.Wc)
-              a.out_nchw[(((long long)tb * (a.N_f32 / rr) + c) * a.Hc + yy) * a.Wc + xx] = fmaf(o[j], a.post_scale, a.post_shift[c & 3]);
+              a.out_nchw[(((long long)tb * (a.n_real / rr) + c) * a.Hc + yy) * a.Wc + xx] = fmaf(o[j], a.post_scale, a.post_shift[c & 3]);
           }
         }
         if (out16) {
@@ -299,8 +309,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                              pack16(o[j + 6], o[j + 7], fmt));
         }
       }
-    } else if (a.epi_mode == 1) {
-      const int Cw = (EPI == EPI_LN) ? a.C : a.N_f32;  // real fp32 columns of this tile row (n0 == 0 when wide)
+    } else if (pl.epi_mode == 1) {
+      const int Cw = (EPI == EPI_LN) ? a.C : a.n_real;  // real fp32 columns of this tile row (n0 == 0 when wide)
       const int pitch = stage_pitch32(Cw);
       float* stg = reinterpret_cast<float*>(smem + S::OFF_STG);
       // ---------------- residual tile -> staging, asynchronously (cp.async, 16 B per request, the whole 128 x C
@@ -443,7 +453,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       // ---------------- 16-bit outputs only: phase A packs into a [128][BN + 8] tile
       constexpr int P16 = BN + 8;
       uint16_t* stg = reinterpret_cast<uint16_t*>(smem + S::OFF_STG);
-      const int ncols = min(BN, a.N - n0);  // columns of this tile that exist (multiple of 32)
+      const int ncols = min(BN, a.n_store - n0);  // columns of this tile that exist (multiple of 32)
       for (int c0 = 32 * half; c0 < ncols; c0 += 64) {
         acc_row32(accs + row * AP + c0, v);
         float o[32];
@@ -471,13 +481,13 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                          pack16(o[j + 6], o[j + 7], fmt));
       }
       epi_barrier();
-      const int nvec = min((long long)ncols, a.ldo_bf16 - n0) >> 3;  // 16-byte vectors per row
+      const int nvec = min((long long)ncols, (long long)a.ldo_bf16 - n0) >> 3;  // 16-byte vectors per row
       const int ew = et >> 5;
       if (CONV && a.ps_r > 0) {
         // PixelShuffle folded into the store (upsample.py:6-30): the weights are packed so that column n' = q * Cq + c
         // holds torch's channel c r^2 + q, i.e. Cq consecutive columns are ONE output pixel's channels
-        const int ps = a.ps_r, Cq = a.N / (ps * ps);
-        const int nv = min(BN, a.N - n0) >> 3;
+        const int ps = a.ps_r, Cq = a.n_store / (ps * ps);
+        const int nv = min(BN, a.n_store - n0) >> 3;
 #pragma unroll 4
         for (int r = ew; r < kBM; r += kEpiWarps) {
           if (s_tok[r] < 0) continue;
@@ -518,7 +528,8 @@ static int make_map(CUtensorMap* m, const void* base, int rank, const cuuint64_t
 }
 
 template <int BN, int EPI, bool CONV>
-static int launch_one(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmTcArgs& a, dim3 grid, cudaStream_t st) {
+static int launch_one(const CUtensorMap& tmA, const CUtensorMap& tmB, const GrlTcGemm& a, const GemmTcPlan& pl, dim3 grid,
+                      cudaStream_t st) {
   auto kern = gemm_tc_kernel<BN, EPI, CONV>;
   // the attribute is per device: a process that drives several GPUs configures each one once
   static bool configured[kMaxDevices] = {false};
@@ -528,24 +539,24 @@ static int launch_one(const CUtensorMap& tmA, const CUtensorMap& tmB, const Gemm
     GRL_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmSmem<BN>::TOTAL));
     if (dev >= 0 && dev < kMaxDevices) configured[dev] = true;
   }
-  kern<<<grid, kThreads, GemmSmem<BN>::TOTAL, st>>>(tmA, tmB, a);
+  kern<<<grid, kThreads, GemmSmem<BN>::TOTAL, st>>>(tmA, tmB, a, pl);
   GRL_LAUNCH_CHECK("gemm_tc_kernel");
   return GRL_OK;
 }
 
 template <int EPI, bool CONV>
-static int dispatch_bn(int bn, const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmTcArgs& a, dim3 grid,
-                       cudaStream_t st) {
+static int dispatch_bn(int bn, const CUtensorMap& tmA, const CUtensorMap& tmB, const GrlTcGemm& a, const GemmTcPlan& pl,
+                       dim3 grid, cudaStream_t st) {
   switch (bn) {
-    case 64: return launch_one<64, EPI, CONV>(tmA, tmB, a, grid, st);
-    case 128: return launch_one<128, EPI, CONV>(tmA, tmB, a, grid, st);
-    case 192: return launch_one<192, EPI, CONV>(tmA, tmB, a, grid, st);
-    case 256: return launch_one<256, EPI, CONV>(tmA, tmB, a, grid, st);
+    case 64: return launch_one<64, EPI, CONV>(tmA, tmB, a, pl, grid, st);
+    case 128: return launch_one<128, EPI, CONV>(tmA, tmB, a, pl, grid, st);
+    case 192: return launch_one<192, EPI, CONV>(tmA, tmB, a, pl, grid, st);
+    case 256: return launch_one<256, EPI, CONV>(tmA, tmB, a, pl, grid, st);
   }
   return fail(GRL_ERR_INVALID, "gemm_tc: unsupported tile width %d", bn);
 }
 
-int pick_bn(int npad) {
+static int pick_bn(int npad) {
   if (npad <= 64) return 64;
   if (npad <= 128) return 128;
   if (npad % 192 == 0 || npad <= 192) return 192;
@@ -553,90 +564,121 @@ int pick_bn(int npad) {
   return npad % 128 == 0 ? 128 : 192;
 }
 
-// Host-side launch selection, shared by launch_gemm_tc and grl_tc_gemm_path (so the path a test asks about is the path
-// that runs): validates the problem, sets the launch fields of `a` (epi_mode, nk, taps, M, conv tiling, n_tiles,
-// total_tiles = grid) and returns the N tile width in *bn.  Needs no device.
-int plan_gemm_tc(const GemmTcProblem& p, GemmTcArgs& a, int* bn_out) {
+// Host-side validation and launch selection, shared by grl_tc_gemm and grl_tc_gemm_path (so the path a test asks about is
+// the path that runs): checks every argument of p but its null test, fills the plan (epi_mode, nk, M, conv tiling,
+// n_tiles, total_tiles = grid) and returns the N tile width in *bn.  Needs no device.
+static int plan_gemm_tc(const GrlTcGemm& p, GemmTcPlan& pl, int* bn_out) {
+  pl = GemmTcPlan{};
+  pl.nchw_r = p.nchw_r > 0 ? p.nchw_r : 1;
+  if (check_fmt(p.fmt)) return GRL_ERR_INVALID;
+  GRL_REQUIRE(p.bias != nullptr, "tc_gemm: bias is required (pass zeros)");
+  GRL_REQUIRE(p.n_store <= p.npad && p.n_real <= p.npad, "tc_gemm: n_store/n_real exceed npad");
+  if (p.epi == EPI_QKV) GRL_REQUIRE(p.slot_scale && p.out_bf16 && p.ldo_bf16 >= p.npad, "tc_gemm: QKV epilogue arguments");
+  if (p.epi == EPI_LN)
+    GRL_REQUIRE(p.gamma && p.beta && p.res_f32 && p.out_f32 && p.out_bf16 && p.C > 0 && p.C <= p.npad &&
+                    p.L > 0 && (p.ldo_f32 % 4) == 0 && (p.ldo_bf16 % 8) == 0,
+                "tc_gemm: LN epilogue arguments");
+  if (p.out_bf16) GRL_REQUIRE((p.ldo_bf16 % 8) == 0, "tc_gemm: bf16 output pitch must be a multiple of 8");
   GRL_REQUIRE(p.kpad % kBK == 0 && p.kpad > 0, "gemm_tc: K pad %d must be a multiple of 64", p.kpad);
   GRL_REQUIRE(p.npad % 32 == 0 && p.npad > 0, "gemm_tc: N pad %d must be a multiple of 32", p.npad);
   int bn = (p.epi == EPI_LN) ? (p.npad <= 64 ? 64 : p.npad <= 128 ? 128 : p.npad <= 192 ? 192 : 256) : pick_bn(p.npad);
   GRL_REQUIRE(p.epi != EPI_LN || p.npad <= 256, "gemm_tc: LayerNorm epilogue needs the whole row in one tile (N=%d)",
               p.npad);
   const bool conv = p.taps == 9;
-  if (a.ps_r > 0)
-    GRL_REQUIRE(conv && p.epi == EPI_BIAS_ACT && !a.out_f32 && !a.res_f32 && a.out_bf16 && a.N % (a.ps_r * a.ps_r) == 0 &&
-                    (a.N / (a.ps_r * a.ps_r)) % 8 == 0 && a.ldo_bf16 >= a.N / (a.ps_r * a.ps_r),
+  if (p.ps_r > 0)
+    GRL_REQUIRE(conv && p.epi == EPI_BIAS_ACT && !p.out_f32 && !p.res_f32 && p.out_bf16 && p.n_store % (p.ps_r * p.ps_r) == 0 &&
+                    (p.n_store / (p.ps_r * p.ps_r)) % 8 == 0 && p.ldo_bf16 >= p.n_store / (p.ps_r * p.ps_r),
                 "gemm_tc: pixel-shuffle store needs a 16-bit-only conv epilogue with N %% r^2 == 0 and N / r^2 %% 8 == 0");
-  if (a.out_nchw)
-    GRL_REQUIRE(conv && p.epi == EPI_BIAS_ACT && a.nchw_r >= 1 && a.N_f32 % (a.nchw_r * a.nchw_r) == 0 &&
-                    a.N_f32 / (a.nchw_r * a.nchw_r) <= 4 && a.Hc > 0 && a.Wc > 0,
+  if (p.out_nchw)
+    GRL_REQUIRE(conv && p.epi == EPI_BIAS_ACT && pl.nchw_r >= 1 && p.n_real % (pl.nchw_r * pl.nchw_r) == 0 &&
+                    p.n_real / (pl.nchw_r * pl.nchw_r) <= 4 && p.Hc > 0 && p.Wc > 0,
                 "gemm_tc: NCHW tail store needs a conv with <= 4 output channels");
   GRL_REQUIRE(p.taps == 1 || p.taps == 9, "gemm_tc: taps must be 1 or 9");
   // Epilogue mode.  fp32 staging (LayerNorm, fp32 output, residual) needs the whole output row in one tile, 16-byte
   // aligned fp32 rows and a tile that fits the staging area; anything else with an fp32 side takes the direct path.
-  a.epi_mode = 0;
-  if (p.epi == EPI_LN || (p.epi == EPI_BIAS_ACT && (a.out_f32 || a.res_f32))) {
-    const int cw = p.epi == EPI_LN ? a.C : a.N_f32;
+  pl.epi_mode = 0;
+  if (p.epi == EPI_LN || (p.epi == EPI_BIAS_ACT && (p.out_f32 || p.res_f32))) {
+    const int cw = p.epi == EPI_LN ? p.C : p.n_real;
     const int cap = bn == 64 ? GemmSmem<64>::STG : bn == 128 ? GemmSmem<128>::STG : bn == 192 ? GemmSmem<192>::STG
                                                                                                : GemmSmem<256>::STG;
     const bool ok = p.npad <= bn && cw > 0 && cw % 4 == 0 && kBM * stage_pitch32(cw) * 4 <= cap &&
-                    (!a.out_f32 || a.ldo_f32 % 4 == 0) && (!a.res_f32 || a.ldr % 4 == 0) &&
-                    (!a.out_bf16 || a.ldo_bf16 % 4 == 0);
+                    (!p.out_f32 || p.ldo_f32 % 4 == 0) && (!p.res_f32 || p.ldr % 4 == 0) &&
+                    (!p.out_bf16 || p.ldo_bf16 % 4 == 0);
     GRL_REQUIRE(ok || p.epi != EPI_LN, "gemm_tc: LayerNorm epilogue needs C %% 4 == 0 and C <= 188 (got %d)", cw);
-    a.epi_mode = ok ? 1 : 2;
+    pl.epi_mode = ok ? 1 : 2;
   }
-  if (a.out_nchw) a.epi_mode = 2;
+  if (p.out_nchw) pl.epi_mode = 2;
   GRL_REQUIRE(p.epi == EPI_BIAS_ACT || p.epi == EPI_QKV || p.epi == EPI_LN, "gemm_tc: unknown epilogue %d", p.epi);
   GRL_REQUIRE(!conv || p.epi == EPI_BIAS_ACT, "gemm_tc: %s epilogue is linear-only", p.epi == EPI_QKV ? "QKV" : "LN");
-  a.nk = p.kpad / kBK;
-  a.taps = p.taps;
-  a.n_tiles = ceil_div(p.npad, bn);
+  pl.nk = p.kpad / kBK;
+  pl.n_tiles = ceil_div(p.npad, bn);
   if (conv) {
-    a.H = p.H, a.W = p.W;
-    a.tiles_x = ceil_div(p.W, kTW), a.tiles_y = ceil_div(p.H, kTH);
-    a.M = (long long)p.B * p.H * p.W;
-    GRL_REQUIRE((long long)a.tiles_x * a.tiles_y * p.B * a.n_tiles < (1ll << 31), "gemm_tc: grid too large");
-    a.total_tiles = a.tiles_x * a.tiles_y * p.B * a.n_tiles;
+    pl.tiles_x = ceil_div(p.W, kTW), pl.tiles_y = ceil_div(p.H, kTH);
+    pl.M = (long long)p.B * p.H * p.W;
+    GRL_REQUIRE((long long)pl.tiles_x * pl.tiles_y * p.B * pl.n_tiles < (1ll << 31), "gemm_tc: grid too large");
+    pl.total_tiles = pl.tiles_x * pl.tiles_y * p.B * pl.n_tiles;
   } else {
-    a.M = p.M;
-    GRL_REQUIRE((long long)ceil_div(p.M, kBM) * a.n_tiles < (1ll << 31), "gemm_tc: grid too large");
-    a.total_tiles = (int)(ceil_div(p.M, kBM) * a.n_tiles);
+    pl.M = p.M;
+    GRL_REQUIRE((long long)ceil_div(p.M, kBM) * pl.n_tiles < (1ll << 31), "gemm_tc: grid too large");
+    pl.total_tiles = (int)(ceil_div(p.M, kBM) * pl.n_tiles);
   }
   *bn_out = bn;
   return GRL_OK;
 }
 
-// x: bf16 (M, Kpad) row-major or (B, H, W, Kpad) channels-last; w: bf16 (Npad, taps*Kpad) K-major.
-int launch_gemm_tc(const GemmTcProblem& p, GemmTcArgs a, cudaStream_t st) {
-  int bn = 0, rc;
-  if ((rc = plan_gemm_tc(p, a, &bn)) != GRL_OK) return rc;
-  if (a.M == 0) return GRL_OK;
-  CUtensorMap tmA, tmB;
-  if (p.taps == 9) {
-    cuuint64_t dims[4] = {(cuuint64_t)p.kpad, (cuuint64_t)p.W, (cuuint64_t)p.H, (cuuint64_t)p.B};
-    cuuint64_t str[3] = {(cuuint64_t)p.kpad * 2, (cuuint64_t)p.W * p.kpad * 2, (cuuint64_t)p.H * p.W * p.kpad * 2};
-    cuuint32_t box[4] = {(cuuint32_t)kBK, (cuuint32_t)kTW, (cuuint32_t)kTH, 1};
-    if ((rc = make_map(&tmA, p.x, 4, dims, str, box, a.fmt)) != GRL_OK) return rc;
-  } else {
-    cuuint64_t dims[2] = {(cuuint64_t)p.kpad, (cuuint64_t)p.M};
-    cuuint64_t str[1] = {(cuuint64_t)p.kpad * 2};
-    cuuint32_t box[2] = {(cuuint32_t)kBK, (cuuint32_t)kBM};
-    if ((rc = make_map(&tmA, p.x, 2, dims, str, box, a.fmt)) != GRL_OK) return rc;
-  }
-  {
-    cuuint64_t dims[2] = {(cuuint64_t)p.kpad * p.taps, (cuuint64_t)p.npad};
-    cuuint64_t str[1] = {(cuuint64_t)p.kpad * p.taps * 2};
-    cuuint32_t box[2] = {(cuuint32_t)kBK, (cuuint32_t)bn};
-    if ((rc = make_map(&tmB, p.w, 2, dims, str, box, a.fmt)) != GRL_OK) return rc;
-  }
-  const dim3 grid((unsigned)a.total_tiles);
-  switch (p.epi) {
-    case EPI_QKV: return dispatch_bn<EPI_QKV, false>(bn, tmA, tmB, a, grid, st);
-    case EPI_LN: return dispatch_bn<EPI_LN, false>(bn, tmA, tmB, a, grid, st);
-  }
-  return p.taps == 9 ? dispatch_bn<EPI_BIAS_ACT, true>(bn, tmA, tmB, a, grid, st)
-                     : dispatch_bn<EPI_BIAS_ACT, false>(bn, tmA, tmB, a, grid, st);
-}
-
 }  // namespace tc
 }  // namespace grl
+
+using namespace grl;
+using namespace grl::tc;
+
+extern "C" {
+
+// x: bf16 (M, Kpad) row-major or (B, H, W, Kpad) channels-last; w: bf16 (Npad, taps*Kpad) K-major.
+int grl_tc_gemm(const GrlTcGemm* p, void* stream) {
+  GRL_REQUIRE(p != nullptr, "tc_gemm: null problem");
+  if (!grl_device_ok()) return fail(GRL_ERR_ARCH, "tc_gemm: wgmma kernels need an sm_90 device");
+  GemmTcPlan pl;
+  int bn = 0, rc;
+  if ((rc = plan_gemm_tc(*p, pl, &bn)) != GRL_OK) return rc;
+  if (pl.M == 0) return GRL_OK;
+  CUtensorMap tmA, tmB;
+  if (p->taps == 9) {
+    cuuint64_t dims[4] = {(cuuint64_t)p->kpad, (cuuint64_t)p->W, (cuuint64_t)p->H, (cuuint64_t)p->B};
+    cuuint64_t str[3] = {(cuuint64_t)p->kpad * 2, (cuuint64_t)p->W * p->kpad * 2, (cuuint64_t)p->H * p->W * p->kpad * 2};
+    cuuint32_t box[4] = {(cuuint32_t)kBK, (cuuint32_t)kTW, (cuuint32_t)kTH, 1};
+    if ((rc = make_map(&tmA, p->x, 4, dims, str, box, p->fmt)) != GRL_OK) return rc;
+  } else {
+    cuuint64_t dims[2] = {(cuuint64_t)p->kpad, (cuuint64_t)p->M};
+    cuuint64_t str[1] = {(cuuint64_t)p->kpad * 2};
+    cuuint32_t box[2] = {(cuuint32_t)kBK, (cuuint32_t)kBM};
+    if ((rc = make_map(&tmA, p->x, 2, dims, str, box, p->fmt)) != GRL_OK) return rc;
+  }
+  {
+    cuuint64_t dims[2] = {(cuuint64_t)p->kpad * p->taps, (cuuint64_t)p->npad};
+    cuuint64_t str[1] = {(cuuint64_t)p->kpad * p->taps * 2};
+    cuuint32_t box[2] = {(cuuint32_t)kBK, (cuuint32_t)bn};
+    if ((rc = make_map(&tmB, p->w, 2, dims, str, box, p->fmt)) != GRL_OK) return rc;
+  }
+  const dim3 grid((unsigned)pl.total_tiles);
+  const cudaStream_t st = (cudaStream_t)stream;
+  switch (p->epi) {
+    case EPI_QKV: return dispatch_bn<EPI_QKV, false>(bn, tmA, tmB, *p, pl, grid, st);
+    case EPI_LN: return dispatch_bn<EPI_LN, false>(bn, tmA, tmB, *p, pl, grid, st);
+  }
+  return p->taps == 9 ? dispatch_bn<EPI_BIAS_ACT, true>(bn, tmA, tmB, *p, pl, grid, st)
+                      : dispatch_bn<EPI_BIAS_ACT, false>(bn, tmA, tmB, *p, pl, grid, st);
+}
+
+int grl_tc_gemm_path(const GrlTcGemm* p, GrlTcGemmPath* out) {
+  GRL_REQUIRE(out != nullptr, "tc_gemm_path: null output");
+  GRL_REQUIRE(p != nullptr, "tc_gemm: null problem");
+  GemmTcPlan pl;
+  int bn = 0, rc;
+  if ((rc = plan_gemm_tc(*p, pl, &bn)) != GRL_OK) return rc;
+  out->bn = bn, out->epi_mode = pl.epi_mode, out->conv = p->taps == 9, out->n_tiles = pl.n_tiles;
+  out->nk_total = p->taps * pl.nk, out->grid = pl.total_tiles;
+  return GRL_OK;
+}
+
+}  // extern "C"

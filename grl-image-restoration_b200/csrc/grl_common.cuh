@@ -41,6 +41,11 @@ inline int fail(int code, const char* fmt, ...) {
       return ::grl::fail(GRL_ERR_CUDA, "launch of %s failed: %s", name, cudaGetErrorString(e__));      \
   } while (0)
 
+// channel_gate_kernel (ops_f32.cu) on per-chunk channel sums (B, chunks, C): the second half of grl_channel_gate_f32,
+// shared with grl_tc_channel_gate (misc_tc.cu), which computes the sums from 16-bit features.
+int channel_gate_from_partial(const float* partial, int chunks, int B, long long L, int C, const float* w1, const float* b1,
+                              const float* w2, const float* b2, int R, float* gate, cudaStream_t st);
+
 constexpr int kMaxDevices = 64;  // per-device one-time kernel attributes (cudaFuncSetAttribute is per device)
 
 inline int ceil_div(long long a, long long b) { return (int)((a + b - 1) / b); }

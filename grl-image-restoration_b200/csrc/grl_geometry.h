@@ -2,7 +2,7 @@
 //
 // The reference builds int64 index tensors and -100 masks on the CPU (models/common/ops.py) and
 // keeps ~1.5 GB of them as module buffers (models/networks/grl.py:386-429).  Here they are O(1)
-// functions evaluated in registers; grl_*_host() in capi.cu expand them into tensors so the tests can
+// functions evaluated in registers; the grl_*_host() functions expand them into tensors so the tests can
 // check them bit-exactly against the reference's golden digests.
 #pragma once
 #include <stdint.h>
@@ -55,6 +55,17 @@ GRL_HD int rel_index(int qh, int qw, int kh, int kw, int qww, int kwh, int kww) 
 }
 
 GRL_HD int windows_per_image(const GrlGrid& g) { return (g.H / g.wh) * (g.W / g.ww); }
+
+// Host check of a grid before anything above is evaluated on it; `what` names the caller in the message.
+int fail(int code, const char* fmt, ...);  // grl_common.cuh
+inline int check_grid(const GrlGrid& g, const char* what) {
+  if (!(g.H > 0 && g.W > 0 && g.wh > 0 && g.ww > 0)) return fail(GRL_ERR_INVALID, "%s: empty grid", what);
+  if (!(g.H % g.wh == 0 && g.W % g.ww == 0))
+    return fail(GRL_ERR_INVALID, "%s: grid %dx%d is not a multiple of the window %dx%d", what, g.H, g.W, g.wh, g.ww);
+  if (!(g.sh >= 0 && g.sh < g.H && g.sw >= 0 && g.sw < g.W && g.sh <= g.wh && g.sw <= g.ww))
+    return fail(GRL_ERR_INVALID, "%s: bad shift (%d,%d)", what, g.sh, g.sw);
+  return GRL_OK;
+}
 
 // The 8 dihedral views of augment_img_tensor4 (utils/utils_bsr/utils_image.py:444-460) as closed forms.  The mode's
 // bits are: 1 = transpose (the view is W x H), 2 = flip the source rows, 4 = flip the source columns:

@@ -12,7 +12,6 @@
 
 #include "grl_common.cuh"
 #include "grl_ssim.h"
-#include "ops_f32.h"
 
 namespace grl {
 
@@ -86,22 +85,6 @@ __global__ void psnr_finalize_kernel(const unsigned long long* __restrict__ sse,
   const double m_rgb = (double)sse[2 * i] / (65025.0 * (double)n_pix * (double)C);
   psnr_rgb[i] = (float)(-10.0 * log10(m_rgb));
   if (psnr_y) psnr_y[i] = (C == 3) ? (float)(-10.0 * log10((double)sse[2 * i + 1] / (65025.0 * (double)n_pix))) : psnr_rgb[i];
-}
-
-int launch_psnr(const float* restored, const float* target, int B, int C, int H, int W, int border,
-                unsigned long long* workspace, float* psnr_rgb, float* psnr_y, cudaStream_t st) {
-  GRL_REQUIRE(B >= 0 && C >= 1 && C <= 4 && H > 2 * border && W > 2 * border && border >= 0, "psnr: bad shape (%d,%d,%d,%d) border %d",
-              B, C, H, W, border);
-  if (B == 0) return GRL_OK;
-  GRL_CUDA(cudaMemsetAsync(workspace, 0, sizeof(unsigned long long) * 2 * (size_t)B, st));
-  const long long n = (long long)(H - 2 * border) * (W - 2 * border);
-  const int threads = 256;
-  const int bx = (int)std::min<long long>((n + threads * 4 - 1) / (threads * 4), 592);  // ~4 CTAs per SM per image at most
-  psnr_sse_kernel<<<dim3((unsigned)std::max(bx, 1), (unsigned)B), threads, 0, st>>>(restored, target, C, H, W, border, workspace);
-  GRL_LAUNCH_CHECK("psnr_sse_kernel");
-  psnr_finalize_kernel<<<(B + 127) / 128, 128, 0, st>>>(workspace, B, C, n, psnr_rgb, psnr_y);
-  GRL_LAUNCH_CHECK("psnr_finalize_kernel");
-  return GRL_OK;
 }
 
 // ---- PSNR-B (utils/metrics/psnrb.py:22-115) -------------------------------------------------------------------------
@@ -191,25 +174,6 @@ __global__ void psnrb_finalize_kernel(const unsigned long long* __restrict__ sum
   psnrb_rgb[i] = t / C;
   if (psnrb_y) psnrb_y[i] = C == 3 ? v[3] : psnrb_rgb[i];
 }
-
-int launch_psnrb(const float* restored, const float* target, int B, int C, int H, int W, unsigned long long* workspace,
-                 double* psnrb_rgb, double* psnrb_y, cudaStream_t st) {
-  GRL_REQUIRE(B >= 0 && (C == 1 || C == 3), "psnrb: needs C == 1 or 3, got %d", C);
-  GRL_REQUIRE(H >= 16 && W >= 16, "psnrb: needs at least 16 x 16 pixels (the blocking-effect factor divides 0 by 0 below), got %d x %d",
-              H, W);
-  if (B == 0) return GRL_OK;
-  GRL_CUDA(cudaMemsetAsync(workspace, 0, psnrb_workspace(B), st));
-  const long long n = (long long)H * W;
-  const int threads = 256;
-  const int bx = (int)std::min<long long>((n + threads * 4 - 1) / (threads * 4), 592);
-  psnrb_sums_kernel<<<dim3((unsigned)std::max(bx, 1), (unsigned)B), threads, 0, st>>>(restored, target, C, H, W, workspace);
-  GRL_LAUNCH_CHECK("psnrb_sums_kernel");
-  psnrb_finalize_kernel<<<(B + 127) / 128, 128, 0, st>>>(workspace, B, C, H, W, psnrb_rgb, psnrb_y);
-  GRL_LAUNCH_CHECK("psnrb_finalize_kernel");
-  return GRL_OK;
-}
-
-size_t psnrb_workspace(int B) { return sizeof(unsigned long long) * kPsnrbSets * kPsnrbSums * (size_t)(B > 0 ? B : 0); }
 
 // ---- SSIM (utils/metrics/ssim.py:17-85; the closed form is grl_ssim.h) -----------------------------------------------
 // One CTA owns a 32 x 16 tile of output pixels of one image and produces every plane of it: the C channels and, for
@@ -374,11 +338,6 @@ static bool ssim_shape_ok(int B, int C, int H, int W, int border) {
   return B >= 0 && (C == 1 || C == 3) && border >= 0 && H > 0 && W > 0 && 2LL * border < std::min(H, W);
 }
 
-size_t ssim_workspace(int B, int C, int H, int W, int border) {
-  if (!ssim_shape_ok(B, C, H, W, border)) return 0;
-  return sizeof(double) * 2 * (size_t)B * (size_t)ssim_tiles(H, W, border);
-}
-
 #define GRL_SSIM_SHAPE(B, C, H, W, border)                                                                                     \
   do {                                                                                                                         \
     GRL_REQUIRE(C == 1 || C == 3, "ssim: needs C == 1 or 3, got %d", C);                                                       \
@@ -386,12 +345,70 @@ size_t ssim_workspace(int B, int C, int H, int W, int border) {
     GRL_REQUIRE(2LL * border < std::min(H, W), "ssim: border %d leaves no pixel of a %d x %d image", border, H, W);            \
   } while (0)
 
-int launch_ssim(const float* restored, const float* target, int B, int C, int H, int W, int border, void* workspace,
-                size_t workspace_bytes, double* ssim_rgb, double* ssim_y, double* map_rgb, double* map_y, cudaStream_t st) {
+}  // namespace grl
+
+using namespace grl;
+
+extern "C" {
+
+int grl_psnr_f32(const float* restored, const float* target, int B, int C, int H, int W, int border, void* workspace,
+                 size_t workspace_bytes, float* psnr_rgb, float* psnr_y, void* stream) {
+  GRL_REQUIRE(restored && target && psnr_rgb, "psnr: null argument");
+  GRL_REQUIRE(workspace && workspace_bytes >= sizeof(unsigned long long) * 2 * (size_t)(B > 0 ? B : 0),
+              "psnr: workspace %zu bytes < %zu", workspace_bytes, sizeof(unsigned long long) * 2 * (size_t)(B > 0 ? B : 0));
+  GRL_REQUIRE(B >= 0 && C >= 1 && C <= 4 && H > 2 * border && W > 2 * border && border >= 0, "psnr: bad shape (%d,%d,%d,%d) border %d",
+              B, C, H, W, border);
+  if (B == 0) return GRL_OK;
+  const cudaStream_t st = (cudaStream_t)stream;
+  unsigned long long* sse = (unsigned long long*)workspace;
+  GRL_CUDA(cudaMemsetAsync(sse, 0, sizeof(unsigned long long) * 2 * (size_t)B, st));
+  const long long n = (long long)(H - 2 * border) * (W - 2 * border);
+  const int threads = 256;
+  const int bx = (int)std::min<long long>((n + threads * 4 - 1) / (threads * 4), 592);  // ~4 CTAs per SM per image at most
+  psnr_sse_kernel<<<dim3((unsigned)std::max(bx, 1), (unsigned)B), threads, 0, st>>>(restored, target, C, H, W, border, sse);
+  GRL_LAUNCH_CHECK("psnr_sse_kernel");
+  psnr_finalize_kernel<<<(B + 127) / 128, 128, 0, st>>>(sse, B, C, n, psnr_rgb, psnr_y);
+  GRL_LAUNCH_CHECK("psnr_finalize_kernel");
+  return GRL_OK;
+}
+
+size_t grl_psnrb_workspace(int B) { return sizeof(unsigned long long) * kPsnrbSets * kPsnrbSums * (size_t)(B > 0 ? B : 0); }
+
+int grl_psnrb_f32(const float* restored, const float* target, int B, int C, int H, int W, void* workspace,
+                  size_t workspace_bytes, double* psnrb_rgb, double* psnrb_y, void* stream) {
+  GRL_REQUIRE(restored && target && psnrb_rgb, "psnrb: null argument");
+  GRL_REQUIRE(workspace && workspace_bytes >= grl_psnrb_workspace(B), "psnrb: workspace %zu bytes < %zu", workspace_bytes,
+              grl_psnrb_workspace(B));
+  GRL_REQUIRE(B >= 0 && (C == 1 || C == 3), "psnrb: needs C == 1 or 3, got %d", C);
+  GRL_REQUIRE(H >= 16 && W >= 16, "psnrb: needs at least 16 x 16 pixels (the blocking-effect factor divides 0 by 0 below), got %d x %d",
+              H, W);
+  if (B == 0) return GRL_OK;
+  const cudaStream_t st = (cudaStream_t)stream;
+  unsigned long long* sums = (unsigned long long*)workspace;
+  GRL_CUDA(cudaMemsetAsync(sums, 0, grl_psnrb_workspace(B), st));
+  const long long n = (long long)H * W;
+  const int threads = 256;
+  const int bx = (int)std::min<long long>((n + threads * 4 - 1) / (threads * 4), 592);
+  psnrb_sums_kernel<<<dim3((unsigned)std::max(bx, 1), (unsigned)B), threads, 0, st>>>(restored, target, C, H, W, sums);
+  GRL_LAUNCH_CHECK("psnrb_sums_kernel");
+  psnrb_finalize_kernel<<<(B + 127) / 128, 128, 0, st>>>(sums, B, C, H, W, psnrb_rgb, psnrb_y);
+  GRL_LAUNCH_CHECK("psnrb_finalize_kernel");
+  return GRL_OK;
+}
+
+size_t grl_ssim_workspace(int B, int C, int H, int W, int border) {
+  if (!ssim_shape_ok(B, C, H, W, border)) return 0;
+  return sizeof(double) * 2 * (size_t)B * (size_t)ssim_tiles(H, W, border);
+}
+
+int grl_ssim_f32(const float* restored, const float* target, int B, int C, int H, int W, int border, void* workspace,
+                 size_t workspace_bytes, double* ssim_rgb, double* ssim_y, double* map_rgb, double* map_y, void* stream) {
+  GRL_REQUIRE(restored && target && ssim_rgb, "ssim: null argument");
   GRL_SSIM_SHAPE(B, C, H, W, border);
   if (B == 0) return GRL_OK;
-  GRL_REQUIRE(workspace && workspace_bytes >= ssim_workspace(B, C, H, W, border), "ssim: workspace %zu bytes < %zu", workspace_bytes,
-              ssim_workspace(B, C, H, W, border));
+  GRL_REQUIRE(workspace && workspace_bytes >= grl_ssim_workspace(B, C, H, W, border), "ssim: workspace %zu bytes < %zu",
+              workspace_bytes, grl_ssim_workspace(B, C, H, W, border));
+  const cudaStream_t st = (cudaStream_t)stream;
   const int h = H - 2 * border, w = W - 2 * border;
   const int gx = ceil_div(w, kSsimTW), gy = ceil_div(h, kSsimTH);
   GRL_REQUIRE(gy <= 65535 && B <= 65535, "ssim: %d tile rows / %d images exceed the grid", gy, B);
@@ -403,13 +420,16 @@ int launch_ssim(const float* restored, const float* target, int B, int C, int H,
   return GRL_OK;
 }
 
-void ssim_taps(double* t11) {
-  for (int i = 0; i < kSsimTaps; ++i) t11[i] = ssim_tap(i);
+int grl_ssim_taps_host(double* taps11) {
+  GRL_REQUIRE(taps11, "ssim_taps_host: null output");
+  for (int i = 0; i < kSsimTaps; ++i) taps11[i] = ssim_tap(i);
+  return GRL_OK;
 }
 
 // The same computation on the CPU (HOST pointers): the scores and, when asked for, the maps.  Scratch is host memory.
-int ssim_host(const float* restored, const float* target, int B, int C, int H, int W, int border, double* ssim_rgb,
-              double* ssim_y, double* map_rgb, double* map_y) {
+int grl_ssim_host(const float* restored, const float* target, int B, int C, int H, int W, int border, double* ssim_rgb,
+                  double* ssim_y, double* map_rgb, double* map_y) {
+  GRL_REQUIRE(restored && target && ssim_rgb, "ssim_host: null argument");
   GRL_SSIM_SHAPE(B, C, H, W, border);
   const int h = H - 2 * border, w = W - 2 * border, planes = C == 3 ? 4 : C;
   const size_t n = (size_t)h * w, plane = (size_t)H * W;
@@ -469,4 +489,4 @@ int ssim_host(const float* restored, const float* target, int B, int C, int H, i
   return GRL_OK;
 }
 
-}  // namespace grl
+}  // extern "C"

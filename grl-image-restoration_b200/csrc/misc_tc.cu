@@ -3,7 +3,6 @@
 // preparation of the attention constants.
 #include "grl_common.cuh"
 #include "grl_demosaic.h"
-#include "ops_tc.h"
 #include "tc_common.cuh"
 
 namespace grl {
@@ -161,53 +160,81 @@ static int launch_head(Src src, int B, int Cin, int H, int W, int Hp, int Wp, co
   GRL_LAUNCH_CHECK("head_pack_kernel");
   return GRL_OK;
 }
-int launch_head_pack(const float* x, int B, int Cin, int H, int W, int Hp, int Wp, const float* mean4, float range, void* y16,
-                     int Cpad, float* y32, int fmt, cudaStream_t st) {
-  return launch_head(PlanarSrc{x, Cin, H, W}, B, Cin, H, W, Hp, Wp, mean4, range, y16, Cpad, y32, fmt, st);
-}
-int launch_head_pack_rggb(const float* cfa4, int B, int h, int w, int Hp, int Wp, const float* mean4, float range, void* y16,
-                          int Cpad, float* y32, int fmt, cudaStream_t st) {
-  GRL_REQUIRE(h >= 2 && w >= 2, "head_pack_rggb: packed RGGB planes need h, w >= 2, got %dx%d", h, w);
-  return launch_head(RggbSrc{cfa4, h, w}, B, 3, 2 * h, 2 * w, Hp, Wp, mean4, range, y16, Cpad, y32, fmt, st);
-}
-int launch_pack_bf16(const float* x, long long ldx, void* y, long long M, int C, int Cpad, int fmt, cudaStream_t st) {
+
+}  // namespace tc
+}  // namespace grl
+
+using namespace grl;
+using namespace grl::tc;
+
+extern "C" {
+
+int grl_tc_pack16(const float* x, int64_t ldx, void* y, int64_t M, int C, int Cpad, int fmt, void* stream) {
+  if (check_fmt(fmt)) return GRL_ERR_INVALID;
   GRL_REQUIRE(Cpad % 8 == 0 && Cpad >= C, "pack_bf16: bad padding %d for %d channels", Cpad, C);
   if (M == 0) return GRL_OK;
-  pack_bf16_kernel<<<ceil_div(M * (Cpad / 8), 256), 256, 0, st>>>(x, ldx, (uint16_t*)y, M, C, Cpad, fmt);
+  pack_bf16_kernel<<<ceil_div(M * (Cpad / 8), 256), 256, 0, (cudaStream_t)stream>>>(x, ldx, (uint16_t*)y, M, C, Cpad, fmt);
   GRL_LAUNCH_CHECK("pack_bf16_kernel");
   return GRL_OK;
 }
-int launch_unpack_bf16(const void* x, long long ldx, int x_off, float* y, long long ldy, long long M, int C, int fmt,
-                       cudaStream_t st) {
+
+int grl_tc_unpack16(const void* x, int64_t ldx, int x_off, float* y, int64_t ldy, int64_t M, int C, int fmt,
+                    void* stream) {
+  if (check_fmt(fmt)) return GRL_ERR_INVALID;
   if (M == 0) return GRL_OK;
-  unpack_bf16_kernel<<<ceil_div(M * C, 256), 256, 0, st>>>((const uint16_t*)x, ldx, x_off, y, ldy, M, C, fmt);
+  unpack_bf16_kernel<<<ceil_div(M * C, 256), 256, 0, (cudaStream_t)stream>>>((const uint16_t*)x, ldx, x_off, y, ldy, M, C, fmt);
   GRL_LAUNCH_CHECK("unpack_bf16_kernel");
   return GRL_OK;
 }
-int launch_avgpool_bf16(const void* x, void* y, int B, int H, int W, int Cpad, int df, int fmt, cudaStream_t st) {
+
+int grl_tc_head_pack(const float* x, int B, int Cin, int H, int W, int Hp, int Wp, const float* mean4, float range, void* y16,
+                     int Cpad, float* y32, int fmt, void* stream) {
+  if (check_fmt(fmt)) return GRL_ERR_INVALID;
+  GRL_REQUIRE(x && y16, "head_pack: null argument");
+  return launch_head(PlanarSrc{x, Cin, H, W}, B, Cin, H, W, Hp, Wp, mean4, range, y16, Cpad, y32, fmt, (cudaStream_t)stream);
+}
+
+int grl_tc_head_pack_rggb(const float* cfa4, int B, int h, int w, int Hp, int Wp, const float* mean4, float range, void* y16,
+                          int Cpad, float* y32, int fmt, void* stream) {
+  if (check_fmt(fmt)) return GRL_ERR_INVALID;
+  GRL_REQUIRE(cfa4 && y16, "head_pack_rggb: null argument");
+  GRL_REQUIRE(h >= 2 && w >= 2, "head_pack_rggb: packed RGGB planes need h, w >= 2, got %dx%d", h, w);
+  return launch_head(RggbSrc{cfa4, h, w}, B, 3, 2 * h, 2 * w, Hp, Wp, mean4, range, y16, Cpad, y32, fmt, (cudaStream_t)stream);
+}
+
+int grl_tc_avgpool16(const void* x, void* y, int B, int H, int W, int Cpad, int df, int fmt, void* stream) {
+  if (check_fmt(fmt)) return GRL_ERR_INVALID;
   GRL_REQUIRE(df >= 1 && H % df == 0 && W % df == 0 && Cpad % 8 == 0, "avgpool_bf16: bad shape");
   long long total = (long long)B * (H / df) * (W / df) * (Cpad / 8);
   if (total == 0) return GRL_OK;
-  avgpool_bf16_kernel<<<ceil_div(total, 256), 256, 0, st>>>((const uint16_t*)x, (uint16_t*)y, B, H, W, Cpad, df, fmt);
+  avgpool_bf16_kernel<<<ceil_div(total, 256), 256, 0, (cudaStream_t)stream>>>((const uint16_t*)x, (uint16_t*)y, B, H, W, Cpad,
+                                                                              df, fmt);
   GRL_LAUNCH_CHECK("avgpool_bf16_kernel");
   return GRL_OK;
 }
-size_t channel_partial_bf16_ws(int B, long long L, int C) { return sizeof(float) * (size_t)B * ceil_div(L, kPoolRowsTc) * C; }
-int launch_channel_partial_bf16(const void* y, int B, long long L, long long ld, int C, int fmt, float* partial,
-                                int* chunks_out, cudaStream_t st) {
-  const int chunks = ceil_div(L, kPoolRowsTc);
-  *chunks_out = chunks;
-  if (B == 0) return GRL_OK;
-  channel_partial_bf16_kernel<<<dim3(chunks, B), 256, 0, st>>>((const uint16_t*)y, L, ld, C, fmt, partial, chunks);
-  GRL_LAUNCH_CHECK("channel_partial_bf16_kernel");
-  return GRL_OK;
-}
-int launch_slot_scale(const float* ls_w, const float* ls_s1, const float* ls_s2, int hw, int hs, float* out,
-                      cudaStream_t st) {
-  slot_scale_kernel<<<1, 64, 0, st>>>(ls_w, ls_s1, ls_s2, hw, hs, out);
+
+int grl_tc_slot_scale(const float* ls_w, const float* ls_s1, const float* ls_s2, int hw, int hs, float* out,
+                      void* stream) {
+  GRL_REQUIRE(hw >= 1 && hs >= 1 && hw <= 8 && hs <= 8, "slot_scale: bad head counts");
+  slot_scale_kernel<<<1, 64, 0, (cudaStream_t)stream>>>(ls_w, ls_s1, ls_s2, hw, hs, out);
   GRL_LAUNCH_CHECK("slot_scale_kernel");
   return GRL_OK;
 }
 
-}  // namespace tc
-}  // namespace grl
+size_t grl_tc_channel_gate_workspace(int B, int64_t L, int C) {
+  return sizeof(float) * (size_t)B * ceil_div(L, kPoolRowsTc) * C;
+}
+
+int grl_tc_channel_gate(const void* y, int64_t ld, int fmt, int B, int64_t L, int C, const float* w1, const float* b1,
+                        const float* w2, const float* b2, int R, float* gate, void* ws, size_t ws_bytes, void* stream) {
+  if (check_fmt(fmt)) return GRL_ERR_INVALID;
+  if (ws_bytes < grl_tc_channel_gate_workspace(B, L, C)) return fail(GRL_ERR_WORKSPACE, "tc_channel_gate: workspace too small");
+  if (B == 0) return GRL_OK;
+  const cudaStream_t st = (cudaStream_t)stream;
+  const int chunks = ceil_div(L, kPoolRowsTc);
+  channel_partial_bf16_kernel<<<dim3(chunks, B), 256, 0, st>>>((const uint16_t*)y, L, ld, C, fmt, (float*)ws, chunks);
+  GRL_LAUNCH_CHECK("channel_partial_bf16_kernel");
+  return channel_gate_from_partial((const float*)ws, chunks, B, L, C, w1, b1, w2, b2, R, gate, st);
+}
+
+}  // extern "C"

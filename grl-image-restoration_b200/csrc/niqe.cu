@@ -20,7 +20,6 @@
 
 #include "grl_common.cuh"
 #include "grl_niqe.h"
-#include "ops_f32.h"
 
 namespace grl {
 
@@ -219,31 +218,10 @@ __global__ void __launch_bounds__(kFeatThreads) niqe_feat_kernel(const float* __
 
 static int grid_1d(long long n) { return (int)std::max<long long>(1, std::min<long long>((n + 255) / 256, 1184)); }
 
-int launch_niqe_luma(const float* x, int B, int C, int H, int W, int border, float* y, cudaStream_t st) {
-  GRL_REQUIRE(C == 3, "niqe: needs RGB images (C == 3), got C = %d", C);
-  GRL_REQUIRE(B >= 0 && border >= 0 && H - 2 * border >= 96 && W - 2 * border >= 96,
-              "niqe: needs at least 96 x 96 pixels after cropping border %d, got %d x %d", border, H, W);
-  if (B == 0) return GRL_OK;
-  const int Hc = (H - 2 * border) / 96 * 96, Wc = (W - 2 * border) / 96 * 96;
-  niqe_luma_kernel<<<dim3(grid_1d((long long)Hc * Wc), B), 256, 0, st>>>(x, H, W, border, Hc, Wc, y);
-  GRL_LAUNCH_CHECK("niqe_luma_kernel");
-  return GRL_OK;
-}
-
-int launch_niqe_mscn(const float* in, int B, int H, int W, const double* window49, float* out, cudaStream_t st) {
-  GRL_REQUIRE(B >= 0 && H >= 1 && W >= 1 && window49, "niqe_mscn: bad arguments B=%d H=%d W=%d", B, H, W);
-  if (B == 0) return GRL_OK;
-  NiqeWin win;
-  for (int i = 0; i < 49; ++i) win.w[i] = window49[48 - i];  // convolve = correlate with the flipped window
-  niqe_mscn_kernel<<<dim3(ceil_div(W, kTx), ceil_div(H, kTy), B), dim3(kTx, kTy), 0, st>>>(in, H, W, win, out);
-  GRL_LAUNCH_CHECK("niqe_mscn_kernel");
-  return GRL_OK;
-}
-
 // imresize's weights for x0.5 with antialiasing (niqe.py:169-238): kernel width 8, distances 3.5 - k for the 8 taps that
 // survive, 0.5 * cubic(0.5 * d) normalised by their sum.  Every value is a short dyadic fraction and the sum is exactly 1,
 // so the fp32 weights are exact whatever the order of evaluation.
-void niqe_half_taps(float* w8) {
+static void niqe_half_taps(float* w8) {
   double s = 0.0, c[8];
   for (int k = 0; k < 8; ++k) {
     const double x = fabs(0.5 * (3.5 - k)), x2 = x * x, x3 = x2 * x;
@@ -254,46 +232,93 @@ void niqe_half_taps(float* w8) {
   for (int k = 0; k < 8; ++k) w8[k] = (float)(c[k] / s);
 }
 
-int launch_niqe_half(const float* in, int B, int H, int W, float* tmp, float* out, cudaStream_t st) {
+static size_t align256(size_t b) { return (b + 255) / 256 * 256; }
+
+}  // namespace grl
+
+using namespace grl;
+
+extern "C" {
+
+int grl_niqe_luma_host(const uint8_t* rgb, int64_t n, float* y) {
+  GRL_REQUIRE(rgb && y && n >= 0, "niqe_luma_host: bad arguments");
+  for (int64_t i = 0; i < n; ++i) y[i] = niqe_luma(rgb[3 * i], rgb[3 * i + 1], rgb[3 * i + 2]);
+  return GRL_OK;
+}
+
+int grl_niqe_half_taps_host(float* w8) {
+  GRL_REQUIRE(w8, "niqe_half_taps_host: null output");
+  niqe_half_taps(w8);
+  return GRL_OK;
+}
+
+int grl_niqe_luma_f32(const float* restored, int B, int C, int H, int W, int border, float* y, void* stream) {
+  GRL_REQUIRE(restored && y, "niqe_luma: null argument");
+  GRL_REQUIRE(C == 3, "niqe: needs RGB images (C == 3), got C = %d", C);
+  GRL_REQUIRE(B >= 0 && border >= 0 && H - 2 * border >= 96 && W - 2 * border >= 96,
+              "niqe: needs at least 96 x 96 pixels after cropping border %d, got %d x %d", border, H, W);
+  if (B == 0) return GRL_OK;
+  const int Hc = (H - 2 * border) / 96 * 96, Wc = (W - 2 * border) / 96 * 96;
+  niqe_luma_kernel<<<dim3(grid_1d((long long)Hc * Wc), B), 256, 0, (cudaStream_t)stream>>>(restored, H, W, border, Hc, Wc, y);
+  GRL_LAUNCH_CHECK("niqe_luma_kernel");
+  return GRL_OK;
+}
+
+int grl_niqe_mscn_f32(const float* img, int B, int H, int W, const double* window49, float* out, void* stream) {
+  GRL_REQUIRE(img && out, "niqe_mscn: null argument");
+  GRL_REQUIRE(B >= 0 && H >= 1 && W >= 1 && window49, "niqe_mscn: bad arguments B=%d H=%d W=%d", B, H, W);
+  if (B == 0) return GRL_OK;
+  NiqeWin win;
+  for (int i = 0; i < 49; ++i) win.w[i] = window49[48 - i];  // convolve = correlate with the flipped window
+  niqe_mscn_kernel<<<dim3(ceil_div(W, kTx), ceil_div(H, kTy), B), dim3(kTx, kTy), 0, (cudaStream_t)stream>>>(img, H, W, win, out);
+  GRL_LAUNCH_CHECK("niqe_mscn_kernel");
+  return GRL_OK;
+}
+
+int grl_niqe_half_f32(const float* img, int B, int H, int W, float* tmp, float* out, void* stream) {
+  GRL_REQUIRE(img && tmp && out, "niqe_half: null argument");
   GRL_REQUIRE(B >= 0 && H >= 4 && W >= 4 && H % 2 == 0 && W % 2 == 0, "niqe_half: needs even sizes >= 4, got %d x %d", H, W);
   if (B == 0) return GRL_OK;
+  const cudaStream_t st = (cudaStream_t)stream;
   NiqeTaps taps;
   niqe_half_taps(taps.w);
-  niqe_half_rows_kernel<<<dim3(grid_1d((long long)H / 2 * W), B), 256, 0, st>>>(in, H, W, taps, tmp);
+  niqe_half_rows_kernel<<<dim3(grid_1d((long long)H / 2 * W), B), 256, 0, st>>>(img, H, W, taps, tmp);
   GRL_LAUNCH_CHECK("niqe_half_rows_kernel");
   niqe_half_cols_kernel<<<dim3(grid_1d((long long)H / 2 * W / 2), B), 256, 0, st>>>(tmp, H, W, taps, out);
   GRL_LAUNCH_CHECK("niqe_half_cols_kernel");
   return GRL_OK;
 }
 
-int launch_niqe_feat(const float* m1, const float* m2, int B, int nbh, int nbw, const double* tables, double* feats,
-                     cudaStream_t st) {
+int grl_niqe_feat_f32(const float* mscn1, const float* mscn2, int B, int nbh, int nbw, const double* tables, double* feats,
+                      void* stream) {
+  GRL_REQUIRE(mscn1 && mscn2 && feats, "niqe_feat: null argument");
   GRL_REQUIRE(B >= 0 && nbh >= 1 && nbw >= 1 && (long long)nbh * nbw <= 0x7fffffffLL && tables,
               "niqe_feat: bad arguments B=%d blocks %d x %d", B, nbh, nbw);
   if (B == 0) return GRL_OK;
-  niqe_feat_kernel<<<dim3(nbh * nbw, 2, B), kFeatThreads, 0, st>>>(m1, m2, nbh, nbw, tables, feats);
+  niqe_feat_kernel<<<dim3(nbh * nbw, 2, B), kFeatThreads, 0, (cudaStream_t)stream>>>(mscn1, mscn2, nbh, nbw, tables, feats);
   GRL_LAUNCH_CHECK("niqe_feat_kernel");
   return GRL_OK;
 }
 
-static size_t align256(size_t b) { return (b + 255) / 256 * 256; }
-
-size_t niqe_ws(int B, int H, int W, int border) {
+size_t grl_niqe_workspace(int B, int H, int W, int border) {
   if (B <= 0 || H - 2 * border < 96 || W - 2 * border < 96) return 0;
   const size_t Hc = (H - 2 * border) / 96 * 96, Wc = (W - 2 * border) / 96 * 96;
   const size_t full = align256(sizeof(float) * B * Hc * Wc), half = align256(sizeof(float) * B * (Hc / 2) * (Wc / 2));
   return 2 * full + align256(sizeof(float) * B * (Hc / 2) * Wc) + 2 * half;
 }
 
-int launch_niqe_features(const float* x, int B, int C, int H, int W, int border, const double* window49, const double* tables,
-                         void* ws, size_t ws_bytes, double* feats, cudaStream_t st) {
+// The four stages above on one workspace: luma, MSCN, x0.5 resize, MSCN of the resized image, features.
+int grl_niqe_features_f32(const float* restored, int B, int C, int H, int W, int border, const double* window49,
+                          const double* tables, void* workspace, size_t workspace_bytes, double* feats, void* stream) {
+  GRL_REQUIRE(restored && window49 && tables && feats, "niqe: null argument");
   GRL_REQUIRE(C == 3, "niqe: needs RGB images (C == 3), got C = %d", C);
   GRL_REQUIRE(B >= 0 && border >= 0 && H - 2 * border >= 96 && W - 2 * border >= 96,
               "niqe: needs at least 96 x 96 pixels after cropping border %d, got %d x %d", border, H, W);
   if (B == 0) return GRL_OK;
-  GRL_REQUIRE(ws && ws_bytes >= niqe_ws(B, H, W, border), "niqe: workspace %zu bytes < %zu", ws_bytes, niqe_ws(B, H, W, border));
+  GRL_REQUIRE(workspace && workspace_bytes >= grl_niqe_workspace(B, H, W, border), "niqe: workspace %zu bytes < %zu",
+              workspace_bytes, grl_niqe_workspace(B, H, W, border));
   const int Hc = (H - 2 * border) / 96 * 96, Wc = (W - 2 * border) / 96 * 96;
-  char* p = (char*)ws;
+  char* p = (char*)workspace;
   float* y = (float*)p;
   p += align256(sizeof(float) * B * (size_t)Hc * Wc);
   float* m1 = (float*)p;
@@ -304,11 +329,11 @@ int launch_niqe_features(const float* x, int B, int C, int H, int W, int border,
   p += align256(sizeof(float) * B * (size_t)(Hc / 2) * (Wc / 2));
   float* m2 = (float*)p;
   int rc;
-  if ((rc = launch_niqe_luma(x, B, C, H, W, border, y, st)) != GRL_OK) return rc;
-  if ((rc = launch_niqe_mscn(y, B, Hc, Wc, window49, m1, st)) != GRL_OK) return rc;
-  if ((rc = launch_niqe_half(y, B, Hc, Wc, t, y2, st)) != GRL_OK) return rc;
-  if ((rc = launch_niqe_mscn(y2, B, Hc / 2, Wc / 2, window49, m2, st)) != GRL_OK) return rc;
-  return launch_niqe_feat(m1, m2, B, Hc / 96, Wc / 96, tables, feats, st);
+  if ((rc = grl_niqe_luma_f32(restored, B, C, H, W, border, y, stream)) != GRL_OK) return rc;
+  if ((rc = grl_niqe_mscn_f32(y, B, Hc, Wc, window49, m1, stream)) != GRL_OK) return rc;
+  if ((rc = grl_niqe_half_f32(y, B, Hc, Wc, t, y2, stream)) != GRL_OK) return rc;
+  if ((rc = grl_niqe_mscn_f32(y2, B, Hc / 2, Wc / 2, window49, m2, stream)) != GRL_OK) return rc;
+  return grl_niqe_feat_f32(m1, m2, B, Hc / 96, Wc / 96, tables, feats, stream);
 }
 
-}  // namespace grl
+}  // extern "C"

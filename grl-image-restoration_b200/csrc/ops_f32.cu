@@ -4,10 +4,50 @@
 // (gemm_tc.cu / attn_tc.cu) is the throughput path and is gated on PSNR.
 //
 // Reference semantics cited per kernel (paths relative to the reference root).
+#include <string.h>
+
 #include "grl_common.cuh"
-#include "ops_f32.h"
 
 namespace grl {
+
+struct GemmArgs {
+  const float* x;
+  long long ldx;
+  const float* w;  // (N, K) row-major
+  const float* b;
+  const float* res;
+  long long ldr;
+  float* y;
+  long long ldy;
+  long long M;
+  int N, K;
+  int act;
+  float slope;
+  int H, W, Cin;  // conv only
+};
+
+struct AttnArgs {
+  GrlGrid gq, gk;  // query / key token grids (same number of windows)
+  const float* q;
+  long long ldq;
+  int q_off;  // channel offset of head 0 in a token row
+  const float* k;
+  long long ldk;
+  int k_off;
+  const float* v;
+  long long ldv;
+  int v_off;
+  int v_dense;  // V is the dense (B_, heads, Nk, d) X1 buffer
+  float* out;
+  long long ldo;
+  int o_off;
+  int o_dense;  // write dense (B_, heads, Nq, d)
+  int B, heads, d;
+  const float* logit_scale;  // (heads)
+  const float* bias;         // (heads, rows)
+  int rows;
+  int use_mask;
+};
 
 // =====================================================================================
 // bias table: out[h, r] = 16 * sigmoid( W2[h,:] . relu(W1 t_r + b1) )
@@ -398,10 +438,10 @@ __global__ void __launch_bounds__(kQT) attn_f32_kernel(AttnArgs a) {
 }
 
 // -------------------------------------------------------------------------------------
-// host launchers
+// host side
 // -------------------------------------------------------------------------------------
-int launch_bias_table(const float* table, int rows, const float* w1, const float* b1, const float* w2, int hidden,
-                      int heads, float mul, int copies, int rows_pad, float* out, cudaStream_t st) {
+static int launch_bias_table(const float* table, int rows, const float* w1, const float* b1, const float* w2, int hidden,
+                             int heads, float mul, int copies, int rows_pad, float* out, cudaStream_t st) {
   GRL_REQUIRE(copies >= 1 && copies <= 4 && rows_pad >= rows + copies - 1, "bias_table: bad copies / pitch");
   GRL_REQUIRE(heads >= 1 && heads <= kMaxHeads, "bias_table: heads=%d unsupported (max %d)", heads, kMaxHeads);
   GRL_REQUIRE(rows > 0 && hidden > 0, "bias_table: empty");
@@ -412,18 +452,7 @@ int launch_bias_table(const float* table, int rows, const float* w1, const float
   return GRL_OK;
 }
 
-int launch_affine(float* attn, long long B_, int heads, int n1, int n2, const float* logit_scale, const float* bias,
-                  int rows, const long long* index, const float* mask, int nW, cudaStream_t st) {
-  long long total = B_ * heads * n1 * n2;
-  if (total == 0) return GRL_OK;
-  GRL_REQUIRE(!mask || (nW > 0 && B_ % nW == 0), "affine: batch %lld not a multiple of nW=%d", B_, nW);
-  affine_kernel<<<ceil_div(total, 256), 256, 0, st>>>(attn, total, heads, n1, n2, logit_scale, bias, rows, index, mask,
-                                                     nW > 0 ? nW : 1);
-  GRL_LAUNCH_CHECK("affine_kernel");
-  return GRL_OK;
-}
-
-int launch_gemm(const GemmArgs& a, bool conv, cudaStream_t st) {
+static int launch_gemm(const GemmArgs& a, bool conv, cudaStream_t st) {
   if (a.M == 0 || a.N == 0) return GRL_OK;
   GRL_REQUIRE(a.K > 0, "gemm: K must be positive");
   dim3 grid(ceil_div(a.M, BM), ceil_div(a.N, BN));
@@ -436,63 +465,16 @@ int launch_gemm(const GemmArgs& a, bool conv, cudaStream_t st) {
   return GRL_OK;
 }
 
-int launch_avgpool(const float* x, float* y, int B, int H, int W, int C, int df, cudaStream_t st) {
-  GRL_REQUIRE(df >= 1 && H % df == 0 && W % df == 0, "avgpool: %dx%d not divisible by %d", H, W, df);
-  long long total = (long long)B * (H / df) * (W / df) * C;
-  if (total == 0) return GRL_OK;
-  avgpool_kernel<<<ceil_div(total, 256), 256, 0, st>>>(x, y, B, H, W, C, df);
-  GRL_LAUNCH_CHECK("avgpool_kernel");
-  return GRL_OK;
-}
-
-int launch_ln_residual(const float* x, const float* u, const float* gamma, const float* beta, float eps,
-                       float res_scale, const float* cab_y, const float* cab_gate, long long L, float* out,
-                       long long M, int C, cudaStream_t st) {
-  if (M == 0) return GRL_OK;
-  GRL_REQUIRE((cab_y == nullptr) == (cab_gate == nullptr), "ln_residual: cab_y and cab_gate go together");
-  GRL_REQUIRE(L > 0 && M % L == 0, "ln_residual: M=%lld not a multiple of L=%lld", M, L);
-  ln_residual_kernel<<<ceil_div(M, 8), 256, 0, st>>>(x, u, gamma, beta, eps, res_scale, cab_y, cab_gate, L, out, M, C);
-  GRL_LAUNCH_CHECK("ln_residual_kernel");
-  return GRL_OK;
-}
-
-size_t channel_gate_ws(int B, long long L, int C) {
-  return sizeof(float) * (size_t)B * ceil_div(L, kPoolRows) * C;
-}
-
-int launch_channel_gate(const float* y, int B, long long L, int C, const float* w1, const float* b1, const float* w2,
-                        const float* b2, int R, float* gate, void* ws, size_t ws_bytes, cudaStream_t st) {
-  if (B == 0) return GRL_OK;
-  GRL_REQUIRE(L > 0 && C > 0 && R > 0, "channel_gate: empty");
-  if (ws_bytes < channel_gate_ws(B, L, C))
-    return fail(GRL_ERR_WORKSPACE, "channel_gate: workspace %zu < %zu", ws_bytes, channel_gate_ws(B, L, C));
-  const int chunks = ceil_div(L, kPoolRows);
-  channel_partial_kernel<<<dim3(chunks, B), 256, 0, st>>>(y, L, C, (float*)ws, chunks);
-  GRL_LAUNCH_CHECK("channel_partial_kernel");
-  channel_gate_kernel<<<B, 256, sizeof(float) * (C + R), st>>>((const float*)ws, chunks, L, C, w1, b1, w2, b2, R, gate);
-  GRL_LAUNCH_CHECK("channel_gate_kernel");
-  return GRL_OK;
-}
-
-int launch_channel_gate_from_partial(const float* partial, int chunks, int B, long long L, int C, const float* w1,
-                                     const float* b1, const float* w2, const float* b2, int R, float* gate,
-                                     cudaStream_t st) {
+int channel_gate_from_partial(const float* partial, int chunks, int B, long long L, int C, const float* w1, const float* b1,
+                              const float* w2, const float* b2, int R, float* gate, cudaStream_t st) {
   if (B == 0) return GRL_OK;
   channel_gate_kernel<<<B, 256, sizeof(float) * (C + R), st>>>(partial, chunks, L, C, w1, b1, w2, b2, R, gate);
   GRL_LAUNCH_CHECK("channel_gate_kernel");
   return GRL_OK;
 }
 
-int check_grid(const GrlGrid& g, const char* what) {
-  GRL_REQUIRE(g.H > 0 && g.W > 0 && g.wh > 0 && g.ww > 0, "%s: empty grid", what);
-  GRL_REQUIRE(g.H % g.wh == 0 && g.W % g.ww == 0, "%s: grid %dx%d is not a multiple of the window %dx%d", what, g.H,
-              g.W, g.wh, g.ww);
-  GRL_REQUIRE(g.sh >= 0 && g.sh < g.H && g.sw >= 0 && g.sw < g.W && g.sh <= g.wh && g.sw <= g.ww,
-              "%s: bad shift (%d,%d)", what, g.sh, g.sw);
-  return GRL_OK;
-}
-
-int launch_attn(const AttnArgs& a, cudaStream_t st) {
+// the window attention and both passes of the stripe attention
+static int launch_attn(const AttnArgs& a, cudaStream_t st) {
   if (a.B == 0) return GRL_OK;
   int rc;
   if ((rc = check_grid(a.gq, "attn(q grid)")) != GRL_OK) return rc;
@@ -515,3 +497,143 @@ int launch_attn(const AttnArgs& a, cudaStream_t st) {
 }
 
 }  // namespace grl
+
+using namespace grl;
+
+extern "C" {
+
+int grl_bias_table_f32(const float* table, int rows, const float* w1, const float* b1, const float* w2, int hidden,
+                       int heads, float* out, void* stream) {
+  return launch_bias_table(table, rows, w1, b1, w2, hidden, heads, 1.0f, 1, rows, out, (cudaStream_t)stream);
+}
+
+int grl_tc_bias_table4(const float* table, int rows, const float* w1, const float* b1, const float* w2, int hidden,
+                       int heads, float mul, int rows_pad, float* out, void* stream) {
+  GRL_REQUIRE(rows_pad % 4 == 0 && rows_pad >= rows + 4, "tc_bias_table4: rows_pad must be a multiple of 4 and >= rows + 4");
+  return launch_bias_table(table, rows, w1, b1, w2, hidden, heads, mul, 4, rows_pad, out, (cudaStream_t)stream);
+}
+
+int grl_affine_f32(float* attn, int64_t B_, int heads, int n1, int n2, const float* logit_scale, const float* bias,
+                   int rows, const int64_t* index, const float* mask, int nW, void* stream) {
+  long long total = B_ * heads * n1 * n2;
+  if (total == 0) return GRL_OK;
+  GRL_REQUIRE(!mask || (nW > 0 && B_ % nW == 0), "affine: batch %lld not a multiple of nW=%d", (long long)B_, nW);
+  affine_kernel<<<ceil_div(total, 256), 256, 0, (cudaStream_t)stream>>>(attn, total, heads, n1, n2, logit_scale, bias, rows,
+                                                                       (const long long*)index, mask, nW > 0 ? nW : 1);
+  GRL_LAUNCH_CHECK("affine_kernel");
+  return GRL_OK;
+}
+
+int grl_linear_f32(const float* x, int64_t ldx, const float* w, const float* b, const float* res, int64_t ldr,
+                   float* y, int64_t ldy, int64_t M, int N, int K, int act, float slope, void* stream) {
+  GRL_REQUIRE(M >= 0 && N >= 0 && K > 0 && ldx >= K && ldy >= N, "linear: bad shape M=%lld N=%d K=%d", (long long)M, N,
+              K);
+  GemmArgs a = {x, ldx, w, b, res, ldr, y, ldy, M, N, K, act, slope, 0, 0, 0};
+  return launch_gemm(a, false, (cudaStream_t)stream);
+}
+
+int grl_conv3x3_f32(const float* x, const float* w, const float* b, const float* res, float* y, int B, int H, int W,
+                    int Cin, int Cout, int act, float slope, void* stream) {
+  GRL_REQUIRE(B >= 0 && H > 0 && W > 0 && Cin > 0 && Cout > 0, "conv3x3: bad shape");
+  GemmArgs a = {x, 0, w, b, res, Cout, y, Cout, (long long)B * H * W, Cout, 9 * Cin, act, slope, H, W, Cin};
+  return launch_gemm(a, true, (cudaStream_t)stream);
+}
+
+int grl_avgpool_f32(const float* x, float* y, int B, int H, int W, int C, int df, void* stream) {
+  GRL_REQUIRE(df >= 1 && H % df == 0 && W % df == 0, "avgpool: %dx%d not divisible by %d", H, W, df);
+  long long total = (long long)B * (H / df) * (W / df) * C;
+  if (total == 0) return GRL_OK;
+  avgpool_kernel<<<ceil_div(total, 256), 256, 0, (cudaStream_t)stream>>>(x, y, B, H, W, C, df);
+  GRL_LAUNCH_CHECK("avgpool_kernel");
+  return GRL_OK;
+}
+
+int grl_ln_residual_f32(const float* x, const float* u, const float* gamma, const float* beta, float eps,
+                        float res_scale, const float* cab_y, const float* cab_gate, int64_t L, float* out, int64_t M,
+                        int C, void* stream) {
+  if (M == 0) return GRL_OK;
+  GRL_REQUIRE((cab_y == nullptr) == (cab_gate == nullptr), "ln_residual: cab_y and cab_gate go together");
+  GRL_REQUIRE(L > 0 && M % L == 0, "ln_residual: M=%lld not a multiple of L=%lld", (long long)M, (long long)L);
+  ln_residual_kernel<<<ceil_div(M, 8), 256, 0, (cudaStream_t)stream>>>(x, u, gamma, beta, eps, res_scale, cab_y, cab_gate, L,
+                                                                      out, M, C);
+  GRL_LAUNCH_CHECK("ln_residual_kernel");
+  return GRL_OK;
+}
+
+size_t grl_channel_gate_workspace(int B, int64_t L, int C) {
+  return sizeof(float) * (size_t)B * ceil_div(L, kPoolRows) * C;
+}
+
+int grl_channel_gate_f32(const float* y, int B, int64_t L, int C, const float* w1, const float* b1, const float* w2,
+                         const float* b2, int R, float* gate, void* workspace, size_t workspace_bytes, void* stream) {
+  if (B == 0) return GRL_OK;
+  GRL_REQUIRE(L > 0 && C > 0 && R > 0, "channel_gate: empty");
+  const size_t need = grl_channel_gate_workspace(B, L, C);
+  if (workspace_bytes < need) return fail(GRL_ERR_WORKSPACE, "channel_gate: workspace %zu < %zu", workspace_bytes, need);
+  const cudaStream_t st = (cudaStream_t)stream;
+  const int chunks = ceil_div(L, kPoolRows);
+  channel_partial_kernel<<<dim3(chunks, B), 256, 0, st>>>(y, L, C, (float*)workspace, chunks);
+  GRL_LAUNCH_CHECK("channel_partial_kernel");
+  channel_gate_kernel<<<B, 256, sizeof(float) * (C + R), st>>>((const float*)workspace, chunks, L, C, w1, b1, w2, b2, R, gate);
+  GRL_LAUNCH_CHECK("channel_gate_kernel");
+  return GRL_OK;
+}
+
+int grl_window_attn_f32(const float* qkv, int64_t ld_qkv, float* out, int64_t ld_out, int B, GrlGrid grid, int heads,
+                        int d, const float* logit_scale, const float* bias, int use_mask, void* stream) {
+  AttnArgs a;
+  memset(&a, 0, sizeof(a));
+  const int c = heads * d;
+  a.gq = grid;
+  a.gk = grid;
+  a.q = qkv, a.ldq = ld_qkv, a.q_off = 0;
+  a.k = qkv, a.ldk = ld_qkv, a.k_off = c;
+  a.v = qkv, a.ldv = ld_qkv, a.v_off = 2 * c;
+  a.out = out, a.ldo = ld_out, a.o_off = 0;
+  a.B = B, a.heads = heads, a.d = d;
+  a.logit_scale = logit_scale;
+  a.bias = bias;
+  a.rows = (2 * grid.wh - 1) * (2 * grid.ww - 1);
+  a.use_mask = use_mask;
+  return launch_attn(a, (cudaStream_t)stream);
+}
+
+size_t grl_stripe_attn_workspace(int B, GrlGrid tok, GrlGrid anc, int heads, int d) {
+  (void)tok;
+  return sizeof(float) * (size_t)B * anc.H * anc.W * heads * d;
+}
+
+int grl_stripe_attn_f32(const float* qkv, int64_t ld_qkv, const float* anchor, int64_t ld_anchor, float* out,
+                        int64_t ld_out, int B, GrlGrid tok, GrlGrid anc, int heads, int d, const float* logit_scale1,
+                        const float* bias1, const float* logit_scale2, const float* bias2, int use_mask,
+                        void* workspace, size_t workspace_bytes, void* stream) {
+  const size_t need = grl_stripe_attn_workspace(B, tok, anc, heads, d);
+  if (workspace_bytes < need) return fail(GRL_ERR_WORKSPACE, "stripe_attn: workspace %zu < %zu", workspace_bytes, need);
+  const int c = heads * d;
+  const int rows = (tok.wh + anc.wh - 1) * (tok.ww + anc.ww - 1);
+  float* x1 = (float*)workspace;
+  AttnArgs a;
+  memset(&a, 0, sizeof(a));
+  // pass 1: anchors attend to the stripe's tokens (a2w)   efficient.py:256-258
+  a.gq = anc, a.gk = tok;
+  a.q = anchor, a.ldq = ld_anchor, a.q_off = 0;
+  a.k = qkv, a.ldk = ld_qkv, a.k_off = c;
+  a.v = qkv, a.ldv = ld_qkv, a.v_off = 2 * c;
+  a.out = x1, a.o_dense = 1;
+  a.B = B, a.heads = heads, a.d = d;
+  a.logit_scale = logit_scale1, a.bias = bias1, a.rows = rows, a.use_mask = use_mask;
+  int rc = launch_attn(a, (cudaStream_t)stream);
+  if (rc != GRL_OK) return rc;
+  // pass 2: tokens attend to the anchors, values = X1 (w2a)   efficient.py:259
+  memset(&a, 0, sizeof(a));
+  a.gq = tok, a.gk = anc;
+  a.q = qkv, a.ldq = ld_qkv, a.q_off = 0;
+  a.k = anchor, a.ldk = ld_anchor, a.k_off = 0;
+  a.v = x1, a.v_dense = 1;
+  a.out = out, a.ldo = ld_out, a.o_off = 0;
+  a.B = B, a.heads = heads, a.d = d;
+  a.logit_scale = logit_scale2, a.bias = bias2, a.rows = rows, a.use_mask = use_mask;
+  return launch_attn(a, (cudaStream_t)stream);
+}
+
+}  // extern "C"

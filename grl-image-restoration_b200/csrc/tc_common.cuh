@@ -8,6 +8,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "grl_common.cuh"
+
 namespace grl {
 namespace tc {
 
@@ -160,6 +162,12 @@ __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
 }
 // Operand formats of the tensor-core path: FMT_F16 (default: 11-bit mantissa, saturating converts) or FMT_BF16.
 enum : int { FMT_F16 = 0, FMT_BF16 = 1 };
+inline int check_fmt(int fmt) {
+  GRL_REQUIRE(fmt == 0 || fmt == 1, "tc: operand format must be 0 (fp16) or 1 (bf16), got %d", fmt);
+  return GRL_OK;
+}
+// GrlTcGemm::epi: the fused epilogues of gemm_tc_kernel
+enum { EPI_BIAS_ACT = 0, EPI_QKV = 1, EPI_LN = 2 };
 __device__ __forceinline__ uint32_t pack_f16(float lo, float hi) {
   uint32_t d;
   asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(d) : "f"(hi), "f"(lo));

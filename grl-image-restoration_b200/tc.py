@@ -40,7 +40,7 @@ LN_MAX_C = 188  # the LayerNorm epilogue keeps a whole 128 x C fp32 row tile in 
 
 def supported(C, heads_w, heads_s):
     """Architectures the tensor-core path covers: head_dim <= 32 (one 32-wide slot per head), <= 8 heads per
-    attention, C % 4 == 0 and C <= LN_MAX_C (launch_gemm_tc's LayerNorm-epilogue limit).  Anything else runs on the
+    attention, C % 4 == 0 and C <= LN_MAX_C (plan_gemm_tc's LayerNorm-epilogue limit).  Anything else runs on the
     fp32 kernels ("auto") or is rejected up front (explicit "fp16" / "bf16")."""
     c = C // 2
     return (C % 4 == 0 and C <= LN_MAX_C and c % heads_w == 0 and c % heads_s == 0 and c // heads_w <= SLOT

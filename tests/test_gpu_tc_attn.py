@@ -127,7 +127,7 @@ EXTRAS = [
     AttnCase("extra: lazy rescale, generic KW (jpeg window)", "window", (36, 36), 1, True, 3, 30, 6.0),
 ]
 
-# key-window widths with their own template instance in launch_attn_tc's switch (attn_tc.cu); any other width runs KW = 0
+# key-window widths with their own template instance in grl_tc_attn's switch (attn_tc.cu); any other width runs KW = 0
 KW_TEMPLATES = (8, 16, 32, 64, 128)
 
 
