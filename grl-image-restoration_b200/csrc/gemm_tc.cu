@@ -8,11 +8,12 @@
 // 9 taps is the same TMA box shifted by (dy, dx) -- the zero padding of the convolution is TMA's out-of-bounds
 // fill, no im2col buffer exists (CAB convs mixed_attn_block.py:973-977, TransformerStage.conv grl.py:164-170).
 //
-// Warp roles (288 threads): warps 0-7 = two consumer warpgroups (rows 0-63 / 64-127 of the tile, wgmma m64n64k16 per
-// 64 output columns, accumulators in registers), warp 8 = TMA producer feeding a 4-stage ring.  After the main loop the
-// accumulators go to an fp32 tile in shared memory, and the same 256 threads run the epilogue with two threads per
-// accumulator row (the row's 32-column chunks split between them, LayerNorm moments merged through shared memory).
-// These GEMMs are short-K and HBM / epilogue bound, not tensor bound (DESIGN.md).
+// 256 threads = two warpgroups (rows 0-63 / 64-127 of the tile, wgmma m64n64k16 per 64 output columns, accumulators
+// in registers); thread 0 also issues the TMA loads into a 2-4 stage ring.  The epilogue works on the accumulator
+// fragments themselves: the 4 threads of a quad hold whole rows, so LayerNorm moments and per-slot norms are quad
+// shuffles.  No fp32 tile goes through shared memory, and up to BN = 192 two CTAs share an SM, one tile's epilogue
+// overlapping the other's loads and MMAs.  These GEMMs are short-K and HBM / epilogue bound, not tensor bound
+// (DESIGN.md).
 //
 // Epilogues:
 //   EPI_BIAS_ACT : y = act(acc + b) (+ res)                       -> bf16 and/or fp32     (fc1, CAB, convs, heads)
@@ -64,61 +65,54 @@ __device__ __forceinline__ float tc_act(float v, int act, float slope) {
   return v;
 }
 
-constexpr int kStages = 4;
 constexpr int kBM = 128, kBK = 64;
 constexpr int kTH = 8, kTW = 16;  // conv patch (kTH * kTW == kBM)
-constexpr int kEpiWarps = 8, kEpiThreads = kEpiWarps * 32, kThreads = kEpiThreads + 32;
+constexpr int kWarps = 8, kThreads = kWarps * 32;
+// CTAs per SM.  Up to BN = 192 two CTAs share an SM, so that one tile's epilogue runs while the other tile's loads and
+// MMAs are in flight: 2 x 8 warps leave 128 registers per thread (each quarter of the register file serves 4 warps;
+// BN = 192 holds 96 accumulators) and ~113 KB of shared memory per CTA.  BN = 256 holds 128 accumulators: one CTA.
+__host__ __device__ constexpr int ctas_per_sm(int bn) { return bn <= 192 ? 2 : 1; }
 
-// Epilogue staging: the accumulator tile is first written to shared memory by its row owners (phase A, thread = row),
-// then streamed to global memory row-major by all epilogue threads with 16-byte accesses (phase B) -- fully coalesced
-// residual reads and stores with many independent requests in flight.
-//   fp32 staging (LayerNorm / fp32 outputs): [128][pitch32] floats, pitch32 % 8 == 4  -> conflict-free 16 B rows
-//   16-bit staging (fp16/bf16-only outputs): [128][BN + 8] halves
-__host__ __device__ constexpr int stage_pitch32(int c) { return (c % 8 == 4) ? c : ((c + 3) / 4 * 4 % 8 == 4 ? (c + 3) / 4 * 4 : (c + 3) / 4 * 4 + 4); }
-
-// Shared memory: the operand ring and, once the main loop is over, the fp32 accumulator tile [128][BN + 4] followed by
-// the staging tile (both alias the ring).
+// Shared memory: the operand ring (up to 4 stages, at most 100 KB when two CTAs share the SM) and, once the main loop
+// is over, the epilogue's staging (aliases the ring): the 16-bit output tile [128][BN + 8] that makes row-major 16-byte
+// stores, or two fp32 row chunks [128][72]; then the per-CTA tables.
 template <int BN>
 struct GemmSmem {
   static constexpr int A_BYTES = kBM * kBK * 2;
   static constexpr int B_BYTES = BN * kBK * 2;
   static constexpr int STAGE = A_BYTES + B_BYTES;
-  static constexpr int PIPE = kStages * STAGE;
-  static constexpr int AP = BN + 4;  // accumulator pitch (floats): AP % 8 == 4, conflict-free 16-byte row reads
-  static constexpr int ACC = kBM * AP * 4;
-  static constexpr int STG32 = kBM * stage_pitch32(BN <= 192 ? (BN == 192 ? 188 : BN) : 4) * 4;  // C <= 188 at BN = 192
-  static constexpr int STG16 = kBM * (BN + 8) * 2;
-  static constexpr int STG = (STG32 > STG16 ? STG32 : STG16);
-  static constexpr int OFF_STG = ACC;
-  static constexpr int OFF_TOK = ((PIPE > ACC + STG ? PIPE : ACC + STG) + 15) / 16 * 16;  // long long tok[128]
-  static constexpr int OFF_PAR = OFF_TOK + 128 * 8 + 128 * 4;  // (+ int img[128]) float bias[BN], gamma[BN], beta[BN]
-  static constexpr int OFF_MOM = OFF_PAR + 3 * BN * 4;         // float mom[2][128][3]
-  static constexpr int OFF_BAR = OFF_MOM + 2 * 128 * 3 * 4;
-  static constexpr int TOTAL = OFF_BAR + 128 + 1024 /*align slack*/;
-  static_assert(AP % 8 == 4, "accumulator pitch");
-  static_assert(TOTAL <= 232448, "shared memory budget");
+  static constexpr int RING = ctas_per_sm(BN) == 2 ? 100 * 1024 : 4 * STAGE;
+  static constexpr int STAGES = RING / STAGE < 4 ? RING / STAGE : 4;
+  static constexpr int PIPE = STAGES * STAGE;
+  static constexpr int P16 = BN + 8;  // 16-bit tile pitch (halves): (BN + 8) / 2 % 32 == 4, conflict-free quad writes
+  static constexpr int OFF_TOK = PIPE;                         // long long tok[128], int img[128]
+  static constexpr int OFF_PAR = OFF_TOK + 128 * 8 + 128 * 4;  // float bias[BN], gamma[BN], beta[BN]
+  static constexpr int OFF_BAR = OFF_PAR + 3 * BN * 4;
+  static constexpr int TOTAL = OFF_BAR + STAGES * 8 + 1024 /*align slack*/;
+  static_assert(STAGES >= 2, "operand ring");
+  static_assert(kBM * P16 * 2 <= PIPE, "16-bit tile fits the ring");
+  static_assert(ctas_per_sm(BN) * (TOTAL + 1024) <= 232448, "shared memory per SM (1 KB reserved per CTA)");
 };
 
-__device__ __forceinline__ void epi_barrier() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
-
-// 32 consecutive fp32 accumulator values of one row
-__device__ __forceinline__ void acc_row32(const float* p, uint32_t (&v)[32]) {
-#pragma unroll
-  for (int j = 0; j < 32; j += 4) {
-    const uint4 x = *reinterpret_cast<const uint4*>(p + j);
-    v[j] = x.x, v[j + 1] = x.y, v[j + 2] = x.z, v[j + 3] = x.w;
-  }
+// sum over the 4 threads of a quad (the threads that hold one accumulator row)
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
 
-// Main loop of consumer warpgroup `half`: rows [64 half, 64 half + 64) of the tile, BN / 64 accumulators of m64n64.
+// Main loop of warpgroup `half`: rows [64 half, 64 half + 64) of the tile, BN / 64 accumulators of m64n64.  Thread 0
+// issues the TMA loads (load(kc) fills stage kc % STAGES and arms its full barrier): the first STAGES chunks up front,
+// then chunk kc - 1 + STAGES once both warpgroups have finished the MMAs that read chunk kc - 1.
 // FMT is a template argument so that no branch separates the wgmma instructions of one k step.
-template <int BN, int FMT>
-__device__ __forceinline__ void mma_loop(float (&acc)[BN / 64][32], uint8_t* smem, uint64_t* full, uint64_t* empty,
-                                         int nk_total, int half, int et) {
+template <int BN, int FMT, class Load>
+__device__ __forceinline__ void mma_loop(float (&acc)[BN / 64][32], uint8_t* smem, uint64_t* full, int nk_total,
+                                         int half, const Load& load) {
   using S = GemmSmem<BN>;
   for (int kc = 0; kc < nk_total; ++kc) {
-    const int s = kc % kStages;
-    mbar_wait(&full[s], (kc / kStages) & 1);
+    const int s = kc % S::STAGES;
+    // The previous step's MMAs are in flight here.  ptxas reports C7517 for every instance: it puts a wait for them on
+    // mbar_wait's trap branch (a protocol fault), not on this path, which keeps one k step in flight.
+    mbar_wait(&full[s], (kc / S::STAGES) & 1);
     const uint32_t sa = smem_u32(smem + s * S::STAGE) + half * (64 * 128);
     const uint32_t sb = smem_u32(smem + s * S::STAGE + S::A_BYTES);
     wgmma_fence();
@@ -133,9 +127,12 @@ __device__ __forceinline__ void mma_loop(float (&acc)[BN / 64][32], uint8_t* sme
       }
     }
     wgmma_commit();
-    // this k step's MMAs stay in flight; the previous step's are complete, so its stage goes back to the producer
+    // this k step's MMAs stay in flight; the previous step's are complete, so its stage can be refilled
     wgmma_wait<1>();
-    if (kc > 0 && (et & 127) == 0) mbar_arrive(&empty[(kc - 1) % kStages]);
+    if (kc > 0 && kc - 1 + S::STAGES < nk_total) {
+      __syncthreads();  // ... by both warpgroups
+      if (threadIdx.x == 0) load(kc - 1 + S::STAGES);
+    }
   }
   wgmma_wait<0>();
 }
@@ -146,29 +143,28 @@ struct GemmTcPlan {
   int nk;        // 64-wide k chunks per tap
   int n_tiles, total_tiles;
   int tiles_x, tiles_y;  // conv: 8 x 16 pixel patches per image
-  int epi_mode;  // 0 = 16-bit staging, 1 = fp32 staging, 2 = direct
+  int epi_mode;  // 0 = 16-bit outputs, 1 = whole fp32 rows (LayerNorm / fp32 output / residual), 2 = direct
   int nchw_r;    // GrlTcGemm::nchw_r, at least 1
 };
 
 template <int BN, int EPI, bool CONV>
-__global__ void __launch_bounds__(kThreads, 1)
+__global__ void __launch_bounds__(kThreads, ctas_per_sm(BN))
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GrlTcGemm a,
               const GemmTcPlan pl) {
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  // 1024-byte aligned (SWIZZLE_128B operands) by pointer arithmetic, so that the compiler keeps the shared state space
+  // (LDS / STS with 32-bit addresses in the epilogue, not generic accesses)
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   using S = GemmSmem<BN>;
-  constexpr int AP = S::AP;
+  constexpr int NJ = BN / 64;
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + S::OFF_BAR);
-  uint64_t* empty = full + kStages;
   long long* s_tok = reinterpret_cast<long long*>(smem + S::OFF_TOK);
   int* s_img = reinterpret_cast<int*>(smem + S::OFF_TOK + 128 * 8);  // image (batch) index of every row (CAB gate)
   float* s_bias = reinterpret_cast<float*>(smem + S::OFF_PAR);      // this tile's columns [n0, n0 + BN)
   float* s_gamma = s_bias + BN;
   float* s_beta = s_gamma + BN;
-  float* s_mom = reinterpret_cast<float*>(smem + S::OFF_MOM);  // [2][128][3]: (mean, M2, n) of each column half of a row
-  float* accs = reinterpret_cast<float*>(smem);                // [128][AP] after the main loop
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int lane = threadIdx.x & 31;
   // 1-D grid, N tile fastest: the CTAs that share an A tile (same rows, different output columns) are scheduled
   // together, so the tile is read from DRAM once and from L2 afterwards (QKV: 3 column tiles, fc1: 2).
   const int n_tiles = pl.n_tiles;
@@ -188,328 +184,319 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     m0 = m_idx * kBM;
   }
 
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < kStages; ++s) {
-      mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 2);  // one arrival per consumer warpgroup
+  // TMA: chunk kc of the A tile (a tap's shifted box for a conv) and of the W tile into stage kc % STAGES
+  auto load = [&](int kc) {
+    const int s = kc % S::STAGES;
+    uint8_t* sa = smem + s * S::STAGE;
+    uint8_t* sb = sa + S::A_BYTES;
+    mbar_expect_tx(&full[s], S::STAGE);
+    if (CONV) {
+      const int tap = kc / pl.nk, c0 = (kc - tap * pl.nk) * kBK;
+      tma_load_4d(sa, &tmA, &full[s], c0, tx0 + (tap % 3) - 1, ty0 + (tap / 3) - 1, tb);
+    } else {
+      tma_load_2d(sa, &tmA, &full[s], kc * kBK, m0);
     }
+    tma_load_2d(sb, &tmB, &full[s], kc * kBK, n0);
+  };
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < S::STAGES; ++s) mbar_init(&full[s], 1);
     mbar_init_fence();
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
+    for (int kc = 0; kc < S::STAGES && kc < nk_total; ++kc) load(kc);
   }
-  __syncthreads();
 
-  if (warp == kEpiWarps) {
-    // ================================================================== TMA producer
-    if (lane == 0) {
-      for (int kc = 0; kc < nk_total; ++kc) {
-        const int s = kc % kStages;
-        mbar_wait(&empty[s], ((kc / kStages) & 1) ^ 1);
-        uint8_t* sa = smem + s * S::STAGE;
-        uint8_t* sb = sa + S::A_BYTES;
-        mbar_expect_tx(&full[s], S::STAGE);
-        if (CONV) {
-          const int tap = kc / pl.nk, c0 = (kc - tap * pl.nk) * kBK;
-          tma_load_4d(sa, &tmA, &full[s], c0, tx0 + (tap % 3) - 1, ty0 + (tap / 3) - 1, tb);
-        } else {
-          tma_load_2d(sa, &tmA, &full[s], kc * kBK, m0);
+  const int et = threadIdx.x;  // 0..255
+  const int half = et >> 7;    // MMA warpgroup: rows [64 half, 64 half + 64)
+  const int fmt = a.fmt;
+  uint16_t* out16 = reinterpret_cast<uint16_t*>(a.out_bf16);
+  // per-tile tables: token (global row) of every accumulator row (-1 = outside the problem), its image, and the
+  // per-column constants of this N tile
+  if (et < kBM) {
+    long long tok;
+    if (CONV) {
+      const int y = ty0 + et / kTW, x = tx0 + et % kTW;
+      tok = (y < a.H && x < a.W) ? ((long long)tb * a.H + y) * a.W + x : -1;
+    } else {
+      tok = (long long)m0 + et;
+      if (tok >= pl.M) tok = -1;
+    }
+    s_tok[et] = tok;
+    s_img[et] = (EPI == EPI_LN && tok >= 0) ? (int)(tok / a.L) : 0;  // one 64-bit division per row, not per access
+  }
+  for (int c = et; c < BN; c += kThreads) {
+    const int n = n0 + c;
+    s_bias[c] = (n < a.n_store) ? a.bias[n] : 0.f;
+    if (EPI == EPI_LN) {
+      s_gamma[c] = (c < a.C) ? a.gamma[c] : 0.f;
+      s_beta[c] = (c < a.C) ? a.beta[c] : 0.f;
+    }
+  }
+
+  float acc[NJ][32];
+#pragma unroll
+  for (int j = 0; j < NJ; ++j)
+#pragma unroll
+    for (int e = 0; e < 32; ++e) acc[j][e] = 0.f;
+  __syncthreads();  // the barriers are initialised and the tables written
+  if (fmt == FMT_BF16) mma_loop<BN, FMT_BF16>(acc, smem, full, nk_total, half, load);
+  else mma_loop<BN, FMT_F16>(acc, smem, full, nk_total, half, load);
+  __syncthreads();  // both warpgroups are done reading the ring: it becomes the epilogue's staging area
+
+  // ---------------- epilogue on the accumulator fragments (tc_common.cuh): this thread holds rows r0 and r0 + 8
+  // (h = 0, 1), columns 64 j + 8 i + cq + {0, 1}; the 4 threads of a quad hold the whole of both rows.
+  // acc[j][4 i + 2 h + e]  <->  row r0 + 8 h, column 64 j + 8 i + cq + e
+  const int r0 = half * 64 + 16 * ((et >> 5) & 3) + (lane >> 2), cq = 2 * (lane & 3);
+#pragma unroll
+  for (int j = 0; j < NJ; ++j)
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const float2 b = *reinterpret_cast<const float2*>(s_bias + 64 * j + 8 * i + cq);
+      acc[j][4 * i] += b.x, acc[j][4 * i + 1] += b.y, acc[j][4 * i + 2] += b.x, acc[j][4 * i + 3] += b.y;
+    }
+  uint16_t* stg = reinterpret_cast<uint16_t*>(smem);  // [128][P16]
+  constexpr int P16 = S::P16;
+
+  // epi_mode (chosen on the host): 1 = whole fp32 rows in this tile (LayerNorm / fp32 result / residual), 0 = 16-bit
+  // outputs only, 2 = direct per-element stores (odd widths such as the 3-channel image head)
+  if (EPI == EPI_BIAS_ACT && pl.epi_mode == 2) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = r0 + 8 * h;
+      const long long t = s_tok[row];
+      if (t < 0) continue;
+#pragma unroll
+      for (int j = 0; j < NJ; ++j)
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const int c = 64 * j + 8 * i + cq;
+          if (n0 + (c & ~31) >= a.n_store) continue;  // 32-column chunks past the stored columns are not written
+          float o[2];
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int n = n0 + c + e;
+            float val = tc_act(acc[j][4 * i + 2 * h + e], a.act, a.slope);
+            if (a.res_f32 && n < a.n_real) val += __ldg(a.res_f32 + t * a.ldr + n);
+            o[e] = (n < a.n_store) ? val : 0.f;
+            if (a.out_f32 && n < a.n_real) a.out_f32[t * a.ldo_f32 + n] = o[e];
+            if (CONV && a.out_nchw && n < a.n_real) {
+              // tail fusion: x / img_range + mean (grl.py:549), the crop (:551), channels-last -> bchw and, for the
+              // one-step head, PixelShuffle (upsample.py:33-50; torch order n = c r^2 + dy r + dx) folded into the store
+              const int r = pl.nchw_r, rr = r * r;
+              const int ch = n / rr, q = n - ch * rr;
+              const int yy = (ty0 + row / kTW) * r + q / r, xx = (tx0 + row % kTW) * r + q % r;
+              if (yy < a.Hc && xx < a.Wc)
+                a.out_nchw[(((long long)tb * (a.n_real / rr) + ch) * a.Hc + yy) * a.Wc + xx] =
+                    fmaf(o[e], a.post_scale, a.post_shift[ch & 3]);
+            }
+          }
+          if (out16 && n0 + (c & ~7) < a.ldo_bf16)
+            *reinterpret_cast<uint32_t*>(out16 + t * a.ldo_bf16 + n0 + c) = pack16(o[0], o[1], fmt);
         }
-        tma_load_2d(sb, &tmB, &full[s], kc * kBK, n0);
-      }
     }
     return;
   }
 
-  // ================================================================== consumers: MMA, then the epilogue (256 threads)
-  const int et = threadIdx.x;      // 0..255
-  const int q = warp & 3;          // row quarter of this warp in phase A
-  const int row = q * 32 + lane;   // accumulator row owned in phase A
-  const int half = et >> 7;        // which chunks of the row: c0 = 32 * half, + 64, ...  (also: the MMA warpgroup)
-  const int fmt = a.fmt;
-  uint16_t* out16 = reinterpret_cast<uint16_t*>(a.out_bf16);
-  // per-tile tables: token (global row) of every accumulator row (-1 = outside the problem), its image, and the
-  // per-column constants of this N tile (every row-owner thread needs all of them: smem broadcast)
-  {
-    long long tok;
-    if (CONV) {
-      const int y = ty0 + row / kTW, x = tx0 + row % kTW;
-      tok = (y < a.H && x < a.W) ? ((long long)tb * a.H + y) * a.W + x : -1;
-    } else {
-      tok = (long long)m0 + row;
-      if (tok >= pl.M) tok = -1;
-    }
-    if (half == 0) {
-      s_tok[row] = tok;
-      s_img[row] = (EPI == EPI_LN && tok >= 0) ? (int)(tok / a.L) : 0;  // one 64-bit division per row, not per access
-    }
-    for (int c = et; c < BN; c += kEpiThreads) {
-      const int n = n0 + c;
-      s_bias[c] = (n < a.n_store) ? a.bias[n] : 0.f;
-      if (EPI == EPI_LN) {
-        s_gamma[c] = (c < a.C) ? a.gamma[c] : 0.f;
-        s_beta[c] = (c < a.C) ? a.beta[c] : 0.f;
+  if (EPI == EPI_LN || pl.epi_mode == 1) {  // LayerNorm always has mode 1
+    // n0 == 0: the tile holds whole rows.  The rows go through shared memory 64 columns at a time, in two fp32 buffers
+    // [128][72] that alias the idle ring: the residual of chunk j + 1 is fetched with cp.async (16 B per request) while
+    // chunk j is finished, the fragments add their result in place, and the chunk is streamed row-major (CAB term,
+    // fp32 store, 16-bit copy) -- coalesced residual reads and stores with many requests in flight.
+    const int Cw = (EPI == EPI_LN) ? a.C : a.n_real;  // real fp32 columns, Cw % 4 == 0
+    constexpr int RP = 72;                             // pitch % 32 == 8: conflict-free float2 quad writes
+    static_assert(2 * kBM * RP * 4 <= S::PIPE, "two fp32 chunk buffers fit the ring");
+    float* rbuf = reinterpret_cast<float*>(smem);
+    const bool has_res = a.res_f32 != nullptr;
+    auto fetch = [&](int j) {  // residual columns [64 j, 64 j + 64) of every row -> buffer j % 2
+      if (has_res)
+        for (int idx = et; idx < kBM * 16; idx += kThreads) {
+          const int r = idx >> 4, c = 64 * j + 4 * (idx & 15);
+          const long long t = s_tok[r];
+          if (c < Cw) cp_async_16(rbuf + (j & 1) * kBM * RP + r * RP + (c & 63), a.res_f32 + (t >= 0 ? t : 0) * a.ldr + c, t >= 0);
+        }
+      cp_async_commit();
+    };
+    fetch(0);
+    float mean[2] = {0.f, 0.f}, rstd[2] = {0.f, 0.f};
+    if (EPI == EPI_LN) {
+      // Shifted single-pass moments of each row: x0 = the row's first element (no catastrophic cancellation),
+      // mean = x0 + S1/n, M2 = S2 - S1^2/n with S1 = sum(x - x0), S2 = sum((x - x0)^2); the quad's partial sums are added.
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const float x0 = __shfl_sync(0xffffffffu, acc[0][2 * h], lane & ~3);
+        float s1 = 0.f, s2 = 0.f;
+#pragma unroll
+        for (int j = 0; j < NJ; ++j)
+#pragma unroll
+          for (int i = 0; i < 8; ++i)
+            if (64 * j + 8 * i < Cw - cq) {  // both columns of the pair: Cw and cq are even
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                const float d = acc[j][4 * i + 2 * h + e] - x0;
+                s1 += d;
+                s2 = fmaf(d, d, s2);
+              }
+            }
+        s1 = quad_sum(s1);
+        s2 = quad_sum(s2);
+        const float fn = (float)Cw, m1 = s1 / fn;
+        mean[h] = x0 + m1;
+        rstd[h] = rsqrtf(fmaxf(s2 - s1 * m1, 0.f) / fn + a.eps);
       }
     }
-  }
-  {
-    // warpgroup `half` computes rows [64 half, 64 half + 64): BN / 64 accumulators of m64n64
-    float acc[BN / 64][32];
+    const bool has_cab = (EPI == EPI_LN) && a.cab_y != nullptr;
+    const uint16_t* caby = reinterpret_cast<const uint16_t*>(a.cab_y);
+    const int ew = et >> 5, c4 = lane & 15;  // row-major pass: a warp covers 2 rows of a chunk per step
 #pragma unroll
-    for (int j = 0; j < BN / 64; ++j)
-#pragma unroll
-      for (int e = 0; e < 32; ++e) acc[j][e] = 0.f;
-    if (fmt == FMT_BF16) mma_loop<BN, FMT_BF16>(acc, smem, full, empty, nk_total, half, et);
-    else mma_loop<BN, FMT_F16>(acc, smem, full, empty, nk_total, half, et);
-    epi_barrier();  // both warpgroups are done reading the ring: it becomes the accumulator / staging tile
-    const int w = (et >> 5) & 3, r0 = half * 64 + 16 * w + (lane >> 2), cq = 2 * (lane & 3);
-#pragma unroll
-    for (int j = 0; j < BN / 64; ++j)
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const int c = j * 64 + 8 * i + cq;
-        *reinterpret_cast<float2*>(accs + r0 * AP + c) = make_float2(acc[j][4 * i], acc[j][4 * i + 1]);
-        *reinterpret_cast<float2*>(accs + (r0 + 8) * AP + c) = make_float2(acc[j][4 * i + 2], acc[j][4 * i + 3]);
+    for (int j = 0; j < NJ; ++j) {
+      if (64 * j >= Cw) break;
+      if (j > 0) __syncthreads();  // every thread is done reading chunk j - 1's buffer, which chunk j + 1 refills
+      if (64 * (j + 1) < Cw) {
+        fetch(j + 1);
+        cp_async_wait<1>();
+      } else {
+        cp_async_wait<0>();
       }
-  }
-  epi_barrier();
-  uint32_t v[32];
-
-    // epi_mode (chosen on the host): 1 = fp32 staging (LayerNorm / fp32 result / residual, whole row in this tile),
-    // 0 = 16-bit staging, 2 = direct per-row stores (odd widths such as the 3-channel image head)
-    if (EPI == EPI_BIAS_ACT && pl.epi_mode == 2) {
-      const long long tok = s_tok[row];
-      for (int c0 = 32 * half; c0 < BN; c0 += 64) {
-        if (n0 + c0 >= a.n_store) break;
-        acc_row32(accs + row * AP + c0, v);
-        if (tok < 0) continue;
-        float o[32];
+      __syncthreads();  // chunk j's residual has landed for every thread
+      float* buf = rbuf + (j & 1) * kBM * RP;
 #pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          const int n = n0 + c0 + j;
-          float val = tc_act(__uint_as_float(v[j]) + s_bias[c0 + j], a.act, a.slope);
-          if (a.res_f32 && n < a.n_real) val += __ldg(a.res_f32 + tok * a.ldr + n);
-          o[j] = (n < a.n_store) ? val : 0.f;
-          if (a.out_f32 && n < a.n_real) a.out_f32[tok * a.ldo_f32 + n] = o[j];
-          if (CONV && a.out_nchw && n < a.n_real) {
-            // tail fusion: x / img_range + mean (grl.py:549), the crop (:551), channels-last -> bchw and, for the one-step
-            // head, PixelShuffle (upsample.py:33-50; torch order n = c r^2 + dy r + dx) folded into the store
-            const int r = pl.nchw_r, rr = r * r;
-            const int c = n / rr, q = n - c * rr;
-            const int yy = (ty0 + row / kTW) * r + q / r, xx = (tx0 + row % kTW) * r + q % r;
-            if (yy < a.Hc && xx < a.Wc)
-              a.out_nchw[(((long long)tb * (a.n_real / rr) + c) * a.Hc + yy) * a.Wc + xx] = fmaf(o[j], a.post_scale, a.post_shift[c & 3]);
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int i = 0; i < 8; ++i)
+          if (64 * j + 8 * i < Cw - cq) {
+            float2* p = reinterpret_cast<float2*>(buf + (r0 + 8 * h) * RP + 8 * i + cq);
+            float2 o = has_res ? *p : make_float2(0.f, 0.f);
+            const float v0 = acc[j][4 * i + 2 * h], v1 = acc[j][4 * i + 2 * h + 1];
+            if (EPI == EPI_LN) {
+              const int c = 64 * j + 8 * i + cq;
+              const float2 g = *reinterpret_cast<const float2*>(s_gamma + c), be = *reinterpret_cast<const float2*>(s_beta + c);
+              o.x += ((v0 - mean[h]) * rstd[h] * g.x + be.x) * a.res_scale;
+              o.y += ((v1 - mean[h]) * rstd[h] * g.y + be.y) * a.res_scale;
+            } else {
+              o.x += tc_act(v0, a.act, a.slope);
+              o.y += tc_act(v1, a.act, a.slope);
+            }
+            *p = o;
+          }
+      __syncthreads();
+      // rows ew + 8 k (k = 0..15), two per step; the loads of RB steps are issued before their stores (the compiler
+      // cannot prove the output and CAB pointers distinct).  The LayerNorm instance batches 2 steps: its CAB operands
+      // are 6 registers per step, and at BN = 192 a batch of 4 spills next to the chunks' accumulators.
+      const int c = 64 * j + 4 * c4;
+      const bool col_real = c < Cw;
+      constexpr int RB = EPI == EPI_LN ? 2 : 4;
+#pragma unroll
+      for (int k0 = 0; k0 < 16; k0 += 2 * RB) {
+        long long tk[RB];
+        uint2 cy[RB];
+        float4 gg[RB];
+#pragma unroll
+        for (int u = 0; u < RB; ++u) {
+          const int r = ew + 8 * (k0 + 2 * u + (lane >> 4));
+          tk[u] = s_tok[r];
+          cy[u] = make_uint2(0u, 0u);
+          gg[u] = make_float4(0.f, 0.f, 0.f, 0.f);
+          if (has_cab && tk[u] >= 0 && col_real) {
+            cy[u] = __ldg(reinterpret_cast<const uint2*>(caby + tk[u] * a.ld_caby + c));
+            gg[u] = __ldg(reinterpret_cast<const float4*>(a.cab_gate + (long long)s_img[r] * Cw + c));
           }
         }
-        if (out16) {
 #pragma unroll
-          for (int j = 0; j < 32; j += 8)
-            if (n0 + c0 + j < a.ldo_bf16)
-              *reinterpret_cast<uint4*>(out16 + tok * a.ldo_bf16 + n0 + c0 + j) =
-                  make_uint4(pack16(o[j], o[j + 1], fmt), pack16(o[j + 2], o[j + 3], fmt), pack16(o[j + 4], o[j + 5], fmt),
-                             pack16(o[j + 6], o[j + 7], fmt));
+        for (int u = 0; u < RB; ++u) {
+          const int r = ew + 8 * (k0 + 2 * u + (lane >> 4));
+          if (tk[u] < 0) continue;
+          float4 val = make_float4(0.f, 0.f, 0.f, 0.f);
+          if (col_real) {
+            val = *reinterpret_cast<const float4*>(buf + r * RP + 4 * c4);
+            if (has_cab) {
+              const float2 c01 = unpack16(cy[u].x, fmt), c23 = unpack16(cy[u].y, fmt);
+              val.x = fmaf(c01.x, gg[u].x, val.x), val.y = fmaf(c01.y, gg[u].y, val.y);
+              val.z = fmaf(c23.x, gg[u].z, val.z), val.w = fmaf(c23.y, gg[u].w, val.w);
+            }
+            if (a.out_f32) *reinterpret_cast<float4*>(a.out_f32 + tk[u] * a.ldo_f32 + c) = val;
+          }
+          if (out16 && c < a.ldo_bf16)
+            *reinterpret_cast<uint2*>(out16 + tk[u] * a.ldo_bf16 + c) =
+                make_uint2(pack16(val.x, val.y, fmt), pack16(val.z, val.w, fmt));
         }
       }
-    } else if (pl.epi_mode == 1) {
-      const int Cw = (EPI == EPI_LN) ? a.C : a.n_real;  // real fp32 columns of this tile row (n0 == 0 when wide)
-      const int pitch = stage_pitch32(Cw);
-      float* stg = reinterpret_cast<float*>(smem + S::OFF_STG);
-      // ---------------- residual tile -> staging, asynchronously (cp.async, 16 B per request, the whole 128 x C
-      // tile in flight at once); it lands while the row moments are computed from the accumulator tile.  Phase A then adds its
-      // result in place, so phase B has no fp32 loads left.
-      const bool res_in_stage = a.res_f32 != nullptr;
-      if (res_in_stage) {
-        const int C4r = Cw >> 2, ewr = et >> 5;
-        for (int r = ewr; r < kBM; r += kEpiWarps) {
-          const long long rtok = s_tok[r];
-          for (int c4 = lane; c4 < C4r; c4 += 32)
-            cp_async_16(stg + r * pitch + c4 * 4, a.res_f32 + (rtok >= 0 ? rtok : 0) * a.ldr + c4 * 4, rtok >= 0);
-        }
-        cp_async_commit();
+    }
+    // the 16-bit copy is written up to its pitch: zero beyond the last chunk
+    if (out16) {
+      const int cz = (Cw + 63) / 64 * 64;
+      for (int idx = et; idx < kBM * ((a.ldo_bf16 - cz) >> 2); idx += kThreads) {
+        const int per = (a.ldo_bf16 - cz) >> 2, r = idx / per, c = cz + 4 * (idx - r * per);
+        const long long t = s_tok[r];
+        if (t >= 0) *reinterpret_cast<uint2*>(out16 + t * a.ldo_bf16 + c) = make_uint2(0u, 0u);
       }
-      // ---------------- phase A
-      if (EPI == EPI_LN) {
-        // One pass over the accumulator row for the moments of THIS THREAD'S HALF of the row (its 32-column chunks), shifted by the half's
-        // first element (no catastrophic cancellation): mean_h = x0 + S1/n, M2_h = S2 - S1^2/n with S1 = sum(x - x0),
-        // S2 = sum((x - x0)^2).  The two halves are merged with the pairwise update (Chan et al.):
-        //   mean = mean_0 + d n_1 / n,  M2 = M2_0 + M2_1 + d^2 n_0 n_1 / n,  d = mean_1 - mean_0.
-        float s1 = 0.f, s2 = 0.f, x0 = 0.f;
-        int nh = 0;
-        for (int c0 = 32 * half; c0 < Cw; c0 += 64) {
-          acc_row32(accs + row * AP + c0, v);
-          if (c0 == 32 * half) x0 = __uint_as_float(v[0]) + s_bias[c0];
+    }
+    return;
+  }
+  {
+    // 16-bit outputs only
 #pragma unroll
-          for (int j = 0; j < 32; ++j)
-            if (c0 + j < Cw) {
-              const float d = __uint_as_float(v[j]) + s_bias[c0 + j] - x0;
-              s1 += d;
-              s2 = fmaf(d, d, s2);
-              ++nh;
-            }
-        }
-        {
-          const float fn = (float)nh;
-          const float m1 = nh > 0 ? s1 / fn : 0.f;
-          s_mom[(half * kBM + row) * 3 + 0] = x0 + m1;
-          s_mom[(half * kBM + row) * 3 + 1] = nh > 0 ? fmaxf(s2 - s1 * m1, 0.f) : 0.f;
-          s_mom[(half * kBM + row) * 3 + 2] = fn;
-        }
-        if (res_in_stage) cp_async_wait<0>();  // this thread's share of the residual tile has landed ...
-        epi_barrier();                         // ... and is visible to the row owners; so are both halves' moments
-        float mean, rstd;
-        {
-          const float m0 = s_mom[row * 3 + 0], q0 = s_mom[row * 3 + 1], c0n = s_mom[row * 3 + 2];
-          const float m1 = s_mom[(kBM + row) * 3 + 0], q1 = s_mom[(kBM + row) * 3 + 1], c1n = s_mom[(kBM + row) * 3 + 2];
-          const float n = c0n + c1n, d = (c1n > 0.f) ? m1 - m0 : 0.f;
-          mean = m0 + d * (c1n / n);
-          const float M2 = q0 + q1 + d * d * (c0n * c1n / n);
-          rstd = rsqrtf(M2 / n + a.eps);
-        }
-        for (int c0 = 32 * half; c0 < Cw; c0 += 64) {
-          acc_row32(accs + row * AP + c0, v);
+    for (int j = 0; j < NJ; ++j) {
+      if (EPI == EPI_QKV) {
+        // per 32-wide head slot: x / max(||x||, 1e-12) == x * rsqrt(max(||x||^2, 1e-24)); scale <= 0 marks a value slot
 #pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            if (c0 + j < Cw) {  // Cw % 4 == 0
-              float4* sp = reinterpret_cast<float4*>(stg + row * pitch + c0 + j);
-              float4 acc4 = res_in_stage ? *sp : make_float4(0.f, 0.f, 0.f, 0.f);
-              float o4[4] = {acc4.x, acc4.y, acc4.z, acc4.w};
+        for (int sh = 0; sh < 2; ++sh) {
+          const int n = n0 + 64 * j + 32 * sh;
+          const float sc = n < a.n_store ? __ldg(a.slot_scale + (n >> 5)) : 0.f;
 #pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                const int c = c0 + j + e;
-                o4[e] += ((__uint_as_float(v[j + e]) + s_bias[c] - mean) * rstd * s_gamma[c] + s_beta[c]) * a.res_scale;
-              }
-              *sp = make_float4(o4[0], o4[1], o4[2], o4[3]);
-            }
+          for (int h = 0; h < 2; ++h) {
+            float ss = 0.f;
+#pragma unroll
+            for (int i = 4 * sh; i < 4 * sh + 4; ++i)
+#pragma unroll
+              for (int e = 0; e < 2; ++e) ss = fmaf(acc[j][4 * i + 2 * h + e], acc[j][4 * i + 2 * h + e], ss);
+            ss = quad_sum(ss);
+            const float mul = sc > 0.f ? sc * rsqrtf(fmaxf(ss, 1e-24f)) : 1.0f;
+#pragma unroll
+            for (int i = 4 * sh; i < 4 * sh + 4; ++i) acc[j][4 * i + 2 * h] *= mul, acc[j][4 * i + 2 * h + 1] *= mul;
           }
         }
       } else {
-        if (res_in_stage) {
-          cp_async_wait<0>();
-          epi_barrier();
-        }
-        for (int c0 = 32 * half; c0 < Cw; c0 += 64) {
-          acc_row32(accs + row * AP + c0, v);
 #pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            if (c0 + j < Cw) {
-              float4* sp = reinterpret_cast<float4*>(stg + row * pitch + c0 + j);
-              float4 acc4 = res_in_stage ? *sp : make_float4(0.f, 0.f, 0.f, 0.f);
-              float o4[4] = {acc4.x, acc4.y, acc4.z, acc4.w};
-#pragma unroll
-              for (int e = 0; e < 4; ++e) o4[e] += tc_act(__uint_as_float(v[j + e]) + s_bias[c0 + j + e], a.act, a.slope);
-              *sp = make_float4(o4[0], o4[1], o4[2], o4[3]);
-            }
-          }
-        }
+        for (int e = 0; e < 32; ++e) acc[j][e] = tc_act(acc[j][e], a.act, a.slope);
       }
-      epi_barrier();
-      // ---------------- phase B: row-major streaming, 4 columns per thread, warp = row group.
-      // All global loads of a batch of RB rows are issued before any store (the compiler cannot prove the output
-      // and residual pointers distinct, so interleaving would serialise every row on a DRAM round trip).
-      const int C4 = Cw >> 2;                              // float4 items with real data
-      const int P4 = out16 ? (int)(a.ldo_bf16 >> 2) : C4;  // the 16-bit copy is written up to its (zero) pad
-      const int ew = et >> 5;
-      const bool has_cab = (EPI == EPI_LN) && a.cab_y != nullptr;
-      const uint16_t* caby = reinterpret_cast<const uint16_t*>(a.cab_y);
-      constexpr int RB = 8;
-      for (int cbase = 0; cbase < P4; cbase += 32) {
-        const int c4 = cbase + lane;
-        const bool col_real = c4 < C4, col_any = c4 < P4;
-        for (int rb = 0; rb < kBM / kEpiWarps; rb += RB) {  // this warp's rows: ew, ew + 8, ...
-          long long tok[RB];
-          float4 gg[RB];
-          uint2 cy[RB];
 #pragma unroll
-          for (int i = 0; i < RB; ++i) {
-            tok[i] = s_tok[ew + kEpiWarps * (rb + i)];
-            gg[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-            cy[i] = make_uint2(0u, 0u);
-            if (tok[i] >= 0 && col_real) {
-              if (has_cab) {
-                cy[i] = __ldg(reinterpret_cast<const uint2*>(caby + tok[i] * a.ld_caby + c4 * 4));
-                gg[i] = __ldg(reinterpret_cast<const float4*>(a.cab_gate + (long long)s_img[ew + kEpiWarps * (rb + i)] * Cw + c4 * 4));
-              }
-            }
-          }
+      for (int i = 0; i < 8; ++i)
 #pragma unroll
-          for (int i = 0; i < RB; ++i) {
-            if (tok[i] < 0 || !col_any) continue;
-            float4 val = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (col_real) {
-              val = *reinterpret_cast<const float4*>(stg + (ew + kEpiWarps * (rb + i)) * pitch + c4 * 4);
-              if (has_cab) {
-                const float2 c01 = unpack16(cy[i].x, fmt), c23 = unpack16(cy[i].y, fmt);
-                val.x = fmaf(c01.x, gg[i].x, val.x), val.y = fmaf(c01.y, gg[i].y, val.y);
-                val.z = fmaf(c23.x, gg[i].z, val.z), val.w = fmaf(c23.y, gg[i].w, val.w);
-              }
-              if (a.out_f32) *reinterpret_cast<float4*>(a.out_f32 + tok[i] * a.ldo_f32 + c4 * 4) = val;
-            }
-            if (out16)
-              *reinterpret_cast<uint2*>(out16 + tok[i] * a.ldo_bf16 + c4 * 4) =
-                  make_uint2(pack16(val.x, val.y, fmt), pack16(val.z, val.w, fmt));
-          }
-        }
-      }
-    } else {
-      // ---------------- 16-bit outputs only: phase A packs into a [128][BN + 8] tile
-      constexpr int P16 = BN + 8;
-      uint16_t* stg = reinterpret_cast<uint16_t*>(smem + S::OFF_STG);
-      const int ncols = min(BN, a.n_store - n0);  // columns of this tile that exist (multiple of 32)
-      for (int c0 = 32 * half; c0 < ncols; c0 += 64) {
-        acc_row32(accs + row * AP + c0, v);
-        float o[32];
-        if (EPI == EPI_QKV) {
-          const int slot = (n0 + c0) >> 5;
-          float ss = 0.f;
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            o[j] = __uint_as_float(v[j]) + s_bias[c0 + j];
-            ss = fmaf(o[j], o[j], ss);
-          }
-          const float sc = __ldg(a.slot_scale + slot);
-          // x / max(||x||, 1e-12) == x * rsqrt(max(||x||^2, 1e-24));  scale <= 0 marks a value slot
-          const float mul = sc > 0.f ? sc * rsqrtf(fmaxf(ss, 1e-24f)) : 1.0f;
-#pragma unroll
-          for (int j = 0; j < 32; ++j) o[j] *= mul;
-        } else {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) o[j] = tc_act(__uint_as_float(v[j]) + s_bias[c0 + j], a.act, a.slope);
-        }
-#pragma unroll
-        for (int j = 0; j < 32; j += 8)
-          *reinterpret_cast<uint4*>(stg + row * P16 + c0 + j) =
-              make_uint4(pack16(o[j], o[j + 1], fmt), pack16(o[j + 2], o[j + 3], fmt), pack16(o[j + 4], o[j + 5], fmt),
-                         pack16(o[j + 6], o[j + 7], fmt));
-      }
-      epi_barrier();
-      const int nvec = min((long long)ncols, (long long)a.ldo_bf16 - n0) >> 3;  // 16-byte vectors per row
-      const int ew = et >> 5;
-      if (CONV && a.ps_r > 0) {
-        // PixelShuffle folded into the store (upsample.py:6-30): the weights are packed so that column n' = q * Cq + c
-        // holds torch's channel c r^2 + q, i.e. Cq consecutive columns are ONE output pixel's channels
-        const int ps = a.ps_r, Cq = a.n_store / (ps * ps);
-        const int nv = min(BN, a.n_store - n0) >> 3;
+        for (int h = 0; h < 2; ++h)
+          *reinterpret_cast<uint32_t*>(stg + (r0 + 8 * h) * P16 + 64 * j + 8 * i + cq) =
+              pack16(acc[j][4 * i + 2 * h], acc[j][4 * i + 2 * h + 1], fmt);
+    }
+  }
+  if (!out16) return;
+  __syncthreads();
+  // ---------------- the 16-bit tile -> global memory, row-major with 16-byte stores, warp = row group
+  const int ew = et >> 5;
+  if (CONV && a.ps_r > 0) {
+    // PixelShuffle folded into the store (upsample.py:6-30): the weights are packed so that column n' = q * Cq + c
+    // holds torch's channel c r^2 + q, i.e. Cq consecutive columns are ONE output pixel's channels
+    const int ps = a.ps_r, Cq = a.n_store / (ps * ps);
+    const int nv = min(BN, a.n_store - n0) >> 3;
 #pragma unroll 4
-        for (int r = ew; r < kBM; r += kEpiWarps) {
-          if (s_tok[r] < 0) continue;
-          const int y = ty0 + r / kTW, x = tx0 + r % kTW;
-          for (int vv = lane; vv < nv; vv += 32) {
-            const int n = n0 + vv * 8;
-            const int q = n / Cq, c = n - q * Cq;
-            const long long dtok = ((long long)tb * a.H * ps + y * ps + q / ps) * ((long long)a.W * ps) + x * ps + q % ps;
-            *reinterpret_cast<uint4*>(out16 + dtok * a.ldo_bf16 + c) = *reinterpret_cast<const uint4*>(stg + r * P16 + vv * 8);
-          }
-        }
-      } else {
-#pragma unroll 4
-        for (int r = ew; r < kBM; r += kEpiWarps) {
-          const long long tok = s_tok[r];
-          if (tok < 0) continue;
-          for (int vv = lane; vv < nvec; vv += 32)
-            *reinterpret_cast<uint4*>(out16 + tok * a.ldo_bf16 + n0 + vv * 8) = *reinterpret_cast<const uint4*>(stg + r * P16 + vv * 8);
-        }
+    for (int r = ew; r < kBM; r += kWarps) {
+      if (s_tok[r] < 0) continue;
+      const int y = ty0 + r / kTW, x = tx0 + r % kTW;
+      for (int vv = lane; vv < nv; vv += 32) {
+        const int n = n0 + vv * 8;
+        const int q = n / Cq, c = n - q * Cq;
+        const long long dtok = ((long long)tb * a.H * ps + y * ps + q / ps) * ((long long)a.W * ps) + x * ps + q % ps;
+        *reinterpret_cast<uint4*>(out16 + dtok * a.ldo_bf16 + c) = *reinterpret_cast<const uint4*>(stg + r * P16 + vv * 8);
       }
     }
-
+  } else {
+    const int nvec = (int)(min((long long)min(BN, a.n_store - n0), (long long)a.ldo_bf16 - n0) >> 3);
+#pragma unroll 4
+    for (int r = ew; r < kBM; r += kWarps) {
+      const long long t = s_tok[r];
+      if (t < 0) continue;
+      for (int vv = lane; vv < nvec; vv += 32)
+        *reinterpret_cast<uint4*>(out16 + t * a.ldo_bf16 + n0 + vv * 8) = *reinterpret_cast<const uint4*>(stg + r * P16 + vv * 8);
+    }
+  }
 }
 
 // -------------------------------------------------------------------------------------
@@ -594,14 +581,14 @@ static int plan_gemm_tc(const GrlTcGemm& p, GemmTcPlan& pl, int* bn_out) {
                     p.n_real / (pl.nchw_r * pl.nchw_r) <= 4 && p.Hc > 0 && p.Wc > 0,
                 "gemm_tc: NCHW tail store needs a conv with <= 4 output channels");
   GRL_REQUIRE(p.taps == 1 || p.taps == 9, "gemm_tc: taps must be 1 or 9");
-  // Epilogue mode.  fp32 staging (LayerNorm, fp32 output, residual) needs the whole output row in one tile, 16-byte
-  // aligned fp32 rows and a tile that fits the staging area; anything else with an fp32 side takes the direct path.
+  // Epilogue mode.  Whole fp32 rows (LayerNorm, fp32 output, residual) need the whole output row in one tile, rows of
+  // 4-column multiples, and at most 188 fp32 columns (132 at BN = 256: the widths the mode has always covered, so that
+  // a launch keeps its path); anything else with an fp32 side takes the direct path.
   pl.epi_mode = 0;
   if (p.epi == EPI_LN || (p.epi == EPI_BIAS_ACT && (p.out_f32 || p.res_f32))) {
     const int cw = p.epi == EPI_LN ? p.C : p.n_real;
-    const int cap = bn == 64 ? GemmSmem<64>::STG : bn == 128 ? GemmSmem<128>::STG : bn == 192 ? GemmSmem<192>::STG
-                                                                                               : GemmSmem<256>::STG;
-    const bool ok = p.npad <= bn && cw > 0 && cw % 4 == 0 && kBM * stage_pitch32(cw) * 4 <= cap &&
+    const int cw_max = bn == 256 ? 132 : bn == 192 ? 188 : bn;
+    const bool ok = p.npad <= bn && cw > 0 && cw % 4 == 0 && cw <= cw_max &&
                     (!p.out_f32 || p.ldo_f32 % 4 == 0) && (!p.res_f32 || p.ldr % 4 == 0) &&
                     (!p.out_bf16 || p.ldo_bf16 % 4 == 0);
     GRL_REQUIRE(ok || p.epi != EPI_LN, "gemm_tc: LayerNorm epilogue needs C %% 4 == 0 and C <= 188 (got %d)", cw);

@@ -35,7 +35,7 @@ def round_up(a, b):
     return (a + b - 1) // b * b
 
 
-LN_MAX_C = 188  # the LayerNorm epilogue keeps a whole 128 x C fp32 row tile in the GEMM's staging area (gemm_tc.cu)
+LN_MAX_C = 188  # the widest LayerNorm row plan_gemm_tc takes (gemm_tc.cu)
 
 
 def supported(C, heads_w, heads_s):
