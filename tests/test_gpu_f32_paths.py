@@ -4,11 +4,10 @@ Launch paths.  An attention launch's signature (`attn_path`) is the kernel speci
 (window, stripe pass 1, stripe pass 2: this fixes dense V and dense output), the head_dim template D, d < D, a partial
 and a second 128-query tile, a partial and a second 32-key tile, the shift mask and a non-zero roll.  A GEMM's
 (`gemm_path`) is conv or linear, a partial last 16-wide k tile, the number of k tiles, a partial and a second 64-wide N
-tile, the activation, bias and residual.  The CPU tests walk the released configs (tiny / small / base x SR x2 x3 x4,
-dn, deblur, jpeg, dm at their smallest padded size) through f32_launches, the fp32 forward run in listing mode: its
-K.linear / K.conv3x3 calls and the passes of its K.window_attention / K.stripe_attention calls, and fail naming any path
-without a case.  test_recorded_launches_match_lists checks that list one for one against the C-ABI calls of real fp32
-forwards.
+tile, the activation, bias and residual.  The CPU tests walk every architecture of archs.architectures through
+f32_launches, the fp32 forward run in listing mode: its K.linear / K.conv3x3 calls and the passes of its
+K.window_attention / K.stripe_attention calls, and fail naming any path without a case.
+test_recorded_launches_match_lists checks that list one for one against the C-ABI calls of real fp32 forwards.
 
 Cases call the C ABI directly and write into NaN-filled buffers with guard rows (and guard columns where a pitch
 allows): every owned element must be written and nothing else.  Attention: 2 x 2 windows of the pass's grid, B = 2, the
@@ -35,13 +34,13 @@ of them the old operator tests' 2e-4 max-abs bound would have missed.
 """
 import ctypes
 import math
-from functools import lru_cache
 from typing import NamedTuple
 
 import pytest
 import torch
 import torch.nn.functional as F
 
+import archs
 import grl_oracle as O
 
 B = 2
@@ -52,28 +51,11 @@ EXPF_ULP = 2
 OLD_TOL = 2e-4     # the max-abs bound of the operator tests this file replaces
 GATE_ATTN = 1695.0   # fp32 ulps at max(|ref|, row rms): 2 x the worst case, 847.2 (small/sr window; H100 80GB HBM3, 400 W)
 GATE_CHAIN = 2165.0  # both stripe passes against the float64 chain: 2 x the worst case, 1082.3 (same card)
-TASKS = (("sr", 2), ("sr", 3), ("sr", 4), ("dn", 1), ("deblur", 1), ("jpeg", 1), ("dm", 1))
 ACT_NONE, ACT_GELU, ACT_LEAKY = 0, 1, 2
 
 
 def gamma(n):
     return n * U / (1 - n * U)
-
-
-@lru_cache(maxsize=None)
-def released_model(pkg, variant, task, scale):
-    """(model, fp32 launch descriptors) of a released config at its smallest padded size, on the CPU."""
-    from grl_image_restoration_b200 import modules
-
-    cfg = pkg.configs.grl_config(variant, task, scale)
-    model = pkg.GRL(**dict(cfg, img_size=math.lcm(cfg["window_size"], *cfg["stripe_size"])))
-    return model, modules.f32_launches(model, (1, model.in_channels) + tuple(model.input_resolution))
-
-
-def released_models(pkg):
-    for variant in ("tiny", "small", "base"):
-        for task, s in TASKS:
-            yield f"{variant}/{task}x{s}", *released_model(pkg, variant, task, s)
 
 
 def launches_of(launches, kind):
@@ -173,6 +155,12 @@ ATTN_EXTRAS = [  # limits no released config uses, and the earlier operator test
     AttnCase("extra: stripe groups, 32x8 stripes shifted by (0, 4)", "stripe2", (32, 8), 2, True, 2, 8, (0, 4)),
     AttnCase("extra: df 3, 1 head", "stripe2", (6, 12), 3, True, 1, 32),
 ]
+# released paths outside the VARIANTS x TASKS grid of archs: GRL-Base blind SR's stripe pass 1 (head_dim 30 on 8 x 16
+# anchors, 2048 keys).  They come after the extras because a case's seed is its index in the case list.
+ATTN_ZOO_CASES = [
+    AttnCase("base/bsr", "stripe1", (32, 64), 4, False, 3, 30),
+    AttnCase("base/bsr", "stripe1", (32, 64), 4, True, 3, 30),
+]
 
 
 def attn_case_launch(case):
@@ -191,24 +179,16 @@ def attn_case_launch(case):
 
 
 def test_released_attention_paths_have_cases(pkg):
-    """Every attention path of every block of every released config has a case, and every case of ATTN_CASES is a
-    released path."""
-    have = {attn_path(attn_case_launch(c)[1]): c for c in ATTN_CASES}
-    assert len(have) == len(ATTN_CASES), "two cases share a path"
-    released, missing = set(), {}
-    for name, _, launches in released_models(pkg):
-        for ln in launches_of(launches, "AttnF32"):
-            s = attn_path(ln)
-            released.add(s)
-            if s not in have:
-                missing.setdefault(s, f"{name} {ln.name} {ln.role}")
-    for s, name in missing.items():
-        print(f"fp32 attention path without a case: {s}, first launched by {name}")
-    assert not missing, f"{len(missing)} released fp32 attention paths have no case: " + "; ".join(
-        f"{s} ({name})" for s, name in missing.items())
-    stale = [c for c in ATTN_CASES if attn_path(attn_case_launch(c)[1]) not in released]
-    assert not stale, f"cases that no released config launches: {stale}"
-    print(f"{len(released)} released fp32 attention paths")
+    """Every attention path of every block of every architecture of archs.architectures has a case, and every case of
+    ATTN_CASES and ATTN_ZOO_CASES is a launched path."""
+    from grl_image_restoration_b200 import modules
+
+    cases = [(attn_path(attn_case_launch(c)[1]), c) for c in ATTN_CASES + ATTN_ZOO_CASES]
+    assert len(dict(cases)) == len(cases), "two cases share a path"
+    launched = [(attn_path(ln), f"{name} {ln.name} {ln.role}")
+                for name, model, shape in archs.architectures(pkg, "fp32")
+                for ln in launches_of(modules.f32_launches(model, shape), "AttnF32")]
+    archs.check_walk("fp32 attention", launched, cases, [(attn_path(attn_case_launch(c)[1]), c) for c in ATTN_EXTRAS])
 
 
 # ------------------------------------------------------------------------------------------------------------ GEMM
@@ -275,26 +255,29 @@ GEMM_EXTRAS = [  # the earlier operator tests' shapes whose paths no released fo
     GemmCase("extra: conv Cin 64 N 12 LeakyReLU + residual", True, 576, 12, ACT_LEAKY, True),
     GemmCase("extra: conv Cin 180 N 45 GELU + residual", True, 1620, 45, ACT_GELU, True),
 ]
+# released paths outside the grid of archs, after the extras for the same reason: 1- and 6-channel heads, the 3-channel
+# tail without the input residual, the nearest+conv head's convs
+GEMM_ZOO_CASES = [
+    GemmCase("tiny/dnx1 c1 conv_first", True, 9, 64),
+    GemmCase("small/dnx1 c1 conv_first", True, 9, 128),
+    GemmCase("base/dnx1 c1 conv_first", True, 9, 180),
+    GemmCase("base/bsrx4 conv_up1", True, 576, 64, ACT_LEAKY, slope=0.2),
+    GemmCase("base/defocus_dual conv_first", True, 54, 180),
+    GemmCase("base/defocus_dual conv_last", True, 1620, 3),
+]
 
 
 def test_released_gemm_paths_have_cases(pkg):
-    """Every GEMM path of every released fp32 forward has a case, and every case of GEMM_CASES is a released path."""
-    have = {gemm_path(c.call()): c for c in GEMM_CASES + GEMM_EXTRAS}
-    assert len(have) == len(GEMM_CASES + GEMM_EXTRAS), "two cases share a path"
-    released, missing = set(), {}
-    for name, _, launches in released_models(pkg):
-        for g in launches_of(launches, "GemmF32"):
-            s = gemm_path(g)
-            released.add(s)
-            if s not in have:
-                missing.setdefault(s, f"{name} {g.name}")
-    for s, name in missing.items():
-        print(f"fp32 gemm path without a case: {s}, first launched by {name}")
-    assert not missing, f"{len(missing)} released fp32 gemm paths have no case: " + "; ".join(
-        f"{s} ({name})" for s, name in missing.items())
-    stale = [c for c in GEMM_CASES if gemm_path(c.call()) not in released]
-    assert not stale, f"cases that no released config launches: {stale}"
-    print(f"{len(released)} released fp32 gemm paths")
+    """Every GEMM path of the fp32 forward of every architecture of archs.architectures has a case, and every case of
+    GEMM_CASES and GEMM_ZOO_CASES is a launched path."""
+    from grl_image_restoration_b200 import modules
+
+    released = GEMM_CASES + GEMM_ZOO_CASES
+    cases = [(gemm_path(c.call()), c) for c in released + GEMM_EXTRAS]
+    assert len(dict(cases)) == len(cases), "two cases share a path"
+    launched = [(gemm_path(g), f"{name} {g.name}") for name, model, shape in archs.architectures(pkg, "fp32")
+                for g in launches_of(modules.f32_launches(model, shape), "GemmF32")]
+    archs.check_walk("fp32 gemm", launched, cases[:len(released)], cases[len(released):])
 
 
 # ----------------------------------------------------------------------------------------------------------------- GPU
@@ -491,7 +474,7 @@ def attn_id(c):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("case", ATTN_CASES + ATTN_EXTRAS, ids=attn_id)
+@pytest.mark.parametrize("case", ATTN_CASES + ATTN_EXTRAS + ATTN_ZOO_CASES, ids=attn_id)
 def test_attention_path(lib, device, case):
     from grl_image_restoration_b200 import capi
 
@@ -501,7 +484,7 @@ def test_attention_path(lib, device, case):
     c = h * d
     H, W = x_size
     L = H * W
-    seed = (ATTN_CASES + ATTN_EXTRAS).index(case)
+    seed = (ATTN_CASES + ATTN_EXTRAS + ATTN_ZOO_CASES).index(case)
     qkv, anc = attn_inputs(case, x_size, device, seed)
     merged, mbuf = nan_rows(B * L, 2 * c, device)
     if case.role == "window":
@@ -634,11 +617,11 @@ def gemm_id(c):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("case", GEMM_CASES + GEMM_EXTRAS, ids=gemm_id)
+@pytest.mark.parametrize("case", GEMM_CASES + GEMM_EXTRAS + GEMM_ZOO_CASES, ids=gemm_id)
 def test_gemm_path(lib, device, case):
     from grl_image_restoration_b200 import capi
 
-    x, w, b, res = gemm_operands(case, device, (GEMM_CASES + GEMM_EXTRAS).index(case))
+    x, w, b, res = gemm_operands(case, device, (GEMM_CASES + GEMM_EXTRAS + GEMM_ZOO_CASES).index(case))
     slope = case.call().slope
     K, N = case.K, case.N
     if case.conv:
@@ -974,7 +957,7 @@ def test_recorded_launches_match_lists(pkg, lib, device, monkeypatch, variant, t
     from grl_image_restoration_b200 import capi, modules
 
     cfg = pkg.configs.grl_config(variant, task, scale)
-    model = pkg.GRL(**dict(cfg, img_size=math.lcm(cfg["window_size"], *cfg["stripe_size"])))
+    model = pkg.GRL(**dict(cfg, img_size=archs.smallest_size(cfg)))
     model.set_precision("fp32")
     model = model.to(device).eval()
     S = model.pad_size
@@ -1024,7 +1007,7 @@ def test_listing_calls_only_host_helpers(pkg, monkeypatch, input_format):
     from grl_image_restoration_b200 import capi, modules
 
     cfg = pkg.configs.grl_config("base", "dm", 1)
-    model = pkg.GRL(input_format=input_format, **dict(cfg, img_size=math.lcm(cfg["window_size"], *cfg["stripe_size"])))
+    model = pkg.GRL(input_format=input_format, **dict(cfg, img_size=archs.smallest_size(cfg)))
     S = model.pad_size
     shape = (2, 4, S // 2 + 3, S - 1) if input_format == "rggb" else (2, 3, S + 5, 2 * S - 1)
     host = HostOnly(capi.lib())
@@ -1045,19 +1028,14 @@ def test_listing_calls_only_host_helpers(pkg, monkeypatch, input_format):
 def test_fp32_and_tensor_core_listings_name_the_same_gemms(pkg):
     """Both paths run the same network: their listings name the same GEMMs in the same order, except that a tensor-core
     block runs its CAB convs before the output projection, whose LayerNorm epilogue adds the CAB branch."""
-    from grl_image_restoration_b200 import tc
+    from grl_image_restoration_b200 import modules, tc
 
     def no_cab(names):
         return [n for n in names if not n.endswith((".cab1", ".cab2"))]
 
-    for name, model, launches in released_models(pkg):
-        shape = (1, model.in_channels) + tuple(model.input_resolution)
-        model.set_precision("fp16")
-        try:
-            names16 = [ln.name for ln in tc.gemm_launches(model, shape)]
-        finally:
-            model.set_precision("fp32")
-        names32 = [g.name for g in launches_of(launches, "GemmF32")]
+    for (name, m32, shape), (_, m16, _) in zip(archs.architectures(pkg, "fp32"), archs.architectures(pkg, "fp16")):
+        names16 = [ln.name for ln in tc.gemm_launches(m16, shape)]
+        names32 = [g.name for g in launches_of(modules.f32_launches(m32, shape), "GemmF32")]
         assert sorted(names32) == sorted(names16), name
         assert no_cab(names32) == no_cab(names16), name
 
@@ -1072,7 +1050,7 @@ def test_listing_first_leaves_the_forward_unchanged(pkg, device, task, input_for
     from grl_image_restoration_b200 import modules
 
     cfg = pkg.configs.grl_config("tiny", task, 2 if task == "sr" else 1)
-    cfg = dict(cfg, img_size=math.lcm(cfg["window_size"], *cfg["stripe_size"]), input_format=input_format)
+    cfg = dict(cfg, img_size=archs.smallest_size(cfg), input_format=input_format)
     torch.manual_seed(0)
     listed = pkg.GRL(**cfg)
     fresh = copy.deepcopy(listed)

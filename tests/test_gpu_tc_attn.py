@@ -3,11 +3,11 @@ emulation of its own algorithm (grl_oracle.attn_launch_reference).
 
 A launch's path is its signature (`path`): the key-window template KW, whether the last query tile (128 rows) and key tile
 (64 keys) are full, the TMA box widths of the query and key grids, dense V / dense output, the ones column and the shift
-mask.  The image size does not enter it.  CASES holds one minimal problem per signature, taken from the first released
-(config, block, pass) that launches it: 2 x 2 windows of that pass's grid and B = 2 (an interior window, a masked and
-wrapped boundary window and a batch offset), the config's heads and head_dim, in the packed production layout.
-test_released_attention_paths_have_cases (CPU) walks every block of every released config through
-tc.attention_launches, the descriptors BlockPlan.run launches, and fails on a signature without a case.
+mask.  The image size does not enter it.  CASES and ZOO_CASES hold one minimal problem per signature, taken from the
+first released (config, block, pass) that launches it: 2 x 2 windows of that pass's grid and B = 2 (an interior window, a
+masked and wrapped boundary window and a batch offset), the config's heads and head_dim, in the packed production
+layout.  test_released_attention_paths_have_cases (CPU) walks every block of every architecture of archs.architectures
+through tc.attention_launches, the descriptors BlockPlan.run launches, and fails on a signature without a case.
 
 The gate bounds |got - emulated| in ulps of the output format, taken at max(|emulated|, the row's rms).  The emulation
 differs from the kernel only in the fp32 summation order of the wgmma products and in ex2.approx, so almost every element
@@ -21,6 +21,7 @@ from typing import NamedTuple
 import pytest
 import torch
 
+import archs
 import grl_oracle as O
 
 ATTN_VARIANTS = [5, 0]  # grl_tc_attn_variant: 5 = TMA boxes where the geometry has them (default), 0 = cp.async gathers
@@ -126,6 +127,12 @@ EXTRAS = [
     AttnCase("extra: lazy rescale, generic KW (jpeg window)", "window", (36, 36), 1, False, 3, 32, 0.6),
     AttnCase("extra: lazy rescale, generic KW (jpeg window)", "window", (36, 36), 1, True, 3, 30, 6.0),
 ]
+# released paths outside the VARIANTS x TASKS grid of archs: GRL-Base blind SR's stripe pass 1 over 64 x 32 stripes
+# with df 4 (16 x 8 anchor windows).  They come after EXTRAS because a case's seed is its index in the case list.
+ZOO_CASES = [
+    AttnCase("base/bsr/b1", "stripe1", (64, 32), 4, False, 3, 30),
+    AttnCase("base/bsr/b3", "stripe1", (64, 32), 4, True, 3, 30),
+]
 
 # key-window widths with their own template instance in grl_tc_attn's switch (attn_tc.cu); any other width runs KW = 0
 KW_TEMPLATES = (8, 16, 32, 64, 128)
@@ -155,38 +162,18 @@ def case_launch(case):
     return x_size, tc.attention_launch(case.role, gq, gk, case.heads, case.heads, case.heads * case.d, case.shifted)
 
 
-def released_launches(pkg):
-    from grl_image_restoration_b200 import tc
-
-    for variant in ("tiny", "small", "base"):
-        for task in ("sr", "dn", "deblur", "jpeg", "dm"):
-            cfg = pkg.configs.grl_config(variant, task)
-            S = math.lcm(cfg["window_size"], *cfg["stripe_size"])  # any size the grids tile gives the same signatures
-            model = pkg.GRL(**dict(cfg, img_size=S))
-            for si, layer in enumerate(model.layers):
-                for bi, blk in enumerate(layer.blocks):
-                    for ln in tc.attention_launches(blk, (S, S)):
-                        yield f"{variant}/{task} stage {si} block {bi} {ln.role}", ln
-
-
 def test_released_attention_paths_have_cases(pkg):
-    """Every launch path of every block of every released config has a case in CASES, and every case of CASES is a
-    released path."""
-    from grl_image_restoration_b200 import capi
+    """Every launch path of every block of every architecture of archs.architectures has a case, and every case of CASES
+    and ZOO_CASES is a launched path."""
+    from grl_image_restoration_b200 import capi, tc
 
-    have = {path(capi, case_launch(c)[1]): c for c in CASES + EXTRAS}
-    released, missing = set(), {}
-    for name, ln in released_launches(pkg):
-        s = path(capi, ln)
-        released.add(s)
-        if s not in have:
-            missing.setdefault(s, name)
-    for s, name in missing.items():
-        print(f"attention path without a case: {s}, first launched by {name}")
-    assert not missing, f"{len(missing)} released attention paths have no case: " + "; ".join(
-        f"{s} ({name})" for s, name in missing.items())
-    stale = [c for c in CASES if path(capi, case_launch(c)[1]) not in released]
-    assert not stale, f"cases that no released config launches: {stale}"
+    cases = [(path(capi, case_launch(c)[1]), c) for c in CASES + ZOO_CASES]
+    assert len(dict(cases)) == len(cases), "two cases share a path"
+    launched = [(path(capi, ln), f"{name} stage {si} block {bi} {ln.role}")
+                for name, model, shape in archs.architectures(pkg, "fp16")
+                for si, layer in enumerate(model.layers) for bi, blk in enumerate(layer.blocks)
+                for ln in tc.attention_launches(blk, shape[2:])]
+    archs.check_walk("tensor-core attention", launched, cases, [(path(capi, case_launch(c)[1]), c) for c in EXTRAS])
 
 
 # ----------------------------------------------------------------------------------------------------------------- GPU
@@ -350,7 +337,7 @@ def mutations(ref_fn, ln, q, k, v, table, index, mask, tokens, variant):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("fmt", [0, 1], ids=["fp16", "bf16"])
-@pytest.mark.parametrize("case", CASES + EXTRAS, ids=lambda c: f"{c.src.split(':')[0]}-{c.role}-{c.win[0]}x{c.win[1]}"
+@pytest.mark.parametrize("case", CASES + EXTRAS + ZOO_CASES, ids=lambda c: f"{c.src.split(':')[0]}-{c.role}-{c.win[0]}x{c.win[1]}"
                          f"-df{c.df}-{'s' if c.shifted else 'u'}-h{c.heads}d{c.d}" + (f"-grow{c.grow}" if c.grow else ""))
 def test_attention_path(tc, device, case, fmt):
     from grl_image_restoration_b200 import capi
@@ -364,7 +351,7 @@ def test_attention_path(tc, device, case, fmt):
         if first != case:
             pytest.skip(f"same cp.async path as {first.src} {first.role}")
     dtype = tc.DTYPE[fmt]
-    seed = (CASES + EXTRAS).index(case) * 2 + fmt
+    seed = (CASES + EXTRAS + ZOO_CASES).index(case) * 2 + fmt
     H, W = x_size
     qkv, anc = block_inputs(case, x_size, dtype, device, seed)
     h, d = case.heads, case.d

@@ -7,8 +7,8 @@ partial last N tile and min(k chunks, 5) (5 and more wrap the 4-stage operand ri
 activation, a residual, 16-bit / fp32 / PixelShuffle / NCHW-tail outputs, the residual on the NCHW tail, the CAB add and
 a 16-bit pitch wider than the stored columns.  The image size does not enter it.  tc.gemm_launches lists the launches of
 one forward (checked one for one against the launches of real forwards by test_recorded_launches_match_descriptors);
-test_released_gemm_paths_have_cases (CPU) walks every released config through it and fails on a signature without a
-case.
+test_released_gemm_paths_have_cases (CPU) walks every architecture of archs.architectures through it and fails on a
+signature without a case.
 
 Every case is the released launch (or an extra) at a small size with its edges built in: B = 2, a partial last row tile
 (linear: M = 200 rows, 2 images of L = 100, so the image boundary lies inside a row tile), conv images of 13 x 21 pixels
@@ -29,13 +29,13 @@ gate on every case where they apply.
 """
 import copy
 import math
-from functools import lru_cache
 from typing import NamedTuple
 
 import numpy as np
 import pytest
 import torch
 
+import archs
 import grl_oracle as O
 
 GATE32 = 255.0         # 2 x the worst case, 127.4 ulp (fp16 operands, base stage conv: K = 9 x 192)
@@ -45,7 +45,6 @@ M_CASE = B * L_CASE
 HIGH_MEAN_ROWS = (5, 133)
 ZERO_QKV_ROW = 3
 GUARD = 3  # guard rows before and after every output buffer
-TASKS = (("sr", 2), ("sr", 3), ("sr", 4), ("dn", 1), ("deblur", 1), ("jpeg", 1), ("dm", 1))
 
 
 def path(launch):
@@ -60,24 +59,6 @@ def path(launch):
             a["act"], a["res_f32"] is not None, o16 is not None, a["out_f32"] is not None, a["ps_r"],
             a["nchw_r"] if nchw else 0, nchw and a["res_f32"] is not None, a["cab_y"] is not None,
             o16 is not None and o16.shape[-1] > a["n_store"])
-
-
-@lru_cache(maxsize=None)
-def released_config(pkg, variant, task, scale):
-    """(model, descriptors) of one released config at its smallest padded size, fp16 operands."""
-    from grl_image_restoration_b200 import tc
-
-    cfg = pkg.configs.grl_config(variant, task, scale)
-    model = pkg.GRL(**dict(cfg, img_size=math.lcm(cfg["window_size"], *cfg["stripe_size"])))
-    model.set_precision("fp16")
-    return model, tc.gemm_launches(model, (1, 3, model.pad_size, model.pad_size))
-
-
-def released_launches(pkg):
-    for variant in ("tiny", "small", "base"):
-        for task, s in TASKS:
-            for ln in released_config(pkg, variant, task, s)[1]:
-                yield f"{variant}/{task}x{s} {ln.name}", ln
 
 
 # one case per released path: (variant, task, scale, launch) of its first launcher
@@ -146,28 +127,24 @@ EXTRA_NAMES = ["extra: linear, direct stores, 2 N tiles, GELU", "extra: linear, 
 
 
 def case_launch(pkg, case):
+    from grl_image_restoration_b200 import tc
+
     if isinstance(case, str):
         return next(e for e in _extras() if e.name == case)
     v, t, s, name = case
-    return next(ln for ln in released_config(pkg, v, t, s)[1] if ln.name == name)
+    return next(ln for ln in tc.gemm_launches(*archs.model(pkg, v, t, s, 3, "fp16")) if ln.name == name)
 
 
 def test_released_gemm_paths_have_cases(pkg):
-    """Every launch path of every released config has a case, and every case of CASES is a released path."""
-    have = {path(case_launch(pkg, c)): c for c in CASES + EXTRA_NAMES}
-    assert len(have) == len(CASES + EXTRA_NAMES), "two cases share a path"
-    released, missing = set(), {}
-    for name, ln in released_launches(pkg):
-        s = path(ln)
-        released.add(s)
-        if s not in have:
-            missing.setdefault(s, name)
-    for s, name in missing.items():
-        print(f"gemm path without a case: {s}, first launched by {name}")
-    assert not missing, f"{len(missing)} released gemm paths have no case: " + "; ".join(
-        f"{s} ({name})" for s, name in missing.items())
-    stale = [c for c in CASES if path(case_launch(pkg, c)) not in released]
-    assert not stale, f"cases that no released config launches: {stale}"
+    """Every launch path of every architecture of archs.architectures has a case, and every case of CASES is a
+    launched path."""
+    from grl_image_restoration_b200 import tc
+
+    cases = [(path(case_launch(pkg, c)), c) for c in CASES + EXTRA_NAMES]
+    assert len(dict(cases)) == len(cases), "two cases share a path"
+    launched = [(path(ln), f"{name} {ln.name}") for name, model, shape in archs.architectures(pkg, "fp16")
+                for ln in tc.gemm_launches(model, shape)]
+    archs.check_walk("tensor-core gemm", launched, cases[:len(CASES)], cases[len(CASES):])
 
 
 def test_gelu_as_bound():
@@ -484,7 +461,7 @@ def test_recorded_launches_match_descriptors(pkg, tc, device, monkeypatch, varia
     """tc.gemm_launches lists, one for one and in order, the tc.gemm calls of a real forward (smallest padded size, an
     input that needs padding)."""
     cfg = pkg.configs.grl_config(variant, task, scale)
-    model = pkg.GRL(**dict(cfg, img_size=math.lcm(cfg["window_size"], *cfg["stripe_size"])))
+    model = pkg.GRL(**dict(cfg, img_size=archs.smallest_size(cfg)))
     model.use_cuda_graph = False
     model = model.to(device).eval()
     model.set_precision("fp16")
@@ -513,7 +490,7 @@ def test_listing_first_leaves_the_forward_unchanged(pkg, tc, device):
     coordinate tables): bitwise the forward of an identical model that was never listed.  A listing run packs weights
     on the device, but its attention constants are meta tensors and must not be kept for the forward."""
     cfg = pkg.configs.grl_config("tiny", "sr", 2)
-    cfg = dict(cfg, img_size=math.lcm(cfg["window_size"], *cfg["stripe_size"]))
+    cfg = dict(cfg, img_size=archs.smallest_size(cfg))
     torch.manual_seed(0)
     listed = pkg.GRL(**cfg)
     fresh = copy.deepcopy(listed)
