@@ -75,17 +75,22 @@ _SIGNATURES = {
     "grl_tc_attn": (c_int, [ctypes.POINTER(GrlTcAttn), c_vp]),
     "grl_tc_attn_variant": (c_int, [c_int]),
     "grl_psnr_f32": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_sz, c_vp, c_vp, c_vp]),
+    "grl_psnr_u8": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_sz, c_vp, c_vp, c_vp]),
     "grl_psnrb_workspace": (c_sz, [c_int]),
     "grl_psnrb_f32": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_sz, c_vp, c_vp, c_vp]),
+    "grl_psnrb_u8": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_sz, c_vp, c_vp, c_vp]),
     "grl_ssim_workspace": (c_sz, [c_int, c_int, c_int, c_int, c_int]),
     "grl_ssim_f32": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "grl_ssim_u8": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "grl_ssim_taps_host": (c_int, [c_vp]),
     "grl_ssim_host": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp]),
     "grl_niqe_workspace": (c_sz, [c_int, c_int, c_int, c_int]),
     "grl_niqe_features_f32": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_sz, c_vp, c_vp]),
+    "grl_niqe_features_u8": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_sz, c_vp, c_vp]),
     "grl_niqe_luma_host": (c_int, [c_vp, c_i64, c_vp]),
     "grl_niqe_half_taps_host": (c_int, [c_vp]),
     "grl_niqe_luma_f32": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp]),
+    "grl_niqe_luma_u8": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp]),
     "grl_niqe_mscn_f32": (c_int, [c_vp, c_int, c_int, c_int, c_vp, c_vp, c_vp]),
     "grl_niqe_half_f32": (c_int, [c_vp, c_int, c_int, c_int, c_vp, c_vp, c_vp]),
     "grl_niqe_feat_f32": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_vp, c_vp, c_vp]),
@@ -105,6 +110,10 @@ _SIGNATURES = {
     "grl_ens_merge_f32": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp]),
     "grl_demosaic_host": (c_int, [c_vp, c_int, c_int, c_int, c_vp]),
     "grl_demosaic_f32": (c_int, [c_vp, c_int, c_int, c_int, c_vp, c_vp]),
+    "grl_u8_to_f32": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp]),
+    "grl_f32_to_u8": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp]),
+    "grl_u8_to_f32_host": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_vp]),
+    "grl_f32_to_u8_host": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_vp]),
 }
 
 _lib = None

@@ -1,24 +1,22 @@
 // metric.cu -- the validation step's PSNR on the device in one pass (engines/base.py:255-268, utils/utils_image.py:8-11
 // shave, :30-33 tensor_round, :43-80 rgb2ycbcr; utils/metrics/psnr.py:44-48).
 //
-// restored / target are (B, C, H, W) fp32 planes.  Both are rounded to the 8-bit grid (clamp to [0, 1], x255, round half
-// to even like torch.round), `border` pixels are shaved on every side, and the squared error is accumulated EXACTLY as an
-// integer (a rounded pixel is k/255; (k1 - k2)^2 <= 65025): the per-image sums are 64-bit integer atomics, so the result
-// is independent of the block schedule.  C == 3 additionally accumulates the error of the luma of MATLAB's rgb2ycbcr
-// (coefficients 65.481, 128.553, 24.966, offset 16, rounded to 8 bit).  HBM-bound: 2 x 4 bytes read per element.
+// restored / target are (B, C, H, W) fp32 planes or (B, H, W, C) 8-bit pixels: every kernel is a template on the pixel
+// reader of grl_image_u8.h, the rest of it is shared.  fp32 planes are rounded to the 8-bit grid (clamp to [0, 1], x255,
+// round half to even like torch.round), `border` pixels are shaved on every side, and the squared error is accumulated
+// EXACTLY as an integer (a rounded pixel is k/255; (k1 - k2)^2 <= 65025): the per-image sums are 64-bit integer atomics,
+// so the result is independent of the block schedule.  C == 3 additionally accumulates the error of the luma of MATLAB's
+// rgb2ycbcr (coefficients 65.481, 128.553, 24.966, offset 16, rounded to 8 bit).  HBM-bound: 2 x 4 bytes read per
+// element from fp32 planes, 2 x 1 from 8-bit pixels.
 // PSNR-B and SSIM (RGB and luma, float64 on the same 8-bit integers) follow below.
 #include <algorithm>
 #include <vector>
 
 #include "grl_common.cuh"
+#include "grl_image_u8.h"
 #include "grl_ssim.h"
 
 namespace grl {
-
-__host__ __device__ __forceinline__ float round8(float v) {
-  v = fminf(fmaxf(v, 0.f), 1.f);
-  return rintf(v * 255.0f);  // round half to even == torch.round
-}
 
 // y = round(65.481/255 * R + 128.553/255 * G + 24.966/255 * B + 16) with R, G, B on the 0..255 grid
 // (metrics.rgb_to_y: (img * 255) @ (coeff / 255) + 16, rounded)
@@ -29,21 +27,20 @@ __host__ __device__ __forceinline__ float luma8(float r, float g, float b) {
   return rintf(acc + 16.0f);
 }
 
-__global__ void psnr_sse_kernel(const float* __restrict__ a, const float* __restrict__ b, int C, int H, int W, int border,
+template <class Img>
+__global__ void psnr_sse_kernel(Img a, Img b, int C, int H, int W, int border,
                                 unsigned long long* __restrict__ sse /* (B, 2): rgb, y */) {
   const int img = blockIdx.y;
   const int h = H - 2 * border, w = W - 2 * border;
   const long long n = (long long)h * w;
-  const long long plane = (long long)H * W;
-  const float* pa = a + (long long)img * C * plane;
-  const float* pb = b + (long long)img * C * plane;
+  const Img pa = a.img(img), pb = b.img(img);
   unsigned long long s_rgb = 0, s_y = 0;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     const int y = (int)(i / w), x = (int)(i - (long long)y * w);
     const long long off = (long long)(y + border) * W + (x + border);
     float ra[3], rb[3];
     for (int c = 0; c < C; ++c) {
-      const float va = round8(pa[c * plane + off]), vb = round8(pb[c * plane + off]);
+      const float va = pa(c, off), vb = pb(c, off);
       if (c < 3) ra[c] = va, rb[c] = vb;
       const int d = (int)va - (int)vb;
       s_rgb += (unsigned)(d * d);
@@ -93,12 +90,11 @@ __global__ void psnr_finalize_kernel(const unsigned long long* __restrict__ sse,
 // (x, x + 1) at block boundaries x = 7, 15, ... < W - 1 and elsewhere, and the same for vertical neighbours.
 constexpr int kPsnrbSets = 4, kPsnrbSums = 5;  // sse, horizontal boundary, horizontal other, vertical boundary, vertical other
 
-__global__ void psnrb_sums_kernel(const float* __restrict__ a, const float* __restrict__ b, int C, int H, int W,
-                                  unsigned long long* __restrict__ sums /* (B, 4, 5) */) {
+template <class Img>
+__global__ void psnrb_sums_kernel(Img a, Img b, int C, int H, int W, unsigned long long* __restrict__ sums /* (B, 4, 5) */) {
   const int img = blockIdx.y;
-  const long long plane = (long long)H * W, n = plane;
-  const float* pa = a + (long long)img * C * plane;
-  const float* pb = b + (long long)img * C * plane;
+  const long long n = (long long)H * W;
+  const Img pa = a.img(img), pb = b.img(img);
   unsigned long long s[kPsnrbSets][kPsnrbSums] = {};
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     const int y = (int)(i / W), x = (int)(i - (long long)y * W);
@@ -109,10 +105,9 @@ __global__ void psnrb_sums_kernel(const float* __restrict__ a, const float* __re
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
       if (c < C) {
-        const float* p = pa + c * plane + i;
-        va[c] = round8(p[0]), vb[c] = round8(pb[c * plane + i]);
-        if (right) vr[c] = round8(p[1]);
-        if (down) vd[c] = round8(p[W]);
+        va[c] = pa(c, i), vb[c] = pb(c, i);
+        if (right) vr[c] = pa(c, i + 1);
+        if (down) vd[c] = pa(c, i + W);
       }
       d[c] = (int)va[c] - (int)vb[c], e[c] = right ? (int)va[c] - (int)vr[c] : 0, f[c] = down ? (int)va[c] - (int)vd[c] : 0;
     }
@@ -194,8 +189,9 @@ static_assert(kSsimRows <= 32 && kSsimTW == 32 && kSsimThreads == 4 * 32 && kSsi
 // exact double of an integer 0 <= k < 2^32 without the conversion pipe: 2^52 + k is exact, minus 2^52
 __device__ __forceinline__ double ssim_u2d(unsigned k) { return __hiloint2double(0x43300000, (int)k) - 4503599627370496.0; }
 
+template <class Img>
 __global__ void __launch_bounds__(kSsimThreads)
-ssim_tile_kernel(const float* __restrict__ a, const float* __restrict__ b, int C, int H, int W, int border,
+ssim_tile_kernel(Img a, Img b, int C, int H, int W, int border,
                  double* __restrict__ partial /* (B, 2, tiles) */, double* __restrict__ map_rgb, double* __restrict__ map_y) {
   __shared__ __align__(16) unsigned char sk[2][4][kSsimRows][kSsimRowBytes];
   __shared__ double hs[5][kSsimRows][kSsimHStride];
@@ -203,9 +199,8 @@ ssim_tile_kernel(const float* __restrict__ a, const float* __restrict__ b, int C
   const int img = blockIdx.z, h = H - 2 * border, w = W - 2 * border;
   const int x0 = blockIdx.x * kSsimTW, y0 = blockIdx.y * kSsimTH;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const long long plane = (long long)H * W, n = (long long)h * w;
-  const float* pa = a + (long long)img * C * plane;
-  const float* pb = b + (long long)img * C * plane;
+  const long long n = (long long)h * w;
+  const Img pa = a.img(img), pb = b.img(img);
 
   // tensor_round + shave + luma, staged as bytes
   for (int i = threadIdx.x; i < kSsimRows * kSsimRowBytes; i += kSsimThreads) {
@@ -217,7 +212,7 @@ ssim_tile_kernel(const float* __restrict__ a, const float* __restrict__ b, int C
 #pragma unroll
     for (int ch = 0; ch < 3; ++ch)
       if (ch < C) {
-        if (in) va[ch] = round8(pa[ch * plane + off]), vb[ch] = round8(pb[ch * plane + off]);
+        if (in) va[ch] = pa(ch, off), vb[ch] = pb(ch, off);
         sk[0][ch][r][c] = (unsigned char)va[ch], sk[1][ch][r][c] = (unsigned char)vb[ch];
       }
     if (C == 3) {
@@ -345,15 +340,11 @@ static bool ssim_shape_ok(int B, int C, int H, int W, int border) {
     GRL_REQUIRE(2LL * border < std::min(H, W), "ssim: border %d leaves no pixel of a %d x %d image", border, H, W);            \
   } while (0)
 
-}  // namespace grl
-
-using namespace grl;
-
-extern "C" {
-
-int grl_psnr_f32(const float* restored, const float* target, int B, int C, int H, int W, int border, void* workspace,
-                 size_t workspace_bytes, float* psnr_rgb, float* psnr_y, void* stream) {
-  GRL_REQUIRE(restored && target && psnr_rgb, "psnr: null argument");
+// The launches behind grl_psnr_f32 / grl_psnr_u8 and their siblings; a and b are the pixel readers of the two images.
+template <class Img>
+int psnr_run(Img a, Img b, int B, int C, int H, int W, int border, void* workspace, size_t workspace_bytes, float* psnr_rgb,
+             float* psnr_y, void* stream) {
+  GRL_REQUIRE(a.p && b.p && psnr_rgb, "psnr: null argument");
   GRL_REQUIRE(workspace && workspace_bytes >= sizeof(unsigned long long) * 2 * (size_t)(B > 0 ? B : 0),
               "psnr: workspace %zu bytes < %zu", workspace_bytes, sizeof(unsigned long long) * 2 * (size_t)(B > 0 ? B : 0));
   GRL_REQUIRE(B >= 0 && C >= 1 && C <= 4 && H > 2 * border && W > 2 * border && border >= 0, "psnr: bad shape (%d,%d,%d,%d) border %d",
@@ -365,18 +356,17 @@ int grl_psnr_f32(const float* restored, const float* target, int B, int C, int H
   const long long n = (long long)(H - 2 * border) * (W - 2 * border);
   const int threads = 256;
   const int bx = (int)std::min<long long>((n + threads * 4 - 1) / (threads * 4), 592);  // ~4 CTAs per SM per image at most
-  psnr_sse_kernel<<<dim3((unsigned)std::max(bx, 1), (unsigned)B), threads, 0, st>>>(restored, target, C, H, W, border, sse);
+  psnr_sse_kernel<<<dim3((unsigned)std::max(bx, 1), (unsigned)B), threads, 0, st>>>(a, b, C, H, W, border, sse);
   GRL_LAUNCH_CHECK("psnr_sse_kernel");
   psnr_finalize_kernel<<<(B + 127) / 128, 128, 0, st>>>(sse, B, C, n, psnr_rgb, psnr_y);
   GRL_LAUNCH_CHECK("psnr_finalize_kernel");
   return GRL_OK;
 }
 
-size_t grl_psnrb_workspace(int B) { return sizeof(unsigned long long) * kPsnrbSets * kPsnrbSums * (size_t)(B > 0 ? B : 0); }
-
-int grl_psnrb_f32(const float* restored, const float* target, int B, int C, int H, int W, void* workspace,
-                  size_t workspace_bytes, double* psnrb_rgb, double* psnrb_y, void* stream) {
-  GRL_REQUIRE(restored && target && psnrb_rgb, "psnrb: null argument");
+template <class Img>
+int psnrb_run(Img a, Img b, int B, int C, int H, int W, void* workspace, size_t workspace_bytes, double* psnrb_rgb,
+              double* psnrb_y, void* stream) {
+  GRL_REQUIRE(a.p && b.p && psnrb_rgb, "psnrb: null argument");
   GRL_REQUIRE(workspace && workspace_bytes >= grl_psnrb_workspace(B), "psnrb: workspace %zu bytes < %zu", workspace_bytes,
               grl_psnrb_workspace(B));
   GRL_REQUIRE(B >= 0 && (C == 1 || C == 3), "psnrb: needs C == 1 or 3, got %d", C);
@@ -389,11 +379,66 @@ int grl_psnrb_f32(const float* restored, const float* target, int B, int C, int 
   const long long n = (long long)H * W;
   const int threads = 256;
   const int bx = (int)std::min<long long>((n + threads * 4 - 1) / (threads * 4), 592);
-  psnrb_sums_kernel<<<dim3((unsigned)std::max(bx, 1), (unsigned)B), threads, 0, st>>>(restored, target, C, H, W, sums);
+  psnrb_sums_kernel<<<dim3((unsigned)std::max(bx, 1), (unsigned)B), threads, 0, st>>>(a, b, C, H, W, sums);
   GRL_LAUNCH_CHECK("psnrb_sums_kernel");
   psnrb_finalize_kernel<<<(B + 127) / 128, 128, 0, st>>>(sums, B, C, H, W, psnrb_rgb, psnrb_y);
   GRL_LAUNCH_CHECK("psnrb_finalize_kernel");
   return GRL_OK;
+}
+
+template <class Img>
+int ssim_run(Img a, Img b, int B, int C, int H, int W, int border, void* workspace, size_t workspace_bytes, double* ssim_rgb,
+             double* ssim_y, double* map_rgb, double* map_y, void* stream) {
+  GRL_REQUIRE(a.p && b.p && ssim_rgb, "ssim: null argument");
+  GRL_SSIM_SHAPE(B, C, H, W, border);
+  if (B == 0) return GRL_OK;
+  GRL_REQUIRE(workspace && workspace_bytes >= grl_ssim_workspace(B, C, H, W, border), "ssim: workspace %zu bytes < %zu",
+              workspace_bytes, grl_ssim_workspace(B, C, H, W, border));
+  const cudaStream_t st = (cudaStream_t)stream;
+  const int h = H - 2 * border, w = W - 2 * border;
+  const int gx = ceil_div(w, kSsimTW), gy = ceil_div(h, kSsimTH);
+  GRL_REQUIRE(gy <= 65535 && B <= 65535, "ssim: %d tile rows / %d images exceed the grid", gy, B);
+  ssim_tile_kernel<<<dim3((unsigned)gx, (unsigned)gy, (unsigned)B), kSsimThreads, 0, st>>>(a, b, C, H, W, border,
+                                                                                         (double*)workspace, map_rgb, map_y);
+  GRL_LAUNCH_CHECK("ssim_tile_kernel");
+  ssim_finalize_kernel<<<dim3(2, (unsigned)B), 256, 0, st>>>((const double*)workspace, C, (long long)gx * gy, (long long)h * w, ssim_rgb, ssim_y);
+  GRL_LAUNCH_CHECK("ssim_finalize_kernel");
+  return GRL_OK;
+}
+
+static F32Planes f32_planes(const float* p, int C, int H, int W) { return {p, (long long)H * W, C}; }
+static U8Pixels u8_pixels(const uint8_t* p, int H, int W, int C) { return {p, (long long)H * W, C}; }
+
+}  // namespace grl
+
+using namespace grl;
+
+extern "C" {
+
+int grl_psnr_f32(const float* restored, const float* target, int B, int C, int H, int W, int border, void* workspace,
+                 size_t workspace_bytes, float* psnr_rgb, float* psnr_y, void* stream) {
+  return psnr_run(f32_planes(restored, C, H, W), f32_planes(target, C, H, W), B, C, H, W, border, workspace, workspace_bytes, psnr_rgb,
+                  psnr_y, stream);
+}
+
+int grl_psnr_u8(const uint8_t* restored, const uint8_t* target, int B, int H, int W, int C, int border, void* workspace,
+                size_t workspace_bytes, float* psnr_rgb, float* psnr_y, void* stream) {
+  return psnr_run(u8_pixels(restored, H, W, C), u8_pixels(target, H, W, C), B, C, H, W, border, workspace, workspace_bytes, psnr_rgb,
+                  psnr_y, stream);
+}
+
+size_t grl_psnrb_workspace(int B) { return sizeof(unsigned long long) * kPsnrbSets * kPsnrbSums * (size_t)(B > 0 ? B : 0); }
+
+int grl_psnrb_f32(const float* restored, const float* target, int B, int C, int H, int W, void* workspace,
+                  size_t workspace_bytes, double* psnrb_rgb, double* psnrb_y, void* stream) {
+  return psnrb_run(f32_planes(restored, C, H, W), f32_planes(target, C, H, W), B, C, H, W, workspace, workspace_bytes, psnrb_rgb,
+                   psnrb_y, stream);
+}
+
+int grl_psnrb_u8(const uint8_t* restored, const uint8_t* target, int B, int H, int W, int C, void* workspace,
+                 size_t workspace_bytes, double* psnrb_rgb, double* psnrb_y, void* stream) {
+  return psnrb_run(u8_pixels(restored, H, W, C), u8_pixels(target, H, W, C), B, C, H, W, workspace, workspace_bytes, psnrb_rgb,
+                   psnrb_y, stream);
 }
 
 size_t grl_ssim_workspace(int B, int C, int H, int W, int border) {
@@ -403,21 +448,14 @@ size_t grl_ssim_workspace(int B, int C, int H, int W, int border) {
 
 int grl_ssim_f32(const float* restored, const float* target, int B, int C, int H, int W, int border, void* workspace,
                  size_t workspace_bytes, double* ssim_rgb, double* ssim_y, double* map_rgb, double* map_y, void* stream) {
-  GRL_REQUIRE(restored && target && ssim_rgb, "ssim: null argument");
-  GRL_SSIM_SHAPE(B, C, H, W, border);
-  if (B == 0) return GRL_OK;
-  GRL_REQUIRE(workspace && workspace_bytes >= grl_ssim_workspace(B, C, H, W, border), "ssim: workspace %zu bytes < %zu",
-              workspace_bytes, grl_ssim_workspace(B, C, H, W, border));
-  const cudaStream_t st = (cudaStream_t)stream;
-  const int h = H - 2 * border, w = W - 2 * border;
-  const int gx = ceil_div(w, kSsimTW), gy = ceil_div(h, kSsimTH);
-  GRL_REQUIRE(gy <= 65535 && B <= 65535, "ssim: %d tile rows / %d images exceed the grid", gy, B);
-  ssim_tile_kernel<<<dim3((unsigned)gx, (unsigned)gy, (unsigned)B), kSsimThreads, 0, st>>>(restored, target, C, H, W, border,
-                                                                                         (double*)workspace, map_rgb, map_y);
-  GRL_LAUNCH_CHECK("ssim_tile_kernel");
-  ssim_finalize_kernel<<<dim3(2, (unsigned)B), 256, 0, st>>>((const double*)workspace, C, (long long)gx * gy, (long long)h * w, ssim_rgb, ssim_y);
-  GRL_LAUNCH_CHECK("ssim_finalize_kernel");
-  return GRL_OK;
+  return ssim_run(f32_planes(restored, C, H, W), f32_planes(target, C, H, W), B, C, H, W, border, workspace, workspace_bytes, ssim_rgb,
+                  ssim_y, map_rgb, map_y, stream);
+}
+
+int grl_ssim_u8(const uint8_t* restored, const uint8_t* target, int B, int H, int W, int C, int border, void* workspace,
+                size_t workspace_bytes, double* ssim_rgb, double* ssim_y, double* map_rgb, double* map_y, void* stream) {
+  return ssim_run(u8_pixels(restored, H, W, C), u8_pixels(target, H, W, C), B, C, H, W, border, workspace, workspace_bytes, ssim_rgb,
+                  ssim_y, map_rgb, map_y, stream);
 }
 
 int grl_ssim_taps_host(double* taps11) {

@@ -4,7 +4,8 @@
 // (metrics.niqe).
 //
 // Stages, each one kernel over all B images:
-//   luma    tensor_round, the BGR-weighted luma of grl_niqe.h, crop `border`, crop to 96 * floor(. / 96) from the top left;
+//   luma    tensor_round (or the bytes of 8-bit (B, H, W, 3) pixels), the BGR-weighted luma of grl_niqe.h, crop
+//           `border`, crop to 96 * floor(. / 96) from the top left;
 //   mscn    (img - mu) / (sigma + 1) with mu, E[img^2] the 7 x 7 window correlated with mode "nearest" (a shared-memory tile
 //           with a 3-pixel halo); float64 accumulation stored to fp32 as scipy.ndimage.convolve does for an fp32 input,
 //           then every step in fp32 with explicitly rounded operations (nvcc would contract them into FMAs otherwise).
@@ -19,6 +20,7 @@
 #include <algorithm>
 
 #include "grl_common.cuh"
+#include "grl_image_u8.h"
 #include "grl_niqe.h"
 
 namespace grl {
@@ -32,19 +34,15 @@ struct NiqeTaps {
   float w[8];
 };
 
-__device__ __forceinline__ float nq_round8(float v) {
-  v = fminf(fmaxf(v, 0.f), 1.f);
-  return rintf(v * 255.0f);  // tensor_round: x255, round half to even
-}
-
-__global__ void niqe_luma_kernel(const float* __restrict__ x, int H, int W, int border, int Hc, int Wc, float* __restrict__ y) {
+template <class Img>
+__global__ void niqe_luma_kernel(Img x, int H, int W, int border, int Hc, int Wc, float* __restrict__ y) {
   const int img = blockIdx.y;
-  const long long n = (long long)Hc * Wc, plane = (long long)H * W;
-  const float* p = x + (long long)img * 3 * plane;
+  const long long n = (long long)Hc * Wc;
+  const Img p = x.img(img);
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     const int r = (int)(i / Wc), c = (int)(i - (long long)r * Wc);
     const long long off = (long long)(r + border) * W + (c + border);
-    y[img * n + i] = niqe_luma((int)nq_round8(p[off]), (int)nq_round8(p[plane + off]), (int)nq_round8(p[2 * plane + off]));
+    y[img * n + i] = niqe_luma((int)p(0, off), (int)p(1, off), (int)p(2, off));
   }
 }
 
@@ -234,6 +232,49 @@ static void niqe_half_taps(float* w8) {
 
 static size_t align256(size_t b) { return (b + 255) / 256 * 256; }
 
+template <class Img>
+int niqe_luma_run(Img x, int B, int C, int H, int W, int border, float* y, void* stream) {
+  GRL_REQUIRE(x.p && y, "niqe_luma: null argument");
+  GRL_REQUIRE(C == 3, "niqe: needs RGB images (C == 3), got C = %d", C);
+  GRL_REQUIRE(B >= 0 && border >= 0 && H - 2 * border >= 96 && W - 2 * border >= 96,
+              "niqe: needs at least 96 x 96 pixels after cropping border %d, got %d x %d", border, H, W);
+  if (B == 0) return GRL_OK;
+  const int Hc = (H - 2 * border) / 96 * 96, Wc = (W - 2 * border) / 96 * 96;
+  niqe_luma_kernel<<<dim3(grid_1d((long long)Hc * Wc), B), 256, 0, (cudaStream_t)stream>>>(x, H, W, border, Hc, Wc, y);
+  GRL_LAUNCH_CHECK("niqe_luma_kernel");
+  return GRL_OK;
+}
+
+// The four stages on one workspace: luma, MSCN, x0.5 resize, MSCN of the resized image, features.
+template <class Img>
+int niqe_features_run(Img x, int B, int C, int H, int W, int border, const double* window49, const double* tables,
+                      void* workspace, size_t workspace_bytes, double* feats, void* stream) {
+  GRL_REQUIRE(x.p && window49 && tables && feats, "niqe: null argument");
+  GRL_REQUIRE(C == 3, "niqe: needs RGB images (C == 3), got C = %d", C);
+  GRL_REQUIRE(B >= 0 && border >= 0 && H - 2 * border >= 96 && W - 2 * border >= 96,
+              "niqe: needs at least 96 x 96 pixels after cropping border %d, got %d x %d", border, H, W);
+  if (B == 0) return GRL_OK;
+  GRL_REQUIRE(workspace && workspace_bytes >= grl_niqe_workspace(B, H, W, border), "niqe: workspace %zu bytes < %zu",
+              workspace_bytes, grl_niqe_workspace(B, H, W, border));
+  const int Hc = (H - 2 * border) / 96 * 96, Wc = (W - 2 * border) / 96 * 96;
+  char* p = (char*)workspace;
+  float* y = (float*)p;
+  p += align256(sizeof(float) * B * (size_t)Hc * Wc);
+  float* m1 = (float*)p;
+  p += align256(sizeof(float) * B * (size_t)Hc * Wc);
+  float* t = (float*)p;
+  p += align256(sizeof(float) * B * (size_t)(Hc / 2) * Wc);
+  float* y2 = (float*)p;
+  p += align256(sizeof(float) * B * (size_t)(Hc / 2) * (Wc / 2));
+  float* m2 = (float*)p;
+  int rc;
+  if ((rc = niqe_luma_run(x, B, C, H, W, border, y, stream)) != GRL_OK) return rc;
+  if ((rc = grl_niqe_mscn_f32(y, B, Hc, Wc, window49, m1, stream)) != GRL_OK) return rc;
+  if ((rc = grl_niqe_half_f32(y, B, Hc, Wc, t, y2, stream)) != GRL_OK) return rc;
+  if ((rc = grl_niqe_mscn_f32(y2, B, Hc / 2, Wc / 2, window49, m2, stream)) != GRL_OK) return rc;
+  return grl_niqe_feat_f32(m1, m2, B, Hc / 96, Wc / 96, tables, feats, stream);
+}
+
 }  // namespace grl
 
 using namespace grl;
@@ -253,15 +294,11 @@ int grl_niqe_half_taps_host(float* w8) {
 }
 
 int grl_niqe_luma_f32(const float* restored, int B, int C, int H, int W, int border, float* y, void* stream) {
-  GRL_REQUIRE(restored && y, "niqe_luma: null argument");
-  GRL_REQUIRE(C == 3, "niqe: needs RGB images (C == 3), got C = %d", C);
-  GRL_REQUIRE(B >= 0 && border >= 0 && H - 2 * border >= 96 && W - 2 * border >= 96,
-              "niqe: needs at least 96 x 96 pixels after cropping border %d, got %d x %d", border, H, W);
-  if (B == 0) return GRL_OK;
-  const int Hc = (H - 2 * border) / 96 * 96, Wc = (W - 2 * border) / 96 * 96;
-  niqe_luma_kernel<<<dim3(grid_1d((long long)Hc * Wc), B), 256, 0, (cudaStream_t)stream>>>(restored, H, W, border, Hc, Wc, y);
-  GRL_LAUNCH_CHECK("niqe_luma_kernel");
-  return GRL_OK;
+  return niqe_luma_run(F32Planes{restored, (long long)H * W, C}, B, C, H, W, border, y, stream);
+}
+
+int grl_niqe_luma_u8(const uint8_t* restored, int B, int H, int W, int C, int border, float* y, void* stream) {
+  return niqe_luma_run(U8Pixels{restored, (long long)H * W, C}, B, C, H, W, border, y, stream);
 }
 
 int grl_niqe_mscn_f32(const float* img, int B, int H, int W, const double* window49, float* out, void* stream) {
@@ -307,33 +344,16 @@ size_t grl_niqe_workspace(int B, int H, int W, int border) {
   return 2 * full + align256(sizeof(float) * B * (Hc / 2) * Wc) + 2 * half;
 }
 
-// The four stages above on one workspace: luma, MSCN, x0.5 resize, MSCN of the resized image, features.
 int grl_niqe_features_f32(const float* restored, int B, int C, int H, int W, int border, const double* window49,
                           const double* tables, void* workspace, size_t workspace_bytes, double* feats, void* stream) {
-  GRL_REQUIRE(restored && window49 && tables && feats, "niqe: null argument");
-  GRL_REQUIRE(C == 3, "niqe: needs RGB images (C == 3), got C = %d", C);
-  GRL_REQUIRE(B >= 0 && border >= 0 && H - 2 * border >= 96 && W - 2 * border >= 96,
-              "niqe: needs at least 96 x 96 pixels after cropping border %d, got %d x %d", border, H, W);
-  if (B == 0) return GRL_OK;
-  GRL_REQUIRE(workspace && workspace_bytes >= grl_niqe_workspace(B, H, W, border), "niqe: workspace %zu bytes < %zu",
-              workspace_bytes, grl_niqe_workspace(B, H, W, border));
-  const int Hc = (H - 2 * border) / 96 * 96, Wc = (W - 2 * border) / 96 * 96;
-  char* p = (char*)workspace;
-  float* y = (float*)p;
-  p += align256(sizeof(float) * B * (size_t)Hc * Wc);
-  float* m1 = (float*)p;
-  p += align256(sizeof(float) * B * (size_t)Hc * Wc);
-  float* t = (float*)p;
-  p += align256(sizeof(float) * B * (size_t)(Hc / 2) * Wc);
-  float* y2 = (float*)p;
-  p += align256(sizeof(float) * B * (size_t)(Hc / 2) * (Wc / 2));
-  float* m2 = (float*)p;
-  int rc;
-  if ((rc = grl_niqe_luma_f32(restored, B, C, H, W, border, y, stream)) != GRL_OK) return rc;
-  if ((rc = grl_niqe_mscn_f32(y, B, Hc, Wc, window49, m1, stream)) != GRL_OK) return rc;
-  if ((rc = grl_niqe_half_f32(y, B, Hc, Wc, t, y2, stream)) != GRL_OK) return rc;
-  if ((rc = grl_niqe_mscn_f32(y2, B, Hc / 2, Wc / 2, window49, m2, stream)) != GRL_OK) return rc;
-  return grl_niqe_feat_f32(m1, m2, B, Hc / 96, Wc / 96, tables, feats, stream);
+  return niqe_features_run(F32Planes{restored, (long long)H * W, C}, B, C, H, W, border, window49, tables, workspace,
+                           workspace_bytes, feats, stream);
+}
+
+int grl_niqe_features_u8(const uint8_t* restored, int B, int H, int W, int C, int border, const double* window49,
+                         const double* tables, void* workspace, size_t workspace_bytes, double* feats, void* stream) {
+  return niqe_features_run(U8Pixels{restored, (long long)H * W, C}, B, C, H, W, border, window49, tables, workspace,
+                           workspace_bytes, feats, stream);
 }
 
 }  // extern "C"

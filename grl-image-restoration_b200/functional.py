@@ -218,6 +218,50 @@ def demosaic_host(x):
     return y
 
 
+def u8_to_f32(img):
+    """Decoded 8-bit images (B, H, W, C) uint8 on the GPU, 1 <= C <= 8 -> (B, C, H, W) float32 = k / 255, correctly
+    rounded: what every dataset's transforms.functional.to_tensor gives (img.float().div(255) on the CPU).  One kernel."""
+    capi.require_device(img)
+    if img.dtype != torch.uint8 or img.dim() != 4 or not 1 <= img.shape[3] <= 8:
+        raise RuntimeError(f"grl_b200: u8_to_f32 needs (B, H, W, C) uint8 images with 1 <= C <= 8, got {img.dtype} "
+                           f"{tuple(img.shape)}")
+    img = img.contiguous()
+    B, H, W, C = img.shape
+    y = torch.empty(B, C, H, W, device=img.device, dtype=torch.float32)
+    capi.check(capi.lib().grl_u8_to_f32(capi.ptr(img), B, H, W, C, capi.ptr(y), capi.stream()))
+    return y
+
+
+def f32_to_u8(y):
+    """(B, C, H, W) float32 on the GPU, 1 <= C <= 8 -> (B, H, W, C) uint8 = round(clamp(v, 0, 1) * 255) with ties to
+    even: the validation step's tensor_round times 255, the bytes of a saved image.  NaN gives 0.  One kernel."""
+    y = _f32c(y, "y")
+    if y.dim() != 4 or not 1 <= y.shape[1] <= 8:
+        raise RuntimeError(f"grl_b200: f32_to_u8 needs (B, C, H, W) float32 images with 1 <= C <= 8, got {tuple(y.shape)}")
+    B, C, H, W = y.shape
+    img = torch.empty(B, H, W, C, device=y.device, dtype=torch.uint8)
+    capi.check(capi.lib().grl_f32_to_u8(capi.ptr(y), B, C, H, W, capi.ptr(img), capi.stream()))
+    return img
+
+
+def u8_to_f32_host(img):
+    """u8_to_f32 evaluated on the CPU by the library's host copy of the same closed form (tests)."""
+    img = img.contiguous()
+    B, H, W, C = img.shape
+    y = torch.empty(B, C, H, W, dtype=torch.float32)
+    capi.check(capi.lib().grl_u8_to_f32_host(ctypes.c_void_p(img.data_ptr()), B, H, W, C, ctypes.c_void_p(y.data_ptr())))
+    return y
+
+
+def f32_to_u8_host(y):
+    """f32_to_u8 evaluated on the CPU by the library's host copy of the same closed form (tests)."""
+    y = y.float().contiguous()
+    B, C, H, W = y.shape
+    img = torch.empty(B, H, W, C, dtype=torch.uint8)
+    capi.check(capi.lib().grl_f32_to_u8_host(ctypes.c_void_p(y.data_ptr()), B, C, H, W, ctypes.c_void_p(img.data_ptr())))
+    return img
+
+
 def stripe_attention(qkv, anchor, B, tok_grid, anc_grid, heads, scale1, bias1, scale2, bias2, use_mask, out=None):
     """qkv (B, L, 3c) view (stripe half), anchor (B, Ha, Wa, c) -> (B, L, c)."""
     qp, ldq = _token_rows(qkv, "qkv")

@@ -6,6 +6,9 @@ utils/metrics/ssim.py:17-82 (Gaussian-window SSIM, 11 taps, sigma 1.5, taps roun
 psnr_fused() and ssim_fused() are the hand-written kernels (csrc/metric.cu, grl_psnr_f32 and grl_ssim_f32) behind
 validation_metrics_fused(), the validation step's four numbers without torch math on the images; the torch-op functions
 below define the same quantities on any device and are what the CPU tests pin against the reference's own functions.
+The kernel-backed functions (psnr_fused, ssim_fused, psnrb_fused, niqe_features, niqe) take either float (B, C, H, W)
+images, rounded to the 8-bit grid inside, or 8-bit (B, H, W, C) uint8 images, read as they are (the _u8 entry points);
+an image and u8_to_f32 of it score the same bit for bit.
 """
 import math
 
@@ -39,22 +42,38 @@ def psnr(restored, target, border=0, channel="rgb"):
     return -10 * (a - b).pow(2).mean([-3, -2, -1]).log10()
 
 
-def psnr_fused(restored, target, border=0):
-    """(psnr_rgb, psnr_y), each (B,), from ONE fused kernel over CUDA fp32 (B, C, H, W) images: tensor_round + shave +
-    exact integer squared-error reduction (csrc/metric.cu).  No torch math on the images."""
+def _image_pair(name, restored, target):
+    """The two images of a fused metric call -> (a, b, u8, (B, C, H, W)): 8-bit (B, H, W, C) uint8 images contiguous as
+    they are, anything else as contiguous float32 (B, C, H, W).  Both must be uint8 or neither."""
     from . import capi
 
     capi.require_device(restored)
     capi.require_device(target)
+    u8 = restored.dtype == torch.uint8
+    if u8 != (target.dtype == torch.uint8):
+        raise RuntimeError(f"grl_b200: {name} needs two uint8 images or two float images, got {restored.dtype} / {target.dtype}")
+    layout = "(B, H, W, C) uint8" if u8 else "(B, C, H, W)"
     if restored.shape != target.shape or restored.dim() != 4:
-        raise RuntimeError(f"grl_b200: psnr_fused needs two (B, C, H, W) tensors of one shape, got {tuple(restored.shape)} / {tuple(target.shape)}")
+        raise RuntimeError(f"grl_b200: {name} needs two {layout} tensors of one shape, got {tuple(restored.shape)} / {tuple(target.shape)}")
+    if u8:
+        B, H, W, C = restored.shape
+        return restored.contiguous(), target.contiguous(), True, (B, C, H, W)
     a = restored if (restored.dtype == torch.float32 and restored.is_contiguous()) else restored.float().contiguous()
     b = target if (target.dtype == torch.float32 and target.is_contiguous()) else target.float().contiguous()
-    B, C, H, W = a.shape
+    return a, b, False, tuple(a.shape)
+
+
+def psnr_fused(restored, target, border=0):
+    """(psnr_rgb, psnr_y), each (B,), from ONE fused kernel over CUDA fp32 (B, C, H, W) or uint8 (B, H, W, C) images:
+    tensor_round + shave + exact integer squared-error reduction (csrc/metric.cu).  No torch math on the images."""
+    from . import capi
+
+    a, b, u8, (B, C, H, W) = _image_pair("psnr_fused", restored, target)
     ws = torch.empty(2 * max(B, 1), device=a.device, dtype=torch.int64)
     out = torch.empty(2, B, device=a.device, dtype=torch.float32)
-    capi.check(capi.lib().grl_psnr_f32(capi.ptr(a), capi.ptr(b), B, C, H, W, int(border), capi.ptr(ws), ws.numel() * 8,
-                                       capi.ptr(out[0]), capi.ptr(out[1]), capi.stream()))
+    fn, dims = (capi.lib().grl_psnr_u8, (B, H, W, C)) if u8 else (capi.lib().grl_psnr_f32, (B, C, H, W))
+    capi.check(fn(capi.ptr(a), capi.ptr(b), *dims, int(border), capi.ptr(ws), ws.numel() * 8, capi.ptr(out[0]),
+                  capi.ptr(out[1]), capi.stream()))
     return out[0], out[1]
 
 
@@ -85,23 +104,18 @@ def ssim(restored, target, border=0, channel="rgb", window_size=11, sigma=1.5):
 
 
 def ssim_fused(restored, target, border=0):
-    """(ssim_rgb, ssim_y), each (B,) float64, from one fused kernel over CUDA fp32 (B, C, H, W) images, C = 1 or 3
-    (csrc/metric.cu, grl_ssim_f32): tensor_round + shave + luma + separable float64 window sums on the 8-bit integers;
-    ssim_y is a copy of ssim_rgb for C = 1."""
+    """(ssim_rgb, ssim_y), each (B,) float64, from one fused kernel over CUDA fp32 (B, C, H, W) or uint8 (B, H, W, C)
+    images, C = 1 or 3 (csrc/metric.cu, grl_ssim_f32 / grl_ssim_u8): tensor_round + shave + luma + separable float64
+    window sums on the 8-bit integers; ssim_y is a copy of ssim_rgb for C = 1."""
     from . import capi
 
-    capi.require_device(restored)
-    capi.require_device(target)
-    if restored.shape != target.shape or restored.dim() != 4:
-        raise RuntimeError(f"grl_b200: ssim_fused needs two (B, C, H, W) tensors of one shape, got {tuple(restored.shape)} / {tuple(target.shape)}")
-    a = restored if (restored.dtype == torch.float32 and restored.is_contiguous()) else restored.float().contiguous()
-    b = target if (target.dtype == torch.float32 and target.is_contiguous()) else target.float().contiguous()
-    B, C, H, W = a.shape
+    a, b, u8, (B, C, H, W) = _image_pair("ssim_fused", restored, target)
     nbytes = capi.lib().grl_ssim_workspace(B, C, H, W, int(border))
     ws = torch.empty(max(nbytes // 8, 1), device=a.device, dtype=torch.float64)
     out = torch.empty(2, B, device=a.device, dtype=torch.float64)
-    capi.check(capi.lib().grl_ssim_f32(capi.ptr(a), capi.ptr(b), B, C, H, W, int(border), capi.ptr(ws), ws.numel() * 8,
-                                       capi.ptr(out[0]), capi.ptr(out[1]), None, None, capi.stream()))
+    fn, dims = (capi.lib().grl_ssim_u8, (B, H, W, C)) if u8 else (capi.lib().grl_ssim_f32, (B, C, H, W))
+    capi.check(fn(capi.ptr(a), capi.ptr(b), *dims, int(border), capi.ptr(ws), ws.numel() * 8, capi.ptr(out[0]),
+                  capi.ptr(out[1]), None, None, capi.stream()))
     return out[0], out[1]
 
 
@@ -148,22 +162,17 @@ def psnrb(restored, target, channel="rgb"):
 
 
 def psnrb_fused(restored, target):
-    """(psnrb_rgb, psnrb_y), each (B,) float64, from one fused kernel over CUDA fp32 (B, C, H, W) images, C = 1 or 3
-    (csrc/metric.cu, grl_psnrb_f32); psnrb_y is a copy of psnrb_rgb for C = 1."""
+    """(psnrb_rgb, psnrb_y), each (B,) float64, from one fused kernel over CUDA fp32 (B, C, H, W) or uint8 (B, H, W, C)
+    images, C = 1 or 3 (csrc/metric.cu, grl_psnrb_f32 / grl_psnrb_u8); psnrb_y is a copy of psnrb_rgb for C = 1."""
     from . import capi
 
-    capi.require_device(restored)
-    capi.require_device(target)
-    if restored.shape != target.shape or restored.dim() != 4:
-        raise RuntimeError(f"grl_b200: psnrb_fused needs two (B, C, H, W) tensors of one shape, got {tuple(restored.shape)} / {tuple(target.shape)}")
-    a = restored if (restored.dtype == torch.float32 and restored.is_contiguous()) else restored.float().contiguous()
-    b = target if (target.dtype == torch.float32 and target.is_contiguous()) else target.float().contiguous()
-    B, C, H, W = a.shape
+    a, b, u8, (B, C, H, W) = _image_pair("psnrb_fused", restored, target)
     nbytes = capi.lib().grl_psnrb_workspace(B)
     ws = torch.empty(max(nbytes // 8, 1), device=a.device, dtype=torch.int64)
     out = torch.empty(2, B, device=a.device, dtype=torch.float64)
-    capi.check(capi.lib().grl_psnrb_f32(capi.ptr(a), capi.ptr(b), B, C, H, W, capi.ptr(ws), ws.numel() * 8,
-                                        capi.ptr(out[0]), capi.ptr(out[1]), capi.stream()))
+    fn, dims = (capi.lib().grl_psnrb_u8, (B, H, W, C)) if u8 else (capi.lib().grl_psnrb_f32, (B, C, H, W))
+    capi.check(fn(capi.ptr(a), capi.ptr(b), *dims, capi.ptr(ws), ws.numel() * 8, capi.ptr(out[0]), capi.ptr(out[1]),
+                  capi.stream()))
     return out[0], out[1]
 
 
@@ -219,33 +228,41 @@ def niqe_params(params):
 
 
 def _niqe_check(restored, border):
+    """-> (x, u8, (B, C, H, W)): 8-bit (B, H, W, 3) uint8 images contiguous as they are, anything else as contiguous
+    float32 (B, 3, H, W)."""
     from . import capi
 
     capi.require_device(restored)
-    if restored.dim() != 4 or restored.shape[1] != 3:
-        raise RuntimeError(f"grl_b200: niqe needs (B, 3, H, W) RGB images, got {tuple(restored.shape)}")
-    if min(restored.shape[-2:]) - 2 * border < 96:
-        raise RuntimeError(f"grl_b200: niqe needs at least 96 x 96 pixels after cropping border {border}, got {tuple(restored.shape[-2:])}")
-    return restored if (restored.dtype == torch.float32 and restored.is_contiguous()) else restored.float().contiguous()
+    u8 = restored.dtype == torch.uint8
+    if restored.dim() != 4 or restored.shape[3 if u8 else 1] != 3:
+        raise RuntimeError(f"grl_b200: niqe needs {'(B, H, W, 3) uint8' if u8 else '(B, 3, H, W)'} RGB images, got {tuple(restored.shape)}")
+    hw = restored.shape[1:3] if u8 else restored.shape[2:]
+    if min(hw) - 2 * border < 96:
+        raise RuntimeError(f"grl_b200: niqe needs at least 96 x 96 pixels after cropping border {border}, got {tuple(hw)}")
+    if u8:
+        B, H, W, C = restored.shape
+        return restored.contiguous(), True, (B, C, H, W)
+    x = restored if (restored.dtype == torch.float32 and restored.is_contiguous()) else restored.float().contiguous()
+    return x, False, tuple(x.shape)
 
 
 def niqe_features(restored, params, border=0):
-    """(B, nblocks, 36) float64 per-block features (niqe.py:445-473) from the device kernels (csrc/niqe.cu)."""
+    """(B, nblocks, 36) float64 per-block features (niqe.py:445-473) from the device kernels (csrc/niqe.cu); restored is
+    fp32 (B, 3, H, W) or uint8 (B, H, W, 3)."""
     import ctypes
 
     from . import capi
 
     _, _, win = niqe_params(params)
-    x = _niqe_check(restored, border)
-    B, C, H, W = x.shape
+    x, u8, (B, C, H, W) = _niqe_check(restored, border)
     nb = ((H - 2 * border) // 96) * ((W - 2 * border) // 96)
     nbytes = capi.lib().grl_niqe_workspace(B, H, W, int(border))
     ws = torch.empty(max(nbytes, 1), device=x.device, dtype=torch.uint8)
     feats = torch.empty(B, nb, 36, device=x.device, dtype=torch.float64)
     win_host = (ctypes.c_double * 49)(*win.flatten().tolist())
-    capi.check(capi.lib().grl_niqe_features_f32(capi.ptr(x), B, C, H, W, int(border), win_host,
-                                                capi.ptr(_niqe_device_tables(x.device)), capi.ptr(ws), ws.numel(),
-                                                capi.ptr(feats), capi.stream()))
+    fn, dims = (capi.lib().grl_niqe_features_u8, (B, H, W, C)) if u8 else (capi.lib().grl_niqe_features_f32, (B, C, H, W))
+    capi.check(fn(capi.ptr(x), *dims, int(border), win_host, capi.ptr(_niqe_device_tables(x.device)), capi.ptr(ws),
+                  ws.numel(), capi.ptr(feats), capi.stream()))
     return feats
 
 
@@ -257,8 +274,7 @@ def niqe_stages(restored, params, border=0):
     from . import capi
 
     _, _, win = niqe_params(params)
-    x = _niqe_check(restored, border)
-    B, C, H, W = x.shape
+    x, u8, (B, C, H, W) = _niqe_check(restored, border)
     Hc, Wc = (H - 2 * border) // 96 * 96, (W - 2 * border) // 96 * 96
     win_host = (ctypes.c_double * 49)(*win.flatten().tolist())
     f32 = dict(device=x.device, dtype=torch.float32)
@@ -266,7 +282,10 @@ def niqe_stages(restored, params, border=0):
          "half": torch.empty(B, Hc // 2, Wc // 2, **f32), "mscn2": torch.empty(B, Hc // 2, Wc // 2, **f32),
          "feats": torch.empty(B, (Hc // 96) * (Wc // 96), 36, device=x.device, dtype=torch.float64)}
     L, st = capi.lib(), capi.stream()
-    capi.check(L.grl_niqe_luma_f32(capi.ptr(x), B, C, H, W, int(border), capi.ptr(s["y"]), st))
+    if u8:
+        capi.check(L.grl_niqe_luma_u8(capi.ptr(x), B, H, W, C, int(border), capi.ptr(s["y"]), st))
+    else:
+        capi.check(L.grl_niqe_luma_f32(capi.ptr(x), B, C, H, W, int(border), capi.ptr(s["y"]), st))
     capi.check(L.grl_niqe_mscn_f32(capi.ptr(s["y"]), B, Hc, Wc, win_host, capi.ptr(s["mscn1"]), st))
     capi.check(L.grl_niqe_half_f32(capi.ptr(s["y"]), B, Hc, Wc, capi.ptr(s["tmp"]), capi.ptr(s["half"]), st))
     capi.check(L.grl_niqe_mscn_f32(capi.ptr(s["half"]), B, Hc // 2, Wc // 2, win_host, capi.ptr(s["mscn2"]), st))
@@ -299,7 +318,7 @@ def niqe_distance(feats, mu_pris, cov_pris):
 
 def niqe(restored, params, border=0):
     """Per-image NIQE (B,) float64 of the blind-SR test command (NaturalImageQualityEvaluator.update, niqe.py:566-576):
-    restored (B, 3, H, W) CUDA fp32, the model's output (tensor_round is applied inside).  params: a path to the
+    restored (B, 3, H, W) CUDA fp32, the model's output (tensor_round is applied inside), or its bytes (B, H, W, 3) uint8.  params: a path to the
     reference's niqe_pris_params.npz (utils/metrics/ in a reference checkout) or a mapping with its three arrays; nothing
     of it ships with this package.  `border` pixels are cropped on every side first.  The luma is the reference's:
     bgr2ycbcr weights on RGB data (grl_niqe.h)."""
@@ -319,8 +338,8 @@ def validation_metrics(restored, target, scale=1, is_sr=False):
 
 
 def validation_metrics_fused(restored, target, scale=1, is_sr=False):
-    """validation_metrics from the two fused kernels, psnr_fused and ssim_fused, on CUDA images: the same four keys,
-    psnr / psnr_y as float32 and ssim / ssim_y as float64 (B,) tensors."""
+    """validation_metrics from the two fused kernels, psnr_fused and ssim_fused, on CUDA images, fp32 (B, C, H, W) or
+    uint8 (B, H, W, C): the same four keys, psnr / psnr_y as float32 and ssim / ssim_y as float64 (B,) tensors."""
     border = scale if is_sr else 0
     p, py = psnr_fused(restored, target, border)
     s, sy = ssim_fused(restored, target, border)

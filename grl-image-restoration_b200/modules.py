@@ -843,6 +843,19 @@ class GRL(nn.Module):
         return self._forward_self_ensemble(x) if self.self_ensemble else self._forward_once(x)
 
     @torch.no_grad()
+    def forward_u8(self, img):
+        """The forward on decoded 8-bit images: img (B, H, W, in_channels) uint8 on the GPU -> (B, H*s, W*s,
+        out_channels) uint8.  Exactly f32_to_u8(forward_rgb(u8_to_f32(img))): the datasets' to_tensor and the validation
+        step's tensor_round as one kernel each around the forward, so precision, self_ensemble and use_cuda_graph apply."""
+        if self.input_format == "rggb":
+            raise ValueError("forward_u8 takes (B, H, W, C) 8-bit images; packed 8-bit Bayer input (input_format='rggb') "
+                             "is not supported")
+        K.capi.require_device(img)
+        if img.dim() != 4 or img.shape[3] != self.in_channels:
+            raise ValueError(f"forward_u8 takes (B, H, W, {self.in_channels}) uint8 images, got {tuple(img.shape)}")
+        return K.f32_to_u8(self.forward_rgb(K.u8_to_f32(img)))
+
+    @torch.no_grad()
     def _forward_self_ensemble(self, x):
         """y = 0.125 * (V_0 + ... + V_7), V_m = inverse_m(forward(augment_img_tensor4(x, m))) (utils/utils_bsr/
         utils_image.py:444-460): 8 independent forwards, each with its own padding, on the views gathered by one kernel

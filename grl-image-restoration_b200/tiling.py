@@ -104,3 +104,15 @@ def forward_tile_sharded(model, x, tile, tile_overlap, scale=None, max_batch=16,
         idx = shard_tiles(len(origins), r, world)
         _accumulate(E, W, [origins[j] for j in idx], recv[r * per_rank: r * per_rank + len(idx)], tile, scale)
     return E.div_(W)
+
+
+@torch.no_grad()
+def forward_tile_u8(model, img, tile, tile_overlap, scale=None, max_batch=16, group=None):
+    """forward_tile_sharded on decoded 8-bit images: img (B, H, W, C) uint8 on the GPU -> (B, H*scale, W*scale, C_out)
+    uint8 = f32_to_u8(forward_tile_sharded(model, u8_to_f32(img), ...)); without a process group that is forward_tile.
+    Packed 8-bit Bayer input (a model with input_format="rggb") is not supported."""
+    if getattr(model, "input_format", "rgb") == "rggb":
+        raise ValueError("forward_tile_u8 takes (B, H, W, C) 8-bit images; packed 8-bit Bayer input "
+                         "(input_format='rggb') is not supported")
+    y = forward_tile_sharded(model, K.u8_to_f32(img), tile, tile_overlap, scale=scale, max_batch=max_batch, group=group)
+    return K.f32_to_u8(y)

@@ -281,6 +281,12 @@ int grl_tc_attn_variant(int variant);
  * geometry.  workspace: 16 * B bytes of device memory (zeroed by the call). */
 int grl_psnr_f32(const float* restored, const float* target, int B, int C, int H, int W, int border, void* workspace,
                  size_t workspace_bytes, float* psnr_rgb, float* psnr_y, void* stream);
+/* Every metric entry point below has a _u8 sibling that takes 8-bit images, restored / target (B, H, W, C) uint8 (note the
+ * argument order B, H, W, C), as they come out of grl_f32_to_u8 or an image decoder: the bytes are the 8-bit integers
+ * tensor_round gives, so the result equals that of the _f32 entry point on grl_u8_to_f32 of the same images bit for bit.
+ * Shapes, workspaces and outputs are those of the _f32 entry point. */
+int grl_psnr_u8(const uint8_t* restored, const uint8_t* target, int B, int H, int W, int C, int border, void* workspace,
+                size_t workspace_bytes, float* psnr_rgb, float* psnr_y, void* stream);
 
 /* Per-image PSNR-B of the JPEG test commands (PeakSignalNoiseRatioBlock.update, utils/metrics/psnrb.py:141-163) on
  * tensor_round'ed images, no shave: per channel 10 log10(1 / (mse + bef)) with the blocking-effect factor bef of the
@@ -292,6 +298,8 @@ int grl_psnr_f32(const float* restored, const float* target, int B, int C, int H
 size_t grl_psnrb_workspace(int B);
 int grl_psnrb_f32(const float* restored, const float* target, int B, int C, int H, int W, void* workspace,
                   size_t workspace_bytes, double* psnrb_rgb, double* psnrb_y, void* stream);
+int grl_psnrb_u8(const uint8_t* restored, const uint8_t* target, int B, int H, int W, int C, void* workspace,
+                 size_t workspace_bytes, double* psnrb_rgb, double* psnrb_y, void* stream);
 
 /* Per-image SSIM of the validation step (StructuralSimilarityIndexMeasure.update, utils/metrics/ssim.py:167-193 ->
  * ssim / _ssim, ssim.py:36-85, after engines/base.py:255-268): both images tensor_round'ed, `border` pixels shaved, local
@@ -306,6 +314,8 @@ int grl_psnrb_f32(const float* restored, const float* target, int B, int C, int 
 size_t grl_ssim_workspace(int B, int C, int H, int W, int border);
 int grl_ssim_f32(const float* restored, const float* target, int B, int C, int H, int W, int border, void* workspace,
                  size_t workspace_bytes, double* ssim_rgb, double* ssim_y, double* map_rgb, double* map_y, void* stream);
+int grl_ssim_u8(const uint8_t* restored, const uint8_t* target, int B, int H, int W, int C, int border, void* workspace,
+                size_t workspace_bytes, double* ssim_rgb, double* ssim_y, double* map_rgb, double* map_y, void* stream);
 /* The 11 normalised float64 window taps (gaussian(11, 1.5), ssim.py:17-24); HOST pointer. */
 int grl_ssim_taps_host(double* taps11);
 /* grl_ssim_f32 on the CPU from the same closed form, HOST pointers; its maps equal the kernel's bit for bit.  Allocates
@@ -325,12 +335,15 @@ int grl_ssim_host(const float* restored, const float* target, int B, int C, int 
 size_t grl_niqe_workspace(int B, int H, int W, int border);
 int grl_niqe_features_f32(const float* restored, int B, int C, int H, int W, int border, const double* window49,
                           const double* tables, void* workspace, size_t workspace_bytes, double* feats, void* stream);
+int grl_niqe_features_u8(const uint8_t* restored, int B, int H, int W, int C, int border, const double* window49,
+                         const double* tables, void* workspace, size_t workspace_bytes, double* feats, void* stream);
 /* The rounded luma (an integer in [16, 235] as fp32) of n 8-bit RGB triples rgb (n, 3); HOST pointers (csrc/grl_niqe.h). */
 int grl_niqe_luma_host(const uint8_t* rgb, int64_t n, float* y);
 /* The 8 fp32 taps of the x0.5 antialiased bicubic resize (niqe.py:169-238); HOST pointer. */
 int grl_niqe_half_taps_host(float* w8);
 /* luma + crops: y (B, Hc, Wc). */
 int grl_niqe_luma_f32(const float* restored, int B, int C, int H, int W, int border, float* y, void* stream);
+int grl_niqe_luma_u8(const uint8_t* restored, int B, int H, int W, int C, int border, float* y, void* stream);
 /* MSCN of img (B, H, W) -> out (B, H, W) (niqe.py:447-455). */
 int grl_niqe_mscn_f32(const float* img, int B, int H, int W, const double* window49, float* out, void* stream);
 /* 255 * imresize(img / 255, 0.5) (niqe.py:470-471): img (B, H, W), H and W even; tmp (B, H/2, W); out (B, H/2, W/2). */
@@ -363,6 +376,19 @@ int grl_ens_merge_f32(const float* ya, const float* yb, int B, int C, int Hs, in
 /* Host evaluation (tests): cfa4 and out are HOST pointers. */
 int grl_demosaic_host(const float* cfa4, int B, int h, int w, float* out);
 int grl_demosaic_f32(const float* cfa4, int B, int h, int w, float* out, void* stream);
+
+/* ---- 8-bit images (the datasets' to_tensor and the validation step's tensor_round, csrc/grl_image_u8.h) -------------
+ * The 8-bit grid at both ends of the pipeline, as two layout transposes: 8-bit HWC pixels, as image decoders give them,
+ * and fp32 CHW planes, as the network and the metrics take them.  1 <= C <= 8 (the 6-channel dual-pixel input). */
+/* src (B, H, W, C) uint8 -> dst (B, C, H, W) fp32 = k / 255, correctly rounded: transforms.functional.to_tensor of every
+ * dataset (data/datasets/restoration_sr.py:114-115), i.e. torch's img.float().div(255) on the CPU. */
+int grl_u8_to_f32(const uint8_t* src, int B, int H, int W, int C, float* dst, void* stream);
+/* src (B, C, H, W) fp32 -> dst (B, H, W, C) uint8 = rint(clamp(v, 0, 1) * 255), ties to even: tensor_round
+ * (utils/utils_image.py:30-33) times 255, the bytes of a saved image.  NaN, which torch leaves undefined, gives 0. */
+int grl_f32_to_u8(const float* src, int B, int C, int H, int W, uint8_t* dst, void* stream);
+/* The same two maps on the CPU from the same closed forms (tests); HOST pointers, any C >= 1. */
+int grl_u8_to_f32_host(const uint8_t* src, int B, int H, int W, int C, float* dst);
+int grl_f32_to_u8_host(const float* src, int B, int C, int H, int W, uint8_t* dst);
 
 #ifdef __cplusplus
 }
