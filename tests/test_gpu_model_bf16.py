@@ -77,17 +77,18 @@ def test_harsh_weights_report(pkg, oracle, device, variant, task, scale, size, h
     assert p_cr >= 25.0
 
 
-def test_bf16_fp32_switch_and_batch_invariance(pkg, oracle, device):
+def test_fp16_fp32_switch(pkg, oracle, device):
+    """Switching one model from the fp16 tensor-core path to the fp32 path.  (Batch composition, bit for bit, is
+    test_gpu_tc_scale.py::test_batch_composition_bitwise.)"""
     cfg = pkg.configs.grl_config("base", "sr", 4, 256)
     m = build(pkg, oracle, cfg, device, seed=1, style="init")
-    x = oracle.synth_input((2, 3, 256, 256), seed=1234).to(device)
+    x = oracle.synth_input((1, 3, 256, 256), seed=1234).to(device)
     y = m(x)
-    assert y.shape == (2, 3, 1024, 1024) and torch.isfinite(y).all()
-    assert (m(x[:1]) - y[:1]).abs().max().item() <= 1e-4
+    assert y.shape == (1, 3, 1024, 1024) and torch.isfinite(y).all()
     m.set_precision("fp32")
-    y32 = m(x[:1])
-    p = (-10 * torch.log10(((y[:1] - y32) ** 2).mean())).item()
-    print(f"base sr 256: PSNR(fp16 path, fp32 path) = {p:.1f} dB, max-abs {(y[:1] - y32).abs().max().item():.3e}")
+    y32 = m(x)
+    p = (-10 * torch.log10(((y - y32) ** 2).mean())).item()
+    print(f"base sr 256: PSNR(fp16 path, fp32 path) = {p:.1f} dB, max-abs {(y - y32).abs().max().item():.3e}")
     assert p >= 25.0
 
 

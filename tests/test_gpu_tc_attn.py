@@ -219,16 +219,16 @@ def old_bound_catches(m, exact, d):
     return bool(err.max() > 4e-2 * max(1.0, float(exact[..., :d].abs().max())) or err.mean() > 6e-3)
 
 
-def block_inputs(case, x_size, dtype, device, seed):
+def block_inputs(case, x_size, dtype, device, seed, batch=B):
     """Packed operands of one block, as the projection epilogues write them: qkv (B*L, 6*heads*32) in slot order
     [window q|k|v][stripe q|k|v] x head and anchor (B*La, heads*32).  q, k and anchors are L2-normalised over head_dim;
     window q, stripe q and stripe k carry exp(min(s, ln 100)) log2 e with a per-head s in [ln 5, ln 150]; with
-    head_dim < 32 column 31 of every value slot is 1."""
+    head_dim < 32 column 31 of every value slot is 1.  `batch` images of x_size."""
     h, d = case.heads, case.d
     H, W = x_size
     g = torch.Generator(device=device).manual_seed(seed)
-    qkv = torch.zeros(B * H * W, 6 * h, 32, device=device)
-    qkv[..., :d] = torch.randn(B * H * W, 6 * h, d, generator=g, device=device)
+    qkv = torch.zeros(batch * H * W, 6 * h, 32, device=device)
+    qkv[..., :d] = torch.randn(batch * H * W, 6 * h, d, generator=g, device=device)
     for grp, scaled in ((0, True), (1, False), (3, True), (4, True)):
         s = math.log(5.0) + (math.log(150.0) - math.log(5.0)) * torch.rand(h, generator=g, device=device)
         scale = torch.exp(s.clamp(max=math.log(100.0))) * O.LOG2E if scaled else torch.ones(h, device=device)
@@ -237,9 +237,9 @@ def block_inputs(case, x_size, dtype, device, seed):
         qkv[:, 2 * h:3 * h, 31] = 1.0
         qkv[:, 5 * h:6 * h, 31] = 1.0
     La = (H // case.df) * (W // case.df)
-    anc = torch.zeros(B * La, h, 32, device=device)
-    anc[..., :d] = torch.nn.functional.normalize(torch.randn(B * La, h, d, generator=g, device=device), dim=-1)
-    return qkv.view(B * H * W, -1).to(dtype), anc.view(B * La, -1).to(dtype)
+    anc = torch.zeros(batch * La, h, 32, device=device)
+    anc[..., :d] = torch.nn.functional.normalize(torch.randn(batch * La, h, d, generator=g, device=device), dim=-1)
+    return qkv.view(batch * H * W, -1).to(dtype), anc.view(batch * La, -1).to(dtype)
 
 
 def cpb_table(ln, seed, grow=0.0):
@@ -260,18 +260,18 @@ def cpb_table(ln, seed, grow=0.0):
     return t
 
 
-def operand(buf, spec, grid, heads):
-    """(Bw, heads, N, 32) view of a launch operand, in the kernel's window order."""
+def operand(buf, spec, grid, heads, batch=B):
+    """(Bw, heads, N, 32) view of a launch operand of `batch` images, in the kernel's window order."""
     name, col = spec
     if name == "x1":
         return buf[name].view(-1, heads, grid.wh * grid.ww, 32)
-    t = buf[name].view(B, grid.H, grid.W, -1)[..., col:col + heads * 32]
+    t = buf[name].view(batch, grid.H, grid.W, -1)[..., col:col + heads * 32]
     return O.attn_windows(t, grid_t(grid), heads)
 
 
-def run(tc, ln, buf, table):
+def run(tc, ln, buf, table, batch=B):
     tc.attention(ln.gq, ln.gk, buf[ln.q[0]], ln.q[1], buf[ln.k[0]], ln.k[1], buf[ln.v[0]], ln.v[1], buf[ln.out[0]],
-                 ln.out[1], B, ln.heads, tc.shifted_copies(table.to(buf["qkv"].device)), ln.use_mask, v_dense=ln.v_dense,
+                 ln.out[1], batch, ln.heads, tc.shifted_copies(table.to(buf["qkv"].device)), ln.use_mask, v_dense=ln.v_dense,
                  o_dense=ln.o_dense, ones_col=ln.ones_col)
 
 
