@@ -50,6 +50,13 @@ class GrlTcAttn(ctypes.Structure):
                 ("rows", ctypes.c_int32), ("rows_pad", ctypes.c_int32), ("use_mask", ctypes.c_int32), ("ones_col", ctypes.c_int32)]
 
 
+class GrlImageRef(ctypes.Structure):
+    _fields_ = [("data", c_vp), ("H", ctypes.c_int32), ("W", ctypes.c_int32), ("kind", ctypes.c_int32)]
+
+
+IMAGE_F32, IMAGE_U8, IMAGE_RGGB = 0, 1, 2  # GrlImageKind
+
+
 _SIGNATURES = {
     "grl_last_error": (ctypes.c_char_p, []),
     "grl_abi_version": (c_int, []),
@@ -114,6 +121,8 @@ _SIGNATURES = {
     "grl_f32_to_u8": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp]),
     "grl_u8_to_f32_host": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_vp]),
     "grl_f32_to_u8_host": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_vp]),
+    "grl_list_gather": (c_int, [ctypes.POINTER(GrlImageRef), c_int, c_int, c_int, c_int, c_vp, c_vp]),
+    "grl_list_crop": (c_int, [c_vp, c_int, c_int, c_int, c_int, ctypes.POINTER(GrlImageRef), c_vp]),
 }
 
 _lib = None

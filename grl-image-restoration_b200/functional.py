@@ -262,6 +262,46 @@ def f32_to_u8_host(y):
     return img
 
 
+def _image_refs(images, kind):
+    refs = (capi.GrlImageRef * max(1, len(images)))()
+    for r, t in zip(refs, images):
+        h, w = t.shape[:2] if kind == capi.IMAGE_U8 else t.shape[1:]
+        r.data, r.H, r.W, r.kind = t.data_ptr(), h, w, kind
+    return refs
+
+
+def list_gather(images, kind, C, Hp, Wp):
+    """check_image_size of every image into one padded batch (n, C, Hp, Wp) float32: reflect padding on the bottom /
+    right, zeros on both axes when a pad is not smaller than its axis (grl.py:479-489).  images: contiguous tensors on
+    the GPU, all of `kind`: capi.IMAGE_F32 (C, H, W) float32, capi.IMAGE_U8 (H, W, C) uint8 (k / 255 as u8_to_f32) or
+    capi.IMAGE_RGGB (4, h, w) float32 packed Bayer planes (demosaiced as K.demosaic, C = 3).  Needs (H, W) <= (Hp, Wp)."""
+    want = torch.uint8 if kind == capi.IMAGE_U8 else torch.float32
+    want_c = {capi.IMAGE_U8: (2, C), capi.IMAGE_RGGB: (0, 4)}.get(kind, (0, C))  # (channel dim, channels)
+    for t in images:
+        capi.require_device(t)
+        if t.dtype != want or t.dim() != 3 or not t.is_contiguous() or t.shape[want_c[0]] != want_c[1]:
+            raise RuntimeError(f"grl_b200: list_gather needs contiguous {want} images of {C} channels (kind {kind}), got "
+                               f"{t.dtype} {tuple(t.shape)}")
+    dev = torch.device("cuda", torch.cuda.current_device()) if not images else images[0].device
+    out = torch.empty(len(images), C, Hp, Wp, device=dev, dtype=torch.float32)
+    capi.check(capi.lib().grl_list_gather(_image_refs(images, kind), len(images), C, Hp, Wp, capi.ptr(out), capi.stream()))
+    return out
+
+
+def list_crop(y, sizes, u8=False):
+    """The top-left (H_i, W_i) corner of every image of a batch y (n, C, Hy, Wy) float32 on the GPU, as a list of
+    (C, H_i, W_i) float32 tensors, or with u8 of (H_i, W_i, C) uint8 tensors as f32_to_u8 gives them."""
+    y = _f32c(y, "y")
+    n, C, Hy, Wy = y.shape
+    if len(sizes) != n:
+        raise RuntimeError(f"grl_b200: list_crop got {len(sizes)} sizes for a batch of {n}")
+    outs = [torch.empty((h, w, C) if u8 else (C, h, w), device=y.device, dtype=torch.uint8 if u8 else torch.float32)
+            for h, w in sizes]
+    kind = capi.IMAGE_U8 if u8 else capi.IMAGE_F32
+    capi.check(capi.lib().grl_list_crop(capi.ptr(y), n, C, Hy, Wy, _image_refs(outs, kind), capi.stream()))
+    return outs
+
+
 def stripe_attention(qkv, anchor, B, tok_grid, anc_grid, heads, scale1, bias1, scale2, bias2, use_mask, out=None):
     """qkv (B, L, 3c) view (stripe half), anchor (B, Ha, Wa, c) -> (B, L, c)."""
     qp, ldq = _token_rows(qkv, "qkv")

@@ -23,6 +23,7 @@ import torch.nn.functional as F
 
 from . import functional as K
 from . import geometry as G
+from . import image_list
 from . import tc
 from .geometry import to_2tuple, _get_stripe_info
 
@@ -571,6 +572,9 @@ class GRL(nn.Module):
         # ensemble_max_batch images, which bounds the activation memory of the 8x larger batch.
         self.self_ensemble = bool(self_ensemble)
         self.ensemble_max_batch = 16
+        # forward_list runs the images of one padded size in forwards of at most max_batch_tokens padded pixels each
+        # (default: bench.py's per-GPU batch, 16 images of 256 x 256), which bounds the activation memory of a list
+        self.max_batch_tokens = 16 * 256 * 256
         # "rggb": forward takes the dm task's packed RGGB Bayer planes (B, 4, h, w) and demosaics them on the device with
         # the reference engine's dm_matlab (engines/base.py:127-128) before the network; "rgb" (default): the reference's
         # forward.  Feed "rggb" only data that the caller has not demosaiced already.
@@ -802,9 +806,12 @@ class GRL(nn.Module):
             graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(graph):
                 static_out = tc.forward(self, static_in, rggb)
-            ent = (graph, static_in, static_out)
+            # the graph reads every block's cached attention constants (tc.BlockPlan) at their addresses at capture; a
+            # forward at another resolution replaces that cache, so the graph holds its own references to them
+            consts = [b._tc_plan._consts for layer in self.layers for b in layer.blocks]
+            ent = (graph, static_in, static_out, consts)
             self._graphs[key] = ent
-        graph, static_in, static_out = ent
+        graph, static_in, static_out, _ = ent
         static_in.copy_(x)
         graph.replay()
         return static_out.clone()
@@ -854,6 +861,19 @@ class GRL(nn.Module):
         if img.dim() != 4 or img.shape[3] != self.in_channels:
             raise ValueError(f"forward_u8 takes (B, H, W, {self.in_channels}) uint8 images, got {tuple(img.shape)}")
         return K.f32_to_u8(self.forward_rgb(K.u8_to_f32(img)))
+
+    def forward_list(self, images):
+        """The forward on a list of differently sized images, as a test set comes: images[i] is (in_channels, H_i, W_i)
+        (input_format "rggb": packed Bayer planes (4, h_i, w_i)), all of one float dtype, on the GPU.  Returns the list of
+        outputs in input order; element i equals self(images[i][None])[0] bit for bit, whatever precision,
+        use_cuda_graph and self_ensemble say.  Images that pad to the same size run in one batched forward of at most
+        max_batch_tokens padded pixels (image_list.py); with self_ensemble each image runs on its own."""
+        return image_list.forward_list(self, images)
+
+    def forward_list_u8(self, images):
+        """forward_list of decoded 8-bit images (H_i, W_i, in_channels) uint8 on the GPU -> (H_i*s, W_i*s, out_channels)
+        uint8; element i equals forward_u8(images[i][None])[0] bit for bit."""
+        return image_list.forward_list(self, images, u8=True)
 
     @torch.no_grad()
     def _forward_self_ensemble(self, x):

@@ -390,6 +390,34 @@ int grl_f32_to_u8(const float* src, int B, int C, int H, int W, uint8_t* dst, vo
 int grl_u8_to_f32_host(const uint8_t* src, int B, int H, int W, int C, float* dst);
 int grl_f32_to_u8_host(const float* src, int B, int C, int H, int W, uint8_t* dst);
 
+/* ---- lists of differently sized images (GRL.forward_list, csrc/image_list.cu) -----------------------------------------
+ * The reference forward takes one (B, C, H, W) tensor, so a test set of differently sized images runs as a loop of B = 1
+ * forwards.  A forward's arithmetic depends only on the padded size, so images that check_image_size pads to the same
+ * (Hp, Wp) can share one forward: these two calls move such a group in and out of that batch.
+ * A GrlImageRef describes one image of a list; `data` is a DEVICE pointer, the array of GrlImageRef is a HOST array that
+ * the call copies into kernel parameters (no device copy).  Every ref of one call has the same kind.
+ *   GRL_IMAGE_F32  (C, H, W) fp32 planes
+ *   GRL_IMAGE_U8   (H, W, C) uint8 pixels, as image decoders give them (k / 255 of grl_u8_to_f32 on the way in, round8 of
+ *                  grl_f32_to_u8 on the way out)
+ *   GRL_IMAGE_RGGB (4, H, W) fp32 packed RGGB planes of a (2H, 2W) image, demosaiced as by grl_demosaic_f32 (gather only;
+ *                  C = 3, H, W >= 2) */
+typedef enum { GRL_IMAGE_F32 = 0, GRL_IMAGE_U8 = 1, GRL_IMAGE_RGGB = 2 } GrlImageKind;
+typedef struct {
+  void* data;
+  int32_t H, W; /* the image's size (RGGB: of the packed planes) */
+  int32_t kind; /* GrlImageKind */
+} GrlImageRef;
+/* check_image_size (grl.py:479-489) of every image of the list into one padded batch: out (n, C, Hp, Wp) fp32, image i
+ * (size H x W <= Hp x Wp, demosaiced first for RGGB) reflect-padded on the bottom / right, or zero-padded on both axes
+ * when Hp - H >= H or Wp - W >= W (F.pad raises and the reference falls back to constant padding, grl.py:485-488).
+ * Image i of the batch equals check_image_size(x_i[None])[0] bit for bit when (Hp, Wp) is x_i's padded size.
+ * 1 <= C <= 8. */
+int grl_list_gather(const GrlImageRef* images, int n, int C, int Hp, int Wp, float* out, void* stream);
+/* The crop of the reference's forward (grl.py:549-551) for every image of a batch: y (n, C, Hy, Wy) fp32 -> image i's
+ * top-left (H, W) <= (Hy, Wy) corner, written to images[i].data as fp32 planes or as the uint8 pixels of grl_f32_to_u8.
+ * 1 <= C <= 8; kind GRL_IMAGE_F32 or GRL_IMAGE_U8. */
+int grl_list_crop(const float* y, int n, int C, int Hy, int Wy, const GrlImageRef* images, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
