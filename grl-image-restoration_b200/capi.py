@@ -57,6 +57,14 @@ class GrlImageRef(ctypes.Structure):
 IMAGE_F32, IMAGE_U8, IMAGE_RGGB = 0, 1, 2  # GrlImageKind
 
 
+class GrlTileRef(ctypes.Structure):
+    _fields_ = [("src", GrlImageRef), ("y0", ctypes.c_int32), ("x0", ctypes.c_int32), ("t", ctypes.c_int32)]
+
+
+class GrlTileImage(ctypes.Structure):
+    _fields_ = [("E", c_vp), ("out_u8", c_vp)] + [(n, ctypes.c_int32) for n in ("H", "W", "t", "overlap", "k0", "k1", "slot")]
+
+
 _SIGNATURES = {
     "grl_last_error": (ctypes.c_char_p, []),
     "grl_abi_version": (c_int, []),
@@ -123,6 +131,10 @@ _SIGNATURES = {
     "grl_f32_to_u8_host": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_vp]),
     "grl_list_gather": (c_int, [ctypes.POINTER(GrlImageRef), c_int, c_int, c_int, c_int, c_vp, c_vp]),
     "grl_list_crop": (c_int, [c_vp, c_int, c_int, c_int, c_int, ctypes.POINTER(GrlImageRef), c_vp]),
+    "grl_tile_gather": (c_int, [ctypes.POINTER(GrlTileRef), c_int, c_int, c_int, c_int, c_vp, c_vp]),
+    "grl_tile_accumulate": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(GrlTileImage), c_int, c_vp]),
+    "grl_tile_finish": (c_int, [ctypes.POINTER(GrlTileImage), c_int, c_int, c_int, c_vp]),
+    "grl_tile_cover_host": (c_int, [c_int, c_int, c_int, c_int, c_vp]),
 }
 
 _lib = None

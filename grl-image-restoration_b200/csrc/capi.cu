@@ -4,6 +4,7 @@
 #include <math.h>
 
 #include "grl_common.cuh"
+#include "grl_tiles.h"
 
 namespace grl {
 char* error_buffer() {
@@ -106,6 +107,20 @@ int grl_coords_table_host(int wh, int ww, int df, float* out) {
         out[((size_t)i * nw + j) * 2 + a] = s * log2f(fabsf(v) + 1.0f) / 3.0f;
       }
     }
+  return GRL_OK;
+}
+
+// ---------------------------------------------------------------- tiled inference (host)
+int grl_tile_cover_host(int size, int tile, int overlap, int scale, int32_t* out) {
+  GRL_REQUIRE(out, "tile_cover: null output");
+  GRL_REQUIRE(tile >= 1 && tile <= size && overlap >= 0 && overlap < tile && scale >= 1,
+              "tile_cover: needs 1 <= tile <= size, 0 <= overlap < tile, scale >= 1 (size %d, tile %d, overlap %d, scale %d)",
+              size, tile, overlap, scale);
+  const TileAxis a = tile_axis(size, tile, overlap);
+  for (int Y = 0; Y < size * scale; ++Y) {
+    out[2 * Y] = tile_first(a, Y / scale);
+    out[2 * Y + 1] = tile_last(a, Y / scale);
+  }
   return GRL_OK;
 }
 

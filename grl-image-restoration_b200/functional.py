@@ -302,6 +302,70 @@ def list_crop(y, sizes, u8=False):
     return outs
 
 
+def tile_gather(tiles, kind, C, Hp, Wp):
+    """check_image_size of tile windows into one padded batch (n, C, Hp, Wp) float32, as list_gather pads whole images.
+    tiles: (image, y0, x0, t) with image a contiguous tensor on the GPU of `kind` (see list_gather) and the t x t window
+    at (y0, x0) of the frame the network sees (capi.IMAGE_RGGB: of the demosaiced (2h, 2w) frame).  Hp = Wp = t cuts."""
+    refs = (capi.GrlTileRef * max(1, len(tiles)))()
+    for r, (img, y0, x0, t) in zip(refs, tiles):
+        capi.require_device(img)
+        if not img.is_contiguous() or img.dtype != (torch.uint8 if kind == capi.IMAGE_U8 else torch.float32):
+            raise RuntimeError(f"grl_b200: tile_gather needs contiguous sources of kind {kind}, got {img.dtype}")
+        h, w = img.shape[:2] if kind == capi.IMAGE_U8 else img.shape[1:]
+        r.src.data, r.src.H, r.src.W, r.src.kind = img.data_ptr(), h, w, kind
+        r.y0, r.x0, r.t = y0, x0, t
+    dev = torch.device("cuda", torch.cuda.current_device()) if not tiles else tiles[0][0].device
+    out = torch.empty(len(tiles), C, Hp, Wp, device=dev, dtype=torch.float32)
+    capi.check(capi.lib().grl_tile_gather(refs, len(tiles), C, Hp, Wp, capi.ptr(out), capi.stream()))
+    return out
+
+
+def _tile_images(blends, C, scale, outs_u8=None):
+    refs = (capi.GrlTileImage * max(1, len(blends)))()
+    for j, (r, (E, t, overlap, k0, k1, slot)) in enumerate(zip(refs, blends)):
+        capi.require_device(E)
+        if (E.dtype != torch.float32 or E.dim() != 3 or not E.is_contiguous() or E.shape[0] != C or E.shape[1] % scale
+                or E.shape[2] % scale):
+            raise RuntimeError(f"grl_b200: a tile accumulator must be contiguous float32 ({C}, H*{scale}, W*{scale}), got "
+                               f"{E.dtype} {tuple(E.shape)}")
+        r.E, r.H, r.W = E.data_ptr(), E.shape[1] // scale, E.shape[2] // scale
+        r.t, r.overlap, r.k0, r.k1, r.slot = t, overlap, k0, k1, slot
+        if outs_u8 is not None:
+            o = outs_u8[j]
+            capi.require_device(o)
+            if o.dtype != torch.uint8 or not o.is_contiguous() or tuple(o.shape) != (E.shape[1], E.shape[2], E.shape[0]):
+                raise RuntimeError(f"grl_b200: tile_finish needs contiguous uint8 (H*s, W*s, C) outputs, got {o.dtype} "
+                                   f"{tuple(o.shape)} for an accumulator {tuple(E.shape)}")
+            r.out_u8 = o.data_ptr()
+    return refs
+
+
+def tile_accumulate(y, blends, scale):
+    """Adds the tile outputs of a batch y (n, C, Hy, Wy) float32 (the forward of a tile_gather batch) to their images'
+    accumulators, as the reference's E[...].add_(o) in origin order.  blends: (E, t, overlap, k0, k1, slot) per image with
+    tiles in the batch: E (C, H*scale, W*scale) float32, the image's tiles k0..k1-1 (row-major over its origin grid) at
+    batch indices slot, slot + 1, ...; tile k's output is the top-left (t*scale)^2 of its entry."""
+    y = _f32c(y, "y")
+    n, C, Hy, Wy = y.shape
+    capi.check(capi.lib().grl_tile_accumulate(capi.ptr(y), n, C, Hy, Wy, int(scale), _tile_images(blends, C, scale),
+                                              len(blends), capi.stream()))
+
+
+def tile_finish(blends, scale, outs_u8=None):
+    """E / W of the reference for every image: blends (E, t, overlap) per image; E becomes E / (number of tiles covering
+    the pixel), IEEE division, in place, or with outs_u8 the (H*s, W*s, C) uint8 outputs receive round8 of it."""
+    C = blends[0][0].shape[0] if blends else 1
+    refs = _tile_images([(E, t, overlap, 0, 0, 0) for E, t, overlap in blends], C, scale, outs_u8)
+    capi.check(capi.lib().grl_tile_finish(refs, len(blends), C, int(scale), capi.stream()))
+
+
+def tile_cover_host(size, tile, overlap, scale=1):
+    """(size*scale, 2) int32: the first and last tile, in origin order, covering each output row (CPU, no device)."""
+    out = torch.empty(size * scale, 2, dtype=torch.int32)
+    capi.check(capi.lib().grl_tile_cover_host(int(size), int(tile), int(overlap), int(scale), ctypes.c_void_p(out.data_ptr())))
+    return out
+
+
 def stripe_attention(qkv, anchor, B, tok_grid, anc_grid, heads, scale1, bias1, scale2, bias2, use_mask, out=None):
     """qkv (B, L, 3c) view (stripe half), anchor (B, Ha, Wa, c) -> (B, L, c)."""
     qp, ldq = _token_rows(qkv, "qkv")

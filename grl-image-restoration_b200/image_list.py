@@ -49,8 +49,8 @@ def plan(sizes, pad_size, max_batch_tokens):
     return chunks
 
 
-def _check(model, images, u8, what):
-    """Refuses a bad list before anything launches."""
+def _check(model, images, u8, what, floats=FLOAT_DTYPES):
+    """Refuses a bad list before anything launches; float images must have one of the dtypes `floats`."""
     rggb = model.input_format == "rggb"
     cdim, C, least = (2, model.in_channels, 1) if u8 else (0, 4, 2) if rggb else (0, model.in_channels, 1)
     layout = f"(H, W, {C}) uint8" if u8 else f"({C}, {'h, w' if rggb else 'H, W'}) float"
@@ -58,9 +58,10 @@ def _check(model, images, u8, what):
         if not isinstance(x, torch.Tensor):
             raise ValueError(f"{what}: element {i} is a {type(x).__name__}, not a tensor")
         capi.require_device(x)
-        if x.dtype not in ((torch.uint8,) if u8 else FLOAT_DTYPES):
+        if x.dtype not in ((torch.uint8,) if u8 else floats):
+            names = [str(d).replace("torch.", "") for d in floats]
             raise ValueError(f"{what}: element {i} has dtype {x.dtype}; it takes {layout} images"
-                             + ("" if u8 else " (float32, float16 or bfloat16)"))
+                             + ("" if u8 else f" ({' or '.join([', '.join(names[:-1]), names[-1]] if names[:-1] else names)})"))
         hw = [d for j, d in enumerate(x.shape) if j != cdim]
         if x.dim() != 3 or x.shape[cdim] != C or min(hw) < least:
             raise ValueError(f"{what}: element {i} has shape {tuple(x.shape)}; it takes {layout} images"

@@ -6,9 +6,13 @@ on 8 GPUs).
 Semantics are the reference's exactly: tile = min(tile, h, w); origins range(0, h - tile, stride) + [h - tile] with
 stride = tile - overlap (same for w); every tile is restored independently (so per-tile operators such as the CAB
 global pool see the same data as in the reference), outputs are summed into E, a ones mask into W, result E / W.
+
+forward_tile_list / forward_tile_list_u8 do the same for a list of differently sized images, with the tiles of the
+whole list sharing forwards and the cut and blend on the device (csrc/image_list.cu, csrc/grl_tiles.h).
 """
 import torch
 
+from . import capi, image_list
 from . import functional as K
 
 
@@ -116,3 +120,100 @@ def forward_tile_u8(model, img, tile, tile_overlap, scale=None, max_batch=16, gr
                          "(input_format='rggb') is not supported")
     y = forward_tile_sharded(model, K.u8_to_f32(img), tile, tile_overlap, scale=scale, max_batch=max_batch, group=group)
     return K.f32_to_u8(y)
+
+
+def tile_plan(model, sizes, tile, tile_overlap):
+    """The tiles of a list of images of network sizes `sizes` (image_list.network_sizes) and the forwards that restore
+    them; needs no device.  Returns (tiles, chunks): tiles are (image, y0, x0, t), t = min(tile, H, W), in forward_tile's
+    order: image, then row origin, then column origin (tile_origins).  chunks are image_list.plan of the tiles' (t, t)
+    sizes, chunk.index indexing `tiles`: by model.pad_size, so that tiles of one padded size share a forward of at most
+    model.max_batch_tokens padded pixels; with self_ensemble by exact size (pad size 1), because forward_rgb pads each of
+    a tile's 8 views on its own.
+    The blend is exact only if each image's tiles reach it in origin order, and they do: all tiles of an image have one
+    size, so they fall in one group, and plan keeps input order within a group and cuts it into consecutive chunks."""
+    tiles = []
+    for i, (h, w) in enumerate(sizes):
+        t = min(tile, h, w)
+        tiles += [(i, y0, x0, t) for y0 in tile_origins(h, t, tile_overlap) for x0 in tile_origins(w, t, tile_overlap)]
+    pad = 1 if model.self_ensemble else model.pad_size
+    return tiles, image_list.plan([(t, t) for *_, t in tiles], pad, model.max_batch_tokens)
+
+
+def _check_tiles(sizes, tile, tile_overlap, what):
+    if tile < 1 or tile_overlap < 0:
+        raise ValueError(f"{what}: tile = {tile}, tile_overlap = {tile_overlap}: needs tile >= 1 and tile_overlap >= 0")
+    for i, (h, w) in enumerate(sizes):
+        t = min(tile, h, w)
+        if t <= tile_overlap:  # stride <= 0, or pixels no tile covers
+            raise ValueError(f"{what}: element {i} ({h} x {w}) is tiled with side min(tile, H, W) = {t}, which needs to be "
+                             f"larger than tile_overlap = {tile_overlap}")
+
+
+@torch.no_grad()
+def _forward_tile_list(model, images, tile, tile_overlap, u8):
+    what = "forward_tile_list_u8" if u8 else "forward_tile_list"
+    rggb = model.input_format == "rggb"
+    if u8 and rggb:
+        raise ValueError(f"{what} takes (H, W, C) 8-bit images; packed 8-bit Bayer input (input_format='rggb') is not "
+                         "supported")
+    images = list(images)
+    image_list._check(model, images, u8, what, floats=(torch.float32,))
+    sizes = image_list.network_sizes([tuple(x.shape) for x in images], model.input_format, u8)
+    _check_tiles(sizes, tile, tile_overlap, what)
+    if not images:
+        return []
+    kind = capi.IMAGE_U8 if u8 else capi.IMAGE_RGGB if rggb else capi.IMAGE_F32
+    src = [x.contiguous() for x in images]
+    s = model.upscale
+    tiles, chunks = tile_plan(model, sizes, tile, tile_overlap)
+    first, last = {}, {}
+    for j, (i, *_) in enumerate(tiles):
+        first.setdefault(i, j)
+        last[i] = j
+    E, outs = [None] * len(images), [None] * len(images)
+    for ch in chunks:
+        batch = K.tile_gather([(src[tiles[j][0]],) + tiles[j][1:] for j in ch.index], kind, model.in_channels, ch.hp,
+                              ch.wp)
+        y = model.forward_rgb(batch)  # what forward_tile's model(patches) runs
+        blends, done = [], []  # one run of consecutive tiles per image in this batch
+        for slot, j in enumerate(ch.index):
+            i, t = tiles[j][0], tiles[j][3]
+            if E[i] is None:
+                # zeros like forward_tile's E: the first tile is added to +0, not written (0 + -0 = +0)
+                E[i] = torch.zeros(y.shape[1], sizes[i][0] * s, sizes[i][1] * s, device=y.device, dtype=torch.float32)
+            if blends and blends[-1][0] is E[i]:
+                blends[-1][4] += 1
+            else:
+                blends.append([E[i], t, tile_overlap, j - first[i], j - first[i] + 1, slot])
+            if j == last[i]:
+                done.append(i)
+        K.tile_accumulate(y, [tuple(b) for b in blends], s)
+        if not done:
+            continue
+        fin = [(E[i], tiles[last[i]][3], tile_overlap) for i in done]
+        if u8:
+            o8 = [torch.empty(E[i].shape[1], E[i].shape[2], E[i].shape[0], device=y.device, dtype=torch.uint8) for i in done]
+            K.tile_finish(fin, s, o8)
+        else:
+            o8 = [E[i] for i in done]
+            K.tile_finish(fin, s)
+        for i, o in zip(done, o8):
+            outs[i], E[i] = o, None
+    return outs
+
+
+def forward_tile_list(model, images, tile, tile_overlap):
+    """forward_tile over a list of differently sized images, as a tiled test set comes: images[i] is (in_channels, H_i,
+    W_i) float32 on the GPU (a model with input_format "rggb": packed Bayer planes (4, h_i, w_i) float32).  Returns the
+    outputs in input order; element i equals forward_tile(model, images[i][None], tile, tile_overlap)[0] bit for bit for
+    every precision, use_cuda_graph, self_ensemble and input_format.  The tiles of the whole list share forwards
+    (tile_plan); one kernel cuts each batch of tiles out of their images, one adds the batch's outputs to the images'
+    accumulators in forward_tile's order, one divides an image by its tile counts after its last tile."""
+    return _forward_tile_list(model, images, tile, tile_overlap, u8=False)
+
+
+def forward_tile_list_u8(model, images, tile, tile_overlap):
+    """forward_tile_list of decoded 8-bit images (H_i, W_i, in_channels) uint8 on the GPU -> (H_i*s, W_i*s, out_channels)
+    uint8; element i equals forward_tile_u8(model, images[i][None], tile, tile_overlap)[0] (no process group) bit for
+    bit.  Packed 8-bit Bayer input (input_format="rggb") is not supported."""
+    return _forward_tile_list(model, images, tile, tile_overlap, u8=True)

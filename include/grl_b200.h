@@ -418,6 +418,47 @@ int grl_list_gather(const GrlImageRef* images, int n, int C, int Hp, int Wp, flo
  * 1 <= C <= 8; kind GRL_IMAGE_F32 or GRL_IMAGE_U8. */
 int grl_list_crop(const float* y, int n, int C, int Hy, int Wy, const GrlImageRef* images, void* stream);
 
+/* ---- tiled inference over a list of images (tiling.forward_tile_list, csrc/image_list.cu, csrc/grl_tiles.h) ------------
+ * BaseEngine.forward_tile (engines/base.py:90-116) restores one image as t x t tiles, t = min(tile, H, W), at the origins
+ * range(0, H - t, stride) + [H - t], stride = t - overlap (the same on W), sums each tile's output into E, counts into W
+ * and returns E / W.  Every tile is restored on its own and a forward's result depends only on the padded size, so the
+ * tiles of a whole list of images can share forwards: these three calls cut the tiles into a padded batch and blend the
+ * batch's outputs into each image's accumulator, bit for bit as the per-image loop does.  Tile k of an image is tile
+ * (row k / n_cols, column k % n_cols) of its origin grid, row-major: forward_tile's order. */
+/* One tile of a list: the t x t window at (y0, x0) of image src, in the frame the network sees (RGGB: the demosaiced
+ * (2H, 2W) frame). */
+typedef struct {
+  GrlImageRef src;
+  int32_t y0, x0, t;
+} GrlTileRef;
+/* check_image_size (grl.py:479-489) of every tile's window into one padded batch: out (n, C, Hp, Wp) fp32, tile i's
+ * window reflect-padded on the bottom / right, or zero-padded on both axes when Hp - t >= t or Wp - t >= t, as for the
+ * whole images of grl_list_gather.  With Hp = Wp = t it is a plain cut.  Every source has the same kind; RGGB windows
+ * are read from the demosaic of the whole frame (grl_demosaic_f32), as forward_tile demosaics before cutting.
+ * 1 <= C <= 8, t <= min(Hp, Wp). */
+int grl_tile_gather(const GrlTileRef* tiles, int n, int C, int Hp, int Wp, float* out, void* stream);
+/* The blend state of one image of the list. */
+typedef struct {
+  float* E;         /* (C, H*scale, W*scale) fp32 accumulator, zeroed before the image's first tile */
+  uint8_t* out_u8;  /* grl_tile_finish: NULL -> E / count in place in E; else (H*scale, W*scale, C) uint8 round8(E / count) */
+  int32_t H, W;     /* the image's size in the network's frame */
+  int32_t t, overlap;
+  int32_t k0, k1;   /* grl_tile_accumulate: the image's tiles [k0, k1) are in this batch ... */
+  int32_t slot;     /* ... tile k0 at batch index slot, the rest after it in order */
+} GrlTileImage;
+/* Adds the outputs of the tiles a batch holds to their images' accumulators: y (n, C, Hy, Wy) fp32 is the forward's
+ * output of a grl_tile_gather batch; tile k's output is the top-left (t*scale)^2 of y[slot + k - k0].  At every output
+ * pixel the covering tiles are added in origin order, each as E = E + o, which is what the reference's slice add_ gives;
+ * a later batch continues where an earlier one stopped, so the image's tiles must reach it in order. */
+int grl_tile_accumulate(const float* y, int n, int C, int Hy, int Wy, int scale, const GrlTileImage* images, int m,
+                        void* stream);
+/* E / W of the reference once an image's last tile is accumulated: E / count with IEEE division, count = the number of
+ * tiles covering the pixel, written to E (out_u8 NULL on every image) or as uint8 pixels (on every image). */
+int grl_tile_finish(const GrlTileImage* images, int m, int C, int scale, void* stream);
+/* Host expansion of the coverage (tests): out (size*scale, 2) int32 = the first and last tile, in origin order, that cover
+ * output row Y of an axis of `size` samples tiled with side `tile` and `overlap` (the covering tiles are that run). */
+int grl_tile_cover_host(int size, int tile, int overlap, int scale, int32_t* out);
+
 #ifdef __cplusplus
 }
 #endif
