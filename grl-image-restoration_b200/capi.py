@@ -135,6 +135,11 @@ _SIGNATURES = {
     "grl_tile_accumulate": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(GrlTileImage), c_int, c_vp]),
     "grl_tile_finish": (c_int, [ctypes.POINTER(GrlTileImage), c_int, c_int, c_int, c_vp]),
     "grl_tile_cover_host": (c_int, [c_int, c_int, c_int, c_int, c_vp]),
+    "grl_jpeg_workspace": (c_sz, [ctypes.POINTER(GrlImageRef), c_int, c_int]),
+    "grl_jpeg_roundtrip_u8": (c_int, [ctypes.POINTER(GrlImageRef), ctypes.POINTER(GrlImageRef), c_int, c_int, c_int, c_vp,
+                                      c_sz, c_vp]),
+    "grl_jpeg_roundtrip_host": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_vp]),
+    "grl_jpeg_quant_tables_host": (c_int, [c_int, c_vp]),
 }
 
 _lib = None

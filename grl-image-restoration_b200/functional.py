@@ -366,6 +366,91 @@ def tile_cover_host(size, tile, overlap, scale=1):
     return out
 
 
+def _jpeg_quality(quality):
+    if isinstance(quality, bool) or not isinstance(quality, int) or not 1 <= quality <= 100:
+        raise ValueError(f"grl_b200: JPEG quality must be an int in 1..100, got {quality!r}")
+    return quality
+
+
+def _jpeg_images(images, what):
+    """The list checks of jpeg_roundtrip_list: (H, W, C) uint8 on the current CUDA device, one C in {1, 3}."""
+    C = None
+    for i, t in enumerate(images):
+        if not isinstance(t, torch.Tensor):
+            raise ValueError(f"grl_b200: {what}: element {i} is a {type(t).__name__}, not a tensor")
+        capi.require_device(t)
+        if t.dtype != torch.uint8 or t.dim() != 3 or t.shape[2] not in (1, 3) or t.shape[0] < 1 or t.shape[1] < 1:
+            raise ValueError(f"grl_b200: {what} needs (H, W, C) uint8 images with C in {{1, 3}}, got element {i}: {t.dtype} "
+                             f"{tuple(t.shape)}")
+        if C is not None and t.shape[2] != C:
+            raise ValueError(f"grl_b200: {what}: element {i} has {t.shape[2]} channels, element 0 {C}: one C per call")
+        C = t.shape[2]
+    return C
+
+
+def _jpeg_launch(srcs, dsts, C, quality):
+    src, dst = _image_refs(srcs, capi.IMAGE_U8), _image_refs(dsts, capi.IMAGE_U8)
+    nbytes = capi.lib().grl_jpeg_workspace(src, len(srcs), C)
+    ws = torch.empty(max(nbytes, 1), device=srcs[0].device, dtype=torch.uint8)
+    capi.check(capi.lib().grl_jpeg_roundtrip_u8(src, dst, len(srcs), C, quality, capi.ptr(ws), nbytes, capi.stream()))
+
+
+def jpeg_roundtrip(img, quality):
+    """The JPEG test command's degraded input (JPEGDataset.jpeg_compress, data/datasets/restoration_jpeg.py:62-79):
+    (B, H, W, C) uint8 images on the GPU, C = 1 (gray) or 3 (RGB) -> new (B, H, W, C) uint8 tensor, each image equal byte
+    for byte to cv2.imdecode(cv2.imencode(".jpg", img, [IMWRITE_JPEG_QUALITY, quality])) (colour via BGR, as the dataset
+    does): libjpeg's baseline 4:2:0 encode and default decode.  quality: int in 1..100.  Two kernels (one for gray)."""
+    quality = _jpeg_quality(quality)
+    if not isinstance(img, torch.Tensor):
+        raise ValueError(f"grl_b200: jpeg_roundtrip needs a tensor, got {type(img).__name__}")
+    capi.require_device(img)
+    if img.dtype != torch.uint8 or img.dim() != 4 or img.shape[3] not in (1, 3) or min(img.shape[1:3]) < 1:
+        raise ValueError(f"grl_b200: jpeg_roundtrip needs (B, H, W, C) uint8 images with C in {{1, 3}}, got {img.dtype} "
+                         f"{tuple(img.shape)}")
+    img = img.contiguous()
+    out = torch.empty_like(img)
+    if img.shape[0]:
+        _jpeg_launch(list(img.unbind(0)), list(out.unbind(0)), img.shape[3], quality)
+    return out
+
+
+def jpeg_roundtrip_list(images, quality):
+    """jpeg_roundtrip of a list of differently sized (H_i, W_i, C) uint8 images on the GPU, all with the same C in {1, 3}
+    -> list of new tensors in input order.  The whole list runs in two kernels per 80 images (one for gray)."""
+    quality = _jpeg_quality(quality)
+    images = list(images)
+    C = _jpeg_images(images, "jpeg_roundtrip_list")
+    if not images:
+        return []
+    srcs = [t.contiguous() for t in images]
+    outs = [torch.empty_like(t) for t in srcs]
+    _jpeg_launch(srcs, outs, C, quality)
+    return outs
+
+
+def jpeg_roundtrip_host(img, quality):
+    """jpeg_roundtrip of one (H, W, C) uint8 CPU image, evaluated by the library's host copy of the same closed forms
+    (tests)."""
+    quality = _jpeg_quality(quality)
+    if img.dtype != torch.uint8 or img.dim() != 3 or img.shape[2] not in (1, 3):
+        raise ValueError(f"grl_b200: jpeg_roundtrip_host needs an (H, W, C) uint8 image with C in {{1, 3}}, got {img.dtype} "
+                         f"{tuple(img.shape)}")
+    img = img.contiguous()
+    out = torch.empty_like(img)
+    H, W, C = img.shape
+    capi.check(capi.lib().grl_jpeg_roundtrip_host(ctypes.c_void_p(img.data_ptr()), H, W, C, quality,
+                                                  ctypes.c_void_p(out.data_ptr())))
+    return out
+
+
+def jpeg_quant_tables(quality):
+    """(2, 64) int32 CPU tensor: the luma and chroma quantisation tables the round trip uses at this quality
+    (jpeg_set_quality with baseline limits), natural row-major order."""
+    out = torch.empty(2, 64, dtype=torch.int32)
+    capi.check(capi.lib().grl_jpeg_quant_tables_host(_jpeg_quality(quality), ctypes.c_void_p(out.data_ptr())))
+    return out
+
+
 def stripe_attention(qkv, anchor, B, tok_grid, anc_grid, heads, scale1, bias1, scale2, bias2, use_mask, out=None):
     """qkv (B, L, 3c) view (stripe half), anchor (B, Ha, Wa, c) -> (B, L, c)."""
     qp, ldq = _token_rows(qkv, "qkv")

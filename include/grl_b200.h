@@ -459,6 +459,26 @@ int grl_tile_finish(const GrlTileImage* images, int m, int C, int scale, void* s
  * output row Y of an axis of `size` samples tiled with side `tile` and `overlap` (the covering tiles are that run). */
 int grl_tile_cover_host(int size, int tile, int overlap, int scale, int32_t* out);
 
+/* ---- JPEG round trip (the JPEG test command's degraded input, csrc/jpeg.cu, csrc/grl_jpeg.h) ---------------------------
+ * JPEGDataset.jpeg_compress (data/datasets/restoration_jpeg.py:62-79): cv2.imencode(".jpg", img, [IMWRITE_JPEG_QUALITY,
+ * quality]) then cv2.imdecode, i.e. libjpeg's default baseline encode (colour: YCbCr 4:2:0; islow DCT) and default decode
+ * (islow IDCT, fancy upsampling).  Entropy coding is lossless, so the decoded pixels are integer arithmetic on 8 x 8 blocks,
+ * reproduced here byte for byte.  Images are (H, W, C) uint8, C = 1 (gray, one component) or 3 (RGB in, RGB out, as the
+ * dataset hands them to to_tensor); 1 <= quality <= 100. */
+/* Bytes of device workspace grl_jpeg_roundtrip_u8 needs for this list: H * W + 2 * ceil(H/2) * ceil(W/2) per colour image,
+ * 0 for gray. */
+size_t grl_jpeg_workspace(const GrlImageRef* images, int n, int C);
+/* The round trip of every image of a list: src[i] -> dst[i], both GRL_IMAGE_U8 refs of the same size (a batch is a list
+ * of refs into it).  Two kernels per kJpegPerLaunch (80) images, one for gray. */
+int grl_jpeg_roundtrip_u8(const GrlImageRef* src, const GrlImageRef* dst, int n, int C, int quality, void* workspace,
+                          size_t workspace_bytes, void* stream);
+/* The same for one image on the CPU from the same closed forms (tests); HOST pointers.  Allocates host scratch of
+ * 1.5 planes for colour. */
+int grl_jpeg_roundtrip_host(const uint8_t* src, int H, int W, int C, int quality, uint8_t* dst);
+/* tables (2, 64) int32: the luma and chroma quantisation tables of jpeg_set_quality(quality, force_baseline = TRUE), natural
+ * (row-major) order; HOST pointer. */
+int grl_jpeg_quant_tables_host(int quality, int32_t* tables);
+
 #ifdef __cplusplus
 }
 #endif
