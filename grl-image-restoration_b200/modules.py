@@ -694,10 +694,15 @@ class GRL(nn.Module):
 
     # ---- tables / indices / masks ------------------------------------------------------------
     def _tables(self, x_size):
+        """The coordinate tables of the stripes the blocks run at x_size.  A vertical-stripe block splits the image with
+        stripe_size[::-1] and stripe_groups[::-1] (efficient.py:466-468), which differs from the horizontal stripe
+        transposed when stripe_groups split a non-square image; the reference's table_sv is the transposed one (see
+        set_table_index_mask), so its own forward cannot run there."""
         ss, _ = _get_stripe_info(self.stripe_size, self.stripe_groups, True, x_size)
+        sv, _ = _get_stripe_info(list(self.stripe_size)[::-1], list(self.stripe_groups)[::-1], True, x_size)
         df = self.anchor_window_down_factor
         return {"table_w": G.coords_table(self.window_size), "table_sh": G.coords_table(ss, df),
-                "table_sv": G.coords_table(ss[::-1], df)}
+                "table_sv": G.coords_table(sv, df)}
 
     def set_table_index_mask(self, x_size, materialize=False):
         """grl.py:386-429.  With materialize=True returns the reference's 13 CPU tensors (bit-exact); the default
@@ -711,6 +716,7 @@ class GRL(nn.Module):
             return out
         ss, sss = _get_stripe_info(self.stripe_size, self.stripe_groups, True, x_size)
         df = self.anchor_window_down_factor
+        out["table_sv"] = G.coords_table(ss[::-1], df)
         out["index_w"] = G.position_index(self.window_size)
         out["mask_w"] = G.shift_mask(x_size, self.window_size, self.shift_size)
         for d, s, sh in (("sh", ss, sss), ("sv", ss[::-1], sss[::-1])):
@@ -777,8 +783,24 @@ class GRL(nn.Module):
 
     # ---- CUDA graphs ----------------------------------------------------------------------------
     def reset_cuda_graphs(self):
-        """Drops every captured graph (they bake in the addresses of the packed weights and of their static buffers)."""
+        """Drops every captured graph (they bake in the addresses of the packed weights and of their static buffers).
+        A graph is also dropped and recaptured by itself when a packed-weight plan it reads is no longer current: after
+        set_precision, or after an in-place edit of a parameter (which bumps its version).  An edit through
+        `param.data` bypasses the version counter, so nothing can detect it, neither here nor in the eager path's
+        packed weights: edit parameters in place under torch.no_grad(), or load_state_dict."""
         self._graphs = {}
+
+    def _graph_plans(self):
+        """The packed-weight plans a tensor-core forward reads: every block's tc.BlockPlan and every tc.ConvPlan."""
+        return ([b._tc_plan for layer in self.layers for b in layer.blocks] +
+                [p for m in self.modules() for p in m.__dict__.get("_tc_convs", {}).values()])
+
+    def _graph_current(self, ent):
+        """Whether a captured graph reads the current weights: no parameter changed version since the capture, and
+        every plan is still the one captured (set_precision / an edit rebuild them and free the captured ones)."""
+        plans, vkey = ent[4], ent[5]
+        now = self._graph_plans()
+        return tc._version_key(self) == vkey and len(now) == len(plans) and all(a is b for a, b in zip(now, plans))
 
     def _apply(self, fn, *args, **kwargs):  # .to() / .cuda() / .half() move parameters: captured graphs are stale
         self._graphs = {}
@@ -795,6 +817,9 @@ class GRL(nn.Module):
         tensor (the caller may mutate it in place, engines/base.py:113)."""
         key = (tuple(x.shape), x.device.index, self.precision, "rggb" if rggb else "rgb")
         ent = self._graphs.get(key)
+        if ent is not None and not self._graph_current(ent):
+            del self._graphs[key]
+            ent = None
         if ent is None:
             static_in = x.clone()
             side = torch.cuda.Stream()
@@ -809,9 +834,10 @@ class GRL(nn.Module):
             # the graph reads every block's cached attention constants (tc.BlockPlan) at their addresses at capture; a
             # forward at another resolution replaces that cache, so the graph holds its own references to them
             consts = [b._tc_plan._consts for layer in self.layers for b in layer.blocks]
-            ent = (graph, static_in, static_out, consts)
+            # ... and the packed weights of the plans it was captured with: it replays only while they are current
+            ent = (graph, static_in, static_out, consts, self._graph_plans(), tc._version_key(self))
             self._graphs[key] = ent
-        graph, static_in, static_out, _ = ent
+        graph, static_in, static_out = ent[:3]
         static_in.copy_(x)
         graph.replay()
         return static_out.clone()

@@ -345,6 +345,19 @@ def bias_table_log2(transform, table, out):
                                              heads, LOG2E, out.shape[2], capi.ptr(out), capi.stream()))
 
 
+def slot_scale(ls_w, ls_s1, ls_s2, hw, hs, out):
+    """The QKV epilogue's per-slot scales (nslots,) fp32 into `out` from the logit scales of window attention and of
+    stripe passes 1 / 2, in slot order [window q|k|v][stripe q|k|v] x head (grl_tc_slot_scale)."""
+    capi.check(capi.lib().grl_tc_slot_scale(capi.ptr(ls_w), capi.ptr(ls_s1), capi.ptr(ls_s2), hw, hs, capi.ptr(out),
+                                            capi.stream()))
+
+
+def avgpool16(x16, out, df):
+    """Anchor pooling: the df x df mean of 16-bit (B, H, W, cpad) into 16-bit (B, H / df, W / df, cpad) `out`."""
+    B, H, W, cpad = x16.shape
+    capi.check(capi.lib().grl_tc_avgpool16(capi.ptr(x16), capi.ptr(out), B, H, W, cpad, df, fmt_of(x16), capi.stream()))
+
+
 def channel_gate(y16, ld, B, L, C, ca, gate):
     """CAB gate (B, C) fp32 into `gate` from the 16-bit features y16 (B*L, ld); ca: the packed ChannelAttention weights."""
     lib = capi.lib()
@@ -455,12 +468,11 @@ class BlockPlan:
         # the coordinate tables only, so they are cached until a parameter or the resolution changes
         ckey = (self.key, t["table_w"].data_ptr(), t["table_s"].data_ptr(), t["table_s"].shape)
         if self._const_key == ckey:
-            slot_scale, bias_w, bias_1, bias_2 = self._consts
+            scales, bias_w, bias_1, bias_2 = self._consts
         else:
-            slot_scale = torch.empty(self.nslots, device=dev, dtype=torch.float32)
-            launch.run(lambda: capi.check(capi.lib().grl_tc_slot_scale(
-                capi.ptr(wa.attn_transform.logit_scale), capi.ptr(sa.attn_transform1.logit_scale),
-                capi.ptr(sa.attn_transform2.logit_scale), hw, hs, capi.ptr(slot_scale), capi.stream())))
+            scales = torch.empty(self.nslots, device=dev, dtype=torch.float32)
+            launch.run(slot_scale, wa.attn_transform.logit_scale, sa.attn_transform1.logit_scale,
+                       sa.attn_transform2.logit_scale, hw, hs, scales)
             tables = ((wa.attn_transform, t["table_w"]), (sa.attn_transform1, t["table_s"]),
                       (sa.attn_transform2, t["table_s"]))
             bias_w, bias_1, bias_2 = [torch.zeros(tr.cpb_mlp[2].weight.shape[0], 4, bias_rows_pad(tb.numel() // 2),
@@ -468,15 +480,14 @@ class BlockPlan:
             for (tr, tb), out in zip(tables, (bias_w, bias_1, bias_2)):
                 launch.run(bias_table_log2, tr, tb, out)
             if launch.caches:  # never keep a listing run's meta constants: a later forward would launch with them
-                self._const_key, self._consts = ckey, (slot_scale, bias_w, bias_1, bias_2)
+                self._const_key, self._consts = ckey, (scales, bias_w, bias_1, bias_2)
         # projections
         qkv = _h16(B * L, self.n_qkv, device=dev, fmt=fmt)
         launch.listed(f"{name}.qkv", gemm, x16, self.w_qkv, self.b_qkv, M=B * L, kpad=cpad, npad=self.n_qkv,
-                      epi=EPI_QKV, n_store=self.n_qkv, out_bf16=qkv, slot_scale=slot_scale)
+                      epi=EPI_QKV, n_store=self.n_qkv, out_bf16=qkv, slot_scale=scales)
         df = self.df
         pooled = _h16(B, H // df, W // df, cpad, device=dev, fmt=fmt)
-        launch.run(lambda: capi.check(capi.lib().grl_tc_avgpool16(capi.ptr(x16), capi.ptr(pooled), B, H, W, cpad, df, fmt,
-                                                                  capi.stream())))
+        launch.run(avgpool16, x16.view(B, H, W, cpad), pooled, df)
         La = (H // df) * (W // df)
         n_anc = self.w_anc.shape[0]
         anchor = _h16(B * La, n_anc, device=dev, fmt=fmt)

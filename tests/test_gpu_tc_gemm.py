@@ -311,9 +311,9 @@ def reference(run, bn, mutation=None):
     return O.gemm_launch_reference(o.pop("x"), o.pop("w"), o.pop("bias"), bn=bn, mutation=mutation, **o)
 
 
-def evaluate(tc, run, got, ref, fmt, row0=0):
+def evaluate(tc, run, got, ref, fmt, row0=0, high_mean_rows=HIGH_MEAN_ROWS):
     """Gate results {what: (statistic, passes)} of the kernel outputs `got` against reference `ref`, whose rows are
-    the problem's rows from row0 on."""
+    the problem's rows from row0 on.  LayerNorm rows listed in high_mean_rows are gated by GATE_LN_SHIFT."""
     a, dt = run.kw, tc.DTYPE[fmt]
     epi = a["epi"]
     gelu = a["act"] == 1
@@ -327,7 +327,7 @@ def evaluate(tc, run, got, ref, fmt, row0=0):
         extra = O.GELU_AS_ABS_ERR if gelu else 0.0
         if epi == tc.EPI_LN:
             hm = torch.isin(torch.arange(row0, row0 + y.shape[0], device=y.device),
-                            torch.tensor(HIGH_MEAN_ROWS, device=y.device))
+                            torch.tensor(high_mean_rows, dtype=torch.long, device=y.device))
             s = stats32(g32[~hm], y[~hm, :n])
             out["fp32"] = (s, s <= GATE32)
             if bool(hm.any()):
