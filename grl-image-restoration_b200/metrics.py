@@ -200,14 +200,16 @@ def niqe_tables():
     return torch.tensor(rows, dtype=torch.float64)
 
 
-_niqe_cache = {}
+_niqe_cache = {}  # ("tables", device) -> streams.Produced of niqe_tables() on that device
 
 
 def _niqe_device_tables(device):
+    from .streams import Produced, upload
+
     key = ("tables", device)
     if key not in _niqe_cache:
-        _niqe_cache[key] = niqe_tables().to(device)
-    return _niqe_cache[key]
+        _niqe_cache[key] = Produced(upload(niqe_tables(), device))
+    return _niqe_cache[key].use()
 
 
 def niqe_params(params):

@@ -26,6 +26,7 @@ from . import geometry as G
 from . import image_list
 from . import tc
 from .geometry import to_2tuple, _get_stripe_info
+from .streams import Produced, upload
 
 _LN_MAX = math.log(1.0 / 0.01)
 
@@ -48,15 +49,16 @@ def linear(launch, name, x, lin, act=K.ACT_NONE):
 
 def conv3x3(launch, name, owner, key, x, act=K.ACT_NONE, slope=0.0, res=None):
     """nn.Conv2d(3x3, stride 1, pad 1) `owner.<key>` on channels-last x (B, H, W, Cin), launched as `name`.  Its
-    (Cout, 9*Cin) im2col-ordered weight is cached on the owner under `key` and re-packed when the weight changes."""
+    (Cout, 9*Cin) im2col-ordered weight is cached on the owner under `key` (a streams.Produced) and re-packed when the
+    weight changes."""
     conv = owner.get_submodule(key)
     w = conv.weight
     version = (w.data_ptr(), w._version, w.device)
     cache = owner.__dict__.setdefault("_f32_convs", {})
     if cache.get(key, (None,))[0] != version:
-        cache[key] = (version, K.pack_conv_weight(w))
+        cache[key] = (version, Produced(K.pack_conv_weight(w)))
     y = torch.empty(*x.shape[:-1], w.shape[0], device=x.device, dtype=torch.float32)
-    launch.listed(name, K.conv3x3, x, cache[key][1], conv.bias, act, slope, res, out=y)
+    launch.listed(name, K.conv3x3, x, cache[key][1].use(), conv.bias, act, slope, res, out=y)
     return y
 
 
@@ -737,8 +739,8 @@ class GRL(nn.Module):
             if key not in cache:
                 if len(cache) >= 16:
                     cache.clear()
-                cache[key] = {k: v.to(device) for k, v in self._tables(input_resolution).items()}
-            t = dict(cache[key])
+                cache[key] = Produced({k: upload(v, device) for k, v in self._tables(input_resolution).items()})
+            t = dict(cache[key].use())
         for n in ("index_w", "index_sh_a2w", "index_sh_w2a", "index_sv_a2w", "index_sv_w2a", "mask_w", "mask_sh_a2w",
                   "mask_sh_w2a", "mask_sv_a2w", "mask_sv_w2a"):
             t[n] = _closed_form_marker()
@@ -798,7 +800,7 @@ class GRL(nn.Module):
     def _graph_current(self, ent):
         """Whether a captured graph reads the current weights: no parameter changed version since the capture, and
         every plan is still the one captured (set_precision / an edit rebuild them and free the captured ones)."""
-        plans, vkey = ent[4], ent[5]
+        plans, vkey = ent[3], ent[4]
         now = self._graph_plans()
         return tc._version_key(self) == vkey and len(now) == len(plans) and all(a is b for a, b in zip(now, plans))
 
@@ -814,7 +816,9 @@ class GRL(nn.Module):
     def _forward_graphed(self, x, rggb=False):
         """Replays a captured graph of tc.forward for this input shape and format (captures it on first use, after two
         eager warm-up forwards that build the packed weights / bias tables / kernel attributes).  The result is a fresh
-        tensor (the caller may mutate it in place, engines/base.py:113)."""
+        tensor (the caller may mutate it in place, engines/base.py:113).  Replays of one graph share its static buffers,
+        so they are serialised across streams: the entry's `done` (a streams.Produced of every tensor the graph reads or
+        writes) is recorded after the output's clone, and the next replay's stream waits on it."""
         key = (tuple(x.shape), x.device.index, self.precision, "rggb" if rggb else "rgb")
         ent = self._graphs.get(key)
         if ent is not None and not self._graph_current(ent):
@@ -835,12 +839,17 @@ class GRL(nn.Module):
             # forward at another resolution replaces that cache, so the graph holds its own references to them
             consts = [b._tc_plan._consts for layer in self.layers for b in layer.blocks]
             # ... and the packed weights of the plans it was captured with: it replays only while they are current
-            ent = (graph, static_in, static_out, consts, self._graph_plans(), tc._version_key(self))
+            plans = self._graph_plans()
+            held = (static_in, static_out, [c.value for c in consts], [p.ready.value for p in plans])
+            ent = [graph, Produced(held), consts, plans, tc._version_key(self)]
             self._graphs[key] = ent
-        graph, static_in, static_out = ent[:3]
+        graph, done = ent[:2]
+        static_in, static_out = done.use()[:2]
         static_in.copy_(x)
         graph.replay()
-        return static_out.clone()
+        y = static_out.clone()
+        ent[1] = Produced(done.value)
+        return y
 
     @torch.no_grad()
     def forward_features(self, x, launch=tc.DEVICE):
@@ -945,7 +954,7 @@ class GRL(nn.Module):
             x = rgb
         H, W = x.shape[2:]
         x = self.check_image_size(x)
-        mean = self.mean.to(x)
+        mean = upload(self.mean, x.device).to(x.dtype)
         x = ((x - mean) * self.img_range).float()
         xc = x.permute(0, 2, 3, 1).contiguous()
 

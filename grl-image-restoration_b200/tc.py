@@ -19,6 +19,7 @@ from torch import nn
 from . import capi
 from . import functional as K
 from . import geometry as G
+from .streams import Produced
 
 LOG2E = 1.4426950408889634
 EPI_BIAS_ACT, EPI_QKV, EPI_LN = 0, 1, 2
@@ -99,12 +100,19 @@ def unpack_rows(x16, C, off=0):
     return y
 
 
+def _slot_rows(first, n, d, device):
+    """Rows (first + i) * SLOT + e of slots first .. first + n - 1, e < d, slot-major: an index map built on the device
+    (a host list would be a blocking host-to-device copy)."""
+    return ((first + torch.arange(n, device=device))[:, None] * SLOT + torch.arange(d, device=device)).reshape(-1)
+
+
 def _pad_matrix(w, npad, kpad, row_map=None, col_map=None, fmt=0):
-    """Scatter fp32 (N, K) into 16-bit (npad, kpad): dest row row_map[i] <- src row i, dest col col_map[j] <- src col j."""
+    """Scatter fp32 (N, K) into 16-bit (npad, kpad): dest row row_map[i] <- src row i, dest col col_map[j] <- src col j
+    (maps: index tensors on w's device)."""
     N, Kd = w.shape
     out = torch.zeros(npad, kpad, device=w.device, dtype=torch.float32)
-    r = torch.arange(N, device=w.device) if row_map is None else torch.as_tensor(row_map, device=w.device)
-    c = torch.arange(Kd, device=w.device) if col_map is None else torch.as_tensor(col_map, device=w.device)
+    r = torch.arange(N, device=w.device) if row_map is None else row_map
+    c = torch.arange(Kd, device=w.device) if col_map is None else col_map
     out[r[:, None], c[None, :]] = w.detach().float()
     return out.to(DTYPE[fmt]).contiguous()
 
@@ -112,8 +120,7 @@ def _pad_matrix(w, npad, kpad, row_map=None, col_map=None, fmt=0):
 def _pad_vector(b, npad, row_map=None):
     out = torch.zeros(npad, device=b.device, dtype=torch.float32)
     if b is not None:
-        r = torch.arange(b.numel(), device=b.device) if row_map is None else torch.as_tensor(row_map, device=b.device)
-        out[r] = b.detach().float()
+        out[torch.arange(b.numel(), device=b.device) if row_map is None else row_map] = b.detach().float()
     return out
 
 
@@ -380,7 +387,8 @@ def _version_key(module):
 
 
 class BlockPlan:
-    """Packed weights + launch sequence of one EfficientMixAttnTransformerBlock."""
+    """Packed weights + launch sequence of one EfficientMixAttnTransformerBlock.  `ready` orders the packed weights
+    for the streams that read them, `_consts` the attention constants (streams.Produced)."""
 
     def __init__(self, blk, fmt):
         self.key = (_version_key(blk), fmt)
@@ -393,18 +401,13 @@ class BlockPlan:
         dw, ds = c // hw, c // hs
         self.C, self.cpad, self.hw, self.hs = C, round_up(C, 64), hw, hs
         self.nslots = 3 * hw + 3 * hs
-        # --- QKV: dest row = slot*32 + e
-        rmap = []
-        for half, (h, d) in enumerate(((hw, dw), (hs, ds))):
-            slot_base = 0 if half == 0 else 3 * hw
-            for t in range(3):
-                for head in range(h):
-                    for e in range(d):
-                        rmap.append((slot_base + t * h + head) * SLOT + e)
-        # source rows are already ordered (half, t, head, e) in the reference layout (efficient.py:150,:251,:362)
+        dev = at.qkv.body.weight.device
+        # --- QKV: dest row = slot*32 + e, slots [window q|k|v][stripe q|k|v] x head; source rows are already ordered
+        # (half, t, head, e) in the reference layout (efficient.py:150,:251,:362)
+        rmap = torch.cat([_slot_rows(0, 3 * hw, dw, dev), _slot_rows(3 * hw, 3 * hs, ds, dev)])
         self.n_qkv = self.nslots * SLOT
         self.w_qkv = _pad_matrix(at.qkv.body.weight, self.n_qkv, self.cpad, row_map=rmap, fmt=fmt)
-        self.b_qkv = _pad_vector(at.qkv.body.bias if at.qkv.body.bias is not None else torch.zeros(3 * C, device=at.qkv.body.weight.device), self.n_qkv, rmap)
+        self.b_qkv = _pad_vector(at.qkv.body.bias if at.qkv.body.bias is not None else torch.zeros(3 * C, device=dev), self.n_qkv, rmap)
         # ones-column (attn_tc.cu): with head_dim < 32 the last slot column of every VALUE slot is 1 (set through the
         # bias; its weight row is zero), so the P V MMA also produces the softmax denominator.  The stripe pass-1 output
         # X1 inherits it (O[:, 31] / O[:, 31] == 1) and is the value operand of pass 2.
@@ -412,10 +415,9 @@ class BlockPlan:
         for half, (hh, on) in enumerate(((hw, self.ones_w), (hs, self.ones_s))):
             if on:
                 base = (0 if half == 0 else 3 * hw) + 2 * hh
-                for head in range(hh):
-                    self.b_qkv[(base + head) * SLOT + SLOT - 1] = 1.0
+                self.b_qkv.view(-1, SLOT)[base:base + hh, SLOT - 1].fill_(1.0)  # fill_: a scalar store would sync
         # --- anchor projection: dest row = head*32 + e
-        amap = [head * SLOT + e for head in range(hs) for e in range(ds)]
+        amap = _slot_rows(0, hs, ds, dev)
         red = at.anchor.body[0].reduction
         self.n_anc = hs * SLOT
         self.w_anc = _pad_matrix(red.weight, round_up(self.n_anc, 32), self.cpad, row_map=amap, fmt=fmt)
@@ -423,8 +425,7 @@ class BlockPlan:
         self.anc_scale = torch.ones(hs, device=red.weight.device, dtype=torch.float32)
         self.df = at.anchor.body[0].down_factor
         # --- output projection: K index = slot*32 + e over [window heads | stripe heads]
-        cmap = [head * SLOT + e for head in range(hw) for e in range(dw)] + \
-               [(hw + head) * SLOT + e for head in range(hs) for e in range(ds)]
+        cmap = torch.cat([_slot_rows(0, hw, dw, dev), _slot_rows(hw, hs, ds, dev)])
         self.k_proj = round_up((hw + hs) * SLOT, 64)
         self.n_ln = 64 if C <= 64 else 128 if C <= 128 else 192 if C <= 192 else 256
         self.w_proj = _pad_matrix(at.proj.weight, self.n_ln, self.k_proj, col_map=cmap, fmt=fmt)
@@ -447,6 +448,7 @@ class BlockPlan:
             a1, a3 = blk.conv.cab[3].attention[1], blk.conv.cab[3].attention[3]
             self.ca = (a1.weight.detach().reshape(a1.weight.shape[0], -1).contiguous(), a1.bias.detach(),
                        a3.weight.detach().reshape(a3.weight.shape[0], -1).contiguous(), a3.bias.detach())
+        self.ready = Produced([v for k, v in vars(self).items() if k != "_consts"])
 
     @torch.no_grad()
     def run(self, blk, x32, x16, x_size, all_table_index_mask, launch=DEVICE, name=""):
@@ -468,7 +470,7 @@ class BlockPlan:
         # the coordinate tables only, so they are cached until a parameter or the resolution changes
         ckey = (self.key, t["table_w"].data_ptr(), t["table_s"].data_ptr(), t["table_s"].shape)
         if self._const_key == ckey:
-            scales, bias_w, bias_1, bias_2 = self._consts
+            scales, bias_w, bias_1, bias_2 = self._consts.use()
         else:
             scales = torch.empty(self.nslots, device=dev, dtype=torch.float32)
             launch.run(slot_scale, wa.attn_transform.logit_scale, sa.attn_transform1.logit_scale,
@@ -480,7 +482,7 @@ class BlockPlan:
             for (tr, tb), out in zip(tables, (bias_w, bias_1, bias_2)):
                 launch.run(bias_table_log2, tr, tb, out)
             if launch.caches:  # never keep a listing run's meta constants: a later forward would launch with them
-                self._const_key, self._consts = ckey, (scales, bias_w, bias_1, bias_2)
+                self._const_key, self._consts = ckey, Produced((scales, bias_w, bias_1, bias_2))
         # projections
         qkv = _h16(B * L, self.n_qkv, device=dev, fmt=fmt)
         launch.listed(f"{name}.qkv", gemm, x16, self.w_qkv, self.b_qkv, M=B * L, kpad=cpad, npad=self.n_qkv,
@@ -540,6 +542,7 @@ def block_plan(blk, fmt):
     if plan is None or plan.key != (_version_key(blk), fmt):
         plan = BlockPlan(blk, fmt)
         blk._tc_plan = plan
+    plan.ready.use()
     return plan
 
 
@@ -552,6 +555,7 @@ class ConvPlan:
         self.cin_pad, self.ps_r = cin_pad, ps_r
         self.npad = round_up(self.cout, 64)
         self.w, self.b = pack_conv(conv, cin_pad, self.npad, fmt, ps_r)
+        self.ready = Produced((self.w, self.b))
 
     def run(self, launch, name, x16, *, want16=True, want_f32=False, rows=False, **kw):
         """One launch on x16 (B, H, W, cin_pad) channels-last -> (16-bit out, fp32 out), each None unless asked for:
@@ -578,6 +582,7 @@ def conv_plan(owner, name, conv, cin_pad, fmt, ps_r=0):
     if plan is None or plan.key != (_version_key(conv), fmt, ps_r) or plan.cin_pad != cin_pad:
         plan = ConvPlan(conv, cin_pad, fmt, ps_r)
         cache[name] = plan
+    plan.ready.use()
     return plan
 
 
