@@ -6,10 +6,13 @@ from .modules import (  # noqa: F401
     EfficientMixAttnTransformerBlock, MixedAttention, Mlp, QKVProjection, TransformerStage, Upsample, UpsampleOneStep,
     WindowAttention, build_last_conv,
 )
-from .functional import demosaic, jpeg_quant_tables, jpeg_roundtrip, jpeg_roundtrip_host, jpeg_roundtrip_list  # noqa: F401
+from .functional import (  # noqa: F401
+    awgn, awgn_list, awgn_noise_host, demosaic, dn_seed, jpeg_quant_tables, jpeg_roundtrip, jpeg_roundtrip_host,
+    jpeg_roundtrip_list,
+)
 
 __all__ = ["GRL", "TransformerStage", "EfficientMixAttnTransformerBlock", "MixedAttention", "WindowAttention",
            "AnchorStripeAttention", "AffineTransform", "CAB", "ChannelAttention", "Mlp", "QKVProjection",
            "AnchorProjection", "AnchorLinear", "CPB_MLP", "Upsample", "UpsampleOneStep", "build_last_conv",
            "configs", "geometry", "demosaic", "jpeg_roundtrip", "jpeg_roundtrip_list", "jpeg_roundtrip_host",
-           "jpeg_quant_tables"]
+           "jpeg_quant_tables", "dn_seed", "awgn", "awgn_list", "awgn_noise_host"]

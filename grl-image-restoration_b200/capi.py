@@ -140,6 +140,10 @@ _SIGNATURES = {
                                       c_sz, c_vp]),
     "grl_jpeg_roundtrip_host": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_vp]),
     "grl_jpeg_quant_tables_host": (c_int, [c_int, c_vp]),
+    "grl_awgn_u8": (c_int, [ctypes.POINTER(GrlImageRef), ctypes.POINTER(GrlImageRef), c_vp, c_int, c_int, ctypes.c_double,
+                            c_vp]),
+    "grl_awgn_noise_host": (c_int, [c_vp, c_i64, ctypes.c_double, c_vp]),
+    "grl_awgn_log_host": (c_int, [c_vp, c_i64, c_vp]),
 }
 
 _lib = None

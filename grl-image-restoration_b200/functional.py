@@ -373,7 +373,8 @@ def _jpeg_quality(quality):
 
 
 def _jpeg_images(images, what):
-    """The list checks of jpeg_roundtrip_list: (H, W, C) uint8 on the current CUDA device, one C in {1, 3}."""
+    """The list checks of jpeg_roundtrip_list and awgn_list: (H, W, C) uint8 on the current CUDA device, one C in
+    {1, 3}."""
     C = None
     for i, t in enumerate(images):
         if not isinstance(t, torch.Tensor):
@@ -448,6 +449,121 @@ def jpeg_quant_tables(quality):
     (jpeg_set_quality with baseline limits), natural row-major order."""
     out = torch.empty(2, 64, dtype=torch.int32)
     capi.check(capi.lib().grl_jpeg_quant_tables_host(_jpeg_quality(quality), ctypes.c_void_p(out.data_ptr())))
+    return out
+
+
+def dn_seed(path):
+    """The RandomState key of the denoising test command's noise for one image (DnDataset.__getitem__,
+    data/datasets/restoration_dn.py:136-140): (8,) uint32 numpy array = the words of sha256(path.split("_")[0]), as
+    np.frombuffer(digest, dtype="uint32") gives them.  `path` is the dataset-relative path the reference keys on, e.g.
+    "CBSD68/0001.png".  The reference cuts the path at its first "_", and so does this: every Urban100 image
+    ("Urban100/img_001.png", "Urban100/img_092.png", ...) gets the key of "Urban100/img", so all of them draw the same
+    noise stream."""
+    import hashlib
+
+    import numpy as np
+
+    if not isinstance(path, str):
+        raise ValueError(f"grl_b200: dn_seed needs a path string, got {type(path).__name__}")
+    return np.frombuffer(hashlib.sha256(path.split("_")[0].encode("utf-8")).digest(), dtype="uint32").copy()
+
+
+def _awgn_scale(noise_sigma):
+    """noise_sigma / 255 in Python double, as the reference divides the config's sigma."""
+    import math
+    import numbers
+
+    if isinstance(noise_sigma, bool) or not isinstance(noise_sigma, numbers.Real) or not math.isfinite(noise_sigma) \
+            or noise_sigma < 0:
+        raise ValueError(f"grl_b200: noise_sigma must be a finite real >= 0, got {noise_sigma!r}")
+    return noise_sigma / 255
+
+
+def _awgn_keys(seeds, n, what):
+    """(n, 8) uint32 host array of RandomState keys: a path string goes through dn_seed, anything else must be 8 integers
+    in [0, 2^32)."""
+    import numpy as np
+
+    seeds = list(seeds)
+    if len(seeds) != n:
+        raise ValueError(f"grl_b200: {what}: {len(seeds)} seeds for {n} images")
+    keys = np.empty((n, 8), dtype=np.uint32)
+    for i, s in enumerate(seeds):
+        if isinstance(s, str):
+            keys[i] = dn_seed(s)
+            continue
+        a = np.asarray(s.cpu() if isinstance(s, torch.Tensor) else s)
+        if a.shape != (8,) or a.dtype.kind not in "iu" or (a.astype(np.int64) < 0).any() or (a.astype(np.int64) >> 32).any():
+            raise ValueError(f"grl_b200: {what}: seed {i} must be a path string or 8 integers in [0, 2^32), got {s!r}")
+        keys[i] = a
+    return keys
+
+
+def _awgn_launch(srcs, dsts, keys, C, scale):
+    src, dst = _image_refs(srcs, capi.IMAGE_U8), _image_refs(dsts, capi.IMAGE_F32)
+    capi.check(capi.lib().grl_awgn_u8(src, dst, keys.ctypes.data_as(ctypes.c_void_p), len(srcs), C, scale,
+                                      capi.stream()))
+
+
+def awgn(img, noise_sigma, seeds):
+    """The denoising test command's noisy input (DnDataset.__getitem__, validation branch,
+    data/datasets/restoration_dn.py:134-143): (B, H, W, C) uint8 images on the GPU, C = 1 or 3 -> new (B, C, H, W) float32
+    tensor, image b equal bit for bit to to_tensor(img[b]) + torch.from_numpy(np.random.RandomState(key_b).normal(0,
+    noise_sigma / 255, (C, H, W))).float().  noise_sigma: the config's sigma (15 for the released checkpoints), a finite
+    real >= 0.  seeds: one per image, a dataset-relative path (through dn_seed) or 8 uint32 words.  The reference's crop
+    to multiples of 8 stays with the caller: g[:H // 8 * 8, :W // 8 * 8].  One kernel per 64 images."""
+    scale = _awgn_scale(noise_sigma)
+    if not isinstance(img, torch.Tensor):
+        raise ValueError(f"grl_b200: awgn needs a tensor, got {type(img).__name__}")
+    capi.require_device(img)
+    if img.dtype != torch.uint8 or img.dim() != 4 or img.shape[3] not in (1, 3) or min(img.shape[1:3]) < 1:
+        raise ValueError(f"grl_b200: awgn needs (B, H, W, C) uint8 images with C in {{1, 3}}, got {img.dtype} "
+                         f"{tuple(img.shape)}")
+    keys = _awgn_keys(seeds, img.shape[0], "awgn")
+    img = img.contiguous()
+    B, H, W, C = img.shape
+    out = torch.empty(B, C, H, W, device=img.device, dtype=torch.float32)
+    if B:
+        _awgn_launch(list(img.unbind(0)), list(out.unbind(0)), keys, C, scale)
+    return out
+
+
+def awgn_list(images, noise_sigma, seeds):
+    """awgn of a list of differently sized (H_i, W_i, C) uint8 images on the GPU, all with the same C in {1, 3}, one seed
+    per image -> list of new (C, H_i, W_i) float32 tensors in input order.  The whole list runs in one kernel per 64
+    images, one CTA per image."""
+    scale = _awgn_scale(noise_sigma)
+    images = list(images)
+    C = _jpeg_images(images, "awgn_list")
+    keys = _awgn_keys(seeds, len(images), "awgn_list")
+    if not images:
+        return []
+    srcs = [t.contiguous() for t in images]
+    outs = [torch.empty(C, t.shape[0], t.shape[1], device=t.device, dtype=torch.float32) for t in srcs]
+    _awgn_launch(srcs, outs, keys, C, scale)
+    return outs
+
+
+def awgn_noise_host(seed, count, noise_sigma):
+    """The noise alone, from the library's host copy of the same closed forms with libm's log, as numpy's (tests):
+    (count,) float64 CPU tensor = np.random.RandomState(key).normal(0, noise_sigma / 255, count)."""
+    scale = _awgn_scale(noise_sigma)
+    key = _awgn_keys([seed], 1, "awgn_noise_host")
+    if isinstance(count, bool) or not isinstance(count, int) or count < 0:
+        raise ValueError(f"grl_b200: awgn_noise_host: count must be an int >= 0, got {count!r}")
+    out = torch.empty(count, dtype=torch.float64)
+    capi.check(capi.lib().grl_awgn_noise_host(key.ctypes.data_as(ctypes.c_void_p), count, scale,
+                                              ctypes.c_void_p(out.data_ptr())))
+    return out
+
+
+def awgn_log_host(x):
+    """The device's double-double log of the polar method (awgn_log_cr, csrc/grl_awgn.h), evaluated on the CPU (tests):
+    x float64 CPU tensor of positive normal numbers -> log(x), correctly rounded but for inputs within about 2^-100 of a
+    rounding midpoint."""
+    x = x.to(torch.float64).contiguous()
+    out = torch.empty_like(x)
+    capi.check(capi.lib().grl_awgn_log_host(ctypes.c_void_p(x.data_ptr()), x.numel(), ctypes.c_void_p(out.data_ptr())))
     return out
 
 

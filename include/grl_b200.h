@@ -479,6 +479,22 @@ int grl_jpeg_roundtrip_host(const uint8_t* src, int H, int W, int C, int quality
  * (row-major) order; HOST pointer. */
 int grl_jpeg_quant_tables_host(int quality, int32_t* tables);
 
+/* ---- Seeded AWGN (the denoising test command's noisy input, csrc/awgn.cu, csrc/grl_awgn.h) -----------------------------
+ * DnDataset.__getitem__, validation branch (data/datasets/restoration_dn.py:134-143): noise =
+ * np.random.RandomState(key).normal(0, scale, (C, H, W)) with key the 8 uint32 words of sha256 of the image's name, then
+ * img_gt + torch.from_numpy(noise).float() in float32.  MT19937, init_by_array and the legacy polar Gaussian are exact;
+ * log(r2) is correctly rounded on the device (csrc/grl_awgn.h states the consequence). */
+/* src[i] (H, W, C) uint8 GRL_IMAGE_U8 -> dst[i] (C, H, W) fp32 GRL_IMAGE_F32 = k / 255 + (float)(scale * N_i), both of one
+ * size, C in {1, 3}, C * H * W < 2^31; keys: HOST array (n, 8) uint32, the RandomState(key) of image i;
+ * scale = noise_sigma / 255 (>= 0, finite).  One CTA per image, kAwgnPerLaunch (64) images per launch; no workspace. */
+int grl_awgn_u8(const GrlImageRef* src, const GrlImageRef* dst, const uint32_t* keys, int n, int C, double scale,
+                void* stream);
+/* The noise alone on the CPU from the same closed forms, log from libm as numpy's (tests): out[count] float64 =
+ * RandomState(key).normal(0, scale, count); HOST pointers. */
+int grl_awgn_noise_host(const uint32_t* key, int64_t count, double scale, double* out);
+/* The device's double-double log (awgn_log_cr) evaluated on the CPU (tests): out[i] = log(x[i]), x[i] positive normal. */
+int grl_awgn_log_host(const double* x, int64_t n, double* out);
+
 #ifdef __cplusplus
 }
 #endif
