@@ -12,6 +12,8 @@ LIB = os.path.join(PKG, "libgrl_b200.so")
 NVCC_FLAGS = [
     "-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v",
+    # the host copies of the closed forms (csrc/grl_hd.h) must evaluate each IEEE operation as written, on any host ISA
+    "-Xcompiler", "-ffp-contract=off",
 ]
 
 

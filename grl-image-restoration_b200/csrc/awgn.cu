@@ -85,7 +85,7 @@ __global__ void __launch_bounds__(kAwgnThreads) awgn_kernel(const AwgnList L, in
     k0 += total;
     if (acc && base < npairs) {
       const double f = awgn_polar_f(r2);
-      const double g[2] = {awgn_mul(f, x2), awgn_mul(f, x1)};
+      const double g[2] = {dmul_rn(f, x2), dmul_rn(f, x1)};
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int i = 2 * base + h;
@@ -139,8 +139,8 @@ int grl_awgn_noise_host(const uint32_t* key, int64_t count, double scale, double
       const double r2 = awgn_r2(x1, x2);
       if (!awgn_accept(r2)) continue;
       const double f = awgn_polar_f(r2);
-      out[i++] = awgn_normal(scale, awgn_mul(f, x2));
-      if (i < count) out[i++] = awgn_normal(scale, awgn_mul(f, x1));
+      out[i++] = awgn_normal(scale, dmul_rn(f, x2));
+      if (i < count) out[i++] = awgn_normal(scale, dmul_rn(f, x1));
     }
   }
   return GRL_OK;

@@ -11,9 +11,9 @@
 //     624 words holds exactly 156 candidates and no candidate straddles two twists.
 //   - legacy_normal: loc + scale * gauss, loc = 0; samples fill the tensor in C order.
 //   - torch.from_numpy(noise).float(), then img_gt + noise in float32.
-// Every double operation is written rounded (awgn_add / awgn_mul / awgn_div / awgn_sqrt): nvcc contracts
-// x1 * x1 + x2 * x2 into an FMA by default, and that changes r2.  The host evaluates plain IEEE operations, as numpy's
-// C code does on x86-64 (no FMA contraction without -mfma).
+// Every double operation goes through the rounded operations of grl_hd.h: nvcc contracts x1 * x1 + x2 * x2 into an FMA
+// by default, and that changes r2.  On the host they are plain IEEE operations and the build turns contraction off
+// (-ffp-contract=off), so the host evaluates the operations numpy's C code writes, on any host ISA.
 //
 // The one step that is not exact is log.  The host calls libm's log, as numpy does.  The device evaluates awgn_log_cr,
 // a double-double log accurate to about 2^-100 relative, rounded once: the correctly rounded log(r2) except where log(r2)
@@ -25,59 +25,17 @@
 #include <math.h>
 #include <stdint.h>
 
+#include "grl_hd.h"
 #include "grl_image_u8.h"
-
-#if defined(__CUDACC__)
-#define GRL_AWGN_HD __host__ __device__ __forceinline__
-#else
-#define GRL_AWGN_HD inline
-#endif
 
 namespace grl {
 
 constexpr int kMtN = 624, kMtM = 397;
 constexpr int kAwgnPairsPerTwist = kMtN / 4;  // 156 polar candidates of 4 words each
 
-// ---- rounded double arithmetic (no contraction on the device) -------------------------------------------------------
-GRL_AWGN_HD double awgn_add(double a, double b) {
-#if defined(__CUDA_ARCH__)
-  return __dadd_rn(a, b);
-#else
-  return a + b;
-#endif
-}
-GRL_AWGN_HD double awgn_mul(double a, double b) {
-#if defined(__CUDA_ARCH__)
-  return __dmul_rn(a, b);
-#else
-  return a * b;
-#endif
-}
-GRL_AWGN_HD double awgn_div(double a, double b) {
-#if defined(__CUDA_ARCH__)
-  return __ddiv_rn(a, b);
-#else
-  return a / b;
-#endif
-}
-GRL_AWGN_HD double awgn_sqrt(double a) {
-#if defined(__CUDA_ARCH__)
-  return __dsqrt_rn(a);
-#else
-  return sqrt(a);
-#endif
-}
-GRL_AWGN_HD double awgn_fma(double a, double b, double c) {
-#if defined(__CUDA_ARCH__)
-  return __fma_rn(a, b, c);
-#else
-  return fma(a, b, c);
-#endif
-}
-
 // ---- MT19937 (numpy's randomkit) -------------------------------------------------------------------------------------
 // init_by_array(key, 8) after init_genrand(19650218).
-GRL_AWGN_HD void awgn_mt_seed(uint32_t* mt, const uint32_t* key) {
+GRL_HD void awgn_mt_seed(uint32_t* mt, const uint32_t* key) {
   uint32_t s = 19650218u;
   for (int p = 0; p < kMtN; ++p) {
     mt[p] = s;
@@ -103,17 +61,17 @@ GRL_AWGN_HD void awgn_mt_seed(uint32_t* mt, const uint32_t* key) {
 }
 
 // One word of the twist: new[i] = far ^ twist(old[i], next), far = the word kMtM ahead (mod kMtN), next = word i + 1.
-GRL_AWGN_HD uint32_t awgn_twist_word(uint32_t cur, uint32_t next, uint32_t far) {
+GRL_HD uint32_t awgn_twist_word(uint32_t cur, uint32_t next, uint32_t far) {
   const uint32_t y = (cur & 0x80000000u) | (next & 0x7fffffffu);
   return far ^ (y >> 1) ^ ((0u - (y & 1u)) & 0x9908b0dfu);
 }
 
 // The whole twist in place, in order (host).  The kernel runs it as three parallel passes (awgn.cu).
-GRL_AWGN_HD void awgn_mt_twist(uint32_t* mt) {
+GRL_HD void awgn_mt_twist(uint32_t* mt) {
   for (int i = 0; i < kMtN; ++i) mt[i] = awgn_twist_word(mt[i], mt[(i + 1) % kMtN], mt[(i + kMtM) % kMtN]);
 }
 
-GRL_AWGN_HD uint32_t awgn_temper(uint32_t y) {
+GRL_HD uint32_t awgn_temper(uint32_t y) {
   y ^= y >> 11;
   y ^= (y << 7) & 0x9d2c5680u;
   y ^= (y << 15) & 0xefc60000u;
@@ -122,78 +80,78 @@ GRL_AWGN_HD uint32_t awgn_temper(uint32_t y) {
 
 // ---- the polar method ------------------------------------------------------------------------------------------------
 // 2 * legacy_double - 1 from two tempered words (every step exact).
-GRL_AWGN_HD double awgn_signed_unit(uint32_t w0, uint32_t w1) {
-  const double u = awgn_div(awgn_add(awgn_mul((double)(w0 >> 5), 67108864.0), (double)(w1 >> 6)), 9007199254740992.0);
-  return awgn_add(awgn_mul(2.0, u), -1.0);
+GRL_HD double awgn_signed_unit(uint32_t w0, uint32_t w1) {
+  const double u = ddiv_rn(dadd_rn(dmul_rn((double)(w0 >> 5), 67108864.0), (double)(w1 >> 6)), 9007199254740992.0);
+  return dadd_rn(dmul_rn(2.0, u), -1.0);
 }
 
 // r2 = x1 * x1 + x2 * x2, each product rounded.
-GRL_AWGN_HD double awgn_r2(double x1, double x2) { return awgn_add(awgn_mul(x1, x1), awgn_mul(x2, x2)); }
+GRL_HD double awgn_r2(double x1, double x2) { return dadd_rn(dmul_rn(x1, x1), dmul_rn(x2, x2)); }
 
-GRL_AWGN_HD bool awgn_accept(double r2) { return !(r2 >= 1.0 || r2 == 0.0); }
+GRL_HD bool awgn_accept(double r2) { return !(r2 >= 1.0 || r2 == 0.0); }
 
 // ---- log: double-double, rounded once ---------------------------------------------------------------------------------
 struct AwgnDD {
   double hi, lo;
 };
 
-GRL_AWGN_HD AwgnDD awgn_two_sum(double a, double b) {
-  const double s = awgn_add(a, b), bb = awgn_add(s, -a);
-  return {s, awgn_add(awgn_add(a, -awgn_add(s, -bb)), awgn_add(b, -bb))};
+GRL_HD AwgnDD awgn_two_sum(double a, double b) {
+  const double s = dadd_rn(a, b), bb = dadd_rn(s, -a);
+  return {s, dadd_rn(dadd_rn(a, -dadd_rn(s, -bb)), dadd_rn(b, -bb))};
 }
-GRL_AWGN_HD AwgnDD awgn_fast_two_sum(double a, double b) {  // |a| >= |b|
-  const double s = awgn_add(a, b);
-  return {s, awgn_add(b, -awgn_add(s, -a))};
+GRL_HD AwgnDD awgn_fast_two_sum(double a, double b) {  // |a| >= |b|
+  const double s = dadd_rn(a, b);
+  return {s, dadd_rn(b, -dadd_rn(s, -a))};
 }
-GRL_AWGN_HD AwgnDD awgn_dd_add(AwgnDD x, AwgnDD y) {
+GRL_HD AwgnDD awgn_dd_add(AwgnDD x, AwgnDD y) {
   AwgnDD s = awgn_two_sum(x.hi, y.hi);
   const AwgnDD t = awgn_two_sum(x.lo, y.lo);
-  s = awgn_fast_two_sum(s.hi, awgn_add(s.lo, t.hi));
-  return awgn_fast_two_sum(s.hi, awgn_add(s.lo, t.lo));
+  s = awgn_fast_two_sum(s.hi, dadd_rn(s.lo, t.hi));
+  return awgn_fast_two_sum(s.hi, dadd_rn(s.lo, t.lo));
 }
-GRL_AWGN_HD AwgnDD awgn_dd_mul(AwgnDD x, AwgnDD y) {
-  const double p = awgn_mul(x.hi, y.hi);
-  double e = awgn_fma(x.hi, y.hi, -p);
-  e = awgn_add(e, awgn_add(awgn_mul(x.hi, y.lo), awgn_mul(x.lo, y.hi)));
+GRL_HD AwgnDD awgn_dd_mul(AwgnDD x, AwgnDD y) {
+  const double p = dmul_rn(x.hi, y.hi);
+  double e = dfma_rn(x.hi, y.hi, -p);
+  e = dadd_rn(e, dadd_rn(dmul_rn(x.hi, y.lo), dmul_rn(x.lo, y.hi)));
   return awgn_fast_two_sum(p, e);
 }
 // 1 / d as a double-double.
-GRL_AWGN_HD AwgnDD awgn_dd_recip(double d) {
-  const double q = awgn_div(1.0, d);
-  return {q, awgn_div(awgn_fma(-q, d, 1.0), d)};
+GRL_HD AwgnDD awgn_dd_recip(double d) {
+  const double q = ddiv_rn(1.0, d);
+  return {q, ddiv_rn(dfma_rn(-q, d, 1.0), d)};
 }
 
 // log(x) for a positive normal x, accurate to about 2^-100 relative before the final rounding:
 //   x = 2^e m, m in [sqrt(1/2), sqrt(2));  log m = 2 atanh(s) = 2 s (1 + t P(t)), s = (m - 1) / (m + 1), t = s^2 <= 0.0295,
 //   P(t) = sum_k t^k / (2k + 3): k < 9 in double-double, k = 9..19 in double (below 2^-50 of P), the rest below 2^-101.
-GRL_AWGN_HD double awgn_log_cr(double x) {
+GRL_HD double awgn_log_cr(double x) {
   int e;
   double m = frexp(x, &e);
   if (m < 0.70710678118654752440) {
-    m = awgn_mul(m, 2.0);
+    m = dmul_rn(m, 2.0);
     --e;
   }
-  const double num = awgn_add(m, -1.0);  // exact (Sterbenz)
+  const double num = dadd_rn(m, -1.0);  // exact (Sterbenz)
   const AwgnDD den = awgn_two_sum(m, 1.0);
   // s = num / den
-  const double q1 = awgn_div(num, den.hi);
-  const double r = awgn_add(awgn_fma(-q1, den.hi, num), -awgn_mul(q1, den.lo));  // the fma is the exact remainder
-  const AwgnDD s = awgn_fast_two_sum(q1, awgn_div(r, den.hi));
+  const double q1 = ddiv_rn(num, den.hi);
+  const double r = dadd_rn(dfma_rn(-q1, den.hi, num), -dmul_rn(q1, den.lo));  // the fma is the exact remainder
+  const AwgnDD s = awgn_fast_two_sum(q1, ddiv_rn(r, den.hi));
   const AwgnDD t = awgn_dd_mul(s, s);
-  double tail = awgn_div(1.0, 41.0);
-  for (int k = 18; k >= 9; --k) tail = awgn_fma(tail, t.hi, awgn_div(1.0, (double)(2 * k + 3)));
+  double tail = ddiv_rn(1.0, 41.0);
+  for (int k = 18; k >= 9; --k) tail = dfma_rn(tail, t.hi, ddiv_rn(1.0, (double)(2 * k + 3)));
   AwgnDD p = {tail, 0.0};
   for (int k = 8; k >= 0; --k) p = awgn_dd_add(awgn_dd_mul(p, t), awgn_dd_recip((double)(2 * k + 3)));
   AwgnDD lm = awgn_dd_mul(s, awgn_dd_add({1.0, 0.0}, awgn_dd_mul(t, p)));
-  lm = {awgn_mul(lm.hi, 2.0), awgn_mul(lm.lo, 2.0)};
+  lm = {dmul_rn(lm.hi, 2.0), dmul_rn(lm.lo, 2.0)};
   const double ln2_hi = 0x1.62e42fefa39efp-1, ln2_lo = 0x1.abc9e3b39803fp-56;  // ln 2 to 2^-106
-  const double ed = (double)e, eh = awgn_mul(ed, ln2_hi);
-  const AwgnDD el = awgn_fast_two_sum(eh, awgn_add(awgn_fma(ed, ln2_hi, -eh), awgn_mul(ed, ln2_lo)));
+  const double ed = (double)e, eh = dmul_rn(ed, ln2_hi);
+  const AwgnDD el = awgn_fast_two_sum(eh, dadd_rn(dfma_rn(ed, ln2_hi, -eh), dmul_rn(ed, ln2_lo)));
   const AwgnDD sum = awgn_dd_add(el, lm);
-  return awgn_add(sum.hi, sum.lo);
+  return dadd_rn(sum.hi, sum.lo);
 }
 
-GRL_AWGN_HD double awgn_log(double x) {
+GRL_HD double awgn_log(double x) {
 #if defined(__CUDA_ARCH__)
   return awgn_log_cr(x);
 #else
@@ -202,18 +160,12 @@ GRL_AWGN_HD double awgn_log(double x) {
 }
 
 // f of an accepted candidate: sqrt(-2 log(r2) / r2).
-GRL_AWGN_HD double awgn_polar_f(double r2) { return awgn_sqrt(awgn_div(awgn_mul(-2.0, awgn_log(r2)), r2)); }
+GRL_HD double awgn_polar_f(double r2) { return dsqrt_rn(ddiv_rn(dmul_rn(-2.0, awgn_log(r2)), r2)); }
 
 // legacy_normal(0, scale) of a gauss g, in float64.
-GRL_AWGN_HD double awgn_normal(double scale, double g) { return awgn_add(0.0, awgn_mul(scale, g)); }
+GRL_HD double awgn_normal(double scale, double g) { return dadd_rn(0.0, dmul_rn(scale, g)); }
 
 // img_gt + torch.from_numpy(noise).float(): k / 255 plus the float32-rounded noise, a float32 add.
-GRL_AWGN_HD float awgn_pixel(int k, double noise) {
-#if defined(__CUDA_ARCH__)
-  return __fadd_rn(u8_unit(k), __double2float_rn(noise));
-#else
-  return u8_unit(k) + (float)noise;
-#endif
-}
+GRL_HD float awgn_pixel(int k, double noise) { return fadd_rn(u8_unit(k), (float)noise); }
 
 }  // namespace grl

@@ -8,12 +8,7 @@
 #include <stdint.h>
 
 #include "../../include/grl_b200.h"
-
-#if defined(__CUDACC__)
-#define GRL_HD __host__ __device__ __forceinline__
-#else
-#define GRL_HD inline
-#endif
+#include "grl_hd.h"
 
 namespace grl {
 

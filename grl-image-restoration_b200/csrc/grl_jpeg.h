@@ -15,18 +15,14 @@
 
 #include <stdint.h>
 
-#if defined(__CUDACC__)
-#define GRL_JPEG_HD __host__ __device__ __forceinline__
-#else
-#define GRL_JPEG_HD inline
-#endif
+#include "grl_hd.h"
 
 namespace grl {
 
 typedef long long jpeg_long;  // libjpeg's JLONG: the DCT products and the colour sums
 
 // ITU T.81 Annex K tables K.1 (luminance) and K.2 (chrominance), natural order.
-GRL_JPEG_HD int jpeg_std_table(int chroma, int k) {
+GRL_HD int jpeg_std_table(int chroma, int k) {
   const int r = k >> 3, c = k & 7;
   if (chroma) {
     const uint8_t t[4][4] = {{17, 18, 24, 47}, {18, 21, 26, 66}, {24, 26, 56, 99}, {47, 66, 99, 99}};
@@ -39,7 +35,7 @@ GRL_JPEG_HD int jpeg_std_table(int chroma, int k) {
 }
 
 // jpeg_set_quality(q, force_baseline = TRUE): entry k (natural order) of the luma (chroma = 0) or chroma table.
-GRL_JPEG_HD int jpeg_quant(int quality, int chroma, int k) {
+GRL_HD int jpeg_quant(int quality, int chroma, int k) {
   const int scale = quality < 50 ? 5000 / quality : 200 - 2 * quality;
   const int v = (jpeg_std_table(chroma, k) * scale + 50) / 100;
   return v < 1 ? 1 : (v > 255 ? 255 : v);
@@ -49,16 +45,16 @@ GRL_JPEG_HD int jpeg_quant(int quality, int chroma, int k) {
 constexpr int kJpegScale = 16;
 constexpr jpeg_long kJpegHalf = (jpeg_long)1 << (kJpegScale - 1);
 
-GRL_JPEG_HD int jpeg_y(int r, int g, int b) { return (int)((19595LL * r + 38470LL * g + 7471LL * b + kJpegHalf) >> 16); }
+GRL_HD int jpeg_y(int r, int g, int b) { return (int)((19595LL * r + 38470LL * g + 7471LL * b + kJpegHalf) >> 16); }
 // Cb (comp 1) or Cr (comp 2); the rounding is 0.5 - epsilon, so the result stays <= 255 without a clamp.
-GRL_JPEG_HD int jpeg_chroma(int comp, int r, int g, int b) {
+GRL_HD int jpeg_chroma(int comp, int r, int g, int b) {
   const jpeg_long off = ((jpeg_long)128 << kJpegScale) + kJpegHalf - 1;
   return comp == 1 ? (int)((-11059LL * r - 21709LL * g + 32768LL * b + off) >> 16)
                    : (int)((32768LL * r - 27439LL * g - 5329LL * b + off) >> 16);
 }
-GRL_JPEG_HD int jpeg_clamp255(int v) { return v < 0 ? 0 : (v > 255 ? 255 : v); }
+GRL_HD int jpeg_clamp255(int v) { return v < 0 ? 0 : (v > 255 ? 255 : v); }
 // YCbCr -> one of R (c = 0), G, B, range-limited to 0..255.
-GRL_JPEG_HD int jpeg_rgb(int c, int y, int cb, int cr) {
+GRL_HD int jpeg_rgb(int c, int y, int cb, int cr) {
   cb -= 128;
   cr -= 128;
   int v;
@@ -77,10 +73,10 @@ constexpr jpeg_long F0298 = 2446, F0390 = 3196, F0541 = 4433, F0765 = 6270, F089
                     F1847 = 15137, F1961 = 16069, F2053 = 16819, F2562 = 20995, F3072 = 25172;
 
 // Rounded right shift of a product sum; every result of the two passes fits an int.
-GRL_JPEG_HD int jpeg_descale(jpeg_long x, int n) { return (int)((x + ((jpeg_long)1 << (n - 1))) >> n); }
+GRL_HD int jpeg_descale(jpeg_long x, int n) { return (int)((x + ((jpeg_long)1 << (n - 1))) >> n); }
 
 // One forward pass over 8 values d[0], d[s], ..., d[7 s]; pass 1 (rows) keeps PASS1_BITS of extra precision.
-GRL_JPEG_HD void jpeg_fdct_1d(int* d, int s, bool pass1) {
+GRL_HD void jpeg_fdct_1d(int* d, int s, bool pass1) {
   const jpeg_long tmp0 = d[0] + d[7 * s], tmp7 = d[0] - d[7 * s], tmp1 = d[s] + d[6 * s], tmp6 = d[s] - d[6 * s];
   const jpeg_long tmp2 = d[2 * s] + d[5 * s], tmp5 = d[2 * s] - d[5 * s], tmp3 = d[3 * s] + d[4 * s],
                   tmp4 = d[3 * s] - d[4 * s];
@@ -102,7 +98,7 @@ GRL_JPEG_HD void jpeg_fdct_1d(int* d, int s, bool pass1) {
 
 // One inverse pass over 8 values; pass 1 (columns of dequantised coefficients) keeps PASS1_BITS, pass 2 (rows) also
 // removes the DCT's factor of 8.
-GRL_JPEG_HD void jpeg_idct_1d(int* z, int s, bool pass1) {
+GRL_HD void jpeg_idct_1d(int* z, int s, bool pass1) {
   const jpeg_long e = ((jpeg_long)z[2 * s] + z[6 * s]) * F0541;
   const jpeg_long tmp2 = e - z[6 * s] * F1847, tmp3 = e + z[2 * s] * F0765;
   const jpeg_long tmp0 = ((jpeg_long)z[0] + z[4 * s]) * (1 << kConstBits);
@@ -128,14 +124,14 @@ GRL_JPEG_HD void jpeg_idct_1d(int* z, int s, bool pass1) {
 }
 
 // The coefficient the decoder sees: the FDCT output (8 x the DCT) divided by 8 qv, rounded half away from zero, times qv.
-GRL_JPEG_HD int jpeg_requant(int c, int qv) {
+GRL_HD int jpeg_requant(int c, int qv) {
   const int div = 8 * qv, a = c < 0 ? -c : c, q = (a + (div >> 1)) / div;
   return (c < 0 ? -q : q) * qv;
 }
 
 // One block through the codec: b (64 samples 0..255, row-major) -> FDCT -> quantise -> dequantise -> IDCT -> b, the
 // decoder's samples (the IDCT's + 128, clamped to 0..255).  qt: the component's 64 quantisation values, natural order.
-GRL_JPEG_HD void jpeg_block_roundtrip(int* b, const uint8_t* qt) {
+GRL_HD void jpeg_block_roundtrip(int* b, const uint8_t* qt) {
 #pragma unroll
   for (int i = 0; i < 64; ++i) b[i] -= 128;
 #pragma unroll
@@ -156,19 +152,19 @@ GRL_JPEG_HD void jpeg_block_roundtrip(int* b, const uint8_t* qt) {
 struct JpegImage {
   const uint8_t* src;  // (H, W, C) uint8
   int H, W, C;
-  GRL_JPEG_HD int h2() const { return (H + 1) >> 1; }  // the chroma components' real size
-  GRL_JPEG_HD int w2() const { return (W + 1) >> 1; }
-  GRL_JPEG_HD int px(int y, int x, int c) const {      // clamp-to-edge
+  GRL_HD int h2() const { return (H + 1) >> 1; }  // the chroma components' real size
+  GRL_HD int w2() const { return (W + 1) >> 1; }
+  GRL_HD int px(int y, int x, int c) const {      // clamp-to-edge
     y = y < H ? y : H - 1;
     x = x < W ? x : W - 1;
     return src[((long long)y * W + x) * C + c];
   }
-  GRL_JPEG_HD int luma(int y, int x) const {
+  GRL_HD int luma(int y, int x) const {
     return C == 1 ? px(y, x, 0) : jpeg_y(px(y, x, 0), px(y, x, 1), px(y, x, 2));
   }
   // Downsampled chroma sample (cy, cx) of component comp (1 = Cb, 2 = Cr): the 2 x 2 sum plus a bias of 1, 2, 1, 2, ...
   // along the row, >> 2.  Rows below the component's last real row repeat it.
-  GRL_JPEG_HD int chroma(int comp, int cy, int cx) const {
+  GRL_HD int chroma(int comp, int cy, int cx) const {
     cy = cy < h2() ? cy : h2() - 1;
     int s = 1 + (cx & 1);
 #pragma unroll
@@ -183,13 +179,13 @@ struct JpegImage {
 };
 
 // Coded blocks of component comp (0 = Y or gray, 1 = Cb, 2 = Cr): rows x cols.
-GRL_JPEG_HD int jpeg_blocks_y(const JpegImage& im, int comp) { return ((comp ? im.h2() : im.H) + 7) >> 3; }
-GRL_JPEG_HD int jpeg_blocks_x(const JpegImage& im, int comp) { return ((comp ? im.w2() : im.W) + 7) >> 3; }
+GRL_HD int jpeg_blocks_y(const JpegImage& im, int comp) { return ((comp ? im.h2() : im.H) + 7) >> 3; }
+GRL_HD int jpeg_blocks_x(const JpegImage& im, int comp) { return ((comp ? im.w2() : im.W) + 7) >> 3; }
 
 // Block (by, bx) of component comp through the codec; the decoded samples inside the component's real area go to
 // out (row pitch ld): the image's size for Y, (h2, w2) for chroma.
-GRL_JPEG_HD void jpeg_component_block(const JpegImage& im, int comp, int by, int bx, const uint8_t* qt, uint8_t* out,
-                                      int ld) {
+GRL_HD void jpeg_component_block(const JpegImage& im, int comp, int by, int bx, const uint8_t* qt, uint8_t* out,
+                                 int ld) {
   int b[64];
 #pragma unroll
   for (int r = 0; r < 8; ++r)
@@ -211,7 +207,7 @@ GRL_JPEG_HD void jpeg_component_block(const JpegImage& im, int comp, int by, int
 // nearer chroma row and column weighted 3 against 1 and edge samples replicated: 3 near + far vertically, then
 // (3 this + neighbour + 8) >> 4 on even columns, + 7 on odd ones.  A component at most 2 samples wide is upsampled by
 // plain replication instead (libjpeg's h2v2_upsample).
-GRL_JPEG_HD int jpeg_upsample(const uint8_t* p, int h2, int w2, int y, int x) {
+GRL_HD int jpeg_upsample(const uint8_t* p, int h2, int w2, int y, int x) {
   const int cy = y >> 1, cx = x >> 1;
   if (w2 <= 2) return p[(long long)cy * w2 + cx];
   int ny = (y & 1) ? cy + 1 : cy - 1;
@@ -225,8 +221,8 @@ GRL_JPEG_HD int jpeg_upsample(const uint8_t* p, int h2, int w2, int y, int x) {
 }
 
 // Decoded RGB at pixel (y, x) from the decoded planes: Y (H, W), Cb and Cr (h2, w2).
-GRL_JPEG_HD void jpeg_decode_pixel(const uint8_t* Y, const uint8_t* cb, const uint8_t* cr, int H, int W, int y, int x,
-                                   uint8_t* rgb) {
+GRL_HD void jpeg_decode_pixel(const uint8_t* Y, const uint8_t* cb, const uint8_t* cr, int H, int W, int y, int x,
+                              uint8_t* rgb) {
   const int h2 = (H + 1) >> 1, w2 = (W + 1) >> 1;
   const int l = Y[(long long)y * W + x], u = jpeg_upsample(cb, h2, w2, y, x), v = jpeg_upsample(cr, h2, w2, y, x);
 #pragma unroll

@@ -10,44 +10,24 @@
 
 #include <math.h>
 
-#if defined(__CUDACC__)
-#define GRL_NQ_HD __host__ __device__ __forceinline__
-#else
-#define GRL_NQ_HD inline
-#endif
+#include "grl_hd.h"
 
 namespace grl {
 
 // fp32 value of one channel after p * 255 and / 255 (p = k / 255 from tensor_round).
-GRL_NQ_HD float niqe_chan(int k) {
-#if defined(__CUDA_ARCH__)
-  const float p = __fdiv_rn((float)k, 255.0f);
-  return __fdiv_rn(__fmul_rn(p, 255.0f), 255.0f);
-#else
-  volatile float p = (float)k / 255.0f;
-  volatile float v = p * 255.0f;
-  return v / 255.0f;
-#endif
+GRL_HD float niqe_chan(int k) {
+  const float p = fdiv_rn((float)k, 255.0f);
+  return fdiv_rn(fmul_rn(p, 255.0f), 255.0f);
 }
 
 // Rounded luma (a float holding an integer in [16, 235]) of the 8-bit RGB triple (r, g, b).
-GRL_NQ_HD float niqe_luma(int r, int g, int b) {
-#if defined(__CUDA_ARCH__)
-  double d = __dmul_rn((double)niqe_chan(r), 24.966);
-  d = __dadd_rn(d, __dmul_rn((double)niqe_chan(g), 128.553));
-  d = __dadd_rn(d, __dmul_rn((double)niqe_chan(b), 65.481));
-  d = __dadd_rn(d, 16.0);
-  const float f = (float)__ddiv_rn(d, 255.0);
-  return rintf(__fmul_rn(f, 255.0f));
-#else
-  volatile double d = (double)niqe_chan(r) * 24.966;
-  d = d + (double)niqe_chan(g) * 128.553;
-  d = d + (double)niqe_chan(b) * 65.481;
-  d = d + 16.0;
-  volatile float f = (float)(d / 255.0);
-  volatile float y = f * 255.0f;
-  return rintf(y);
-#endif
+GRL_HD float niqe_luma(int r, int g, int b) {
+  double d = dmul_rn((double)niqe_chan(r), 24.966);
+  d = dadd_rn(d, dmul_rn((double)niqe_chan(g), 128.553));
+  d = dadd_rn(d, dmul_rn((double)niqe_chan(b), 65.481));
+  d = dadd_rn(d, 16.0);
+  const float f = (float)ddiv_rn(d, 255.0);
+  return rintf(fmul_rn(f, 255.0f));
 }
 
 }  // namespace grl

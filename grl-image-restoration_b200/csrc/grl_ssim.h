@@ -10,19 +10,13 @@
 // with the 2-D window float32(t t^T) and sums in fp32; the two windows differ by at most 6e-8 relative per weight.
 #pragma once
 
-#include <math.h>
-
-#if defined(__CUDACC__)
-#define GRL_SSIM_HD __host__ __device__ __forceinline__
-#else
-#define GRL_SSIM_HD inline
-#endif
+#include "grl_hd.h"
 
 namespace grl {
 
 constexpr int kSsimTaps = 11, kSsimHalo = 5;
 // round(exp(-(i - 5)^2 / 4.5), 6) over their sum, in float64 (gaussian(11, 1.5), ssim.py:17-24)
-GRL_SSIM_HD double ssim_tap(int i) {
+GRL_HD double ssim_tap(int i) {
   // the sum as the reference takes it, left to right: 3.7592320000000004
   constexpr double s = 0.003866 + 0.028566 + 0.135335 + 0.411112 + 0.800737 + 1.0 + 0.800737 + 0.411112 + 0.135335 + 0.028566 + 0.003866;
   constexpr double t[kSsimTaps] = {0.003866 / s, 0.028566 / s, 0.135335 / s, 0.411112 / s, 0.800737 / s, 1.0 / s,
@@ -33,32 +27,13 @@ GRL_SSIM_HD double ssim_tap(int i) {
 // C1 = 0.01^2 and C2 = 0.03^2 (ssim.py:57-58) for data in [0, 1], times 255^2 for data in [0, 255]
 constexpr double kSsimC1 = 1e-4 * 65025.0, kSsimC2 = 9e-4 * 65025.0;
 
-GRL_SSIM_HD double ssim_fma(double a, double b, double c) {
-#if defined(__CUDA_ARCH__)
-  return __fma_rn(a, b, c);
-#else
-  return fma(a, b, c);
-#endif
-}
-
 // One value of the SSIM map (ssim.py:42-62) from the five windowed sums of a, b, a^2, b^2 and a * b on the 0..255 scale.
-// Every operation is one correctly rounded multiply, add, fma or divide in this order on host and device.
-GRL_SSIM_HD double ssim_map_value(double sa, double sb, double saa, double sbb, double sab) {
-#if defined(__CUDA_ARCH__)
-  const double mu_aa = __dmul_rn(sa, sa), mu_bb = __dmul_rn(sb, sb), mu_ab = __dmul_rn(sa, sb);
-  const double var_a = __dsub_rn(saa, mu_aa), var_b = __dsub_rn(sbb, mu_bb), cov = __dsub_rn(sab, mu_ab);
-  const double num = __dmul_rn(__fma_rn(2.0, mu_ab, kSsimC1), __fma_rn(2.0, cov, kSsimC2));
-  const double den = __dmul_rn(__dadd_rn(__dadd_rn(mu_aa, mu_bb), kSsimC1), __dadd_rn(__dadd_rn(var_a, var_b), kSsimC2));
-  return __ddiv_rn(num, den);
-#else
-  volatile double mu_aa = sa * sa, mu_bb = sb * sb, mu_ab = sa * sb;  // volatile: no contraction into an fma
-  volatile double var_a = saa - mu_aa, var_b = sbb - mu_bb, cov = sab - mu_ab;
-  volatile double n1 = fma(2.0, mu_ab, kSsimC1), n2 = fma(2.0, cov, kSsimC2);
-  volatile double d1 = mu_aa + mu_bb, d2 = var_a + var_b;
-  volatile double e1 = d1 + kSsimC1, e2 = d2 + kSsimC2;
-  volatile double num = n1 * n2, den = e1 * e2;
-  return num / den;
-#endif
+GRL_HD double ssim_map_value(double sa, double sb, double saa, double sbb, double sab) {
+  const double mu_aa = dmul_rn(sa, sa), mu_bb = dmul_rn(sb, sb), mu_ab = dmul_rn(sa, sb);
+  const double var_a = dsub_rn(saa, mu_aa), var_b = dsub_rn(sbb, mu_bb), cov = dsub_rn(sab, mu_ab);
+  const double num = dmul_rn(dfma_rn(2.0, mu_ab, kSsimC1), dfma_rn(2.0, cov, kSsimC2));
+  const double den = dmul_rn(dadd_rn(dadd_rn(mu_aa, mu_bb), kSsimC1), dadd_rn(dadd_rn(var_a, var_b), kSsimC2));
+  return ddiv_rn(num, den);
 }
 
 }  // namespace grl

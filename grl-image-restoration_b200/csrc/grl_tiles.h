@@ -9,11 +9,7 @@
 // column axis).
 #pragma once
 
-#if defined(__CUDACC__)
-#define GRL_TILE_HD __host__ __device__ __forceinline__
-#else
-#define GRL_TILE_HD inline
-#endif
+#include "grl_hd.h"
 
 namespace grl {
 
@@ -21,21 +17,21 @@ struct TileAxis {
   int size, t, stride, n;
 };
 
-GRL_TILE_HD TileAxis tile_axis(int size, int t, int overlap) {
+GRL_HD TileAxis tile_axis(int size, int t, int overlap) {
   const int stride = t - overlap;
   return {size, t, stride, (size - t + stride - 1) / stride + 1};
 }
 
-GRL_TILE_HD int tile_origin(const TileAxis& a, int k) { return k < a.n - 1 ? k * a.stride : a.size - a.t; }
+GRL_HD int tile_origin(const TileAxis& a, int k) { return k < a.n - 1 ? k * a.stride : a.size - a.t; }
 
 // The first tile whose window reaches past sample r: the first k < n - 1 with k * stride + t > r, else the last tile.
-GRL_TILE_HD int tile_first(const TileAxis& a, int r) {
+GRL_HD int tile_first(const TileAxis& a, int r) {
   const int k = r < a.t ? 0 : (r - a.t) / a.stride + 1;
   return k < a.n - 1 ? k : a.n - 1;
 }
 
 // The last tile whose origin is at or before sample r: the last tile once r >= size - t, else the last k * stride <= r
 // (which is below n - 1, since (n - 1) * stride >= size - t).
-GRL_TILE_HD int tile_last(const TileAxis& a, int r) { return r >= a.size - a.t ? a.n - 1 : r / a.stride; }
+GRL_HD int tile_last(const TileAxis& a, int r) { return r >= a.size - a.t ? a.n - 1 : r / a.stride; }
 
 }  // namespace grl

@@ -59,7 +59,7 @@ __device__ __forceinline__ int pad_source(int p, int n, bool reflect) {
 }
 
 // F.pad(..., "reflect") needs every pad smaller than its axis; otherwise the reference pads both axes with zeros.
-__host__ __device__ __forceinline__ bool reflects(int H, int W, int Hp, int Wp) { return Hp - H < H && Wp - W < W; }
+GRL_HD bool reflects(int H, int W, int Hp, int Wp) { return Hp - H < H && Wp - W < W; }
 
 // Source readers of the fp32 gather: the network image's size, and its channel c at pixel (y, x).
 struct PlanesReader {  // (C, H, W) fp32 planes

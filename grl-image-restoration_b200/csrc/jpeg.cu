@@ -43,14 +43,14 @@ __device__ __forceinline__ int find_image(const int* first, int m, int t) {
   return lo;
 }
 
-__host__ __device__ __forceinline__ long long blocks_of(int H, int W, int C) {
+GRL_HD long long blocks_of(int H, int W, int C) {
   const JpegImage im{nullptr, H, W, C};
   long long n = (long long)jpeg_blocks_y(im, 0) * jpeg_blocks_x(im, 0);
   if (C == 3) n += 2LL * jpeg_blocks_y(im, 1) * jpeg_blocks_x(im, 1);
   return n;
 }
 
-__host__ __device__ __forceinline__ long long workspace_of(int H, int W, int C) {
+GRL_HD long long workspace_of(int H, int W, int C) {
   return C == 3 ? (long long)H * W + 2LL * ((H + 1) >> 1) * ((W + 1) >> 1) : 0;
 }
 

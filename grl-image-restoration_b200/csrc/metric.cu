@@ -20,7 +20,7 @@ namespace grl {
 
 // y = round(65.481/255 * R + 128.553/255 * G + 24.966/255 * B + 16) with R, G, B on the 0..255 grid
 // (metrics.rgb_to_y: (img * 255) @ (coeff / 255) + 16, rounded)
-__host__ __device__ __forceinline__ float luma8(float r, float g, float b) {
+GRL_HD float luma8(float r, float g, float b) {
   float acc = r * (65.481f / 255.0f);
   acc = fmaf(g, 128.553f / 255.0f, acc);
   acc = fmaf(b, 24.966f / 255.0f, acc);
@@ -248,7 +248,7 @@ ssim_tile_kernel(Img a, Img b, int C, int H, int W, int border,
 #pragma unroll
           for (int t = 0; t < kSsimTaps; ++t)
 #pragma unroll
-            for (int i = 0; i < 4; ++i) acc[i] = ssim_fma(ssim_tap(t), v[i + t], acc[i]);
+            for (int i = 0; i < 4; ++i) acc[i] = dfma_rn(ssim_tap(t), v[i + t], acc[i]);
 #pragma unroll
           for (int i = 0; i < 4; ++i) hs[q][lane][4 * xg + i] = acc[i];
         }
@@ -265,7 +265,7 @@ ssim_tile_kernel(Img a, Img b, int C, int H, int W, int border,
       for (int i = 0; i < 4; ++i) {
         double acc = 0.0;
 #pragma unroll
-        for (int t = 0; t < kSsimTaps; ++t) acc = ssim_fma(ssim_tap(t), r[i + t], acc);
+        for (int t = 0; t < kSsimTaps; ++t) acc = dfma_rn(ssim_tap(t), r[i + t], acc);
         s[q][i] = acc;
       }
     }
@@ -496,7 +496,7 @@ int grl_ssim_host(const float* restored, const float* target, int B, int C, int 
             double acc = 0.0;
             for (int t = 0; t < kSsimTaps; ++t) {
               const int xx = x - kSsimHalo + t;
-              acc = ssim_fma(ssim_tap(t), xx >= 0 && xx < w ? src[(size_t)y * w + xx] : 0.0, acc);
+              acc = dfma_rn(ssim_tap(t), xx >= 0 && xx < w ? src[(size_t)y * w + xx] : 0.0, acc);
             }
             hsum[(size_t)y * w + x] = acc;
           }
@@ -505,7 +505,7 @@ int grl_ssim_host(const float* restored, const float* target, int B, int C, int 
             double acc = 0.0;
             for (int t = 0; t < kSsimTaps; ++t) {
               const int yy = y - kSsimHalo + t;
-              acc = ssim_fma(ssim_tap(t), yy >= 0 && yy < h ? hsum[(size_t)yy * w + x] : 0.0, acc);
+              acc = dfma_rn(ssim_tap(t), yy >= 0 && yy < h ? hsum[(size_t)yy * w + x] : 0.0, acc);
             }
             sums[q][(size_t)y * w + x] = acc;
           }
