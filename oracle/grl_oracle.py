@@ -515,6 +515,86 @@ def gemm_launch_reference(x, w, bias, *, taps=1, epi=0, act=0, slope=0.0, n_res=
     return out
 
 
+LN100_F32 = float(torch.tensor(log(100.0), dtype=torch.float32))  # the logit-scale clamp as the kernels hold it
+
+
+def to16(x, fmt):
+    """The 16-bit rounding contract of the pack kernels: round to nearest even; fp16 saturates at +-65504 (cvt.rn.satfinite,
+    where torch's .half() would give inf), bf16 is torch's .bfloat16()."""
+    x = x.float()
+    return x.bfloat16() if fmt else x.clamp(-65504.0, 65504.0).half()
+
+
+def channel_gate_reference(y, w1, b1, w2, b2):
+    """float64 squeeze-excite of the CAB: sigmoid(W2 relu(W1 mean_L(y) + b1) + b2), y (B, L, C).  Returns the gate, the
+    means and the hidden units."""
+    m = y.double().mean(1)
+    h = torch.relu(m @ w1.double().T + b1.double())
+    return torch.sigmoid(h @ w2.double().T + b2.double()), m, h
+
+
+U = 2.0 ** -24  # fp32 unit roundoff
+L_LN = 100      # rows per image of the CAB gate in ln_reference / ln_bound: the boundary lies inside an 8-row block
+
+
+def gamma(n):
+    """gamma_n = n u / (1 - n u): the relative error bound of n fp32 roundings."""
+    return n * U / (1 - n * U)
+
+
+def ln_reference(u, gamma_, beta, eps, rs, x, cy, gate, mutation=None):
+    """float64 LayerNorm residual of the fp32 kernels (K.ln_residual): LN(u) rs + x + cy gate[image of the row], with the
+    images L_LN rows each.  `mutation` names a kernel bug whose effect to compute instead."""
+    C = u.shape[1]
+    if mutation == "naive fp32 E[x^2] - E[x]^2":
+        u32 = u.float()
+        mean32 = u32.mean(1, keepdim=True)
+        mean, var = mean32.double(), ((u32 * u32).mean(1, keepdim=True) - mean32 * mean32).double()
+    else:
+        mean = u.mean(1, keepdim=True)
+        var = (u - mean).pow(2).sum(1, keepdim=True) / (C - 1 if mutation == "n - 1 variance" else C)
+    e = 0.0 if mutation == "no eps" else eps
+    r = (u - mean) / torch.sqrt(var + e) * gamma_ + beta
+    r = r * (1.0 if mutation == "res_scale dropped" else rs)
+    if x is not None:
+        r = r + x
+    if cy is not None:
+        rows = torch.arange(u.shape[0], device=u.device)
+        if mutation == "CAB gate of the wrong image at the boundary":
+            rows = rows // 8 * 8  # every row of an 8-row block takes the image of the block's first row
+        r = r + cy * gate[rows // L_LN]
+    return r
+
+
+def ln_bound(u, gamma_, beta, eps, rs, x, cy, gate):
+    """Per-element bound of ln_reference's fp32 kernel: two-pass moments over C, each a lane-strided sequential sum plus a
+    5-level warp tree."""
+    C = u.shape[1]
+    ns = -(-C // 32) + 5
+    mean = u.mean(1, keepdim=True)
+    e_mean = gamma(ns) * u.abs().sum(1, keepdim=True) / C + U * mean.abs()
+    d = u - mean
+    var = d.pow(2).mean(1, keepdim=True)
+    # the deviations carry the common mean error (its cross term sums to zero) and one rounding each
+    e_var = e_mean ** 2 + (var + e_mean ** 2) * (gamma(ns) + 4 * U)
+    rel_v = (e_var + U * (var + eps)) / (var + eps)
+    rel_r = 0.5 * rel_v * (1 + rel_v) + 2.5 * U  # sqrt, reciprocal
+    rstd = 1 / torch.sqrt(var + eps)
+    n = d * rstd
+    e_n = (e_mean + U * (d.abs() + e_mean)) * rstd + n.abs() * (rel_r + U)
+    t = n * gamma_ + beta
+    e = gamma_.abs() * e_n + U * ((n * gamma_).abs() + t.abs())
+    r = t * rs
+    e = abs(rs) * e + U * r.abs()
+    if x is not None:
+        r = r + x
+        e = e + U * r.abs()
+    if cy is not None:
+        cg = cy * gate[torch.arange(u.shape[0], device=u.device) // L_LN]
+        e = e + U * (cg.abs() + (r + cg).abs())
+    return e * (1 + 1e-6)
+
+
 def window_attention(sd, pre, qkv, x_size, ws, heads, shifted, table, index, mask):
     """mixed_attn_block_efficient.py:128-165."""
     H, W = x_size

@@ -12,6 +12,8 @@ import numpy as np
 import pytest
 import torch
 
+from engine_oracle import to_tensor
+
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 with open(os.path.join(GOLD, "awgn_cases.json")) as f:
@@ -25,11 +27,6 @@ COUNTS = [0, 1, 2, 3, 311, 312, 313, 623, 624, 625, 10 ** 5 + 3]
 def case(name):
     c = CASES[name]
     return c, _NPZ[f"{name}/input"], torch.from_numpy(_NPZ[f"{name}/gt"]), torch.from_numpy(_NPZ[f"{name}/lq"])
-
-
-def to_tensor(img):
-    """transforms.functional.to_tensor of an (H, W, C) uint8 array."""
-    return torch.from_numpy(np.ascontiguousarray(img.transpose(2, 0, 1))).float().div(255)
 
 
 def crop8(img):

@@ -4,22 +4,14 @@ and against a float64 evaluation, with a derived bound; mutation controls that t
 
 Gate: an fp32 response of <= 11 exact-weight products is within gamma_11 * sum|w_i m_i| of the exact value whatever the
 summation order (dm_oracle.dm_matlab_bound), so two fp32 evaluations are within twice that of each other."""
-import json
-import os
-
 import pytest
 import torch
 import torch.nn.functional as F
 
 import dm_oracle  # oracle/dm_oracle.py (conftest puts oracle/ on sys.path)
+from support import dm_cases
 
-GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 NAMES = ["b2_40x56", "zero_pad_4x4", "odd_18x26"]
-
-
-def dm_cases():
-    with open(os.path.join(GOLD, "dm_cases.json")) as f:
-        return json.load(f)
 
 
 def ulp32(v):

@@ -1,28 +1,13 @@
 """x8 self-ensemble, host side: the closed-form view maps (grl_geometry.h d8_src / d8_inv through grl_d8_index_host)
 against augment_img_tensor4's index maps, and the CPU oracle composed as 8 independent forwards against the unmodified
 reference's per-view and merged outputs (tests/golden/ensemble_*.npz, oracle/make_golden_ensemble.py)."""
-import json
-import os
-
 import pytest
 import torch
 
-GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+from engine_oracle import INVERSE, augment
+from support import ensemble_cases
+
 SIZES = [(1, 1), (1, 7), (5, 3), (28, 44), (64, 64)]
-INVERSE = {3: 5, 5: 3}
-
-
-def augment(img, mode):
-    """augment_img_tensor4 (utils/utils_bsr/utils_image.py:444-460) restated with the same torch ops."""
-    ops = [lambda t: t, lambda t: t.rot90(1, [2, 3]).flip([2]), lambda t: t.flip([2]), lambda t: t.rot90(3, [2, 3]),
-           lambda t: t.rot90(2, [2, 3]).flip([2]), lambda t: t.rot90(1, [2, 3]), lambda t: t.rot90(2, [2, 3]),
-           lambda t: t.rot90(3, [2, 3]).flip([2])]
-    return ops[mode](img)
-
-
-def ensemble_cases():
-    with open(os.path.join(GOLD, "ensemble_cases.json")) as f:
-        return json.load(f)
 
 
 @pytest.mark.parametrize("H,W", SIZES)

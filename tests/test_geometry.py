@@ -1,14 +1,9 @@
 """Closed-form index arithmetic (csrc/grl_geometry.h, expanded by the C ABI's *_host functions) must be BIT-EXACT
 against the reference's tensors (golden digests) and the oracle.  CPU only."""
-import hashlib
-
-import numpy as np
 import pytest
 import torch
 
-
-def sha(t):
-    return hashlib.sha256(np.ascontiguousarray(t.numpy()).tobytes()).hexdigest()
+from support import sha
 
 
 NAMES = ["sr_small_128", "dn_small_128", "deblur_96x192", "jpeg_144", "dm_64", "yaml_default_64", "groups_g1_32",

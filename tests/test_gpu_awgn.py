@@ -10,7 +10,8 @@ import numpy as np
 import pytest
 import torch
 
-from test_gpu_image_list import micro
+from engine_oracle import to_tensor
+from support import micro
 
 pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
@@ -30,8 +31,7 @@ def recipe(img, sigma, seed):
     """The dataset's img_lq of one (H, W, C) uint8 image on the CPU: to_tensor, then the float32 RandomState noise."""
     from grl_image_restoration_b200 import functional as F
 
-    a = img.cpu().numpy()
-    gt = torch.from_numpy(np.ascontiguousarray(a.transpose(2, 0, 1))).float().div(255)
+    gt = to_tensor(img).contiguous()
     key = F._awgn_keys([seed], 1, "recipe")[0]
     return gt + torch.from_numpy(np.random.RandomState(key).normal(0, sigma / 255, gt.shape)).float()
 

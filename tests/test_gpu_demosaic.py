@@ -1,34 +1,17 @@
 """Demosaicking on the GPU: the standalone kernel and the fused tensor-core head bit-exact against the library's host
 closed form and the unfused path; GRL(input_format="rggb") against GRL on the demosaiced image (bit for bit) and against
 the unmodified reference's dm pipeline (tests/golden/dm_*.npz); CUDA graphs, the x8 ensemble and tiled inference."""
-import json
-import os
-
 import pytest
 import torch
 
+from support import dm_model
+
 pytestmark = pytest.mark.gpu
-GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 NAMES = ["b2_40x56", "zero_pad_4x4", "odd_18x26"]
 
 
-def dm_cases():
-    with open(os.path.join(GOLD, "dm_cases.json")) as f:
-        return json.load(f)
-
-
-def build(pkg, oracle, device, precision="fp32", **kw):
-    cfg = dm_cases()["cfg"]
-    m = pkg.GRL(**cfg, **kw)
-    m.load_state_dict(oracle.synth_state_dict(cfg, seed=0, style="init"), strict=False)
-    m = m.to(device).eval()
-    m.set_precision(precision)
-    return m
-
-
 def pair(pkg, oracle, device, precision, **kw):
-    return (build(pkg, oracle, device, precision, input_format="rggb", **kw),
-            build(pkg, oracle, device, precision, **kw))
+    return dm_model(pkg, oracle, device, precision, **kw), dm_model(pkg, oracle, device, precision, "rgb", **kw)
 
 
 @pytest.mark.parametrize("h,w", [(2, 2), (5, 3), (9, 13), (16, 33), (40, 70), (33, 8)])
@@ -94,7 +77,7 @@ def test_rggb_forward_equals_forward_of_demosaiced(pkg, oracle, golden_loader, d
 @pytest.mark.parametrize("name", NAMES)
 def test_rggb_fp32_vs_reference(pkg, oracle, golden_loader, device, name):
     g = golden_loader(f"dm_{name}.npz")
-    m = build(pkg, oracle, device, "fp32", input_format="rggb")
+    m = dm_model(pkg, oracle, device, "fp32")
     y = m(g["cfa4"].to(device)).cpu()
     err = (y - g["output"]).abs().max().item()
     print(f"{name}: rggb fp32 max-abs vs reference dm pipeline = {err:.3e}")
@@ -107,7 +90,7 @@ def test_rggb_16bit_psnr_gate(pkg, oracle, golden_loader, device, name, precisio
     """The gate of the 16-bit end-to-end tests: |PSNR(cand, GT) - PSNR(ref, GT)| <= 0.01 dB, PSNR(cand, ref) >= 56 dB
     with fp16 operands (40 dB with bf16)."""
     g = golden_loader(f"dm_{name}.npz")
-    m = build(pkg, oracle, device, precision, input_format="rggb")
+    m = dm_model(pkg, oracle, device, precision)
     assert m.precision == precision
     y = m(g["cfa4"].to(device)).cpu()
     ref = g["output"]
@@ -126,7 +109,7 @@ def test_rggb_cuda_graph_matches_eager(pkg, oracle, golden_loader, device):
     a packed input and an RGB input of the same batch from different graphs."""
     from grl_image_restoration_b200 import functional as K
 
-    m = build(pkg, oracle, device, "fp16", input_format="rggb")
+    m = dm_model(pkg, oracle, device, "fp16")
     x1 = golden_loader("dm_b2_40x56.npz")["cfa4"].to(device)
     x2 = x1.flip(-1).contiguous()
     e1, e2 = m(x1).clone(), m(x2).clone()
@@ -172,7 +155,7 @@ def test_rggb_forward_tile_demosaics_the_whole_frame(pkg, oracle, golden_loader,
 
 
 def test_rggb_rejects_other_shapes(pkg, oracle, device):
-    m = build(pkg, oracle, device, "fp16", input_format="rggb")
+    m = dm_model(pkg, oracle, device, "fp16")
     for bad in ((1, 3, 8, 8), (1, 4, 1, 8), (4, 8, 8)):
         with pytest.raises(ValueError, match=r"\(B, 4, h, w\)"):
             m(torch.rand(*bad, device=device))

@@ -1,55 +1,14 @@
 """x8 self-ensemble on the GPU: the gather / merge kernels bit-exact against torch rot90 / flip, GRL(self_ensemble=True)
 against the unmodified reference's stored ensemble outputs (tests/golden/ensemble_*.npz) and against a Python loop of
 8 plain forwards of the same module, CUDA-graph replay, and tiled inference."""
-import json
-import os
-
 import pytest
 import torch
 
+from engine_oracle import augment, forward_tile, merge_reference
+from support import build, ensemble_cases, loop_ensemble
+
 pytestmark = pytest.mark.gpu
-GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 GATE = 1e-3  # fp32, BASELINE.json
-INVERSE = {3: 5, 5: 3}
-
-
-def augment(img, mode):
-    """augment_img_tensor4 (utils/utils_bsr/utils_image.py:444-460) restated with the same torch ops."""
-    ops = [lambda t: t, lambda t: t.rot90(1, [2, 3]).flip([2]), lambda t: t.flip([2]), lambda t: t.rot90(3, [2, 3]),
-           lambda t: t.rot90(2, [2, 3]).flip([2]), lambda t: t.rot90(1, [2, 3]), lambda t: t.rot90(2, [2, 3]),
-           lambda t: t.rot90(3, [2, 3]).flip([2])]
-    return ops[mode](img)
-
-
-def merge_reference(outs):
-    """outs[m] = view m's output: 0.125 * sequential fp32 sum of the mapped-back views in mode order."""
-    acc = None
-    for mode, o in enumerate(outs):
-        back = augment(o, INVERSE.get(mode, mode))
-        acc = back.clone() if acc is None else acc + back
-    return acc * 0.125
-
-
-def loop_ensemble(m, x):
-    """What a user writes without the feature: 8 plain forwards of the module, mapped back and averaged."""
-    flag, m.self_ensemble = m.self_ensemble, False
-    try:
-        return merge_reference([m(augment(x, mode).contiguous()) for mode in range(8)])
-    finally:
-        m.self_ensemble = flag
-
-
-def ensemble_cases():
-    with open(os.path.join(GOLD, "ensemble_cases.json")) as f:
-        return json.load(f)
-
-
-def build(pkg, oracle, cfg, device, precision="fp32", **kw):
-    m = pkg.GRL(**cfg, **kw)
-    m.load_state_dict(oracle.synth_state_dict(cfg, seed=0, style="init"), strict=False)
-    m = m.to(device).eval()
-    m.set_precision(precision)
-    return m
 
 
 @pytest.mark.parametrize("C", [1, 3, 6])
@@ -85,7 +44,7 @@ def test_merge_kernel_bit_exact(pkg, device, C, Hs, Ws):
 def test_self_ensemble_fp32_vs_reference(pkg, oracle, golden_loader, device, name):
     c = ensemble_cases()[name]
     g = golden_loader(f"ensemble_{name}.npz")
-    m = build(pkg, oracle, c["cfg"], device, self_ensemble=True)
+    m = build(pkg, oracle, c["cfg"], device, "fp32", style="init", self_ensemble=True)
     x = g["input"].to(device)
     y = m(x)
     assert y.dtype == x.dtype and y.device == x.device and y.is_contiguous()
@@ -102,7 +61,7 @@ def test_self_ensemble_16bit_psnr_gate(pkg, oracle, golden_loader, device, name,
     with fp16 operands (40 dB with bf16)."""
     c = ensemble_cases()[name]
     g = golden_loader(f"ensemble_{name}.npz")
-    m = build(pkg, oracle, c["cfg"], device, precision, self_ensemble=True)
+    m = build(pkg, oracle, c["cfg"], device, precision, style="init", self_ensemble=True)
     assert m.precision == precision
     y = m(g["input"].to(device)).cpu()
     ref = g["merged"]
@@ -123,7 +82,7 @@ def test_self_ensemble_16bit_psnr_gate(pkg, oracle, golden_loader, device, name,
 def test_self_ensemble_equals_loop_of_plain_forwards(pkg, oracle, device, precision, hw):
     """Non-square (two view batches) and square (one shared view batch) inputs, 2 images each."""
     cfg = pkg.configs.micro_config()
-    m = build(pkg, oracle, cfg, device, precision, self_ensemble=True)
+    m = build(pkg, oracle, cfg, device, precision, style="init", self_ensemble=True)
     x = oracle.synth_input((2, 3, *hw), seed=21).to(device)
     ref = loop_ensemble(m, x)
     for mb in (1, 16):
@@ -138,8 +97,8 @@ def test_self_ensemble_off_is_the_plain_forward(pkg, oracle, device):
     cfg = pkg.configs.micro_config()
     x = oracle.synth_input((2, 3, 28, 44), seed=3).to(device)
     for precision in ("fp32", "fp16"):
-        plain = build(pkg, oracle, cfg, device, precision)
-        off = build(pkg, oracle, cfg, device, precision, self_ensemble=False)
+        plain = build(pkg, oracle, cfg, device, precision, style="init")
+        off = build(pkg, oracle, cfg, device, precision, style="init", self_ensemble=False)
         assert torch.equal(plain(x), off(x))
         off.self_ensemble = True
         assert not torch.equal(plain(x), off(x))
@@ -149,7 +108,7 @@ def test_self_ensemble_cuda_graph_matches_eager(pkg, oracle, device):
     """Each view chunk shape gets its own captured graph (3 + 3 + 2 views here); gather and merge run outside the graphs.
     The result is a fresh tensor: mutating it leaves the next call untouched."""
     cfg = pkg.configs.micro_config()
-    m = build(pkg, oracle, cfg, device, "fp16", self_ensemble=True)
+    m = build(pkg, oracle, cfg, device, "fp16", style="init", self_ensemble=True)
     m.ensemble_max_batch = 3
     x1 = oracle.synth_input((1, 3, 32, 32), seed=5).to(device)
     x2 = oracle.synth_input((1, 3, 32, 32), seed=6).to(device)
@@ -163,39 +122,20 @@ def test_self_ensemble_cuda_graph_matches_eager(pkg, oracle, device):
     assert len(m._graphs) == 2
 
 
-def reference_forward_tile(fn, x, tile, overlap, scale):
-    """engines/base.py:90-116 restated with `fn` as the model call."""
-    b, c, h, w = x.shape
-    tile = min(tile, h, w)
-    stride = tile - overlap
-    h_idx = list(range(0, h - tile, stride)) + [h - tile]
-    w_idx = list(range(0, w - tile, stride)) + [w - tile]
-    E = W = None
-    for hi in h_idx:
-        for wi in w_idx:
-            out = fn(x[..., hi:hi + tile, wi:wi + tile])
-            if E is None:
-                E = torch.zeros(b, out.shape[1], h * scale, w * scale)
-                W = torch.zeros_like(E)
-            E[..., hi * scale:(hi + tile) * scale, wi * scale:(wi + tile) * scale] += out
-            W[..., hi * scale:(hi + tile) * scale, wi * scale:(wi + tile) * scale] += 1
-    return E / W
-
-
 @pytest.mark.parametrize("precision,tol", [("fp32", 1e-3), ("fp16", 2e-2)])
 def test_forward_tile_ensembles_every_tile(pkg, oracle, device, precision, tol):
     from grl_image_restoration_b200 import tiling
 
     cfg = pkg.configs.micro_config(img_size=32, upscale=2)
     sd = oracle.synth_state_dict(cfg, seed=0, style="init")
-    m = build(pkg, oracle, cfg, device, precision, self_ensemble=True)
+    m = build(pkg, oracle, cfg, device, precision, style="init", self_ensemble=True)
     x = oracle.synth_input((2, 3, 40, 56), seed=11)
 
     def x8_oracle(t):
         with torch.no_grad():
             return merge_reference([oracle.grl_forward(sd, cfg, augment(t, mode).contiguous()) for mode in range(8)])
 
-    ref = reference_forward_tile(x8_oracle, x, 32, 8, 2)
+    ref = forward_tile(x8_oracle, x, 32, 8, 2)
     y = tiling.forward_tile(m, x.to(device), 32, 8, max_batch=5).cpu()
     err = (y - ref).abs().max().item()
     print(f"forward_tile x8 [{precision}]: max-abs vs per-tile x8 reference loop = {err:.3e}")

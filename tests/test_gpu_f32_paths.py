@@ -42,20 +42,17 @@ import torch.nn.functional as F
 
 import archs
 import grl_oracle as O
+from grl_oracle import L_LN, U, gamma, ln_bound, ln_reference
+from support import bound_ratio, grid_t, ulp
 
 B = 2
 GUARD = 3          # NaN guard rows before and after every output buffer
-U = 2.0 ** -24     # fp32 unit roundoff
 ERFF_ULP = 2       # CUDA C++ Programming Guide, maximum ulp error of erff / expf (no fast math)
 EXPF_ULP = 2
 OLD_TOL = 2e-4     # the max-abs bound of the operator tests this file replaces
 GATE_ATTN = 1695.0   # fp32 ulps at max(|ref|, row rms): 2 x the worst case, 847.2 (small/sr window; H100 80GB HBM3, 400 W)
 GATE_CHAIN = 2165.0  # both stripe passes against the float64 chain: 2 x the worst case, 1082.3 (same card)
 ACT_NONE, ACT_GELU, ACT_LEAKY = 0, 1, 2
-
-
-def gamma(n):
-    return n * U / (1 - n * U)
 
 
 def launches_of(launches, kind):
@@ -317,20 +314,10 @@ def check_written(buf, cols, what, guard_cols=0):
         assert bool(inner[:, cols:].isnan().all()), f"{what}: wrote into the guard columns"
 
 
-def ulp32(x):
-    return torch.clamp(torch.finfo(torch.float32).eps * torch.exp2((torch.frexp(x.abs())[1] - 1).double()),
-                       min=2.0 ** -149)
-
-
 def ulp_stats(got, ref):
     """max |got - ref| in fp32 ulps at max(|ref|, the row's rms) (rows: the last dimension)."""
     scale = torch.maximum(ref.abs(), ref.pow(2).mean(-1, keepdim=True).sqrt())
-    return float(((got.double() - ref).abs() / ulp32(scale)).nan_to_num(float("inf")).max())
-
-
-def bound_ratio(got, ref, bound):
-    """max |got - ref| / bound (inf where either side is NaN)."""
-    return float(((got.double() - ref).abs() / bound).nan_to_num(float("inf")).max())
+    return float(((got.double() - ref).abs() / ulp(scale, torch.float32)).nan_to_num(float("inf")).max())
 
 
 def old_misses(mut, ref):
@@ -345,10 +332,6 @@ def report(name, ratio, gate, kind="bound"):
 
 
 # --------------------------------------------------------------------------------------------------- GPU: attention
-
-
-def grid_t(g):
-    return (g.H, g.W, g.wh, g.ww, g.sh, g.sw)
 
 
 def windows(t, g, heads):
@@ -684,58 +667,7 @@ def test_gemm_path(lib, device, case):
 # ------------------------------------------------------------------------------------------- GPU: LayerNorm residual
 
 
-L_LN = 100  # 8-row blocks: the image boundary at row 100 lies inside the block of rows 96..103
 HIGH_MEAN_ROWS, LOW_STD_ROWS = (5, 133), (7, 150)
-
-
-def ln_reference(u, gamma_, beta, eps, rs, x, cy, gate, mutation=None):
-    C = u.shape[1]
-    if mutation == "naive fp32 E[x^2] - E[x]^2":
-        u32 = u.float()
-        mean32 = u32.mean(1, keepdim=True)
-        mean, var = mean32.double(), ((u32 * u32).mean(1, keepdim=True) - mean32 * mean32).double()
-    else:
-        mean = u.mean(1, keepdim=True)
-        var = (u - mean).pow(2).sum(1, keepdim=True) / (C - 1 if mutation == "n - 1 variance" else C)
-    e = 0.0 if mutation == "no eps" else eps
-    r = (u - mean) / torch.sqrt(var + e) * gamma_ + beta
-    r = r * (1.0 if mutation == "res_scale dropped" else rs)
-    if x is not None:
-        r = r + x
-    if cy is not None:
-        rows = torch.arange(u.shape[0], device=u.device)
-        if mutation == "CAB gate of the wrong image at the boundary":
-            rows = rows // 8 * 8  # every row of an 8-row block takes the image of the block's first row
-        r = r + cy * gate[rows // L_LN]
-    return r
-
-
-def ln_bound(u, gamma_, beta, eps, rs, x, cy, gate):
-    """Per-element bound: two-pass moments over C, each a lane-strided sequential sum plus a 5-level warp tree."""
-    C = u.shape[1]
-    ns = -(-C // 32) + 5
-    mean = u.mean(1, keepdim=True)
-    e_mean = gamma(ns) * u.abs().sum(1, keepdim=True) / C + U * mean.abs()
-    d = u - mean
-    var = d.pow(2).mean(1, keepdim=True)
-    # the deviations carry the common mean error (its cross term sums to zero) and one rounding each
-    e_var = e_mean ** 2 + (var + e_mean ** 2) * (gamma(ns) + 4 * U)
-    rel_v = (e_var + U * (var + eps)) / (var + eps)
-    rel_r = 0.5 * rel_v * (1 + rel_v) + 2.5 * U  # sqrt, reciprocal
-    rstd = 1 / torch.sqrt(var + eps)
-    n = d * rstd
-    e_n = (e_mean + U * (d.abs() + e_mean)) * rstd + n.abs() * (rel_r + U)
-    t = n * gamma_ + beta
-    e = gamma_.abs() * e_n + U * ((n * gamma_).abs() + t.abs())
-    r = t * rs
-    e = abs(rs) * e + U * r.abs()
-    if x is not None:
-        r = r + x
-        e = e + U * r.abs()
-    if cy is not None:
-        cg = cy * gate[torch.arange(u.shape[0], device=u.device) // L_LN]
-        e = e + U * (cg.abs() + (r + cg).abs())
-    return e * (1 + 1e-6)
 
 
 LN_CASES = [(C, with_x, cab) for C in (64, 128, 180) for with_x, cab in ((False, False), (True, False), (True, True))]

@@ -3,34 +3,13 @@ against check_image_size / to_tensor / demosaic and slices / tensor_round, and G
 bit for bit, to the loop of B = 1 forwards they replace, on every precision, input format, CUDA-graph and self-ensemble
 setting.  A forward of a batch gives each image what its own forward gives, so any difference here is a kernel whose
 result depends on the rest of the batch."""
-import json
-import os
-
 import pytest
 import torch
-import torch.nn.functional as F
+
+from engine_oracle import check_image_size, to_tensor
+from support import MICRO, assert_equal_lists, build, count_calls, dm_model, micro, random_images, round8_ref
 
 pytestmark = pytest.mark.gpu
-GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
-
-
-def pad_to(x, Hp, Wp):
-    """check_image_size of x (1, C, H, W) padded to (Hp, Wp) (grl.py:479-489): reflect, or zeros when F.pad refuses."""
-    pads = (0, Wp - x.shape[3], 0, Hp - x.shape[2])
-    try:
-        return F.pad(x, pads, "reflect")
-    except BaseException:
-        return F.pad(x, pads, "constant")
-
-
-def to_tensor(img):
-    """(H, W, C) uint8 -> (C, H, W) k / 255 as the datasets compute it, on the CPU."""
-    return img.cpu().permute(2, 0, 1).float().div(255)
-
-
-def round8_ref(v):
-    """(C, H, W) float -> (H, W, C) uint8: tensor_round times 255, NaN -> 0 (grl_image_u8.h)."""
-    return (v.nan_to_num(nan=0.0).clamp(0, 1) * 255).round().byte().permute(1, 2, 0)
 
 
 # sizes against a (48, 40) batch: 1 x 1, a pad >= size on one axis only (zeros on both), the exact batch size, odd sizes,
@@ -56,10 +35,10 @@ def test_gather_bit_exact(pkg, device, C, u8):
     g = torch.Generator().manual_seed(C)
     if u8:
         imgs = [torch.randint(0, 256, (h, w, C), dtype=torch.uint8, generator=g).to(device) for h, w in sizes]
-        refs = [pad_to(to_tensor(x)[None], Hp, Wp)[0] for x in imgs]
+        refs = [check_image_size(to_tensor(x)[None], Hp, Wp)[0] for x in imgs]
     else:
         imgs = [(torch.randn(C, h, w, generator=g) * 2).to(device) for h, w in sizes]
-        refs = [pad_to(x[None].cpu(), Hp, Wp)[0] for x in imgs]
+        refs = [check_image_size(x[None].cpu(), Hp, Wp)[0] for x in imgs]
     out = K.list_gather(imgs, capi.IMAGE_U8 if u8 else capi.IMAGE_F32, C, Hp, Wp)
     assert out.shape == (130, C, Hp, Wp) and out.dtype == torch.float32
     out = out.cpu()
@@ -91,7 +70,7 @@ def test_gather_rggb_equals_padded_demosaic(pkg, device):
     cfa = [torch.rand(4, h, w, generator=g).to(device) for h, w in packed]
     out = K.list_gather(cfa, capi.IMAGE_RGGB, 3, Hp, Wp)
     for i, x in enumerate(cfa):
-        assert torch.equal(out[i:i + 1], pad_to(K.demosaic(x[None]), Hp, Wp)), (i, packed[i])
+        assert torch.equal(out[i:i + 1], check_image_size(K.demosaic(x[None]), Hp, Wp)), (i, packed[i])
 
 
 @pytest.mark.parametrize("C", [1, 3, 6])
@@ -115,54 +94,8 @@ def test_crop_bit_exact(pkg, device, C, u8):
 
 
 # ------------------------------------------------------------------------------------------ end to end
-MICRO = {  # the micro configs of test_gpu_image_u8.py: upscaling with CAB, denoising with the input residual, grayscale
-    "micro_cab_x2": dict(),
-    "micro_pad_dn": dict(embed_dim=36, stripe=(8, 16), df=2, upsampler="", upscale=1, img_size=32),
-    "micro_gray": dict(embed_dim=32, heads=1, window=6, stripe=(6, 12), df=3, local_connection=False, upsampler="",
-                       upscale=1, img_size=24, in_channels=1),
-    "micro_dual": dict(upsampler="", upscale=1, in_channels=6),  # 6 channels in (dual-pixel views), 3 out
-}
 # several buckets, repeats of one bucket, both orientations, zero padding on one axis, a 1-pixel-wide image
 SIZES = [(24, 40), (40, 24), (17, 30), (24, 40), (9, 9), (30, 5), (33, 20), (20, 33), (1, 12), (16, 16)]
-
-
-def build(pkg, oracle, cfg, device, precision, **kw):
-    m = pkg.GRL(**cfg, **kw)
-    m.load_state_dict(oracle.synth_state_dict(cfg, seed=0, style="init"), strict=False)
-    m = m.to(device).eval()
-    m.set_precision(precision)
-    return m
-
-
-def micro(pkg, oracle, name, device, precision, **kw):
-    cfg = pkg.configs.micro_config(**MICRO[name])
-    if name == "micro_dual":
-        cfg["out_channels"] = 3
-    return build(pkg, oracle, cfg, device, precision, **kw)
-
-
-def images(shape_of, sizes, seed, device, dtype=torch.float32):
-    g = torch.Generator().manual_seed(seed)
-    return [torch.rand(shape_of(h, w), generator=g).to(device=device, dtype=dtype) for h, w in sizes]
-
-
-def assert_equal_lists(got, want):
-    assert len(got) == len(want)
-    for i, (a, b) in enumerate(zip(got, want)):
-        assert a.shape == b.shape and a.dtype == b.dtype, (i, a.shape, b.shape, a.dtype, b.dtype)
-        assert torch.equal(a, b), (i, (a.float() - b.float()).abs().max().item())
-
-
-def count_forwards(m):
-    calls = []
-    inner = m._forward_once
-
-    def wrapped(x, rggb=False):
-        calls.append(tuple(x.shape))
-        return inner(x, rggb)
-
-    m._forward_once = wrapped
-    return calls
 
 
 @pytest.mark.parametrize("name", list(MICRO))
@@ -174,10 +107,10 @@ def test_forward_list_equals_loop(pkg, oracle, device, name, precision, ensemble
 
     m = micro(pkg, oracle, name, device, precision, self_ensemble=ensemble)
     m.use_cuda_graph = graph
-    xs = images(lambda h, w: (m.in_channels, h, w), SIZES, list(MICRO).index(name), device)
+    xs = random_images(lambda h, w: (m.in_channels, h, w), SIZES, list(MICRO).index(name), device)
     kept = [x.clone() for x in xs]
     want = [m(x[None])[0] for x in xs]
-    calls = count_forwards(m)
+    calls = count_calls(m, "_forward_once")
     got = m.forward_list(xs)
     assert_equal_lists(got, want)
     assert all(torch.equal(a, b) for a, b in zip(xs, kept)), "forward_list changed its inputs"
@@ -194,10 +127,10 @@ def test_forward_list_equals_loop(pkg, oracle, device, name, precision, ensemble
 def test_forward_list_splits_a_bucket_at_the_budget(pkg, oracle, device, precision):
     m = micro(pkg, oracle, "micro_cab_x2", device, precision)
     sizes = [(24, 40), (20, 33), (32, 48), (24, 40), (30, 35), (17, 40), (32, 33)]  # all pad to 32 x 48
-    xs = images(lambda h, w: (3, h, w), sizes, 11, device)
+    xs = random_images(lambda h, w: (3, h, w), sizes, 11, device)
     want = [m(x[None])[0] for x in xs]
     m.max_batch_tokens = 3 * 32 * 48
-    calls = count_forwards(m)
+    calls = count_calls(m, "_forward_once")
     assert_equal_lists(m.forward_list(xs), want)
     assert [c[0] for c in calls] == [3, 3, 1]
 
@@ -207,14 +140,8 @@ def test_forward_list_splits_a_bucket_at_the_budget(pkg, oracle, device, precisi
 def test_forward_list_other_float_dtypes(pkg, oracle, device, precision, dtype):
     """Half-precision inputs give the dtype and the bits of the image's own forward."""
     m = micro(pkg, oracle, "micro_pad_dn", device, precision)
-    xs = images(lambda h, w: (3, h, w), SIZES[:6], 2, device, dtype)
+    xs = random_images(lambda h, w: (3, h, w), SIZES[:6], 2, device, dtype)
     assert_equal_lists(m.forward_list(xs), [m(x[None])[0] for x in xs])
-
-
-def dm_model(pkg, oracle, device, precision, **kw):
-    with open(os.path.join(GOLD, "dm_cases.json")) as f:
-        cfg = json.load(f)["cfg"]
-    return build(pkg, oracle, cfg, device, precision, input_format="rggb", **kw)
 
 
 @pytest.mark.parametrize("precision,ensemble,graph", [("fp32", False, False), ("fp16", False, False),
@@ -224,9 +151,9 @@ def test_forward_list_rggb(pkg, oracle, device, precision, ensemble, graph):
     m = dm_model(pkg, oracle, device, precision, self_ensemble=ensemble)
     m.use_cuda_graph = graph
     packed = [(10, 14), (9, 13), (2, 2), (10, 14), (14, 10), (20, 28), (16, 3)]
-    xs = images(lambda h, w: (4, h, w), packed, 4, device)
+    xs = random_images(lambda h, w: (4, h, w), packed, 4, device)
     want = [m(x[None])[0] for x in xs]
-    calls = count_forwards(m)
+    calls = count_calls(m, "_forward_once")
     got = m.forward_list(xs)
     assert_equal_lists(got, want)
     assert got[0].shape == (3, 20, 28)
@@ -255,7 +182,7 @@ def test_cuda_graphs_of_several_resolutions_replay_exactly(pkg, oracle, device):
     """Each block caches its attention constants for the last resolution it ran; a captured graph reads them at their
     address, so it must keep them alive when a forward at another resolution replaces the cache."""
     m = micro(pkg, oracle, "micro_cab_x2", device, "fp16")
-    xs = images(lambda h, w: (3, 1, h, w), [(32, 48), (48, 32), (16, 16), (32, 32)], 12, device)
+    xs = random_images(lambda h, w: (3, 1, h, w), [(32, 48), (48, 32), (16, 16), (32, 32)], 12, device)
     eager = [m(x) for x in xs]
     m.use_cuda_graph = True
     for _ in range(2):
@@ -269,10 +196,10 @@ def test_cuda_graphs_of_several_resolutions_replay_exactly(pkg, oracle, device):
 def test_forward_list_base_x4_b100_sizes(pkg, oracle, device):
     """The released GRL-Base x4 SR architecture on whole B100-sized images: both orientations share one forward."""
     cfg = pkg.configs.grl_config("base", "sr", 4, 64)
-    m = build(pkg, oracle, cfg, device, "fp16")
-    xs = images(lambda h, w: (3, h, w), [(120, 80), (80, 120), (120, 80)], 21, device)
+    m = build(pkg, oracle, cfg, device, "fp16", style="init")
+    xs = random_images(lambda h, w: (3, h, w), [(120, 80), (80, 120), (120, 80)], 21, device)
     want = [m(x[None])[0] for x in xs]
-    calls = count_forwards(m)
+    calls = count_calls(m, "_forward_once")
     got = m.forward_list(xs)
     assert calls == [(3, 3, 128, 128)]
     assert_equal_lists(got, want)

@@ -12,6 +12,9 @@ import numpy as np
 import pytest
 import torch
 
+from engine_oracle import to_tensor
+from support import micro, round8_ref, same_bits
+
 pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
@@ -21,16 +24,6 @@ def random_u8(shape, seed, device):
     ends = torch.tensor([255, 0], dtype=torch.uint8)
     img.view(-1)[: min(2, img.numel())] = ends[: min(2, img.numel())]
     return img.to(device)
-
-
-def to_tensor(img):
-    """(B, H, W, C) uint8 -> (B, C, H, W) k / 255, as the datasets compute it (on the CPU), moved to img's device."""
-    return img.cpu().permute(0, 3, 1, 2).float().div(255).to(img.device)
-
-
-def tensor_round_bytes(y):
-    """(B, C, H, W) float -> (B, H, W, C) uint8: tensor_round times 255 (defined where y is not NaN)."""
-    return (y.clamp(0, 1) * 255).round().byte().permute(0, 2, 3, 1)
 
 
 SIZES = [(1, 1), (17, 33), (257, 130)]
@@ -45,7 +38,7 @@ def test_u8_to_f32_bit_exact(pkg, device, B, C, H, W):
     img = random_u8((B, H, W, C), B * 1000 + C * 100 + H, device)
     y = K.u8_to_f32(img)
     assert y.dtype == torch.float32 and y.shape == (B, C, H, W) and y.is_contiguous()
-    assert torch.equal(y.cpu(), to_tensor(img).cpu())
+    assert torch.equal(y.cpu(), to_tensor(img))
     # a non-contiguous input is read as its values
     assert torch.equal(K.u8_to_f32(img.transpose(1, 2).contiguous().transpose(1, 2)), y)
 
@@ -68,7 +61,7 @@ def test_f32_to_u8_bit_exact(pkg, device, B, C, H, W):
     assert out.dtype == torch.uint8 and out.shape == (B, H, W, C) and out.is_contiguous()
     out = out.cpu()
     nan = v.isnan().permute(0, 2, 3, 1)
-    want = tensor_round_bytes(v)
+    want = round8_ref(v)
     assert torch.equal(out[~nan], want[~nan])
     assert (out[nan] == 0).all()
     # round trip
@@ -89,37 +82,22 @@ def test_conversions_reject_bad_input(pkg, device):
         K.f32_to_u8(torch.zeros(1, 3, 4, device=device))
 
 
-# (cfg kwargs of configs.micro_config, input (B, H, W)): an upscaling, a denoising and the grayscale micro config of
-# tests/golden/cases.json
-MODELS = {
-    "micro_cab_x2": (dict(), (2, 24, 40)),
-    "micro_pad_dn": (dict(embed_dim=36, stripe=(8, 16), df=2, upsampler="", upscale=1, img_size=32), (1, 24, 40)),
-    "micro_gray": (dict(embed_dim=32, heads=1, window=6, stripe=(6, 12), df=3, local_connection=False, upsampler="",
-                        upscale=1, img_size=24, in_channels=1), (1, 24, 24)),
-}
+# input (B, H, W) of an upscaling, a denoising and the grayscale micro config of tests/golden/cases.json
+INPUTS = {"micro_cab_x2": (2, 24, 40), "micro_pad_dn": (1, 24, 40), "micro_gray": (1, 24, 24)}
 
 
-def build(pkg, oracle, name, device, precision, **kw):
-    cfg = pkg.configs.micro_config(**MODELS[name][0])
-    m = pkg.GRL(**cfg, **kw)
-    m.load_state_dict(oracle.synth_state_dict(cfg, seed=0, style="init"), strict=False)
-    m = m.to(device).eval()
-    m.set_precision(precision)
-    return m
-
-
-@pytest.mark.parametrize("name", list(MODELS))
+@pytest.mark.parametrize("name", list(INPUTS))
 @pytest.mark.parametrize("precision,ensemble,graph", [("fp32", False, False), ("fp32", True, False), ("fp16", False, False),
                                                       ("fp16", True, False), ("fp16", False, True)])
 def test_forward_u8_equals_torch_composition(pkg, oracle, device, name, precision, ensemble, graph):
-    m = build(pkg, oracle, name, device, precision, self_ensemble=ensemble)
+    m = micro(pkg, oracle, name, device, precision, self_ensemble=ensemble)
     m.use_cuda_graph = graph
-    B, H, W = MODELS[name][1]
-    img = random_u8((B, H, W, m.in_channels), list(MODELS).index(name), device)
+    B, H, W = INPUTS[name]
+    img = random_u8((B, H, W, m.in_channels), list(INPUTS).index(name), device)
     out = m.forward_u8(img)
     s = m.upscale
     assert out.dtype == torch.uint8 and out.shape == (B, H * s, W * s, m.out_channels) and out.is_contiguous()
-    want = tensor_round_bytes(m.forward_rgb(to_tensor(img)))
+    want = round8_ref(m.forward_rgb(to_tensor(img).to(device)))
     assert torch.equal(out, want)
     if graph:
         assert m._graphs, "the forward must have replayed a captured graph"
@@ -131,10 +109,10 @@ def test_forward_u8_equals_torch_composition(pkg, oracle, device, name, precisio
 def test_forward_tile_u8_equals_torch_composition(pkg, oracle, device):
     from grl_image_restoration_b200 import tiling
 
-    m = build(pkg, oracle, "micro_cab_x2", device, "fp16")
+    m = micro(pkg, oracle, "micro_cab_x2", device, "fp16")
     img = random_u8((2, 40, 56, 3), 7, device)
     out = tiling.forward_tile_u8(m, img, 32, 8, max_batch=5)
-    want = tensor_round_bytes(tiling.forward_tile(m, to_tensor(img), 32, 8, max_batch=5))
+    want = round8_ref(tiling.forward_tile(m, to_tensor(img).to(device), 32, 8, max_batch=5))
     assert out.shape == (2, 80, 112, 3) and out.dtype == torch.uint8
     assert torch.equal(out, want)
 
@@ -147,11 +125,6 @@ def pair(shape_hwc, seed, device):
     noise = torch.randint(-12, 13, shape_hwc, generator=torch.Generator().manual_seed(seed + 1)).to(device)
     a = (b.short() + noise).clamp(0, 255).byte()
     return a, b, K.u8_to_f32(a), K.u8_to_f32(b)
-
-
-def same(x, y):
-    """Bit-for-bit equality that lets NaN stand where NaN stands."""
-    return torch.equal(x.isnan(), y.isnan()) and torch.equal(x.nan_to_num(), y.nan_to_num())
 
 
 @pytest.mark.parametrize("C", [1, 3])
@@ -184,10 +157,11 @@ def test_niqe_u8_equals_f32(pkg, device, shape, border):
 
     params = dict(np.load(os.path.join(GOLD, "niqe_pris_params.npz")))
     a, _, fa, _ = pair(shape + (3,), shape[1] + border, device)
-    assert same(metrics.niqe_features(a, params, border), metrics.niqe_features(fa, params, border))
-    assert same(metrics.niqe(a, params, border), metrics.niqe(fa, params, border))
+    same_bits(metrics.niqe_features(a, params, border), metrics.niqe_features(fa, params, border))
+    same_bits(metrics.niqe(a, params, border), metrics.niqe(fa, params, border))
     su, sf = metrics.niqe_stages(a, params, border), metrics.niqe_stages(fa, params, border)
-    assert all(same(su[k], sf[k]) for k in sf)
+    for k in sf:
+        same_bits(su[k], sf[k])
 
 
 def test_metrics_refuse_mixed_dtypes_and_bad_shapes(pkg, device):

@@ -3,15 +3,9 @@ with the reference's PSNR definition (tensor_round + shave + per-image mean), an
 import pytest
 import torch
 
+from support import build
+
 pytestmark = pytest.mark.gpu
-
-
-def build(pkg, oracle, cfg, device, seed=0, precision="fp16", style="spread"):
-    m = pkg.GRL(**cfg)
-    m.load_state_dict(oracle.synth_state_dict(cfg, seed=seed, style=style), strict=False)
-    m = m.to(device).eval()
-    m.set_precision(precision)
-    return m
 
 
 def test_block_and_stage_bf16_vs_reference_taps(pkg, oracle, cases, golden_loader, device):
@@ -19,7 +13,7 @@ def test_block_and_stage_bf16_vs_reference_taps(pkg, oracle, cases, golden_loade
     gold = golden_loader("model_micro_cab_x2.npz")
     for bi in range(4):
         gold.update(golden_loader(f"model_micro_cab_x2_block{bi}.npz"))
-    m = build(pkg, oracle, cfg, device)
+    m = build(pkg, oracle, cfg, device, "fp16", style="spread")
     assert m.precision == "fp16"
     hw = (16, 32)
     xb = gold["block_input"].to(device)
@@ -45,7 +39,7 @@ def test_psnr_gate_vs_oracle(pkg, oracle, device, variant, task, scale, size, hw
     fp16 operands must meet the 0.01 dB gate with PSNR(cand, ref) >= 56 dB (SURVEY.md 8d); bf16 operands are
     reported (they cannot: 8-bit mantissas give ~45-50 dB, as SURVEY.md section 7 predicted)."""
     cfg = pkg.configs.grl_config(variant, task, scale, size)
-    m = build(pkg, oracle, cfg, device, seed=3, precision=precision, style="init")
+    m = build(pkg, oracle, cfg, device, precision, style="init", seed=3)
     sd = oracle.synth_state_dict(cfg, seed=3, style="init")
     x = oracle.synth_input((1, 3, *hw), seed=77, noise_sigma=50.0 if task == "dn" else 0.0)
     with torch.no_grad():
@@ -66,7 +60,7 @@ def test_harsh_weights_report(pkg, oracle, device, variant, task, scale, size, h
     """The "spread" synthetic weights (logit scales up to the clamp at 100, random LayerNorm affine) make the network
     near-chaotic; reported for transparency with a loose sanity bound."""
     cfg = pkg.configs.grl_config(variant, task, scale, size)
-    m = build(pkg, oracle, cfg, device, seed=3, precision="fp16")
+    m = build(pkg, oracle, cfg, device, "fp16", style="spread", seed=3)
     sd = oracle.synth_state_dict(cfg, seed=3)
     x = oracle.synth_input((1, 3, *hw), seed=77)
     with torch.no_grad():
@@ -81,7 +75,7 @@ def test_fp16_fp32_switch(pkg, oracle, device):
     """Switching one model from the fp16 tensor-core path to the fp32 path.  (Batch composition, bit for bit, is
     test_gpu_tc_scale.py::test_batch_composition_bitwise.)"""
     cfg = pkg.configs.grl_config("base", "sr", 4, 256)
-    m = build(pkg, oracle, cfg, device, seed=1, style="init")
+    m = build(pkg, oracle, cfg, device, "fp16", style="init", seed=1)
     x = oracle.synth_input((1, 3, 256, 256), seed=1234).to(device)
     y = m(x)
     assert y.shape == (1, 3, 1024, 1024) and torch.isfinite(y).all()
@@ -132,7 +126,7 @@ def test_cuda_graph_replay_matches_eager(pkg, oracle, device):
     sequence, for new inputs of the captured shape, a second shape gets its own graph, and the caller may mutate the
     result in place (engines/base.py:113) without touching the graph's static buffers."""
     cfg = pkg.configs.grl_config("base", "sr", 4, 64)
-    m = build(pkg, oracle, cfg, device, seed=3, precision="fp16", style="init")
+    m = build(pkg, oracle, cfg, device, "fp16", style="init", seed=3)
     x1 = oracle.synth_input((2, 3, 64, 64), seed=5).to(device)
     x2 = oracle.synth_input((2, 3, 64, 64), seed=6).to(device)
     e1, e2 = m(x1).clone(), m(x2).clone()

@@ -3,15 +3,10 @@ tests/golden, (b) the CPU oracle on fresh seeds.  Gate from BASELINE.json: <= 1e
 import pytest
 import torch
 
+from support import build
+
 pytestmark = pytest.mark.gpu
 GATE = 1e-3
-
-
-def build(pkg, oracle, cfg, device, seed=0):
-    m = pkg.GRL(**cfg)
-    missing, unexpected = m.load_state_dict(oracle.synth_state_dict(cfg, seed=seed), strict=False)
-    assert not unexpected and all(k.startswith("table_") for k in missing)
-    return m.to(device).eval()
 
 
 @pytest.mark.parametrize("name", ["cfg1_tiny_x2_64", "micro_cab_x2", "micro_pad_dn", "micro_groups", "micro_odd_d",
@@ -19,7 +14,7 @@ def build(pkg, oracle, cfg, device, seed=0):
 def test_golden_reference_outputs(pkg, oracle, cases, golden_loader, device, name):
     c = cases[name]
     cfg = c["cfg"]
-    m = build(pkg, oracle, cfg, device)
+    m = build(pkg, oracle, cfg, device, "fp32", style="spread")
     x = oracle.synth_input((c["batch"], cfg["in_channels"], *c["hw"]), seed=1234, noise_sigma=c["sigma"])
     y = m(x.to(device)).cpu()
     ref = golden_loader(f"model_{name}.npz")["output"]
@@ -34,7 +29,7 @@ def test_golden_reference_outputs(pkg, oracle, cases, golden_loader, device, nam
                                                         ("tiny", "deblur", 1, 96, (96, 96))])
 def test_released_configs_vs_oracle(pkg, oracle, device, variant, task, scale, size, hw):
     cfg = pkg.configs.grl_config(variant, task, scale, size)
-    m = build(pkg, oracle, cfg, device, seed=3)
+    m = build(pkg, oracle, cfg, device, "fp32", style="spread", seed=3)
     sd = oracle.synth_state_dict(cfg, seed=3)
     x = oracle.synth_input((1, 3, *hw), seed=77, noise_sigma=50.0 if task == "dn" else 0.0)
     with torch.no_grad():
@@ -50,7 +45,7 @@ def test_full_size_properties_base_sr_256(pkg, oracle, device):
     """BASELINE cfg4 geometry (GRL-Base x4, 256x256 tiles): size-independent properties instead of a 2-minute CPU
     oracle run -- batch invariance (tiles are independent), determinism, finite output, output shape."""
     cfg = pkg.configs.grl_config("base", "sr", 4, 256)
-    m = build(pkg, oracle, cfg, device, seed=1)
+    m = build(pkg, oracle, cfg, device, "fp32", style="spread", seed=1)
     x = oracle.synth_input((2, 3, 256, 256), seed=1234).to(device)
     y = m(x)
     assert y.shape == (2, 3, 1024, 1024) and torch.isfinite(y).all()
@@ -65,7 +60,7 @@ def test_resolution_change_and_engine_contract(pkg, oracle, device):
     """img_size != input size (tables rebuilt on the fly, grl.py:449-453), output is a fresh contiguous tensor the
     caller may mutate in place (engines/base.py:113, utils_image.py:31)."""
     cfg = pkg.configs.micro_config(img_size=32)
-    m = build(pkg, oracle, cfg, device)
+    m = build(pkg, oracle, cfg, device, "fp32", style="spread")
     sd = oracle.synth_state_dict(cfg, seed=0)
     x = oracle.synth_input((1, 3, 48, 80), seed=5)
     with torch.no_grad():

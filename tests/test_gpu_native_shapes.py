@@ -12,15 +12,11 @@ import numpy as np
 import pytest
 import torch
 
+from support import build, native_model
+
 pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
-SHAPES = {  # must match oracle/make_golden_native.py
-    "cfg2": ("small", "sr", 4, 256, (256, 256), 0.0),
-    "cfg3": ("base", "dn", 1, 256, (256, 256), 50.0),
-    "cfg4": ("base", "sr", 4, 256, (256, 256), 0.0),
-    "cfg5": ("base", "deblur", 1, 480, (480, 480), 0.0),
-}
 GT_SEED = 9
 
 
@@ -29,18 +25,6 @@ def load(case):
     if not os.path.exists(path):
         pytest.skip(f"{path} not generated")
     return np.load(path)
-
-
-def build(pkg, oracle, shape_name, style, device, precision):
-    variant, task, scale, img_size, hw, sigma = SHAPES[shape_name]
-    cfg = pkg.configs.grl_config(variant, task, scale, img_size)
-    m = pkg.GRL(**cfg)
-    missing, unexpected = m.load_state_dict(oracle.synth_state_dict(cfg, seed=0, style=style), strict=False)
-    assert not unexpected
-    m = m.to(device).eval()
-    m.set_precision(precision)
-    x = oracle.synth_input((1, 3, *hw), seed=1234, noise_sigma=sigma)
-    return m, x, scale
 
 
 def compare(oracle, y, gold, scale):
@@ -61,7 +45,7 @@ def compare(oracle, y, gold, scale):
 def test_fp32_path_vs_reference_native_shape(pkg, oracle, device, case):
     gold = load(case)
     shape_name, style = case.split("_")
-    m, x, scale = build(pkg, oracle, shape_name, style, device, "fp32")
+    m, x, scale = native_model(pkg, oracle, shape_name, style, device, "fp32")
     y = m(x.to(device)).cpu()
     err, p_cr, d_psnr = compare(oracle, y, gold, scale)
     print(f"{case} [fp32]: max-abs vs reference {err:.3e}  PSNR(cand, ref) {p_cr:.1f} dB  |dPSNR vs GT| {d_psnr:.2e} dB")
@@ -77,7 +61,7 @@ def test_tensor_core_path_psnr_gate_native_shape(pkg, oracle, device, case, prec
     reported (8-bit mantissas: SURVEY.md section 7)."""
     gold = load(case)
     shape_name, style = case.split("_")
-    m, x, scale = build(pkg, oracle, shape_name, style, device, precision)
+    m, x, scale = native_model(pkg, oracle, shape_name, style, device, precision)
     y = m(x.to(device)).cpu()
     assert torch.isfinite(y).all()
     err, p_cr, d_psnr = compare(oracle, y, gold, scale)
@@ -94,9 +78,7 @@ def test_cfg5_whole_frame_tiled(pkg, oracle, device):
 
     gold = load("cfg5_frame")
     cfg = pkg.configs.grl_config("base", "deblur", 1, 480)
-    m = pkg.GRL(**cfg)
-    m.load_state_dict(oracle.synth_state_dict(cfg, seed=0, style="init"), strict=False)
-    m = m.to(device).eval()
+    m = build(pkg, oracle, cfg, device, "fp32", style="init")
     x = oracle.synth_input((1, 3, 720, 1280), seed=1234)
     for precision, gate in (("fp32", 1e-3), ("fp16", None)):
         m.set_precision(precision)

@@ -8,7 +8,7 @@ import pytest
 import torch
 
 import niqe_oracle
-from test_niqe import ALPHA_COLS, CASES, GOLD, SCORE_GATE, params
+from metric_cases import ALPHA_COLS, GOLD, NIQE_CASES, NIQE_SCORE_GATE, niqe_params
 
 pytestmark = pytest.mark.gpu
 ULP255 = 255 * 2.0 ** -23  # one fp32 ulp at the top of the 8-bit range
@@ -27,11 +27,11 @@ def tab():
     return niqe_oracle.tables()
 
 
-@pytest.mark.parametrize("case", CASES)
+@pytest.mark.parametrize("case", NIQE_CASES)
 def test_stages_against_oracle(pkg, device, tab, case):
     from grl_image_restoration_b200 import metrics
 
-    g, prm = golden(case), params()
+    g, prm = golden(case), niqe_params()
     win = prm["gaussian_window"]
     s = {k: v.cpu().numpy() for k, v in metrics.niqe_stages(as_input(g["rgb8"], device), prm, int(g["border"])).items()}
     for i in range(g["rgb8"].shape[0]):
@@ -62,7 +62,7 @@ def test_stages_against_oracle(pkg, device, tab, case):
         assert np.nanmax(np.abs(got[rows] - want[rows]) / (np.abs(want[rows]) + 1e-6)) <= 1e-9
 
 
-@pytest.mark.parametrize("case", CASES)
+@pytest.mark.parametrize("case", NIQE_CASES)
 def test_score_matches_reference(pkg, device, case):
     from grl_image_restoration_b200 import metrics
 
@@ -74,15 +74,15 @@ def test_score_matches_reference(pkg, device, case):
     assert got.dtype == torch.float64 and got.shape == (x.shape[0],)
     err = (got.cpu() - torch.from_numpy(g["score"])).abs().max().item()
     print(f"niqe {case}: device {got.cpu().tolist()} reference {g['score'].tolist()} |diff| {err:.2e}")
-    assert err <= SCORE_GATE
-    again = metrics.niqe(x, params(), border=int(g["border"]))
+    assert err <= NIQE_SCORE_GATE
+    again = metrics.niqe(x, niqe_params(), border=int(g["border"]))
     assert torch.equal(got, again), "two runs must be bit-identical"
 
 
 def test_batch_equals_single_images(pkg, device):
     from grl_image_restoration_b200 import metrics
 
-    g, prm = golden("b2"), params()
+    g, prm = golden("b2"), niqe_params()
     x = as_input(g["rgb8"], device)
     fb = metrics.niqe_features(x, prm, 4)
     for i in range(x.shape[0]):
@@ -101,11 +101,11 @@ def test_realistic_size_against_oracle(pkg, device, tab, hw):
     yy, xx = np.mgrid[0:h, 0:w] / max(h, w)
     base = np.stack([np.sin(9 * xx + 4 * yy), np.cos(7 * yy - 5 * xx), np.sin(6 * (xx + yy))]) * 70 + 128
     rgb8 = np.clip(base + rng.normal(0, 10, (3, h, w)), 0, 255).round().astype(np.uint8)
-    prm = params()
+    prm = niqe_params()
     got = metrics.niqe(as_input(rgb8[None], device), prm).item()
     want = niqe_oracle.niqe(rgb8, prm, 0, tab)["score"]
     print(f"niqe {h}x{w}: device {got:.6f} oracle {want:.6f} |diff| {abs(got - want):.2e}")
-    assert abs(got - want) <= SCORE_GATE
+    assert abs(got - want) <= NIQE_SCORE_GATE
 
 
 def _score_from(feats_rows, prm):
@@ -116,10 +116,10 @@ def test_mutations_fail_the_gate(pkg, device, tab):
     """Each deliberate change, applied to the device's own intermediate images, moves some golden's score past the gate."""
     from grl_image_restoration_b200 import metrics
 
-    prm = params()
+    prm = niqe_params()
     win = prm["gaussian_window"]
     worst = {"rgb_luma": 0.0, "float64_mscn": 0.0, "no_roll_wrap": 0.0}
-    for case in CASES:
+    for case in NIQE_CASES:
         g = golden(case)
         b = int(g["border"])
         s = {k: v.cpu().numpy() for k, v in metrics.niqe_stages(as_input(g["rgb8"], device), prm, b).items()}
@@ -163,4 +163,4 @@ def test_mutations_fail_the_gate(pkg, device, tab):
             worst["no_roll_wrap"] = max(worst["no_roll_wrap"], abs(_score_from(np.concatenate(rows, 1), prm) - want))
     print("mutation worst |score - reference|:", worst)
     for name, v in worst.items():
-        assert v > SCORE_GATE, f"mutation {name} passes the gate"
+        assert v > NIQE_SCORE_GATE, f"mutation {name} passes the gate"

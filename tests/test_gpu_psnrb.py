@@ -2,24 +2,22 @@
 (tests/golden/psnrb.npz) and the torch-op definition metrics.psnrb, plus mutation controls that must fail the 1e-4 dB
 gate."""
 import math
-import os
 
 import numpy as np
 import pytest
 import torch
 
-from test_psnrb import CASES, golden_case
+from metric_cases import PSNRB_CASES, PSNRB_GOLDEN, golden_pair
 
 pytestmark = pytest.mark.gpu
-GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "psnrb.npz")
 
 
-@pytest.mark.parametrize("case", CASES)
+@pytest.mark.parametrize("case", PSNRB_CASES)
 def test_fused_psnrb_matches_reference(pkg, device, case):
     from grl_image_restoration_b200 import metrics
 
-    g = np.load(GOLDEN)
-    restored, target = (t.to(device) for t in golden_case(g, case))
+    g = np.load(PSNRB_GOLDEN)
+    restored, target = (t.to(device) for t in golden_pair(g, case))
     keep = restored.clone()
     p, py = metrics.psnrb_fused(restored, target)
     assert torch.equal(restored, keep)
@@ -73,10 +71,10 @@ def _mutated(restored, target, counts=False, on_target=False):
 
 @pytest.mark.parametrize("mutation", ["counts", "on_target"])
 def test_mutations_fail_the_gate(pkg, device, mutation):
-    g = np.load(GOLDEN)
+    g = np.load(PSNRB_GOLDEN)
     worst = 0.0
-    for case in CASES:
-        restored, target = golden_case(g, case)
+    for case in PSNRB_CASES:
+        restored, target = golden_pair(g, case)
         got = _mutated(restored, target, counts=mutation == "counts", on_target=mutation == "on_target")
         worst = max(worst, (got - torch.from_numpy(g[f"{case}_psnrb"]).double()).abs().max().item())
     assert worst > 1e-4, f"mutation {mutation} passes the gate: the goldens do not pin it"

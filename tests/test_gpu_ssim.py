@@ -10,7 +10,7 @@ import torch
 from torch.utils._pytree import tree_leaves
 from torch.utils._python_dispatch import TorchDispatchMode
 
-from test_ssim import CASES, GOLDEN, SCORE_GATE, golden_case, golden_scores, host_ssim
+from metric_cases import SSIM_CASES, SSIM_GOLDEN, SSIM_SCORE_GATE, golden_pair, golden_scores, host_ssim
 
 pytestmark = pytest.mark.gpu
 METRICS_GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "metrics.npz")
@@ -31,12 +31,13 @@ def device_ssim(a, b, border=0):
     return out[0], out[1], m, my
 
 
-@pytest.mark.parametrize("case", CASES)
+@pytest.mark.parametrize("case", SSIM_CASES)
 def test_kernel_against_host_and_reference(pkg, device, case):
     from grl_image_restoration_b200 import metrics
 
-    g = np.load(GOLDEN)
-    restored, target, border = golden_case(g, case)
+    g = np.load(SSIM_GOLDEN)
+    restored, target = golden_pair(g, case)
+    border = int(g[f"{case}_border"])
     hs, hsy, hm, hmy = host_ssim(restored, target, border, maps=True)
     a, b = restored.to(device), target.to(device)
     keep = a.clone()
@@ -47,7 +48,7 @@ def test_kernel_against_host_and_reference(pkg, device, case):
         assert my.cpu().numpy().tobytes() == hmy.tobytes()
     assert np.abs(s.cpu().numpy() - hs).max() <= 1e-13 and np.abs(sy.cpu().numpy() - hsy).max() <= 1e-13
     want, want_y = golden_scores(g, case)
-    assert np.abs(s.cpu().numpy() - want).max() <= SCORE_GATE and np.abs(sy.cpu().numpy() - want_y).max() <= SCORE_GATE
+    assert np.abs(s.cpu().numpy() - want).max() <= SSIM_SCORE_GATE and np.abs(sy.cpu().numpy() - want_y).max() <= SSIM_SCORE_GATE
     f, fy = metrics.ssim_fused(a, b, border)  # the public call: same kernel, no map output
     assert torch.equal(f, s) and torch.equal(fy, sy)
     if restored.shape[1] == 1:
@@ -65,9 +66,9 @@ def test_fused_ssim_vs_torch_ops(pkg, device, shape, border):
     s, sy = metrics.ssim_fused(a, b, border)
     assert s.dtype == torch.float64 and s.shape == (shape[0],)
     # the torch-op definition on the CPU: its fp32 convolutions do not depend on the device library's math mode there
-    assert (s.cpu() - metrics.ssim(a.cpu(), b.cpu(), border)).abs().max().item() <= SCORE_GATE
+    assert (s.cpu() - metrics.ssim(a.cpu(), b.cpu(), border)).abs().max().item() <= SSIM_SCORE_GATE
     if shape[1] == 3:
-        assert (sy.cpu() - metrics.ssim(a.cpu(), b.cpu(), border, "y")).abs().max().item() <= SCORE_GATE
+        assert (sy.cpu() - metrics.ssim(a.cpu(), b.cpu(), border, "y")).abs().max().item() <= SSIM_SCORE_GATE
     else:
         assert torch.equal(sy, s)
     s2, sy2 = metrics.ssim_fused(a, b, border)
@@ -114,7 +115,7 @@ def test_validation_metrics_fused(pkg, device, case, is_sr):
     got = metrics.validation_metrics_fused(restored, target, scale=scale, is_sr=is_sr)
     want = metrics.validation_metrics(restored.cpu(), target.cpu(), scale=scale, is_sr=is_sr)  # the torch-op definitions
     assert list(got) == list(want)
-    for name, tol in (("psnr", 1e-4), ("psnr_y", 1e-4), ("ssim", SCORE_GATE), ("ssim_y", SCORE_GATE)):
+    for name, tol in (("psnr", 1e-4), ("psnr_y", 1e-4), ("ssim", SSIM_SCORE_GATE), ("ssim_y", SSIM_SCORE_GATE)):
         assert got[name].shape == want[name].shape
         assert (got[name].double().cpu() - want[name].double()).abs().max().item() <= tol, name
         assert (got[name].double().cpu() - torch.from_numpy(g[f"{case}_{name}"]).double()).abs().max().item() <= tol, name

@@ -26,6 +26,8 @@ import sys
 import pytest
 import torch
 
+from support import build
+
 pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 NIQE_PARAMS = os.path.join(GOLD, "niqe_pris_params.npz")
@@ -155,12 +157,8 @@ def side_stream_case(env, monkeypatch, fn, make, graph_only=False):
 # ---------------------------------------------------------------------------------------------------------- models
 
 
-def build(pkg, oracle, precision, **kw):
-    cfg = pkg.configs.micro_config()
-    m = pkg.GRL(**cfg, **kw)
-    m.load_state_dict(oracle.synth_state_dict(cfg, seed=0, style="init"), strict=False)
-    m = m.to("cuda").eval()
-    m.set_precision(precision)
+def micro_model(pkg, oracle, precision, **kw):
+    m = build(pkg, oracle, pkg.configs.micro_config(), "cuda", precision, style="init", **kw)
     m.use_cuda_graph = False
     return m
 
@@ -178,7 +176,7 @@ MODEL_CASES = [(p, f, e, g) for p in ("fp32", "fp16", "bf16") for f in ("rgb", "
 
 @pytest.mark.parametrize("precision,fmt,ensemble,graph", MODEL_CASES)
 def test_model_on_side_stream(pkg, oracle, env, monkeypatch, precision, fmt, ensemble, graph):
-    m = build(pkg, oracle, precision, input_format=fmt, self_ensemble=ensemble)
+    m = micro_model(pkg, oracle, precision, input_format=fmt, self_ensemble=ensemble)
     m.use_cuda_graph = graph
     shape = (2, 4, 12, 20) if fmt == "rggb" else (2, 3, 24, 40)
     side_stream_case(env, monkeypatch, m, lambda s: (rand(s, *shape),), graph_only=graph and not ensemble)
@@ -187,7 +185,7 @@ def test_model_on_side_stream(pkg, oracle, env, monkeypatch, precision, fmt, ens
 def _entry_cases(pkg, oracle):
     from grl_image_restoration_b200 import functional as K, metrics, tiling
 
-    m = build(pkg, oracle, "fp16")
+    m = micro_model(pkg, oracle, "fp16")
     sizes = [(24, 40), (17, 30), (24, 40), (9, 13)]
     flist = lambda s: ([rand(s + i, 3, h, w) for i, (h, w) in enumerate(sizes)],)  # noqa: E731
     ulist = lambda s: ([rand(s + i, h, w, 3, u8=True) for i, (h, w) in enumerate(sizes)],)  # noqa: E731
@@ -224,7 +222,7 @@ def test_entry_point_on_side_stream(pkg, oracle, env, monkeypatch, entry):
 
 def test_misstreamed_launch_is_caught(pkg, oracle, env, monkeypatch):
     """Mutation control: the same race with every grl_tc_attn launch put on another stream must not match."""
-    m = build(pkg, oracle, "fp16")
+    m = micro_model(pkg, oracle, "fp16")
     srcs = (rand(1, 2, 3, 24, 40),)
     ref = m(*srcs)
     torch.cuda.synchronize()
@@ -278,7 +276,7 @@ def test_cross_stream_handoff(pkg, oracle, env, case, precision):
     equal the default-stream reference.  constants: R1 and R2 warmed, the forward at R1 rebuilds the attention constants;
     set_precision / edit: the packed weights (fp32: the im2col conv weights) are rebuilt; new_resolution: the coordinate
     tables, constants and plans of a resolution first seen on A."""
-    m = build(pkg, oracle, {"set_precision": "bf16" if precision == "fp16" else "fp16"}.get(case, precision))
+    m = micro_model(pkg, oracle, {"set_precision": "bf16" if precision == "fp16" else "fp16"}.get(case, precision))
     size = R3 if case == "new_resolution" else R1
     xa, xb = x_at(11, size), x_at(12, size)
     warm_streams(env, m, x_at(3, R2))
@@ -328,7 +326,7 @@ REUSE = [("resolution", "fp16"), ("set_precision", "fp16"), ("set_precision", "b
 def test_reuse_after_free(pkg, oracle, env, case, precision):
     """Hazard 2: a forward queued on the delayed stream S reads entries made on the default stream; the default stream
     then drops them and runs a forward that allocates and writes there.  S's output must still equal the reference."""
-    m = build(pkg, oracle, precision)
+    m = micro_model(pkg, oracle, precision)
     size = R3 if case == "eviction" else R1
     x = x_at(31, size)
     ref = m(x)
@@ -371,7 +369,7 @@ def test_reuse_after_free(pkg, oracle, env, case, precision):
 def test_concurrent_graph_replays(pkg, oracle, env):
     """Hazard 3: one captured graph replayed from two streams at once (A delayed by about half a replay); the two
     executions would overlap without ordering, and both outputs equal the eager results."""
-    m = build(pkg, oracle, "fp16")
+    m = micro_model(pkg, oracle, "fp16")
     xa, xb = rand(41, 32, 3, 192, 192), rand(42, 32, 3, 192, 192)
     ref = (m(xa), m(xb))
     m.use_cuda_graph = True
@@ -456,7 +454,7 @@ def test_every_cached_tensor_is_ordered(pkg, oracle, env):
     from grl_image_restoration_b200 import metrics
 
     name = pkg.__name__
-    m = build(pkg, oracle, "fp16")
+    m = micro_model(pkg, oracle, "fp16")
     x = x_at(51, R2)
     m(x)
     m.use_cuda_graph = True

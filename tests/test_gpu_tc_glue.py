@@ -10,9 +10,11 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from grl_oracle import LN100_F32, channel_gate_reference, to16
+from support import FMTS, same_bits
+
 pytestmark = pytest.mark.gpu
 
-FMTS = [0, 1]
 U = 2.0 ** -24  # fp32 unit roundoff
 GRL_ERR_WORKSPACE = -3
 
@@ -34,25 +36,6 @@ def capi():
 
 def dt(fmt):
     return torch.bfloat16 if fmt else torch.float16
-
-
-def to16(x, fmt):
-    """The 16-bit rounding contract of the pack kernels: round to nearest even; fp16 saturates at +-65504 (cvt.rn.satfinite,
-    where torch's .half() would give inf), bf16 is torch's .bfloat16()."""
-    x = x.float()
-    return x.bfloat16() if fmt else x.clamp(-65504.0, 65504.0).half()
-
-
-def same_bits(a, b):
-    """Bitwise equality of two 16-bit or fp32 tensors, NaN payloads excepted (any NaN matches any NaN)."""
-    assert a.shape == b.shape and a.dtype == b.dtype
-    nan_a, nan_b = torch.isnan(a.float()), torch.isnan(b.float())
-    assert torch.equal(nan_a, nan_b), "NaN positions differ"
-    ib = {2: torch.int16, 4: torch.int32}[a.element_size()]
-    ai, bi = a.contiguous().view(ib), b.contiguous().view(ib)
-    bad = (ai != bi) & ~nan_a
-    assert not bad.any(), f"{int(bad.sum())} of {a.numel()} differ, first at {bad.nonzero()[0].tolist()}: " \
-                          f"{a[tuple(bad.nonzero()[0])].item()!r} vs {b[tuple(bad.nonzero()[0])].item()!r}"
 
 
 def ulp16(x, fmt):
@@ -213,13 +196,6 @@ def test_avgpool16(tc, device, df, Cpad, fmt):
         assert ((got.double() - mean).abs() <= ulp16(mean, fmt)).all()
 
 
-def _gate_ref(y, w1, b1, w2, b2):
-    """float64 squeeze-excite: sigmoid(W2 relu(W1 mean_L(y) + b1) + b2), y (B, L, C)."""
-    m = y.double().mean(1)
-    h = torch.relu(m @ w1.double().T + b1.double())
-    return torch.sigmoid(h @ w2.double().T + b2.double()), m, h
-
-
 @pytest.mark.parametrize("fmt", FMTS)
 @pytest.mark.parametrize("C", [36, 180])
 @pytest.mark.parametrize("B", [1, 3])
@@ -241,7 +217,7 @@ def test_tc_channel_gate(tc, device, L, B, C, fmt):
     y16[..., :C] = y.to(dt(fmt))
     w1, b1 = torch.randn(R, C, generator=g) / C ** 0.5, torch.randn(R, generator=g) * 0.1
     w2, b2 = torch.randn(C, R, generator=g) / R ** 0.5, torch.randn(C, generator=g) * 0.1
-    ref, m, h = _gate_ref(y16[..., :C].float(), w1, b1, w2, b2)
+    ref, m, h = channel_gate_reference(y16[..., :C].float(), w1, b1, w2, b2)
     chunks = (L + 511) // 512
     dm = (512 + chunks) * U * y16[..., :C].double().abs().mean(1)
     dh = dm @ w1.double().abs().T + (C + 1) * U * (m.abs() @ w1.double().abs().T + b1.double().abs())
@@ -262,9 +238,6 @@ def test_tc_channel_gate(tc, device, L, B, C, fmt):
     rc = lib.grl_tc_channel_gate(C_.ptr(yd), cpad, fmt, B, L, C, C_.ptr(w1d), C_.ptr(b1d), C_.ptr(w2d), C_.ptr(b2d), R,
                                  C_.ptr(gate), C_.ptr(ws), nbytes - 4, C_.stream())
     assert rc == GRL_ERR_WORKSPACE
-
-
-LN100_F32 = float(torch.tensor(math.log(100.0), dtype=torch.float32))
 
 
 @pytest.mark.parametrize("hw,hs", [(1, 1), (2, 2), (3, 3), (8, 8), (2, 5)])

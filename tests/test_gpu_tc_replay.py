@@ -4,16 +4,16 @@
 the forward really handed it before the next one runs.  So every kernel is gated on what the previous kernels wrote
 (correlated q / k, trained-like bias tables, real residual streams), not only on the seeded operands of the launch-path
 tests, with the gates of those tests:
-  GEMM (every `listed` launch): grl_oracle.gemm_launch_reference through test_gpu_tc_gemm.evaluate (fp32, 16-bit,
+  GEMM (every `listed` launch): grl_oracle.gemm_launch_reference through gemm_cases.evaluate (fp32, 16-bit,
     PixelShuffle and NCHW-tail outputs and the 16-bit == RNE(own fp32) identity; no high-mean row split);
   attention: grl_oracle.attn_launch_reference of the launch's own q / k / v and copy 0 of its bias table, through
-    test_gpu_tc_attn.compare and GATE_ULP, stripe pass 2 also against the chained emulation (GATE_CHAIN).  At most 16
+    attn_cases.compare and GATE_ULP, stripe pass 2 also against the chained emulation (GATE_CHAIN).  At most 16
     windows per launch (the first, the last (masked and rolled) and 14 seeded others); every window in the first and
     last block of each stage;
   glue: pack_rows, head_pack / head_pack_rggb and avgpool16 bit for bit; slot scales exactly as
     test_slot_scale_layout, from the block's parameters as they are then; bias_table_log2 within test_bias_table4's
     bound of float64 16 sigmoid(MLP(coords)) log2 e, copies 1-3 exact shifts, the pad zero; channel_gate within
-    test_tc_channel_gate's bound; K.ln_residual within test_gpu_f32_paths.ln_bound;
+    test_tc_channel_gate's bound; K.ln_residual within grl_oracle.ln_bound;
   consumers: the slot scales a QKV GEMM receives and the table an attention launch receives are checked whether they
     were computed in this forward or come from the block's constant cache; the 16-bit operand a GEMM reads as the
     residual stream's copy (qkv, cab1, fc1, stage conv, conv_after_body) is bit for bit RNE16 of the latest fp32 stream;
@@ -35,15 +35,11 @@ import pytest
 import torch
 
 import archs
+import attn_cases as A
+import gemm_cases as G
 import grl_oracle as O
 from _pkgload import load_package
-import test_gpu_demosaic as DM
-import test_gpu_f32_paths as F32
-import test_gpu_native_shapes as NS
-import test_gpu_tc_attn as A
-import test_gpu_tc_gemm as G
-import test_gpu_tc_glue as Gl
-import test_gpu_zoo_model as Z
+from support import bound_ratio, build, dm_model, grid_t, native_model, zoo_model
 
 load_package()
 from grl_image_restoration_b200 import functional as KF, tc as TC  # noqa: E402
@@ -86,7 +82,7 @@ def same16(a, b):
 def slot_scale_ref(blk):
     """test_slot_scale_layout's reference from the block's current logit scales."""
     wa, sa = blk.attn.window_attn, blk.attn.stripe_attn
-    sc = lambda ls: torch.exp(ls.detach().double().reshape(-1).clamp(max=Gl.LN100_F32)) / math.log(2.0)  # noqa: E731
+    sc = lambda ls: torch.exp(ls.detach().double().reshape(-1).clamp(max=O.LN100_F32)) / math.log(2.0)  # noqa: E731
     hw, hs = wa.num_heads, sa.num_heads
     d = wa.attn_transform.logit_scale.device
     z = lambda n, v: torch.full((n,), v, dtype=torch.float64, device=d)  # noqa: E731
@@ -317,7 +313,7 @@ class Replay(TC.Device):
 
     # ---- glue -------------------------------------------------------------------------------------
     def _to16(self, x):
-        return Gl.to16(x, self.fmt)
+        return O.to16(x, self.fmt)
 
     def _check_pack_rows(self, x, cpad, fmt=0, out=None, _name=None):
         C = x.shape[-1]
@@ -371,7 +367,7 @@ class Replay(TC.Device):
         w2, b2 = att[3].weight.detach().reshape(att[3].weight.shape[0], -1), att[3].bias.detach()
         R = w1.shape[0]
         y = y16.reshape(B, L, ld)[..., :C].float()
-        ref, m, h = Gl._gate_ref(y, w1, b1, w2, b2)
+        ref, m, h = O.channel_gate_reference(y, w1, b1, w2, b2)
         chunks = (L + 511) // 512
         dm = (512 + chunks) * U * y.double().abs().mean(1)
         dh = dm @ w1.double().abs().T + (C + 1) * U * (m.abs() @ w1.double().abs().T + b1.double().abs())
@@ -386,9 +382,9 @@ class Replay(TC.Device):
         u64 = u.reshape(-1, C).double()
         g64, b64 = gamma.detach().double(), beta.detach().double()
         x64 = None if x is None else x.reshape(-1, C).double()
-        ref = F32.ln_reference(u64, g64, b64, eps, res_scale, x64, None, None)
-        bound = F32.ln_bound(u64, g64, b64, eps, res_scale, x64, None, None)
-        r = F32.bound_ratio(out.reshape(-1, C), ref, bound)
+        ref = O.ln_reference(u64, g64, b64, eps, res_scale, x64, None, None)
+        bound = O.ln_bound(u64, g64, b64, eps, res_scale, x64, None, None)
+        r = bound_ratio(out.reshape(-1, C), ref, bound)
         self._gate("ln_residual (error / bound)", r, 1.0, r <= 1.0, "norm_start" if self.block is None else "norm_end")
         self.stream32 = out
 
@@ -421,7 +417,7 @@ class Replay(TC.Device):
         vv = A.operand(buf, spec("v", v_off, v_dense), gk, heads, B)
         got = A.operand(buf, spec("o", o_off, o_dense), gq, heads, B)
         idx = self._windows(qq.shape[0]).to(q.device)
-        index, mask = O.attn_pair_geometry(A.grid_t(gq), A.grid_t(gk), use_mask)
+        index, mask = O.attn_pair_geometry(grid_t(gq), grid_t(gk), use_mask)
         index = index.to(q.device)
         msel = None if mask is None else mask.to(q.device)[idx % mask.shape[0]]
         table = bias[:, 0, :(gq.wh + gk.wh - 1) * (gq.ww + gk.ww - 1)]
@@ -538,21 +534,18 @@ def _case(pkg, oracle, cases, golden_loader, device, name):
     kind, _, rest = name.partition(":")
     if kind == "native":
         shape_name, precision = rest.split("-")
-        m, x, _ = NS.build(pkg, oracle, shape_name, "spread", device, precision)
+        m, x, _ = native_model(pkg, oracle, shape_name, "spread", device, precision)
         return m, x.to(device), False
     if kind == "zoo":
         zname, precision = rest.rsplit("-", 1)
-        m, gold = Z.golden(pkg, oracle, zname, device, precision)
+        m, gold = zoo_model(pkg, oracle, zname, device, precision)
         return m, torch.from_numpy(gold["x"]).to(device), False
     if kind == "dm":
-        m = DM.build(pkg, oracle, device, "fp16", input_format="rggb")
+        m = dm_model(pkg, oracle, device, "fp16")
         return m, golden_loader("dm_b2_40x56.npz")["cfa4"].to(device), True
     mname, precision = rest.rsplit("-", 1)
     c = cases[mname]
-    m = pkg.GRL(**c["cfg"])
-    m.load_state_dict(oracle.synth_state_dict(c["cfg"], seed=0, style="routed"), strict=False)
-    m = m.to(device).eval()
-    m.set_precision(precision)
+    m = build(pkg, oracle, c["cfg"], device, precision, style="routed")
     x = oracle.synth_input((c["batch"], c["cfg"]["in_channels"], *c["hw"]), seed=1234, noise_sigma=c["sigma"])
     return m, x.to(device), False
 

@@ -23,6 +23,8 @@ import copy
 import pytest
 import torch
 
+from support import build
+
 pytestmark = pytest.mark.gpu
 
 G_BLK = 1e-2
@@ -96,12 +98,6 @@ def mutate(module, name):
     return any(MUTATIONS[name](b) is not False for b in blocks)
 
 
-def build(pkg, oracle, cfg, device, style, seed=0):
-    m = pkg.GRL(**cfg)
-    m.load_state_dict(oracle.synth_state_dict(cfg, seed=seed, style=style), strict=False)
-    return m.to(device).eval()
-
-
 # (name, config, block input size): micro_cab_x2 at the size of its stored reference taps; GRL-Small (C 128, head_dim 32)
 # and GRL-Base (C 180, head_dim 30: the ones-column path), blocks 0 and 1 (no shift / shifted, both stripe directions)
 def block_cases(pkg, cases):
@@ -112,7 +108,7 @@ def block_cases(pkg, cases):
 
 def block_errors(pkg, oracle, cfg, hw, device, style, block_ids, x=None, precision="fp16", mutations=MUTATIONS):
     """{block: {"unmutated": e, mutation: e}} with e = rms(y_tc - y_fp32) / rms(y_fp32 - x), y_fp32 always unmutated."""
-    m = build(pkg, oracle, cfg, device, style)
+    m = build(pkg, oracle, cfg, device, "fp32", style=style)
     C = cfg["embed_dim"]
     if x is None:
         x = torch.randn(1, hw[0] * hw[1], C, generator=torch.Generator().manual_seed(11))
@@ -146,7 +142,7 @@ def psnr(a, b):
 
 
 def net_psnrs(pkg, oracle, cfg, batch, hw, sigma, device, style, precision, mutations=MUTATIONS):
-    m = build(pkg, oracle, cfg, device, style)
+    m = build(pkg, oracle, cfg, device, "fp32", style=style)
     x = oracle.synth_input((batch, cfg["in_channels"], *hw), seed=1234, noise_sigma=sigma).to(device)
     m.set_precision("fp32")
     y32 = m(x)

@@ -8,7 +8,7 @@ micro-batch of 16 images, and the non-square window grids of the stripe passes o
 
 Workloads are read from bench.py's text (WORKLOADS, MICRO_BATCH, CFG5_*; importing bench.py would redirect stdout).  One
 launch's batch is min(tiles per GPU, MICRO_BATCH); cfg5 runs the 6 tiles of its frame in one batch, as one GPU does.
-Operands follow the seeded recipes of the small-size tests (test_gpu_tc_gemm.instantiate, test_gpu_tc_attn.block_inputs)
+Operands follow the seeded recipes of the small-size tests (gemm_cases.instantiate, attn_cases.block_inputs)
 at the production batch and image size, and use the same gates.
 
   GEMM: each distinct launch of tc.gemm_launches (its name modulo the stage / block index) runs on the whole batch;
@@ -36,8 +36,9 @@ import pytest
 import torch
 
 import grl_oracle as O
-import test_gpu_tc_attn as A
-import test_gpu_tc_gemm as G
+import attn_cases as A
+import gemm_cases as G
+from support import grid_t
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 H100_SMS = 132
@@ -109,7 +110,7 @@ def distinct_attention_units(tc, model, shape):
         for blk in layer.blocks:
             w, s1, s2 = tc.attention_launches(blk, shape[2:])
             for lns in ((w,), (s1, s2)):
-                key = tuple((ln.role, A.grid_t(ln.gq), A.grid_t(ln.gk), ln.heads, ln.use_mask, ln.ones_col) for ln in lns)
+                key = tuple((ln.role, grid_t(ln.gq), grid_t(ln.gk), ln.heads, ln.use_mask, ln.ones_col) for ln in lns)
                 out.setdefault(key, (blk, lns))
     return list(out.values())
 
@@ -405,7 +406,7 @@ def test_attention_at_scale(pkg, tc, device, measured, workload):
         first = {int(s): j for j, s in enumerate(sel) if s < nW}
         emulated = {}  # role -> emulated output on the subset (pass 1: the chain's X1)
         for ln in lns:
-            index, mask = O.attn_pair_geometry(A.grid_t(ln.gq), A.grid_t(ln.gk), ln.use_mask)
+            index, mask = O.attn_pair_geometry(grid_t(ln.gq), grid_t(ln.gk), ln.use_mask)
             index, mask = index.to(device), None if mask is None else mask.to(device)[sel % nW]
             q, k, v = (A.operand(buf, s, g, h, batch=Bn)[sel] for s, g in ((ln.q, ln.gq), (ln.k, ln.gk), (ln.v, ln.gk)))
             got = A.operand(buf, ln.out, ln.gq, h, batch=Bn)[sel]
@@ -418,7 +419,7 @@ def test_attention_at_scale(pkg, tc, device, measured, workload):
             stats = A.compare(got, emul, d, dtype)
             nwh, nww = window_grid(ln.gq)
             ctas = attn_ctas(ln, Bn)
-            print(f"\n[{name} {precision}] {ln.role} {A.grid_t(ln.gq)} <- {A.grid_t(ln.gk)} h{h} d{d} mask={ln.use_mask} "
+            print(f"\n[{name} {precision}] {ln.role} {grid_t(ln.gq)} <- {grid_t(ln.gk)} h{h} d{d} mask={ln.use_mask} "
                   f"B={Bn}: window grid {nwh} x {nww}, {ctas} CTAs = {ctas / (CTAS_PER_SM * n_sm):.1f} waves; "
                   f"{sel.numel()} of {Bn * nW} windows vs float64: |got-emulated| {stats[0]:.2f} ulp (gate {A.GATE_ULP}), "
                   f"mismatch {stats[1]:.4f}, |emulated-exact| {float((emul - exact)[..., :d].abs().max()):.2e}, "

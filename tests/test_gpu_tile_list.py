@@ -2,34 +2,14 @@
 check_image_size, the overlap blend bit-exact against forward_tile's slice add_ and E.div_(W), and
 tiling.forward_tile_list / forward_tile_list_u8 equal, bit for bit, to the per-image forward_tile / forward_tile_u8 loop
 they replace, on every precision, input format, CUDA-graph and self-ensemble setting."""
-import json
-import os
-
 import pytest
 import torch
-import torch.nn.functional as F
+
+from engine_oracle import check_image_size, to_tensor
+from support import (MICRO, assert_equal_lists, build, count_calls, dm_model, micro, random_images, round8_ref,
+                     same_bits)
 
 pytestmark = pytest.mark.gpu
-GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
-
-
-def pad_to(x, Hp, Wp):
-    """check_image_size of x (1, C, h, w) padded to (Hp, Wp) (grl.py:479-489): reflect, or zeros when F.pad refuses."""
-    pads = (0, Wp - x.shape[3], 0, Hp - x.shape[2])
-    try:
-        return F.pad(x, pads, "reflect")
-    except BaseException:
-        return F.pad(x, pads, "constant")
-
-
-def to_tensor(img):
-    """(H, W, C) uint8 -> (C, H, W) k / 255 as the datasets compute it, on the CPU."""
-    return img.cpu().permute(2, 0, 1).float().div(255)
-
-
-def round8_ref(v):
-    """(C, H, W) float -> (H, W, C) uint8: tensor_round times 255, NaN -> 0 (grl_image_u8.h)."""
-    return (v.nan_to_num(nan=0.0).clamp(0, 1) * 255).round().byte().permute(1, 2, 0)
 
 
 def windows(sizes, n, seed, k=1):
@@ -73,20 +53,13 @@ def test_tile_gather_bit_exact(pkg, device, kind):
     out = K.tile_gather([(imgs[i], y0, x0, t) for i, y0, x0, t in wins], code, C, 16, 16).cpu()
     assert out.shape == (130, C, 16, 16)
     for j, (i, y0, x0, t) in enumerate(wins):
-        want = pad_to(frames[i][None, :, y0:y0 + t, x0:x0 + t], 16, 16)[0]
+        want = check_image_size(frames[i][None, :, y0:y0 + t, x0:x0 + t], 16, 16)[0]
         assert torch.equal(out[j].view(torch.int32), want.contiguous().view(torch.int32)), (j, i, y0, x0, t)
     for t in (1, 5, 16):  # Hp = Wp = t: a plain cut
         cut = [w for w in wins if w[3] == t][:3] or [(2, 0, 0, t)]
         got = K.tile_gather([(imgs[i], y0, x0, tt) for i, y0, x0, tt in cut], code, C, t, t).cpu()
         for j, (i, y0, x0, _) in enumerate(cut):
             assert torch.equal(got[j].view(torch.int32), frames[i][:, y0:y0 + t, x0:x0 + t].contiguous().view(torch.int32))
-
-
-def same_bits(a, b):
-    """Equal bit for bit, NaN payloads aside."""
-    nan = a.isnan()
-    return a.shape == b.shape and torch.equal(nan, b.isnan()) and torch.equal(a.view(torch.int32)[~nan],
-                                                                                 b.view(torch.int32)[~nan])
 
 
 @pytest.mark.parametrize("scale", [1, 2])
@@ -135,61 +108,15 @@ def test_blend_bit_exact(pkg, device, scale):
     K.tile_finish([(E, s[2], overlap) for E, s in zip(acc, spans)], scale, outs8)
     K.tile_finish([(E, s[2], overlap) for E, s in zip(Es, spans)], scale)
     for i, (E, o8, ref) in enumerate(zip(Es, outs8, refs)):
-        assert same_bits(E.cpu(), ref.cpu()), i
+        same_bits(E.cpu(), ref.cpu())
         assert torch.equal(o8.cpu(), round8_ref(ref.cpu())), i
 
 
 # ------------------------------------------------------------------------------------------ end to end
-MICRO = {  # upscaling with CAB, denoising with the input residual, grayscale, 6 channels in (dual-pixel views), 3 out
-    "micro_cab_x2": dict(),
-    "micro_pad_dn": dict(embed_dim=36, stripe=(8, 16), df=2, upsampler="", upscale=1, img_size=32),
-    "micro_gray": dict(embed_dim=32, heads=1, window=6, stripe=(6, 12), df=3, local_connection=False, upsampler="",
-                       upscale=1, img_size=24, in_channels=1),
-    "micro_dual": dict(upsampler="", upscale=1, in_channels=6),
-}
 # tile 24, overlap 6: several tile rows and columns, images smaller than the tile on one or both axes (t = 17, 12, 9),
 # repeats of one size, both orientations
 SIZES = [(40, 52), (17, 30), (24, 24), (52, 40), (12, 12), (33, 45), (40, 52), (9, 30)]
 TILE, OVERLAP = 24, 6
-
-
-def build(pkg, oracle, cfg, device, precision, **kw):
-    m = pkg.GRL(**cfg, **kw)
-    m.load_state_dict(oracle.synth_state_dict(cfg, seed=0, style="init"), strict=False)
-    m = m.to(device).eval()
-    m.set_precision(precision)
-    return m
-
-
-def micro(pkg, oracle, name, device, precision, **kw):
-    cfg = pkg.configs.micro_config(**MICRO[name])
-    if name == "micro_dual":
-        cfg["out_channels"] = 3
-    return build(pkg, oracle, cfg, device, precision, **kw)
-
-
-def images(shape_of, sizes, seed, device):
-    g = torch.Generator().manual_seed(seed)
-    return [torch.rand(shape_of(h, w), generator=g).to(device) for h, w in sizes]
-
-
-def assert_equal_lists(got, want):
-    assert len(got) == len(want)
-    for i, (a, b) in enumerate(zip(got, want)):
-        assert a.shape == b.shape and a.dtype == b.dtype, (i, a.shape, b.shape, a.dtype, b.dtype)
-        assert torch.equal(a, b), (i, (a.float() - b.float()).abs().max().item())
-
-
-def count_forwards(m):
-    calls = []
-    inner = m.forward_rgb
-
-    def wrapped(x):
-        calls.append(tuple(x.shape))
-        return inner(x)
-
-    m.forward_rgb = wrapped
-    return calls
 
 
 def loop(tiling, m, xs, tile=TILE, overlap=OVERLAP):
@@ -204,10 +131,10 @@ def test_forward_tile_list_equals_loop(pkg, oracle, device, name, precision, ens
 
     m = micro(pkg, oracle, name, device, precision, self_ensemble=ensemble)
     m.use_cuda_graph = graph
-    xs = images(lambda h, w: (m.in_channels, h, w), SIZES, list(MICRO).index(name), device)
+    xs = random_images(lambda h, w: (m.in_channels, h, w), SIZES, list(MICRO).index(name), device)
     kept = [x.clone() for x in xs]
     want = loop(tiling, m, xs)
-    calls = count_forwards(m)
+    calls = count_calls(m, "forward_rgb")
     got = tiling.forward_tile_list(m, xs, TILE, OVERLAP)
     assert_equal_lists(got, want)
     assert all(torch.equal(a, b) for a, b in zip(xs, kept)), "forward_tile_list changed its inputs"
@@ -237,21 +164,15 @@ def test_small_budget_splits_images_across_forwards(pkg, oracle, device, precisi
     from grl_image_restoration_b200 import image_list, tiling
 
     m = micro(pkg, oracle, "micro_cab_x2", device, precision)
-    xs = images(lambda h, w: (3, h, w), SIZES, 11, device)
+    xs = random_images(lambda h, w: (3, h, w), SIZES, 11, device)
     want = loop(tiling, m, xs)
     m.max_batch_tokens = 5 * 32 * 32  # 5 tiles of 24 (padded to 32) per forward: images of 3 x 3 tiles span several
-    calls = count_forwards(m)
+    calls = count_calls(m, "forward_rgb")
     assert_equal_lists(tiling.forward_tile_list(m, xs, TILE, OVERLAP), want)
     tiles, chunks = tiling.tile_plan(m, image_list.network_sizes([tuple(x.shape) for x in xs]), TILE, OVERLAP)
     assert all(n * h * w <= m.max_batch_tokens for n, _, h, w in calls) and (5, 3, 32, 32) in calls
     assert len(calls) == len(chunks)
     assert any(len({k for k, c in enumerate(chunks) if any(tiles[j][0] == i for j in c.index)}) > 1 for i in range(len(xs)))
-
-
-def dm_model(pkg, oracle, device, precision, **kw):
-    with open(os.path.join(GOLD, "dm_cases.json")) as f:
-        cfg = json.load(f)["cfg"]
-    return build(pkg, oracle, cfg, device, precision, input_format="rggb", **kw)
 
 
 @pytest.mark.parametrize("precision,ensemble,graph", [("fp32", False, False), ("fp16", False, False),
@@ -262,7 +183,7 @@ def test_forward_tile_list_rggb(pkg, oracle, device, precision, ensemble, graph)
     m = dm_model(pkg, oracle, device, precision, self_ensemble=ensemble)
     m.use_cuda_graph = graph
     packed = [(20, 26), (9, 13), (12, 12), (26, 20), (5, 16)]  # demosaiced: 40 x 52, 18 x 26, 24 x 24, 52 x 40, 10 x 32
-    xs = images(lambda h, w: (4, h, w), packed, 4, device)
+    xs = random_images(lambda h, w: (4, h, w), packed, 4, device)
     want = loop(tiling, m, xs)
     got = tiling.forward_tile_list(m, xs, TILE, OVERLAP)
     assert_equal_lists(got, want)
@@ -277,11 +198,11 @@ def test_released_jpeg_small_at_288_36(pkg, oracle, device):
     *_, tile, overlap = pkg.configs.RELEASED["jpeg_grl_small_c3q10.ckpt"]
     assert (tile, overlap) == (288, 36)
     cfg = pkg.configs.released_config("jpeg_grl_small_c3q10.ckpt", tile)
-    m = build(pkg, oracle, cfg, device, "fp16")
-    xs = images(lambda h, w: (3, h, w), [(481, 321), (321, 481), (512, 512), (500, 375), (256, 300), (481, 321)], 31,
+    m = build(pkg, oracle, cfg, device, "fp16", style="init")
+    xs = random_images(lambda h, w: (3, h, w), [(481, 321), (321, 481), (512, 512), (500, 375), (256, 300), (481, 321)], 31,
                 device)
     want = loop(tiling, m, xs, tile, overlap)
-    calls = count_forwards(m)
+    calls = count_calls(m, "forward_rgb")
     assert_equal_lists(tiling.forward_tile_list(m, xs, tile, overlap), want)
     assert len(calls) < len(xs)
 

@@ -2,26 +2,9 @@
 import pytest
 import torch
 
+from engine_oracle import forward_tile
+
 pytestmark = pytest.mark.gpu
-
-
-def reference_forward_tile(fn, x, tile, overlap, scale):
-    """engines/base.py:90-116 restated with `fn` as the model call (the oracle on the CPU)."""
-    b, c, h, w = x.shape
-    tile = min(tile, h, w)
-    stride = tile - overlap
-    h_idx = list(range(0, h - tile, stride)) + [h - tile]
-    w_idx = list(range(0, w - tile, stride)) + [w - tile]
-    E = W = None
-    for hi in h_idx:
-        for wi in w_idx:
-            out = fn(x[..., hi:hi + tile, wi:wi + tile])
-            if E is None:
-                E = torch.zeros(b, out.shape[1], h * scale, w * scale)
-                W = torch.zeros_like(E)
-            E[..., hi * scale:(hi + tile) * scale, wi * scale:(wi + tile) * scale] += out
-            W[..., hi * scale:(hi + tile) * scale, wi * scale:(wi + tile) * scale] += 1
-    return E / W
 
 
 @pytest.mark.parametrize("precision,tol", [("fp32", 1e-3), ("fp16", 2e-2)])
@@ -36,7 +19,7 @@ def test_forward_tile_matches_engine_semantics(pkg, oracle, device, precision, t
     m.set_precision(precision)
     x = oracle.synth_input((2, 3, 40, 56), seed=11)
     with torch.no_grad():
-        ref = reference_forward_tile(lambda t: oracle.grl_forward(sd, cfg, t), x, 32, 8, 2)
+        ref = forward_tile(lambda t: oracle.grl_forward(sd, cfg, t), x, 32, 8, 2)
     y = tiling.forward_tile(m, x.to(device), 32, 8, max_batch=5).cpu()
     assert y.shape == ref.shape == (2, 3, 80, 112)
     assert (y - ref).abs().max().item() <= tol

@@ -8,38 +8,18 @@ Gates as in test_gpu_native_shapes.py / test_gpu_model_bf16.py: fp32 <= 1e-3 max
 |PSNR(cand, GT) - PSNR(ref, GT)| <= 0.01 dB, PSNR(cand, ref) >= 56 dB (fp16) / 40 dB (bf16).  The PSNRs are taken on the
 stored output sample (the whole output except for blind SR, every 3rd pixel), without border shave.
 """
-import json
 import math
-import os
 
-import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
 
-import test_gpu_ensemble as E
-import test_gpu_tc_glue as Gl
+from engine_oracle import forward_tile
+from grl_oracle import to16
+from support import FMTS, ZOO, build, loop_ensemble, same_bits, zoo_model
 
 pytestmark = pytest.mark.gpu
-GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
-with open(os.path.join(GOLD, "zoo_cases.json")) as _f:
-    ZOO = json.load(_f)["cases"]
 GT_SEED = 9
-
-
-def build(pkg, oracle, cfg, device, precision, style="init", seed=0, **kw):
-    m = pkg.GRL(**cfg, **kw)
-    missing, unexpected = m.load_state_dict(oracle.synth_state_dict(cfg, seed=seed, style=style), strict=False)
-    assert not unexpected and set(missing) <= {"table_w", "table_sh", "table_sv"}, (missing, unexpected)
-    m = m.to(device).eval()
-    assert m.set_precision(precision) == precision
-    return m
-
-
-def golden(pkg, oracle, name, device, precision):
-    c = ZOO[name]
-    gold = np.load(os.path.join(GOLD, f"zoo_{name}.npz"))
-    return build(pkg, oracle, c["kwargs"], device, precision, c["style"], c["weight_seed"]), gold
 
 
 def gates(y, gold):
@@ -85,7 +65,7 @@ def zoo_params():
 
 @pytest.mark.parametrize("name,precision", zoo_params())
 def test_zoo_vs_reference(pkg, oracle, device, name, precision):
-    m, gold = golden(pkg, oracle, name, device, precision)
+    m, gold = zoo_model(pkg, oracle, name, device, precision)
     check(name, precision, m(torch.from_numpy(gold["x"]).to(device)), gold)
 
 
@@ -93,7 +73,7 @@ def test_zoo_vs_reference(pkg, oracle, device, name, precision):
 def test_defocus_dual_takes_the_concatenated_views(pkg, oracle, device, precision):
     """The engine's dual-pixel input, torch.cat([left, right], 1) (engines/base.py:119-120), is the model's input."""
     name = "defocus_dual_b2_48x80"
-    m, gold = golden(pkg, oracle, name, device, precision)
+    m, gold = zoo_model(pkg, oracle, name, device, precision)
     x = torch.from_numpy(gold["x"]).to(device)
     left, right = x[:, :3].contiguous(), x[:, 3:].contiguous()
     y = m(torch.cat([left, right], 1))
@@ -106,7 +86,7 @@ HEAD_WIDE = [  # B, Cin, H, W, Hp, Wp: no pad | reflect | zero (pad >= size in H
 ]
 
 
-@pytest.mark.parametrize("fmt", Gl.FMTS)
+@pytest.mark.parametrize("fmt", FMTS)
 @pytest.mark.parametrize("per_channel", [False, True])
 @pytest.mark.parametrize("B,Cin,H,W,Hp,Wp", HEAD_WIDE)
 def test_head_pack_wide_input_bit_exact(pkg, device, B, Cin, H, W, Hp, Wp, per_channel, fmt):
@@ -127,10 +107,10 @@ def test_head_pack_wide_input_bit_exact(pkg, device, B, Cin, H, W, Hp, Wp, per_c
         for cpad in (8, 64):
             y16, y32 = tc.head_pack(x.to(device), Hp, Wp, mean, rng, cpad, fmt, want_f32=want_f32)
             y16 = y16.cpu()
-            Gl.same_bits(y16[..., :Cin], Gl.to16(ref32, fmt))
+            same_bits(y16[..., :Cin], to16(ref32, fmt))
             assert not y16[..., Cin:].float().any()
             if want_f32:
-                Gl.same_bits(y32.cpu(), ref32)
+                same_bits(y32.cpu(), ref32)
 
 
 def test_head_pack_rejects_more_than_8_channels(pkg, device):
@@ -141,14 +121,15 @@ def test_head_pack_rejects_more_than_8_channels(pkg, device):
 
 
 def dual(pkg, oracle, device, precision, size=96, **kw):
-    return build(pkg, oracle, pkg.configs.grl_config("base", "defocus_dual", 1, size), device, precision, **kw)
+    cfg = pkg.configs.grl_config("base", "defocus_dual", 1, size)
+    return build(pkg, oracle, cfg, device, precision, style="init", **kw)
 
 
 @pytest.mark.parametrize("name", ["defocus_dual", "dn_c1"])
 def test_cuda_graph_replay_equals_eager(pkg, oracle, device, name):
     cfg = (pkg.configs.grl_config("base", "defocus_dual", 1, 96) if name == "defocus_dual"
            else pkg.configs.grl_config("small", "dn", 1, 128, in_channels=1))
-    m = build(pkg, oracle, cfg, device, "fp16")
+    m = build(pkg, oracle, cfg, device, "fp16", style="init")
     x1 = oracle.synth_input((2, cfg["in_channels"], 90, 70), seed=5).to(device)
     x2 = oracle.synth_input((2, cfg["in_channels"], 90, 70), seed=6).to(device)
     e1, e2 = m(x1).clone(), m(x2).clone()
@@ -164,7 +145,7 @@ def test_self_ensemble_six_channels_equals_loop(pkg, oracle, device, precision, 
     and averaged; non-square (two view batches) and square (one) inputs."""
     m = dual(pkg, oracle, device, precision, self_ensemble=True)
     x = oracle.synth_input((2, 6, *hw), seed=21).to(device)
-    ref = E.loop_ensemble(m, x)
+    ref = loop_ensemble(m, x)
     y = m(x)
     err = (y - ref).abs().max().item()
     print(f"defocus_dual {precision} {hw}: x8 ensemble vs loop of 8 plain forwards max-abs {err:.3e}")
@@ -180,7 +161,7 @@ def test_forward_tile_at_the_released_tile(pkg, oracle, device):
     m = dual(pkg, oracle, device, "fp16", size=480)
     x = oracle.synth_input((1, 6, 800, 900), seed=31).to(device)
     y = tiling.forward_tile(m, x, tile, overlap, max_batch=3)
-    ref = E.reference_forward_tile(lambda t: m(t).cpu(), x, tile, overlap, 1)
+    ref = forward_tile(lambda t: m(t).cpu(), x, tile, overlap, 1)
     err = (y.cpu() - ref).abs().max().item()
     print(f"defocus_dual forward_tile {tile}/{overlap}: out {tuple(y.shape)}, max-abs vs the engine's loop {err:.3e}")
     assert y.shape == (1, 3, 800, 900) and err <= 1e-4
@@ -193,7 +174,7 @@ def test_every_released_entry_runs(pkg, oracle, device, precision):
     for name, (_, task, upscale, cin, _, _) in pkg.configs.RELEASED.items():
         cfg = pkg.configs.released_config(name)
         S = math.lcm(cfg["window_size"], *cfg["stripe_size"])
-        m = build(pkg, oracle, dict(cfg, img_size=S), device, precision)
+        m = build(pkg, oracle, dict(cfg, img_size=S), device, precision, style="init")
         x = oracle.synth_input((1, cin, S - 3, S - 5), seed=41).to(device)
         y = m(x)
         torch.cuda.synchronize()

@@ -6,6 +6,8 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from support import build
+
 
 @pytest.fixture(scope="module")
 def tc(pkg):
@@ -15,9 +17,7 @@ def tc(pkg):
 
 
 def _block(pkg, oracle, **kw):
-    cfg = pkg.configs.micro_config(**kw)
-    model = pkg.GRL(**cfg)
-    model.load_state_dict(oracle.synth_state_dict(cfg, seed=3, style="spread"), strict=False)
+    model = build(pkg, oracle, pkg.configs.micro_config(**kw), "cpu", "fp32", style="spread", seed=3)
     return model, model.layers[0].blocks[0]
 
 

@@ -11,14 +11,9 @@ import numpy as np
 import pytest
 import torch
 
+from metric_cases import ALPHA_COLS, NIQE_CASES, NIQE_SCORE_GATE, niqe_params
+
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
-CASES = ["smooth", "flat", "b2"]
-SCORE_GATE = 2e-3
-ALPHA_COLS = [0, 2, 6, 10, 14, 18, 20, 24, 28, 32]
-
-
-def params():
-    return dict(np.load(os.path.join(GOLD, "niqe_pris_params.npz")))
 
 
 def numpy_luma_chain(rgb8):
@@ -57,7 +52,7 @@ def test_half_taps_match_reference_weights(pkg):
 
     w = np.empty(8, np.float32)
     capi.check(capi.lib().grl_niqe_half_taps_host(ctypes.c_void_p(w.ctypes.data)))
-    for case in CASES:
+    for case in NIQE_CASES:
         ref = np.load(os.path.join(GOLD, f"niqe_{case}.npz"))["weights"]
         assert ref.shape[1] == 8
         assert np.array_equal(ref, np.broadcast_to(w, ref.shape))  # every output row uses the same taps, bit for bit
@@ -80,12 +75,12 @@ def test_gamma_tables_match_numpy_and_scipy(pkg):
     assert np.all(np.diff(t[1]) > 0), "r_gam is increasing: the argmin has one decision midpoint per neighbour"
 
 
-@pytest.mark.parametrize("case", CASES)
+@pytest.mark.parametrize("case", NIQE_CASES)
 def test_oracle_reproduces_reference(pkg, case):
     import niqe_oracle
 
     g = np.load(os.path.join(GOLD, f"niqe_{case}.npz"))
-    prm, tab = params(), niqe_oracle.tables()
+    prm, tab = niqe_params(), niqe_oracle.tables()
     for i, img in enumerate(g["rgb8"]):
         r = niqe_oracle.niqe(img, prm, int(g["border"]), tab)
         assert np.array_equal(r["y"], g["y"][i].astype(np.float32))
@@ -98,7 +93,7 @@ def test_oracle_reproduces_reference(pkg, case):
         rows = agree.all(1)
         rel = np.abs(f[rows] - want[rows]) / (np.abs(want[rows]) + 1e-2)
         assert np.nanmax(rel) <= 5e-3
-        assert abs(r["score"] - g["score"][i]) <= SCORE_GATE, (r["score"], g["score"][i])
+        assert abs(r["score"] - g["score"][i]) <= NIQE_SCORE_GATE, (r["score"], g["score"][i])
 
 
 def test_flat_golden_has_nan_blocks_and_float64_misses_it(pkg):
@@ -107,7 +102,7 @@ def test_flat_golden_has_nan_blocks_and_float64_misses_it(pkg):
     import niqe_oracle
 
     g = np.load(os.path.join(GOLD, "niqe_flat.npz"))
-    prm = params()
+    prm = niqe_params()
     want = g["feats"][0]
     nan_rows = np.isnan(want).any(1)
     assert nan_rows.sum() >= 4
@@ -127,7 +122,7 @@ def test_flat_golden_has_nan_blocks_and_float64_misses_it(pkg):
     f1, _ = niqe_oracle.features(mscn64(y), 96, tab)
     f2, _ = niqe_oracle.features(mscn64(niqe_oracle.half(g["y"][0].astype(np.float32)).astype(np.float64)), 48, tab)
     s64 = niqe_oracle.distance(np.concatenate([f1, f2], 1), prm["mu_pris_param"], prm["cov_pris_param"])
-    assert abs(s64 - g["score"][0]) > 100 * SCORE_GATE
+    assert abs(s64 - g["score"][0]) > 100 * NIQE_SCORE_GATE
 
 
 def test_niqe_params_and_malformed_inputs(pkg, tmp_path):
@@ -135,7 +130,7 @@ def test_niqe_params_and_malformed_inputs(pkg, tmp_path):
 
     from grl_image_restoration_b200 import capi, metrics
 
-    prm = params()
+    prm = niqe_params()
     path = os.path.join(GOLD, "niqe_pris_params.npz")
     for a, b in zip(metrics.niqe_params(path), metrics.niqe_params(prm)):
         assert torch.equal(a, b)

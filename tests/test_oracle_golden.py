@@ -1,14 +1,10 @@
 """The oracle (oracle/grl_oracle.py) replayed against fixtures that were produced by the UNMODIFIED reference
 (oracle/make_golden.py).  CPU only; this is what pins the parity oracle."""
-import hashlib
-
 import numpy as np
 import pytest
 import torch
 
-
-def sha(t):
-    return hashlib.sha256(np.ascontiguousarray(t.numpy()).tobytes()).hexdigest()
+from support import sha
 
 
 GEOS = ["sr_small_128", "dn_small_128", "deblur_96x192", "jpeg_144", "dm_64", "yaml_default_64", "groups_g1_32",

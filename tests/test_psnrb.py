@@ -2,21 +2,12 @@
 (tests/golden/psnrb.npz, written by oracle/make_golden_psnrb.py) and against a float64 restatement that counts nothing
 for itself: the reference's normalisers are formulas of H and W, not counts of the summed positions."""
 import math
-import os
 
 import numpy as np
 import pytest
 import torch
 
-GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "psnrb.npz")
-CASES = ["rgb_b2", "rgb_w20", "gray", "clamp"]
-
-
-def golden_case(g, name):
-    restored = (torch.from_numpy(g[f"{name}_restored"]) if f"{name}_restored" in g
-                else torch.from_numpy(g[f"{name}_restored8"].astype(np.float32) / np.float32(255.0)))
-    target = torch.from_numpy(g[f"{name}_target8"].astype(np.float32) / np.float32(255.0))
-    return restored, target
+from metric_cases import PSNRB_CASES, PSNRB_GOLDEN, golden_pair
 
 
 def restated(restored, target, luma=False):
@@ -46,12 +37,12 @@ def restated(restored, target, luma=False):
     return torch.tensor(out, dtype=torch.float64)
 
 
-@pytest.mark.parametrize("case", CASES)
+@pytest.mark.parametrize("case", PSNRB_CASES)
 def test_psnrb_matches_reference(pkg, case):
     from grl_image_restoration_b200 import metrics
 
-    g = np.load(GOLDEN)
-    restored, target = golden_case(g, case)
+    g = np.load(PSNRB_GOLDEN)
+    restored, target = golden_pair(g, case)
     keep = restored.clone()
     got = metrics.psnrb(restored, target)
     assert torch.equal(restored, keep)
@@ -63,11 +54,11 @@ def test_psnrb_matches_reference(pkg, case):
         assert (got_y - torch.from_numpy(g[f"{case}_psnrb_y"]).double()).abs().max().item() <= 1e-4
 
 
-@pytest.mark.parametrize("case", CASES)
+@pytest.mark.parametrize("case", PSNRB_CASES)
 def test_psnrb_equals_float64_restatement(pkg, case):
     from grl_image_restoration_b200 import metrics
 
-    restored, target = golden_case(np.load(GOLDEN), case)
+    restored, target = golden_pair(np.load(PSNRB_GOLDEN), case)
     assert (metrics.psnrb(restored, target) - restated(restored, target)).abs().max().item() <= 1e-9
     if restored.shape[1] == 3:
         assert (metrics.psnrb(restored, target, "y") - restated(restored, target, luma=True)).abs().max().item() <= 1e-9
@@ -78,8 +69,8 @@ def test_normaliser_is_the_formula_not_the_count(pkg):
     2H summed positions instead is a different number on the golden."""
     from grl_image_restoration_b200 import metrics
 
-    g = np.load(GOLDEN)
-    restored, target = golden_case(g, "rgb_w20")
+    g = np.load(PSNRB_GOLDEN)
+    restored, target = golden_pair(g, "rgb_w20")
     want = torch.from_numpy(g["rgb_w20_psnrb"]).double()
     assert (metrics.psnrb(restored, target) - want).abs().max().item() <= 1e-4
     k = (metrics.tensor_round(restored) * 255).round().double()

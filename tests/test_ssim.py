@@ -2,53 +2,21 @@
 values produced by the reference's own ssim (tests/golden/ssim.npz, written by oracle/make_golden_ssim.py) and against the
 float64 restatement oracle/ssim_oracle.py in both forms: the reference's 2-D float32 window and the kernel's separable one.
 
-SCORE_GATE is the distance allowed between a score of this project and the reference's.  The reference convolves and sums
-in fp32.  Measured on the goldens (RGB / luma): flat 5.0e-7 / 4.6e-6, letterbox 4.5e-6 / 4.9e-6, sr_b2 8.1e-6 / 9.5e-6,
-gray 8.1e-6, tiny 7.4e-8 / 1.9e-8, clamp 3.0e-6 / 7.3e-6.  The float64 oracle with the reference's own 2-D float32 window
-lies within 2.7e-7 of the host computation on every one of them and as far from the reference as the host computation
-does, so the residue is the rounding of the reference's fp32 sums; the gate is twice the worst of it.  The engine logs 4
-decimals.
+SSIM_SCORE_GATE (metric_cases.py) is the distance allowed between a score of this project and the reference's.  The
+reference convolves and sums in fp32.  Measured on the goldens (RGB / luma): flat 5.0e-7 / 4.6e-6, letterbox 4.5e-6 /
+4.9e-6, sr_b2 8.1e-6 / 9.5e-6, gray 8.1e-6, tiny 7.4e-8 / 1.9e-8, clamp 3.0e-6 / 7.3e-6.  The float64 oracle with the
+reference's own 2-D float32 window lies within 2.7e-7 of the host computation on every one of them and as far from the
+reference as the host computation does, so the residue is the rounding of the reference's fp32 sums; the gate is twice
+the worst of it.  The engine logs 4 decimals.
 """
 import ctypes
-import os
 
 import numpy as np
 import pytest
 import torch
 
 import ssim_oracle
-
-GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ssim.npz")
-CASES = ["flat", "letterbox", "sr_b2", "gray", "tiny", "clamp"]
-SCORE_GATE = 2e-5
-
-
-def golden_case(g, name):
-    restored = (torch.from_numpy(g[f"{name}_restored"]) if f"{name}_restored" in g
-                else torch.from_numpy(g[f"{name}_restored8"].astype(np.float32) / np.float32(255.0)))
-    target = torch.from_numpy(g[f"{name}_target8"].astype(np.float32) / np.float32(255.0))
-    return restored, target, int(g[f"{name}_border"])
-
-
-def golden_scores(g, name):
-    """(ssim, ssim_y) of the reference; ssim_y of a one-channel case is its ssim."""
-    s = g[f"{name}_ssim"]
-    return s, (g[f"{name}_ssim_y"] if f"{name}_ssim_y" in g else s)
-
-
-def host_ssim(restored, target, border=0, maps=False):
-    """grl_ssim_host on two fp32 (B, C, H, W) host tensors -> (ssim_rgb, ssim_y[, map_rgb, map_y]) as NumPy float64."""
-    from grl_image_restoration_b200 import capi
-
-    a, b = np.ascontiguousarray(restored.numpy(), np.float32), np.ascontiguousarray(target.numpy(), np.float32)
-    B, C, H, W = a.shape
-    h, w = max(H - 2 * border, 0), max(W - 2 * border, 0)
-    s, sy = np.zeros(B), np.zeros(B)
-    m, my = np.zeros((B, C, h, w)), np.zeros((B, 1, h, w))
-    p = lambda x: x.ctypes.data_as(ctypes.c_void_p)  # noqa: E731
-    capi.check(capi.lib().grl_ssim_host(p(a), p(b), B, C, H, W, border, p(s), p(sy), p(m) if maps else None,
-                                        p(my) if maps and C == 3 else None))
-    return (s, sy, m, my) if maps else (s, sy)
+from metric_cases import SSIM_CASES, SSIM_GOLDEN, SSIM_SCORE_GATE, golden_pair, golden_scores, host_ssim
 
 
 def grid8(img):
@@ -88,17 +56,19 @@ def test_taps_equal_the_reference_window(pkg):
 
     t = np.zeros(11)
     capi.check(capi.lib().grl_ssim_taps_host(t.ctypes.data_as(ctypes.c_void_p)))
-    want = np.load(GOLDEN)["taps"]
+    want = np.load(SSIM_GOLDEN)["taps"]
     assert want.dtype == np.float64 and t.tobytes() == want.tobytes()  # gaussian(11, 1.5), bit for bit
     assert t.tobytes() == ssim_oracle.taps().tobytes()
     assert {"grl_ssim_f32", "grl_ssim_workspace", "grl_ssim_host", "grl_ssim_taps_host"} <= set(capi.header_symbols())
 
 
-@pytest.mark.parametrize("case", CASES)
+@pytest.mark.parametrize("case", SSIM_CASES)
 def test_host_equals_the_separable_oracle(pkg, case):
     """Same taps, same separable order of summation, float64 on both sides: what is left is the fma chains against
     NumPy's multiply-adds, a few ulp per map value."""
-    restored, target, border = golden_case(np.load(GOLDEN), case)
+    g = np.load(SSIM_GOLDEN)
+    restored, target = golden_pair(g, case)
+    border = int(g[f"{case}_border"])
     s, sy, m, my = host_ssim(restored, target, border, maps=True)
     want, want_y = oracle_scores(restored, target, border)
     assert np.abs(s - want).max() <= 1e-13 and np.abs(sy - want_y).max() <= 1e-13
@@ -126,9 +96,11 @@ def window_bound(a, b):
     return 1.01 * per_pixel.mean((-3, -2, -1))  # 1 % for the second-order terms
 
 
-@pytest.mark.parametrize("case", CASES)
+@pytest.mark.parametrize("case", SSIM_CASES)
 def test_host_against_the_2d_window_oracle(pkg, case):
-    restored, target, border = golden_case(np.load(GOLDEN), case)
+    g = np.load(SSIM_GOLDEN)
+    restored, target = golden_pair(g, case)
+    border = int(g[f"{case}_border"])
     s, sy = host_ssim(restored, target, border)
     want, want_y = oracle_scores(restored, target, border, window="2d")
     bound = window_bound(*planes(restored, target, border))
@@ -139,16 +111,17 @@ def test_host_against_the_2d_window_oracle(pkg, case):
     assert max(np.abs(s - want).max(), np.abs(sy - want_y).max()) <= 5e-7
 
 
-@pytest.mark.parametrize("case", CASES)
+@pytest.mark.parametrize("case", SSIM_CASES)
 def test_host_matches_the_reference(pkg, case):
-    g = np.load(GOLDEN)
-    restored, target, border = golden_case(g, case)
+    g = np.load(SSIM_GOLDEN)
+    restored, target = golden_pair(g, case)
+    border = int(g[f"{case}_border"])
     keep = restored.clone()
     s, sy = host_ssim(restored, target, border)
     assert torch.equal(restored, keep)
     want, want_y = golden_scores(g, case)
-    assert np.abs(s - want).max() <= SCORE_GATE, (s, want)
-    assert np.abs(sy - want_y).max() <= SCORE_GATE, (sy, want_y)
+    assert np.abs(s - want).max() <= SSIM_SCORE_GATE, (s, want)
+    assert np.abs(sy - want_y).max() <= SSIM_SCORE_GATE, (sy, want_y)
     if restored.shape[1] == 1:
         assert sy.tobytes() == s.tobytes()
 
@@ -156,7 +129,9 @@ def test_host_matches_the_reference(pkg, case):
 def test_letterbox_map_is_exactly_one(pkg):
     """Where every pixel under the window is black in both images the five sums are exactly 0 and the map is C1 C2 / C1 C2:
     the 12 black rows at either end leave 7 rows whose 11-row window sees nothing else."""
-    restored, target, border = golden_case(np.load(GOLDEN), "letterbox")
+    g = np.load(SSIM_GOLDEN)
+    restored, target = golden_pair(g, "letterbox")
+    border = int(g["letterbox_border"])
     assert not grid8(restored)[..., :12, :].any() and not grid8(target)[..., -12:, :].any()
     _, _, m, my = host_ssim(restored, target, border, maps=True)
     for mm in (m, my):
@@ -196,10 +171,11 @@ def test_refusals(pkg):
 
 # ------------------------------------------------------------------------------------------------ mutation controls
 # Each changes one thing the definition fixes, in the oracle or in what the host computation is given.  Those listed in
-# PINNED move some golden past SCORE_GATE; the others are checked to stay inside it, so that the statement "the goldens
+# PINNED move some golden past the gate; the others are checked to stay inside it, so that the statement "the goldens
 # do not pin this" is itself under test.
 def mutated_scores(g, case, mutation):
-    restored, target, border = golden_case(g, case)
+    restored, target = golden_pair(g, case)
+    border = int(g[f"{case}_border"])
     if mutation == "no_shave":
         return host_ssim(restored, target, 0)
     if mutation == "unrounded_luma":
@@ -211,8 +187,8 @@ def mutated_scores(g, case, mutation):
 
 
 def worst_distance(mutation):
-    g, worst = np.load(GOLDEN), 0.0
-    for case in CASES:
+    g, worst = np.load(SSIM_GOLDEN), 0.0
+    for case in SSIM_CASES:
         if case == "tiny" and mutation in ("reflect_padding", "valid_only"):
             continue  # 7 x 9: no reflection of 5 pixels, no valid window
         if mutation == "no_shave" and not int(g[f"{case}_border"]):
@@ -229,11 +205,11 @@ NOT_PINNED = ["unrounded_taps"]
 
 @pytest.mark.parametrize("mutation", PINNED)
 def test_mutation_fails_the_gate(pkg, mutation):
-    assert worst_distance(mutation) > SCORE_GATE, f"mutation {mutation} passes the gate: the goldens do not pin it"
+    assert worst_distance(mutation) > SSIM_SCORE_GATE, f"mutation {mutation} passes the gate: the goldens do not pin it"
 
 
 @pytest.mark.parametrize("mutation", NOT_PINNED)
 def test_mutation_the_goldens_do_not_pin(pkg, mutation):
     """Taps kept at full precision instead of 6 decimals: 9.3e-6 from the goldens at worst, which is the reference's own
     fp32 residue and no more.  The taps are pinned bit for bit by test_taps_equal_the_reference_window instead."""
-    assert worst_distance(mutation) <= SCORE_GATE
+    assert worst_distance(mutation) <= SSIM_SCORE_GATE
