@@ -144,6 +144,10 @@ _SIGNATURES = {
                             c_vp]),
     "grl_awgn_noise_host": (c_int, [c_vp, c_i64, ctypes.c_double, c_vp]),
     "grl_awgn_log_host": (c_int, [c_vp, c_i64, c_vp]),
+    "grl_mosaic_u8": (c_int, [ctypes.POINTER(GrlImageRef), ctypes.POINTER(GrlImageRef), c_int, c_vp]),
+    "grl_luma_u8": (c_int, [ctypes.POINTER(GrlImageRef), ctypes.POINTER(GrlImageRef), c_int, c_vp]),
+    "grl_mosaic_host": (c_int, [c_vp, c_int, c_int, c_vp]),
+    "grl_luma_host": (c_int, [c_vp, c_i64, c_vp]),
 }
 
 _lib = None

@@ -567,6 +567,109 @@ def awgn_log_host(x):
     return out
 
 
+def _rgb_u8_images(images, what):
+    """The list checks of mosaic_list and luma_list: (H, W, 3) uint8 on the current CUDA device."""
+    for i, t in enumerate(images):
+        if not isinstance(t, torch.Tensor):
+            raise ValueError(f"grl_b200: {what}: element {i} is a {type(t).__name__}, not a tensor")
+        capi.require_device(t)
+        if t.dtype != torch.uint8 or t.dim() != 3 or t.shape[2] != 3 or t.shape[0] < 1 or t.shape[1] < 1:
+            raise ValueError(f"grl_b200: {what} needs (H, W, 3) uint8 RGB images, got element {i}: {t.dtype} "
+                             f"{tuple(t.shape)}")
+
+
+def _rgb_u8_batch(img, what):
+    if not isinstance(img, torch.Tensor):
+        raise ValueError(f"grl_b200: {what} needs a tensor, got {type(img).__name__}")
+    capi.require_device(img)
+    if img.dtype != torch.uint8 or img.dim() != 4 or img.shape[3] != 3 or min(img.shape[1:3]) < 1:
+        raise ValueError(f"grl_b200: {what} needs (B, H, W, 3) uint8 RGB images, got {img.dtype} {tuple(img.shape)}")
+    return img.contiguous()
+
+
+def _mosaic_launch(srcs, outs):
+    capi.check(capi.lib().grl_mosaic_u8(_image_refs(srcs, capi.IMAGE_U8), _image_refs(outs, capi.IMAGE_RGGB), len(srcs),
+                                        capi.stream()))
+
+
+def mosaic(img):
+    """The demosaicking test command's input (DemosaicDataset.__getitem__, data/datasets/restoration_dm.py:33-37):
+    (B, H, W, 3) uint8 RGB images on the GPU -> new (B, 4, H // 2, W // 2) float32 packed RGGB planes (R, G of the even
+    rows, G of the odd rows, B), equal bit for bit to to_tensor(mosaic_CFA_Bayer(img[b])[1]); an odd last row or column is
+    dropped.  What GRL(input_format="rggb") takes.  One kernel per 128 images."""
+    img = _rgb_u8_batch(img, "mosaic")
+    B, H, W, _ = img.shape
+    out = torch.empty(B, 4, H // 2, W // 2, device=img.device, dtype=torch.float32)
+    if B:
+        _mosaic_launch(list(img.unbind(0)), list(out.unbind(0)))
+    return out
+
+
+def mosaic_list(images):
+    """mosaic of a list of differently sized (H_i, W_i, 3) uint8 images on the GPU -> list of new (4, H_i // 2, W_i // 2)
+    float32 tensors in input order, what GRL(input_format="rggb").forward_list takes.  One kernel per 128 images."""
+    images = list(images)
+    _rgb_u8_images(images, "mosaic_list")
+    if not images:
+        return []
+    srcs = [t.contiguous() for t in images]
+    outs = [torch.empty(4, t.shape[0] // 2, t.shape[1] // 2, device=t.device, dtype=torch.float32) for t in srcs]
+    _mosaic_launch(srcs, outs)
+    return outs
+
+
+def mosaic_host(img):
+    """mosaic of one (H, W, 3) uint8 CPU image, evaluated by the library's host copy of the same closed form (tests)."""
+    if img.dtype != torch.uint8 or img.dim() != 3 or img.shape[2] != 3:
+        raise ValueError(f"grl_b200: mosaic_host needs an (H, W, 3) uint8 image, got {img.dtype} {tuple(img.shape)}")
+    img = img.contiguous()
+    H, W, _ = img.shape
+    out = torch.empty(4, H // 2, W // 2, dtype=torch.float32)
+    capi.check(capi.lib().grl_mosaic_host(ctypes.c_void_p(img.data_ptr()), H, W, ctypes.c_void_p(out.data_ptr())))
+    return out
+
+
+def _luma_launch(srcs, outs):
+    capi.check(capi.lib().grl_luma_u8(_image_refs(srcs, capi.IMAGE_U8), _image_refs(outs, capi.IMAGE_U8), len(srcs),
+                                      capi.stream()))
+
+
+def luma(img):
+    """The gray JPEG test command's clean image on LIVE1 / BSDS500 / Urban100 (base_image.imread,
+    data/datasets/base_image.py:233-241): (B, H, W, 3) uint8 RGB images on the GPU -> new (B, H, W, 1) uint8, equal byte for
+    byte to rgb2ycbcr_np(img[b], y_only=True) (MATLAB's rgb2ycbcr luma of k / 255, rounded half to even).  One kernel per
+    128 images."""
+    img = _rgb_u8_batch(img, "luma")
+    out = torch.empty(*img.shape[:3], 1, device=img.device, dtype=torch.uint8)
+    if img.shape[0]:
+        _luma_launch(list(img.unbind(0)), list(out.unbind(0)))
+    return out
+
+
+def luma_list(images):
+    """luma of a list of differently sized (H_i, W_i, 3) uint8 images on the GPU -> list of new (H_i, W_i, 1) uint8
+    tensors in input order.  One kernel per 128 images."""
+    images = list(images)
+    _rgb_u8_images(images, "luma_list")
+    if not images:
+        return []
+    srcs = [t.contiguous() for t in images]
+    outs = [torch.empty(t.shape[0], t.shape[1], 1, device=t.device, dtype=torch.uint8) for t in srcs]
+    _luma_launch(srcs, outs)
+    return outs
+
+
+def luma_host(rgb):
+    """luma of (..., 3) uint8 CPU pixels -> (..., 1) uint8, evaluated by the library's host copy of the same closed form
+    (tests)."""
+    if rgb.dtype != torch.uint8 or rgb.dim() < 1 or rgb.shape[-1] != 3:
+        raise ValueError(f"grl_b200: luma_host needs (..., 3) uint8 pixels, got {rgb.dtype} {tuple(rgb.shape)}")
+    rgb = rgb.contiguous()
+    out = torch.empty(*rgb.shape[:-1], 1, dtype=torch.uint8)
+    capi.check(capi.lib().grl_luma_host(ctypes.c_void_p(rgb.data_ptr()), out.numel(), ctypes.c_void_p(out.data_ptr())))
+    return out
+
+
 def stripe_attention(qkv, anchor, B, tok_grid, anc_grid, heads, scale1, bias1, scale2, bias2, use_mask, out=None):
     """qkv (B, L, 3c) view (stripe half), anchor (B, Ha, Wa, c) -> (B, L, c)."""
     qp, ldq = _token_rows(qkv, "qkv")

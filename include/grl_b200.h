@@ -495,6 +495,21 @@ int grl_awgn_noise_host(const uint32_t* key, int64_t count, double scale, double
 /* The device's double-double log (awgn_log_cr) evaluated on the CPU (tests): out[i] = log(x[i]), x[i] positive normal. */
 int grl_awgn_log_host(const double* x, int64_t n, double* out);
 
+/* ---- Dataset-side inputs of the dm and gray JPEG test commands (csrc/dataset_u8.cu, csrc/grl_dataset_u8.h) ------------
+ * Bayer mosaic: DemosaicDataset.__getitem__ (data/datasets/restoration_dm.py:33-37), to_tensor(mosaic_CFA_Bayer(img)[1])
+ * (utils/utils_mosaic.py:124-147).  MATLAB luma: rgb2ycbcr_np(img, y_only=True) (utils/utils_image.py:143-190), the clean
+ * image of the gray JPEG command on LIVE1 / BSDS500 / Urban100 (data/datasets/base_image.py:233-241).  Both exact. */
+/* src[i] (H, W, 3) uint8 GRL_IMAGE_U8 -> dst[i] (4, H / 2, W / 2) fp32 GRL_IMAGE_RGGB (H, W of the dst ref are the planes'),
+ * planes R, G (even rows), G (odd rows), B of k / 255; an odd last row / column is dropped.  kDatasetPerLaunch (128)
+ * images per launch; no workspace. */
+int grl_mosaic_u8(const GrlImageRef* src, const GrlImageRef* dst, int n, void* stream);
+/* src[i] (H, W, 3) uint8 GRL_IMAGE_U8 -> dst[i] (H, W, 1) uint8 GRL_IMAGE_U8: the luma byte of every pixel. */
+int grl_luma_u8(const GrlImageRef* src, const GrlImageRef* dst, int n, void* stream);
+/* The same closed forms on the CPU (tests); HOST pointers.  mosaic: one (H, W, 3) image -> out (4, H / 2, W / 2) fp32.
+ * luma: n RGB pixels (n, 3) -> out (n) bytes. */
+int grl_mosaic_host(const uint8_t* img, int H, int W, float* out);
+int grl_luma_host(const uint8_t* rgb, int64_t n, uint8_t* out);
+
 #ifdef __cplusplus
 }
 #endif
