@@ -42,17 +42,13 @@ import torch.nn.functional as F
 
 import archs
 import grl_oracle as O
-from grl_oracle import L_LN, U, gamma, ln_bound, ln_reference
-from support import bound_ratio, grid_t, ulp
+from f32_cases import (ACT_GELU, ACT_LEAKY, ACT_NONE, B, GATE_ATTN, GATE_CHAIN, POOL_ROWS, Pass, attn_ref,
+                       bias_table_bound, gate_bound, gate_reference, gemm_bound, im2col, ulp_stats, windows)
+from grl_oracle import L_LN, ln_bound, ln_reference
+from support import bound_ratio, grid_t
 
-B = 2
 GUARD = 3          # NaN guard rows before and after every output buffer
-ERFF_ULP = 2       # CUDA C++ Programming Guide, maximum ulp error of erff / expf (no fast math)
-EXPF_ULP = 2
 OLD_TOL = 2e-4     # the max-abs bound of the operator tests this file replaces
-GATE_ATTN = 1695.0   # fp32 ulps at max(|ref|, row rms): 2 x the worst case, 847.2 (small/sr window; H100 80GB HBM3, 400 W)
-GATE_CHAIN = 2165.0  # both stripe passes against the float64 chain: 2 x the worst case, 1082.3 (same card)
-ACT_NONE, ACT_GELU, ACT_LEAKY = 0, 1, 2
 
 
 def launches_of(launches, kind):
@@ -314,12 +310,6 @@ def check_written(buf, cols, what, guard_cols=0):
         assert bool(inner[:, cols:].isnan().all()), f"{what}: wrote into the guard columns"
 
 
-def ulp_stats(got, ref):
-    """max |got - ref| in fp32 ulps at max(|ref|, the row's rms) (rows: the last dimension)."""
-    scale = torch.maximum(ref.abs(), ref.pow(2).mean(-1, keepdim=True).sqrt())
-    return float(((got.double() - ref).abs() / ulp(scale, torch.float32)).nan_to_num(float("inf")).max())
-
-
 def old_misses(mut, ref):
     """The old operator tests' bound would pass a kernel that computes `mut` instead of `ref`."""
     return float((mut - ref).abs().nan_to_num(float("inf")).max()) <= OLD_TOL
@@ -332,14 +322,6 @@ def report(name, ratio, gate, kind="bound"):
 
 
 # --------------------------------------------------------------------------------------------------- GPU: attention
-
-
-def windows(t, g, heads):
-    """(B, H, W, c) tokens -> (B nW, heads, wh ww, c / heads) in the kernel's window order (roll by -shift, then
-    partition); g = (H, W, wh, ww, sh, sw)."""
-    _, _, wh, ww, sh, sw = g
-    t = torch.roll(t, (-sh, -sw), (1, 2)) if sh or sw else t
-    return O.partition(t, (wh, ww)).reshape(-1, wh * ww, heads, t.shape[-1] // heads).transpose(1, 2)
 
 
 def cpb_like(rows_hw, df, heads, seed, device):
@@ -355,46 +337,6 @@ def logit_scales(heads, reverse, device):
     """Per-head logit scales (natural log) from ln 5 to ln 150: they cross the clamp at ln 100."""
     s = torch.linspace(math.log(5.0), math.log(150.0), heads) if heads > 1 else torch.tensor([math.log(150.0)])
     return (s.flip(0) if reverse else s).float().to(device)
-
-
-def unwindows(o, g, nb):
-    """Inverse of `windows`: (B nW, heads, wh ww, d) -> (B, H, W, heads d)."""
-    H, W, wh, ww, sh, sw = g
-    t = O.unpartition(o.transpose(1, 2).reshape(-1, wh, ww, o.shape[1] * o.shape[3]), (wh, ww), (H, W))
-    assert t.shape[0] == nb
-    return torch.roll(t, (sh, sw), (1, 2)) if sh or sw else t
-
-
-class Pass(NamedTuple):
-    """One attention launch on float64 operands: q, k (B, H, W, c) tokens; v tokens or, for stripe pass 2, the dense
-    X1 (B nW, heads, Nk, d); o_dense: the launch writes dense X1 (stripe pass 1) instead of tokens."""
-    gq: tuple
-    gk: tuple
-    q: torch.Tensor
-    k: torch.Tensor
-    v: torch.Tensor
-    v_dense: bool
-    o_dense: bool
-    scale: torch.Tensor
-    table: torch.Tensor
-    use_mask: bool
-
-
-def attn_ref(p, heads, mutation=None, index=None, mask=None, v=None, roll=True, drop_last_key=False):
-    """float64 reference of one pass in the kernel's window layout (B nW, heads, Nq, d).  roll=False: the kernel read
-    and wrote the un-rolled grids."""
-    gq, gk = (p.gq, p.gk) if roll else (p.gq[:4] + (0, 0), p.gk[:4] + (0, 0))
-    i0, m0 = O.attn_pair_geometry(p.gq, p.gk, p.use_mask)
-    index = i0 if index is None else index
-    mask = (m0 if mask is None else mask) if p.use_mask else None
-    v = p.v if v is None else v
-    q, k, vw = windows(p.q, gq, heads), windows(p.k, gk, heads), v if p.v_dense else windows(v, gk, heads)
-    if drop_last_key:
-        k, vw, index, mask = k[:, :, :-1], vw[:, :, :-1], index[:, :-1], None if mask is None else mask[..., :-1]
-    o = O.attn_f32_reference(q, k, vw, p.scale, p.table, index, mask, mutation)
-    if not roll and not p.o_dense:  # written to the un-rolled token positions
-        o = windows(unwindows(o, gq, B), p.gq, heads)
-    return o
 
 
 def attn_mutations(p, heads, x1_kernel=None):
@@ -531,45 +473,6 @@ def test_attention_path(lib, device, case):
 
 HT, WT, M_LIN = 13, 21, 200
 ZERO_ROWS = (7, 150)  # linear rows of zero input: the accumulator is exactly 0
-
-
-def im2col(x, transposed=False, wrap=False):
-    """(B, H, W, Cin) -> (B H W, 9 Cin) with k = tap Cin + c, tap = 3 (dy + 1) + (dx + 1) (pack_conv_weight's order).
-    Padding reads zero; wrap=True reads the flat neighbour m + dy W + dx instead (the previous row or image)."""
-    Bn, H, W, C = x.shape
-    flat = x.reshape(-1, C)
-    M = flat.shape[0]
-    m = torch.arange(M, device=x.device)
-    yy, xx = (m // W) % H, m % W
-    cols = []
-    for t in range(9):
-        dy, dx = divmod(t, 3)
-        if transposed:
-            dy, dx = dx, dy
-        dy, dx = dy - 1, dx - 1
-        src = m + dy * W + dx
-        ok = (src >= 0) & (src < M) if wrap else (yy + dy >= 0) & (yy + dy < H) & (xx + dx >= 0) & (xx + dx < W)
-        cols.append(torch.where(ok[:, None], flat[src.clamp(0, M - 1)], 0.0))
-    return torch.cat(cols, 1)
-
-
-def gemm_bound(A, w, b, act, slope, res):
-    """Per-element bound on |kernel - float64| of act(A w^T + b) (+ res), for a sequential FMA chain over k."""
-    K = A.shape[1]
-    v = A @ w.T + b
-    e = gamma(K) * (A.abs() @ w.abs().T)
-    e = e + U * (v.abs() + e)                                              # + bias
-    if act == ACT_GELU:
-        y = O._gelu(v)
-        e = 1.13 * e + 0.5 * v.abs() * (ERFF_ULP * U + 3 * U) + U * y.abs()  # |GELU'| <= 1.13; erf term absolute
-    elif act == ACT_LEAKY:
-        y = torch.where(v > 0, v, v * slope)
-        e = max(1.0, slope) * e + U * y.abs()
-    else:
-        y = v
-    if res is not None:
-        e = e + U * ((y + res).abs() + e)
-    return e, v
 
 
 def gemm_operands(case, device, seed):
@@ -721,37 +624,6 @@ def test_ln_residual(lib, device, C, with_x, cab):
 
 # ------------------------------------------------------------------------------------------------ GPU: channel gate
 
-POOL_ROWS = 256  # rows per partial sum (ops_f32.cu: kPoolRows)
-
-
-def gate_reference(y, w1, b1, w2, b2, mutation=None):
-    L = y.shape[1]
-    chunks = -(-L // POOL_ROWS)
-    if mutation == "partial last chunk dropped":
-        mean = y[:, :(chunks - 1) * POOL_ROWS].sum(1) / L
-    elif mutation == "division by chunks x 256":
-        mean = y.sum(1) / (chunks * POOL_ROWS)
-    else:
-        mean = y.mean(1)
-    hpre = mean @ w1.T + b1
-    h = hpre if mutation == "ReLU missing" else torch.relu(hpre)
-    return torch.sigmoid(h @ w2.T + b2)
-
-
-def gate_bound(y, w1, b1, w2, b2):
-    L, C = y.shape[1], y.shape[2]
-    R = w1.shape[0]
-    mean = y.mean(1)
-    e_mean = gamma(POOL_ROWS + -(-L // POOL_ROWS)) * y.abs().sum(1) / L + U * mean.abs()
-    hpre = mean @ w1.T + b1
-    e_h = e_mean @ w1.abs().T + gamma(-(-C // 32) + 5) * (mean.abs() @ w1.abs().T) + U * hpre.abs()
-    h = torch.relu(hpre)
-    s = h @ w2.T + b2
-    e_s = e_h @ w2.abs().T + gamma(R) * (b2.abs() + h @ w2.abs().T)
-    gt = torch.sigmoid(s)
-    return gt * (1 - gt) * e_s + gt * (2 * EXPF_ULP * U * (1 - gt) + 2 * U)
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("L", [1, 100, 1000])
 def test_channel_gate(lib, device, L):
@@ -812,17 +684,6 @@ def test_avgpool_bit_exact(lib, device, df):
             s = s + xc[:, :, dy, :, dx]
     ref = (s / float(df * df)).reshape(-1, C)
     assert torch.equal(out.cpu(), ref), float((out.cpu() - ref).abs().max())
-
-
-def bias_table_bound(t, w1, b1, w2):
-    """16 sigmoid(W2 relu(W1 t + b1)): two FMAs per hidden unit, a sequential FMA chain over them, expf."""
-    hpre = t @ w1.T + b1
-    e_h = gamma(2) * (t.abs() @ w1.abs().T + b1.abs())
-    h = torch.relu(hpre)
-    acc = h @ w2.T
-    e_acc = e_h @ w2.abs().T + gamma(w1.shape[0]) * (h @ w2.abs().T)
-    sg = torch.sigmoid(acc)
-    return (16 * (sg * (1 - sg) * e_acc + sg * (2 * EXPF_ULP * U * (1 - sg) + 2 * U))).T, (16 * sg).T
 
 
 @pytest.mark.gpu

@@ -39,13 +39,13 @@ import attn_cases as A
 import gemm_cases as G
 import grl_oracle as O
 from _pkgload import load_package
-from support import bound_ratio, build, dm_model, grid_t, native_model, zoo_model
+from replay_base import Recorder, ReplayBase, _base, replay_case
+from support import bound_ratio, grid_t
 
 load_package()
 from grl_image_restoration_b200 import functional as KF, tc as TC  # noqa: E402
 
 U = 2.0 ** -24
-MAX_WINDOWS = 16
 STREAM_READERS = (".qkv", ".cab1", ".fc1", ".conv", "conv_after_body")  # GEMMs whose x16 is the residual stream's copy
 MUTATIONS = ("qkv fed the previous block's input", "proj residual of the previous block",
              "window attention with the previous block's constants")
@@ -56,23 +56,6 @@ def checkers(tc, K):
     return {tc.gemm: "gemm", tc.pack_rows: "pack_rows", tc.head_pack: "head_pack", tc.head_pack_rggb: "head_pack_rggb",
             tc.slot_scale: "slot_scale", tc.bias_table_log2: "bias_table", tc.avgpool16: "avgpool16",
             tc.attention: "attention", tc.channel_gate: "channel_gate", K.ln_residual: "ln_residual"}
-
-
-def _base(t):
-    return t if t._base is None else t._base
-
-
-def _checksum(t):
-    w = t.reshape(-1).view({2: torch.int16, 4: torch.int32}[t.element_size()])
-    return torch.stack([w.sum(dtype=torch.int64), w[::2].sum(dtype=torch.int64)])
-
-
-def _tensors(v):
-    if isinstance(v, torch.Tensor):
-        yield v
-    elif isinstance(v, (tuple, list)):
-        for e in v:
-            yield from _tensors(e)
 
 
 def same16(a, b):
@@ -124,97 +107,28 @@ def bias_ratio(transform, coords, out):
     return float(((out[:, 0, :rows].double() - ref).abs() / bound).max())
 
 
-class Replay(TC.Device):
-    """tc.Device that checks every launch (module docstring).  Results: `worst` {family: (statistic, gate, where)},
-    `failures` [(family, where, detail)], `mutations` {name: [caught, applied]}, `rescales`, `sat16`."""
+class Replay(ReplayBase, TC.Device):
+    """tc.Device that checks every launch (module docstring).  Results as replay_base.ReplayBase, plus `rescales` and
+    `sat16`."""
 
     def __init__(self, model, mutate=True, seed=0):
-        self.tc, self.K, self.model = TC, KF, model
+        super().__init__(model, MUTATIONS, mutate, seed)
+        self.tc, self.K = TC, KF
         self.fmt = TC.FMT[model.precision]
         self.dtype = TC.DTYPE[self.fmt]
         self.methods = checkers(TC, KF)
-        self.mutate, self.seed = mutate, seed
-        self.owner = {}  # id(logit_scale / attn_transform) -> block name
-        self.blocks = {}
-        for si, layer in enumerate(model.layers):
-            for bi, blk in enumerate(layer.blocks):
-                name = f"stage{si}.block{bi}"
-                self.blocks[name] = (blk, si, bi, len(layer.blocks))
-                wa, sa = blk.attn.window_attn, blk.attn.stripe_attn
-                for m in (wa.attn_transform, sa.attn_transform1, sa.attn_transform2):
-                    self.owner[id(m)] = name
-                self.owner[id(wa.attn_transform.logit_scale)] = name
-        self.block, self.prev = None, None  # names of the current and the previous block
-        self.saved = {}  # block name -> {"x16", "res", "table_w", "scales"} for the mutation controls
         self.pass1 = {}  # block name -> (window indices, emulated X1 of those windows)
-        self.sums = {}   # base data_ptr -> (weakref to the base, checksum, writer)
         self.stream32 = None
-        self.worst, self.failures = {}, []
-        self.mutations = {m: [0, 0] for m in MUTATIONS}
-        self.below = {}  # mutation -> blocks where it does not move the emulated output past twice the gate
         self.rescales, self.sat16 = 0, 0
 
-    # ---- bookkeeping ------------------------------------------------------------------------------
-    def _gate(self, family, stat, gate, ok, where, detail=""):
-        w = self.worst.get(family)
-        if w is None or stat > w[0]:
-            self.worst[family] = (stat, gate, where)
-        if not ok:
-            self.failures.append((family, where, f"{stat} (gate {gate}) {detail}"))
-
-    def _check_reads(self, tensors, where):
-        for t in tensors:
-            b = _base(t)
-            e = self.sums.get(b.data_ptr())
-            if e is not None and e[0]() is b and not torch.equal(_checksum(b), e[1]):
-                self.failures.append(("integrity", where, f"a buffer {e[2]} wrote changed before this launch read it"))
-
     def _record_writes(self, tensors, where):
+        super()._record_writes(tensors, where)
         for t in tensors:
-            b = _base(t)
-            self.sums[b.data_ptr()] = (weakref.ref(b), _checksum(b), where)
-            if b.dtype == torch.float16:
+            if _base(t).dtype == torch.float16:
                 self.sat16 += int((t.float().abs() == 65504.0).sum())
 
-    def _set_block(self, name):
-        if name != self.block:
-            self.prev, self.block = self.block, name
-            self.saved = {k: v for k, v in self.saved.items() if k == self.prev}
-            self.pass1 = {}
-
-    def _blk(self):
-        return self.blocks[self.block][0]
-
-    def _full_windows(self):
-        _, _, bi, n = self.blocks[self.block]
-        return bi == 0 or bi == n - 1
-
-    def _mutation_here(self):
-        """Mutation controls run at the first and last block of each stage that have a previous block."""
-        return self.mutate and self.prev is not None and self._full_windows()
-
-    def _mut(self, name, caught):
-        self.mutations[name][1] += 1
-        self.mutations[name][0] += bool(caught)
-        if not caught:
-            self.failures.append(("mutation", self.block, f"'{name}' passes its gate"))
-
-    # ---- the launcher -----------------------------------------------------------------------------
-    def listed(self, name, fn, *args, **kw):
-        self.run(fn, *args, _name=name, **kw)
-
-    def run(self, fn, *args, _name=None, **kw):
-        method = self.methods.get(fn)
-        if method is None:
-            raise AssertionError(f"Replay has no checker for {getattr(fn, '__qualname__', fn)}")
-        outs = getattr(self, f"_outs_{method}")(*args, **kw)
-        ins = [t for t in _tensors(list(args) + list(kw.values())) if all(t is not o for o in outs)]
-        where = _name or (f"{self.block}:{method}" if self.block else method)
-        self._check_reads(ins, where)
-        fn(*args, **kw)
-        torch.cuda.synchronize()
-        getattr(self, f"_check_{method}")(*args, _name=_name, **kw)
-        self._record_writes(outs, where)
+    def _block_changed(self):
+        self.pass1 = {}
 
     # ---- outputs of each wrapper ------------------------------------------------------------------
     def _outs_gemm(self, *a, **kw):
@@ -389,13 +303,6 @@ class Replay(TC.Device):
         self.stream32 = out
 
     # ---- attention --------------------------------------------------------------------------------
-    def _windows(self, Bw):
-        if self._full_windows() or Bw <= MAX_WINDOWS:
-            return torch.arange(Bw)
-        g = torch.Generator().manual_seed(self.seed * 7919 + sum(map(ord, self.block)))
-        mid = 1 + torch.randperm(Bw - 2, generator=g)[:MAX_WINDOWS - 2]
-        return torch.cat([torch.tensor([0, Bw - 1]), mid]).sort().values
-
     def _check_attention(self, gq, gk, q, q_off, k, k_off, v, v_off, out, o_off, B, heads, bias, use_mask,
                          v_dense=False, o_dense=False, tag="attn", ones_col=False, _name=None):
         blk = self._blk()
@@ -449,22 +356,12 @@ class Replay(TC.Device):
                 if A.compare(em_m, emul, d, self.dtype)[0] > 2 * A.GATE_ULP:
                     self._mut(MUTATIONS[2], A.compare(got[idx], em_m, d, self.dtype)[0] > A.GATE_ULP)
                 else:
-                    self.below[MUTATIONS[2]] = self.below.get(MUTATIONS[2], 0) + 1
+                    self._below(MUTATIONS[2])
         if role == "window":
             self.saved.setdefault(self.block, {})["table_w"] = table.clone()
 
-    # ---- report -----------------------------------------------------------------------------------
     def report(self, label, seconds, peak):
-        lines = [f"\n[replay] {label}: {seconds:.1f} s, peak memory {peak / 2 ** 30:.2f} GiB, warp rescales "
-                 f"{self.rescales}, fp16 operands at +-65504: {self.sat16}"]
-        for fam, (s, gate, where) in sorted(self.worst.items()):
-            lines.append(f"  {fam}: worst {s:.4g} (gate {gate}) at {where}")
-        for name, (c, n) in self.mutations.items():
-            lines.append(f"  mutation '{name}': fails its gate {c} / {n}"
-                         + (f" ({self.below[name]} more below twice the gate)" if name in self.below else ""))
-        for f in self.failures[:40]:
-            lines.append(f"  FAIL {f}")
-        print("\n".join(lines))
+        super().report(label, seconds, peak, f", warp rescales {self.rescales}, fp16 operands at +-65504: {self.sat16}")
 
 
 def replay(tc, model, x, rggb=False, mutate=True, seed=0, label=""):
@@ -480,21 +377,6 @@ def replay(tc, model, x, rggb=False, mutate=True, seed=0, label=""):
 
 
 # ---------------------------------------------------------------------------------------------------------- CPU
-
-
-class Recorder(TC.Listing):
-    """tc.Listing that also records the wrappers of `run` launches."""
-
-    def __init__(self):
-        super().__init__()
-        self.fns = {}
-
-    def listed(self, name, fn, *a, **kw):
-        self.fns.setdefault(fn, name)
-        super().listed(name, fn, *a, **kw)
-
-    def run(self, fn, *a, **kw):
-        self.fns.setdefault(fn, getattr(fn, "__qualname__", repr(fn)))
 
 
 def test_every_forward_wrapper_has_a_replay_checker(pkg):
@@ -529,27 +411,6 @@ def tc(pkg, device):
     return T
 
 
-def _case(pkg, oracle, cases, golden_loader, device, name):
-    """(model, input, rggb) of a replay case."""
-    kind, _, rest = name.partition(":")
-    if kind == "native":
-        shape_name, precision = rest.split("-")
-        m, x, _ = native_model(pkg, oracle, shape_name, "spread", device, precision)
-        return m, x.to(device), False
-    if kind == "zoo":
-        zname, precision = rest.rsplit("-", 1)
-        m, gold = zoo_model(pkg, oracle, zname, device, precision)
-        return m, torch.from_numpy(gold["x"]).to(device), False
-    if kind == "dm":
-        m = dm_model(pkg, oracle, device, "fp16")
-        return m, golden_loader("dm_b2_40x56.npz")["cfa4"].to(device), True
-    mname, precision = rest.rsplit("-", 1)
-    c = cases[mname]
-    m = build(pkg, oracle, c["cfg"], device, precision, style="routed")
-    x = oracle.synth_input((c["batch"], c["cfg"]["in_channels"], *c["hw"]), seed=1234, noise_sigma=c["sigma"])
-    return m, x.to(device), False
-
-
 MICRO = ["micro_cab_x2", "micro_pad_dn", "micro_groups", "micro_odd_d", "micro_gray"]
 CASES = (["native:cfg2-fp16", "native:cfg3-fp16", "native:cfg4-fp16", "native:cfg4-bf16", "native:cfg5-fp16",
           "zoo:bsr_b2_40x56-fp16", "zoo:defocus_dual_b2_48x80-fp16", "zoo:defocus_dual_b2_48x80-bf16",
@@ -564,7 +425,7 @@ def _assert_clean(rp):
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", CASES)
 def test_replay(pkg, oracle, cases, golden_loader, tc, device, name):
-    model, x, rggb = _case(pkg, oracle, cases, golden_loader, device, name)
+    model, x, rggb = replay_case(pkg, oracle, cases, golden_loader, device, name)
     model.use_cuda_graph = False
     y, rp = replay(tc, model, x, rggb, label=name)  # first: the attention constants are computed under the replay
     assert torch.equal(y, model(x).float()), "the replayed forward differs from model(x)"
