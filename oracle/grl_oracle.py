@@ -745,7 +745,8 @@ def forward_features(sd, cfg, x):
     c = full_config(cfg)
     x_size = (x.shape[2], x.shape[3])
     t = layer_norm(sd, "norm_start.", x.flatten(2).transpose(1, 2))
-    tim = table_index_mask(cfg, x_size)
+    tim = {k: v.to(x.device, x.dtype) if v.is_floating_point() else v.to(x.device)
+           for k, v in table_index_mask(cfg, x_size).items()}
     for s in range(len(c["depths"])):
         t = transformer_stage(sd, cfg, s, t, x_size, tim)
     t = layer_norm(sd, "norm_end.", t)
@@ -764,9 +765,9 @@ def grl_forward(sd, cfg, x):
     except BaseException:
         x = F.pad(x, (0, pw, 0, ph), "constant")
     if c["in_channels"] == 3:
-        mean = torch.tensor((0.4488, 0.4371, 0.4040), dtype=x.dtype).view(1, 3, 1, 1)
+        mean = torch.tensor((0.4488, 0.4371, 0.4040), dtype=x.dtype, device=x.device).view(1, 3, 1, 1)
     else:
-        mean = torch.zeros(1, 1, 1, 1, dtype=x.dtype)
+        mean = torch.zeros(1, 1, 1, 1, dtype=x.dtype, device=x.device)
     x = (x - mean) * c["img_range"]
     up = c["upsampler"]
     if up in ("pixelshuffle", "pixelshuffledirect", "nearest+conv"):

@@ -1,7 +1,8 @@
 """The architectures the launch-path tests walk (test_gpu_tc_gemm.py, test_gpu_tc_attn.py, test_gpu_f32_paths.py): every
 configs.RELEASED entry with its own in_channels, and every grl_config of the VARIANTS x TASKS grid (which also holds
 architectures without a released checkpoint, such as GRL-Tiny deblurring).  Each is built once per precision, at the
-smallest size its windows and stripes tile: any size they tile gives the same launch paths."""
+smallest size its windows and stripes tile: any size they tile gives the same launch paths (test_command_paths.py checks
+this at the sizes the released test commands run)."""
 import math
 from functools import lru_cache
 

@@ -124,10 +124,13 @@ def stats32(got, ref, extra=0.0):
     return float((err / ulp(row_scale(ref), torch.float32)).max())
 
 
-def check16_only(got, ref, dtype, gelu):
+def check16_only(got, ref, dtype, gelu, acc_err=None):
     """16-bit-only output: RNE16(ref) unless ref lies within delta of a rounding boundary.  Returns (ok, fraction of
-    elements allowed either neighbour, fraction that differ from RNE16(ref))."""
+    elements allowed either neighbour, fraction that differ from RNE16(ref)).  acc_err: an absolute bound on the fp32
+    accumulation's error per element, added to delta (through GELU: times max |GELU'| = 1.13)."""
     delta = GATE32 * ulp(row_scale(ref), torch.float32) + (O.GELU_AS_ABS_ERR if gelu else 0.0)
+    if acc_err is not None:
+        delta = delta + (1.13 if gelu else 1.0) * acc_err
     lo, hi, mid = (ref - delta).to(dtype).double(), (ref + delta).to(dtype).double(), ref.to(dtype)
     g = got.double()
     ok = bool(((g >= lo) & (g <= hi)).all())
@@ -240,9 +243,10 @@ def instantiate(tc, launch, fmt, device, seed, batch=B, size=(HT, WT), L=L_CASE)
     return Run(launch, dict(x16=x16, w16=w16, bias=b32, **kw), ops, bufs, path(run_launch))
 
 
-def evaluate(tc, run, got, ref, fmt, row0=0, high_mean_rows=HIGH_MEAN_ROWS):
+def evaluate(tc, run, got, ref, fmt, row0=0, high_mean_rows=HIGH_MEAN_ROWS, acc_err=None):
     """Gate results {what: (statistic, passes)} of the kernel outputs `got` against reference `ref`, whose rows are
-    the problem's rows from row0 on.  LayerNorm rows listed in high_mean_rows are gated by GATE_LN_SHIFT."""
+    the problem's rows from row0 on.  LayerNorm rows listed in high_mean_rows are gated by GATE_LN_SHIFT.  acc_err: see
+    check16_only (16-bit-only outputs of a bias / activation epilogue)."""
     a, dt = run.kw, tc.DTYPE[fmt]
     epi = a["epi"]
     gelu = a["act"] == 1
@@ -275,7 +279,7 @@ def evaluate(tc, run, got, ref, fmt, row0=0, high_mean_rows=HIGH_MEAN_ROWS):
             yr = y[:, :real]
             if epi == tc.EPI_QKV:  # the row of a normalised output is its 32-wide slot
                 g16, yr = g16.reshape(-1, 32), yr.reshape(-1, 32)
-            ok, allowed, differ = check16_only(g16, yr, dt, gelu)
+            ok, allowed, differ = check16_only(g16, yr, dt, gelu, None if acc_err is None else acc_err[:, :real])
             out["16-bit"] = ((allowed, differ), ok)
     if a.get("ps_r"):
         ok, allowed, differ = check16_only(got["out_bf16"], ref["ps"], dt, gelu)

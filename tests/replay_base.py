@@ -8,9 +8,12 @@ import weakref
 
 import torch
 
+import command_cases as CC
+import grl_oracle as O
 from support import build, dm_model, native_model, zoo_model
 
 MAX_WINDOWS = 16  # attention windows checked per launch outside the first and last block of a stage
+GEOMETRIES = 4    # attention geometries a replay keeps (a block's three passes, and the next block's first)
 
 
 def _base(t):
@@ -32,9 +35,13 @@ def _tensors(v):
 
 def replay_case(pkg, oracle, cases, golden_loader, device, name):
     """(model, input, rggb) of a replay case "kind:what-precision": native:<shape> on "spread" weights, zoo:<golden>,
-    dm:<golden> through the packed-Bayer head, micro:<case>[@HxW] on "routed" weights (at its own size or H x W)."""
+    dm:<golden> through the packed-Bayer head, micro:<case>[@HxW] on "routed" weights (at its own size or H x W),
+    command:<checkpoint>@<H>x<W> (command_cases.py: a released checkpoint at the size its test command runs)."""
     kind, _, rest = name.partition(":")
     rest, precision = rest.rsplit("-", 1)
+    if kind == "command":
+        m, x, rggb = CC.model_and_input(pkg, oracle, CC.BY_NAME[f"command:{rest}"], device, precision)
+        return m, x.to(device), rggb
     if kind == "native":
         m, x, _ = native_model(pkg, oracle, rest, "spread", device, precision)
         return m, x.to(device), False
@@ -94,6 +101,7 @@ class ReplayBase:
         self.worst, self.failures = {}, []
         self.mutations = {m: [0, 0] for m in mutations}
         self.below = {}
+        self.geometries = {}  # (gq, gk, use_mask) -> grl_oracle.attn_pair_geometry, the GEOMETRIES latest
 
     # ---- bookkeeping ------------------------------------------------------------------------------
     def _gate(self, family, stat, gate, ok, where, detail=""):
@@ -146,6 +154,18 @@ class ReplayBase:
 
     def _below(self, name):
         self.below[name] = self.below.get(name, 0) + 1
+
+    def _geometry(self, gq, gk, use_mask):
+        """grl_oracle.attn_pair_geometry of a launch, kept for the next launches of the replay: a whole-frame stripe
+        mask is over a GB and takes seconds to build on the host, and every block uses its geometries several times."""
+        key = (tuple(gq), tuple(gk), bool(use_mask))
+        g = self.geometries.pop(key, None)
+        if g is None:
+            g = O.attn_pair_geometry(*key)
+        self.geometries[key] = g  # most recent last
+        while len(self.geometries) > GEOMETRIES:
+            self.geometries.pop(next(iter(self.geometries)))
+        return g
 
     def _windows(self, Bw):
         """Window indices to check: all of them in the first and last block of a stage, else the first, the last and

@@ -28,9 +28,12 @@ correlated q / k), with the bounds and gates of test_gpu_f32_paths.py (tests/f32
     have the same sum when a later launch reads it; a wrapper without a checker fails.
 Mutation controls, computed on the reference side (never an edited kernel), at the first and last block of each stage
 that has a previous block: the QKV linear fed the previous block's input, ln_residual given the previous block's
-residual, window attention with the previous block's table and logit scales, the CAB gate of the previous block.  A
+residual, window attention with the previous block's table and logit scales, the CAB gate of the previous block; and at
+the sizes the test commands run (`command:` cases, tests/command_cases.py) the output cropped at the padded pitch (where
+Wc < Wp) and shifted window attention with the shift mask of the transposed window grid (non-square grids).  A
 mutation applies where it moves the float64 result by more than twice the gate, and must fail its gate wherever it
-applies; the other blocks are counted apart.
+applies; the other blocks are counted apart.  A `command:` case's output is also compared end to end with
+oracle.grl_forward on the device (command_cases.end_to_end).
 """
 import copy
 import time
@@ -41,6 +44,7 @@ import torch
 import torch.nn.functional as F
 
 import archs
+import command_cases as CC
 import f32_cases as C
 import grl_oracle as O
 from _pkgload import load_package
@@ -52,7 +56,8 @@ load_package()
 from grl_image_restoration_b200 import capi, functional as KF, tc as TC  # noqa: E402
 
 MUTATIONS = ("qkv fed the previous block's input", "ln_residual given the previous block's residual",
-             "window attention with the previous block's table and logit scales", "CAB gate of the previous block")
+             "window attention with the previous block's table and logit scales", "CAB gate of the previous block",
+             "output cropped at the padded pitch", "window attention on the transposed window grid's geometry")
 STREAM_READERS = (".qkv", ".cab1", ".fc1", ".conv", "conv_after_body")  # launches whose input is the residual stream
 TAIL = ("conv_first", "conv_after_body", "conv_before_upsample", "upsample.", "conv_up1", "conv_up2", "conv_hr",
         "conv_last")
@@ -249,8 +254,11 @@ class Replay32(ReplayBase, TC.Device):
         else:
             last = nchw(o["conv_last"])
         s = m.upscale
-        ref = (last / m.img_range + m.mean.to(y.device))[:, :, :H * s, :W * s]
+        full = last / m.img_range + m.mean.to(y.device)
+        ref = full[:, :, :H * s, :W * s]
         self._exact("output == tail glue of the last conv", same32(y, ref), "tail")
+        if self.mutate and W * s < full.shape[3]:  # the crop taken at the padded pitch
+            self._mut(MUTATIONS[4], not same32(y, full.flatten(2)[..., :H * s * W * s].reshape(ref.shape)))
 
     # ---- glue -------------------------------------------------------------------------------------
     def _check_ln_residual(self, x, u, gamma, beta, eps=1e-5, res_scale=1.0, cab_y=None, cab_gate=None, out=None,
@@ -352,8 +360,9 @@ class Replay32(ReplayBase, TC.Device):
         """Gates one attention output with f32_cases.attn_ratio (the ulp statistic alone is reported); returns (reference,
         reference on |v|)."""
         v = p.v if v is None else v
-        ref = C.attn_ref(p, heads, v=v, sel=sel)
-        absref = C.attn_ref(p, heads, v=v.abs(), sel=sel)
+        geo = dict(zip(("index", "mask"), self._geometry(p.gq, p.gk, p.use_mask)))
+        ref = C.attn_ref(p, heads, v=v, sel=sel, **geo)
+        absref = C.attn_ref(p, heads, v=v.abs(), sel=sel, **geo)
         nk = p.gk[2] * p.gk[3]  # keys per window
         r = C.attn_ratio(got, ref, absref, nk, gate)
         self._gate(f"{family} (error / bound)", r, 1.0, r <= 1.0, where)
@@ -377,8 +386,15 @@ class Replay32(ReplayBase, TC.Device):
         ref, absref, nk = self._attn("window attention", got, p, heads, sel, GATE_ATTN, f"{where}.window")
         pv = self.saved.get(self.prev, {}).get("window")
         if self._mutation_here() and pv is not None and pv[0].shape == bias.shape:
-            mut = C.attn_ref(p._replace(table=pv[0], scale=pv[1]), heads, sel=sel)
+            mut = C.attn_ref(p._replace(table=pv[0], scale=pv[1]), heads, sel=sel,
+                             **dict(zip(("index", "mask"), self._geometry(g, g, use_mask))))
             self._control(MUTATIONS[2], lambda a, b, _: C.attn_ratio(a, b, absref, nk, GATE_ATTN), got, ref, mut, None,
+                          1.0)
+        if self.mutate and self._full_windows() and use_mask and g[0] // g[2] != g[1] // g[3]:
+            gt = (g[1], g[0], g[3], g[2], g[5], g[4])  # the transposed window grid (square windows)
+            index = self._geometry(g, g, use_mask)[0]
+            mut = C.attn_ref(p, heads, index=index, mask=self._geometry(gt, gt, True)[1], sel=sel)
+            self._control(MUTATIONS[5], lambda a, b, _: C.attn_ratio(a, b, absref, nk, GATE_ATTN), got, ref, mut, None,
                           1.0)
         self.saved.setdefault(self.block, {})["window"] = (bias.clone(), logit_scale.detach().clone())
 
@@ -476,7 +492,7 @@ def lib(pkg, device):
 MICRO = ["micro_cab_x2", "micro_pad_dn", "micro_groups", "micro_odd_d", "micro_gray"]
 CASES = (["native:cfg2-fp32", "native:cfg3-fp32", "native:cfg4-fp32", "native:cfg5-fp32", "zoo:bsr_b2_40x56-fp32",
           "zoo:defocus_dual_b2_48x80-fp32", "zoo:dn_small_c1_b2_100x72-fp32", "dm:b2_40x56-fp32"] +
-         [f"micro:{n}-fp32" for n in MICRO] + ["micro:micro_groups@24x32-fp32"])
+         [f"micro:{n}-fp32" for n in MICRO] + ["micro:micro_groups@24x32-fp32"] + CC.f32_names())
 
 
 @pytest.mark.gpu
@@ -489,6 +505,15 @@ def test_replay_f32(pkg, oracle, cases, golden_loader, lib, device, name):
     if sum(len(layer.blocks) for layer in model.layers) > 1:
         applied = {m: rp.mutations[m][1] for m in MUTATIONS[:2]}
         assert all(applied.values()), applied
+    if name.startswith("command:"):
+        case = CC.BY_NAME[name.rsplit("-", 1)[0]]
+        for m, applies in zip(MUTATIONS[4:], CC.expected_mutations(model, case, rggb)):
+            assert (rp.mutations[m][1] > 0) == applies, (m, applies, rp.mutations[m])
+        del rp
+        torch.cuda.empty_cache()
+        ok, msg = CC.end_to_end(pkg, oracle, case, device, "fp32", y, x, rggb)
+        print(f"  end to end: {msg}")
+        assert ok, msg
 
 
 @pytest.mark.gpu

@@ -22,7 +22,11 @@ tests, with the gates of those tests:
 Mutation controls, computed on the reference side (never an edited kernel), at the first block of every stage after the
 first block of the network and at the last block of every stage: the QKV GEMM fed the previous block's 16-bit input, the
 proj LayerNorm epilogue with the previous block's residual, window attention with the previous block's bias table and
-slot scales.  Each must fail its gate wherever it applies.
+slot scales.  Two more show only at the sizes the test commands run (`command:` cases, tests/command_cases.py): the
+NCHW tail's crop taken at the padded pitch (where Wc < Wp) and, at the first and last block of each stage, shifted
+window attention with the shift mask of the transposed window grid (non-square grids).  Each must fail its gate wherever
+it applies.  A `command:` case's output is also compared end to end with oracle.grl_forward on the device
+(command_cases.end_to_end).
 """
 import copy
 import inspect
@@ -36,11 +40,12 @@ import torch
 
 import archs
 import attn_cases as A
+import command_cases as CC
 import gemm_cases as G
 import grl_oracle as O
 from _pkgload import load_package
 from replay_base import Recorder, ReplayBase, _base, replay_case
-from support import bound_ratio, grid_t
+from support import bound_ratio, grid_t, ulp
 
 load_package()
 from grl_image_restoration_b200 import functional as KF, tc as TC  # noqa: E402
@@ -48,7 +53,8 @@ from grl_image_restoration_b200 import functional as KF, tc as TC  # noqa: E402
 U = 2.0 ** -24
 STREAM_READERS = (".qkv", ".cab1", ".fc1", ".conv", "conv_after_body")  # GEMMs whose x16 is the residual stream's copy
 MUTATIONS = ("qkv fed the previous block's input", "proj residual of the previous block",
-             "window attention with the previous block's constants")
+             "window attention with the previous block's constants", "NCHW tail cropped at the padded pitch",
+             "window attention on the transposed window grid's geometry")
 
 
 def checkers(tc, K):
@@ -120,6 +126,7 @@ class Replay(ReplayBase, TC.Device):
         self.pass1 = {}  # block name -> (window indices, emulated X1 of those windows)
         self.stream32 = None
         self.rescales, self.sat16 = 0, 0
+        self.derived16 = []  # launches whose 16-bit-only output needed the accumulation term
 
     def _record_writes(self, tensors, where):
         super()._record_writes(tensors, where)
@@ -193,12 +200,19 @@ class Replay(ReplayBase, TC.Device):
         got = {k: a[k] for k in ("out_bf16", "out_f32", "out_nchw") if a[k] is not None}
         run = types.SimpleNamespace(kw=a)
 
-        def verdict(xx=x, extra=None):
+        def verdict(xx=x, extra=None, acc_err=None):
             o = dict(ops, **(extra or {}))
             ref = O.gemm_launch_reference(xx, w16, bias, **o)
-            return G.evaluate(tc, run, got, ref, self.fmt, high_mean_rows=())
+            return G.evaluate(tc, run, got, ref, self.fmt, high_mean_rows=(), acc_err=acc_err)
 
         res = verdict()
+        if a["epi"] == tc.EPI_BIAS_ACT and "16-bit" in res and not res["16-bit"][1]:
+            # the seeded gate does not grow with sum |x| |w|: where a real operand cancels, add gamma_K of that sum
+            absdot = O.gemm_launch_reference(x.abs(), w16.abs(), torch.zeros_like(bias), taps=a["taps"])["y"]
+            acc = O.gamma(w16.shape[1]) * absdot
+            res["16-bit"] = verdict(acc_err=acc)["16-bit"]
+            self.derived16.append(_name)
+            self._report16(_name, O.gemm_launch_reference(x, w16, bias, **ops)["y"], a, absdot, acc, res["16-bit"][1])
         for what, (s, ok) in res.items():
             stat = s[1] if isinstance(s, tuple) else s
             self._gate(f"gemm {what}", stat, "evaluate", ok, _name, str(s))
@@ -222,8 +236,29 @@ class Replay(ReplayBase, TC.Device):
                 sv["x16"], sv["scales"] = x.clone(), a["slot_scale"].clone()
             elif _name.endswith(".proj"):
                 sv["res"] = a["res_f32"].clone()
+        if a["out_nchw"] is not None and self.mutate:
+            o, r = a["out_nchw"], a["nchw_r"]
+            full = (x.shape[1] * r, x.shape[2] * r)
+            if o.shape[3] < full[1]:  # a tail that crops Hc x Wc out of the padded image at its pitch Wp
+                ref = O.gemm_launch_reference(x, w16, bias, **dict(ops, crop=full))["nchw"]
+                mut = ref.flatten(2)[..., :o.shape[2] * o.shape[3]].reshape(o.shape)
+                self._mut(MUTATIONS[3], G.stats32(o, mut) > G.GATE32)
         if a["out_f32"] is not None and (a["epi"] == tc.EPI_LN or _name.endswith(".conv")):
             self.stream32 = a["out_f32"]
+
+    def _report16(self, name, y, a, absdot, acc, ok):
+        """Prints the 16-bit-only output's elements outside the seeded gate: the worst, with its float64 value, sum |x||w|
+        and gamma_K of that sum."""
+        n = a["n_real"] or a["n_store"]
+        yr, g = y[:, :n], a["out_bf16"].reshape(y.shape[0], -1)[:, :n].double()
+        delta = G.GATE32 * ulp(G.row_scale(yr), torch.float32) + (O.GELU_AS_ABS_ERR if a["act"] == 1 else 0.0)
+        lo, hi = (yr - delta).to(self.dtype).double(), (yr + delta).to(self.dtype).double()
+        out = torch.maximum(lo - g, g - hi).clamp_min(0.0)
+        r, c = divmod(int(out.argmax()), n)
+        print(f"  {name}: {int((out > 0).sum())} 16-bit elements outside the seeded gate; the worst (row {r}, column "
+              f"{c}): got {float(g[r, c]):.6g}, allowed [{float(lo[r, c]):.6g}, {float(hi[r, c]):.6g}], float64 "
+              f"{float(yr[r, c]):.6g}, sum |x||w| {float(absdot[r, c]):.6g}, gamma_K of it {float(acc[r, c]):.3g}; "
+              f"within the derived gate: {ok}")
 
     # ---- glue -------------------------------------------------------------------------------------
     def _to16(self, x):
@@ -324,7 +359,7 @@ class Replay(ReplayBase, TC.Device):
         vv = A.operand(buf, spec("v", v_off, v_dense), gk, heads, B)
         got = A.operand(buf, spec("o", o_off, o_dense), gq, heads, B)
         idx = self._windows(qq.shape[0]).to(q.device)
-        index, mask = O.attn_pair_geometry(grid_t(gq), grid_t(gk), use_mask)
+        index, mask = self._geometry(grid_t(gq), grid_t(gk), use_mask)
         index = index.to(q.device)
         msel = None if mask is None else mask.to(q.device)[idx % mask.shape[0]]
         table = bias[:, 0, :(gq.wh + gk.wh - 1) * (gq.ww + gk.ww - 1)]
@@ -357,11 +392,22 @@ class Replay(ReplayBase, TC.Device):
                     self._mut(MUTATIONS[2], A.compare(got[idx], em_m, d, self.dtype)[0] > A.GATE_ULP)
                 else:
                     self._below(MUTATIONS[2])
+        if role == "window" and self.mutate and self._full_windows() and use_mask and \
+                gq.H // gq.wh != gq.W // gq.ww:
+            gt = (gq.W, gq.H, gq.ww, gq.wh, gq.sw, gq.sh)  # the transposed window grid (square windows)
+            mt = self._geometry(gt, gt, True)[1].to(q.device)
+            _, em_t, _ = O.attn_launch_reference(qq[idx], kk[idx], vv[idx], table, index, mt[idx % mt.shape[0]],
+                                                 self.dtype)
+            if A.compare(em_t, emul, d, self.dtype)[0] > 2 * A.GATE_ULP:
+                self._mut(MUTATIONS[4], A.compare(got[idx], em_t, d, self.dtype)[0] > A.GATE_ULP)
+            else:
+                self._below(MUTATIONS[4])
         if role == "window":
             self.saved.setdefault(self.block, {})["table_w"] = table.clone()
 
     def report(self, label, seconds, peak):
-        super().report(label, seconds, peak, f", warp rescales {self.rescales}, fp16 operands at +-65504: {self.sat16}")
+        super().report(label, seconds, peak, f", warp rescales {self.rescales}, fp16 operands at +-65504: {self.sat16}"
+                       f", 16-bit outputs gated with the accumulation term: {self.derived16}")
 
 
 def replay(tc, model, x, rggb=False, mutate=True, seed=0, label=""):
@@ -415,7 +461,7 @@ MICRO = ["micro_cab_x2", "micro_pad_dn", "micro_groups", "micro_odd_d", "micro_g
 CASES = (["native:cfg2-fp16", "native:cfg3-fp16", "native:cfg4-fp16", "native:cfg4-bf16", "native:cfg5-fp16",
           "zoo:bsr_b2_40x56-fp16", "zoo:defocus_dual_b2_48x80-fp16", "zoo:defocus_dual_b2_48x80-bf16",
           "zoo:dn_small_c1_b2_100x72-fp16", "dm:b2_40x56-fp16"] +
-         [f"micro:{n}-{p}" for n in MICRO for p in ("fp16", "bf16")])
+         [f"micro:{n}-{p}" for n in MICRO for p in ("fp16", "bf16")] + CC.tc_names())
 
 
 def _assert_clean(rp):
@@ -433,6 +479,15 @@ def test_replay(pkg, oracle, cases, golden_loader, tc, device, name):
     nblocks = sum(len(layer.blocks) for layer in model.layers)
     if nblocks > 1:
         assert all(n > 0 for n, m in ((rp.mutations[m][1], m) for m in MUTATIONS[:2])), rp.mutations
+    if name.startswith("command:"):
+        case = CC.BY_NAME[name.rsplit("-", 1)[0]]
+        for m, applies in zip(MUTATIONS[3:], CC.expected_mutations(model, case, rggb)):
+            assert (rp.mutations[m][1] > 0) == applies, (m, applies, rp.mutations[m])
+        del rp
+        torch.cuda.empty_cache()
+        ok, msg = CC.end_to_end(pkg, oracle, case, device, model.precision, y, x, rggb)
+        print(f"  end to end: {msg}")
+        assert ok, msg
 
 
 @pytest.mark.gpu
