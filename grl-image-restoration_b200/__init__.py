@@ -7,8 +7,8 @@ from .modules import (  # noqa: F401
     WindowAttention, build_last_conv,
 )
 from .functional import (  # noqa: F401
-    awgn, awgn_list, awgn_noise_host, demosaic, dn_seed, jpeg_quant_tables, jpeg_roundtrip, jpeg_roundtrip_host,
-    jpeg_roundtrip_list, luma, luma_list, mosaic, mosaic_list,
+    awgn, awgn_list, awgn_noise_host, demosaic, dn_seed, imresize, imresize_list, jpeg_quant_tables, jpeg_roundtrip,
+    jpeg_roundtrip_host, jpeg_roundtrip_list, luma, luma_list, mosaic, mosaic_list,
 )
 from .evaluation import RECIPES, evaluate  # noqa: F401
 
@@ -17,4 +17,4 @@ __all__ = ["GRL", "TransformerStage", "EfficientMixAttnTransformerBlock", "Mixed
            "AnchorProjection", "AnchorLinear", "CPB_MLP", "Upsample", "UpsampleOneStep", "build_last_conv",
            "configs", "geometry", "demosaic", "jpeg_roundtrip", "jpeg_roundtrip_list", "jpeg_roundtrip_host",
            "jpeg_quant_tables", "dn_seed", "awgn", "awgn_list", "awgn_noise_host", "mosaic", "mosaic_list", "luma",
-           "luma_list", "RECIPES", "evaluate"]
+           "luma_list", "imresize", "imresize_list", "RECIPES", "evaluate"]

@@ -154,6 +154,10 @@ _SIGNATURES = {
     "grl_luma_u8": (c_int, [ctypes.POINTER(GrlImageRef), ctypes.POINTER(GrlImageRef), c_int, c_vp]),
     "grl_mosaic_host": (c_int, [c_vp, c_int, c_int, c_vp]),
     "grl_luma_host": (c_int, [c_vp, c_i64, c_vp]),
+    "grl_imresize_f32": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp]),
+    "grl_imresize_u8_list": (c_int, [ctypes.POINTER(GrlImageRef), ctypes.POINTER(GrlImageRef), c_int, c_int, c_int, c_vp]),
+    "grl_imresize_taps_host": (c_int, [c_int, c_int, c_vp, c_vp]),
+    "grl_imresize_f32_host": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp]),
 }
 
 _lib = None

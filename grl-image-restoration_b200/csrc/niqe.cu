@@ -22,6 +22,7 @@
 #include "grl_common.cuh"
 #include "grl_image_u8.h"
 #include "grl_niqe.h"
+#include "grl_resize.h"  // resize_mirror: imresize's symmetric padding
 
 namespace grl {
 
@@ -77,9 +78,6 @@ __global__ void __launch_bounds__(kTx* kTy) niqe_mscn_kernel(const float* __rest
   out[blockIdx.z * plane + (long long)y * W + x] = __fdiv_rn(__fsub_rn(v0, mu), __fadd_rn(sigma, 1.0f));
 }
 
-// symmetric padding of imresize (edge sample repeated): -1 -> 0, -2 -> 1, n -> n - 1, n + 1 -> n - 2
-__device__ __forceinline__ int nq_sym(int i, int n) { return i < 0 ? -1 - i : (i >= n ? 2 * n - 1 - i : i); }
-
 // vertical pass: t (B, H/2, W) = taps over rows of img / 255
 __global__ void niqe_half_rows_kernel(const float* __restrict__ in, int H, int W, NiqeTaps taps, float* __restrict__ t) {
   const int Ho = H / 2, img = blockIdx.y;
@@ -90,7 +88,7 @@ __global__ void niqe_half_rows_kernel(const float* __restrict__ in, int H, int W
     double acc = 0.0;
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
-      const float v = __fdiv_rn(src[(long long)nq_sym(2 * oy - 3 + k, H) * W + x], 255.0f);  // img / 255.0 in fp32
+      const float v = __fdiv_rn(src[(long long)resize_mirror(2 * oy - 3 + k, H) * W + x], 255.0f);  // img / 255.0 in fp32
       acc = __dadd_rn(acc, __dmul_rn((double)taps.w[k], (double)v));
     }
     t[img * n + i] = (float)acc;
@@ -106,7 +104,7 @@ __global__ void niqe_half_cols_kernel(const float* __restrict__ t, int H, int W,
     const int oy = (int)(i / Wo), ox = (int)(i - (long long)oy * Wo);
     double acc = 0.0;
 #pragma unroll
-    for (int k = 0; k < 8; ++k) acc = __dadd_rn(acc, __dmul_rn((double)taps.w[k], (double)src[(long long)oy * W + nq_sym(2 * ox - 3 + k, W)]));
+    for (int k = 0; k < 8; ++k) acc = __dadd_rn(acc, __dmul_rn((double)taps.w[k], (double)src[(long long)oy * W + resize_mirror(2 * ox - 3 + k, W)]));
     out[img * n + i] = __fmul_rn((float)acc, 255.0f);
   }
 }

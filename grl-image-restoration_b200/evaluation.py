@@ -12,7 +12,8 @@ Reference lines (all paths in the reference checkout):
   crop (VAL)   data/datasets/base_image.py:404-405 (modcrop by the SR scale when a low-quality image is given; scale 1
                for the JPEG and paired deblurring sets: no crop), :419-423 (clean image alone: top-left crop to multiples
                of data_module.modulo, default 8: dn, dm)
-  inputs       restoration_sr.py:100-115 (LR file), restoration_dn.py:134-143 (AWGN keyed on img_info[index][0],
+  inputs       restoration_sr.py:100-115 (LR file; with synthesize_lr the online LR of :127-141, imresize(modcrop(img_gt)
+               / 255, 1 / scale), utils/matlab_functions.py:92-188), restoration_dn.py:134-143 (AWGN keyed on img_info[index][0],
                base_image.py:47-53), restoration_jpeg.py:38-42 + :62-79 (JPEG round trip, colour via BGR),
                base_image.py:233-241 (gray JPEG on live1 / bsds500 / urban100: rgb2ycbcr_np luma of the colour read),
                restoration_dm.py:33-37 (mosaic_CFA_Bayer(img)[1]), restoration_bsr.py:111-118 (uint2single of the image
@@ -134,9 +135,19 @@ def clean_images(name, gts, dataset=None):
     return [_crop(g, r, scale) for g in gts]
 
 
-def model_inputs(name, clean, lqs=None, keys=None):
-    """The recipe's model inputs: (H, W, C) uint8 for the u8 forwards, (C, H, W) float32 for awgn and the mosaic."""
+def _check_synthesize_lr(name, lqs, synthesize_lr):
+    if synthesize_lr and (RECIPES[name].task != "sr" or lqs is not None):
+        raise ValueError(f"grl_b200: evaluate: synthesize_lr=True makes the LR input of an SR recipe from its HR images and "
+                         f"takes no lqs; got {name} ({RECIPES[name].task}) with lqs {'given' if lqs is not None else 'None'}")
+
+
+def model_inputs(name, clean, lqs=None, keys=None, synthesize_lr=False):
+    """The recipe's model inputs: (H, W, C) uint8 for the u8 forwards, (C, H, W) float32 for awgn, the mosaic and, with
+    synthesize_lr (SR recipes, no lqs), the bicubic downscale of the modcropped clean images."""
     r = RECIPES[name]
+    _check_synthesize_lr(name, lqs, synthesize_lr)
+    if synthesize_lr:
+        return K.imresize_list(clean, 1 / configs.RELEASED[name][2])
     if r.input == "awgn":
         if keys is None or len(keys) != len(clean):
             raise ValueError("grl_b200: evaluate: the denoising recipe needs one seed key per image (the reference keys "
@@ -225,7 +236,8 @@ def mean(values):
 
 
 @torch.no_grad()
-def evaluate(model, name, gts, lqs=None, keys=None, dataset=None, niqe_params=None, metric=None, lpips_weights=None):
+def evaluate(model, name, gts, lqs=None, keys=None, dataset=None, niqe_params=None, metric=None, lpips_weights=None,
+             synthesize_lr=False):
     """The test command of the released checkpoint `name` (a configs.RELEASED key) on `model`, over one test set.
 
     gts: decoded (H, W, C) uint8 CUDA images (RGB, or one channel for the gray sets; for the gray JPEG command on
@@ -235,14 +247,17 @@ def evaluate(model, name, gts, lqs=None, keys=None, dataset=None, niqe_params=No
     dataset: the set's name (selects the luma for the gray JPEG command).  niqe_params: the NIQE pristine model (bsr, and
     restorer_perceptual).  metric: the command's metric= override: None keeps the recipe's collection; "restorer_perceptual"
     (recipes whose collection is restorer) adds val_lpips and val_niqe on the same shaved 8-bit images and needs
-    lpips_weights (metrics.lpips_weights accepts it) and niqe_params.  model.precision and model.self_ensemble apply as
-    they are set.
+    lpips_weights (metrics.lpips_weights accepts it) and niqe_params.  synthesize_lr: for an SR recipe without lqs, make
+    each LR input on the device from its modcropped HR image as the SR dataset's online branch does, imresize(img / 255,
+    1 / scale) (functional.imresize_list), instead of reading an LR file; the scores may differ slightly from those on
+    MATLAB-made LR files.  model.precision and model.self_ensemble apply as they are set.
 
     Returns {"scores": {metric: (N,) CPU tensor in image order}, "means": {metric: float}} with the reference's metric
     names (val_psnr, val_psnr_y, val_ssim, ...)."""
     if name not in RECIPES:
         raise ValueError(f"grl_b200: evaluate: unknown checkpoint name {name!r} (configs.RELEASED)")
     names = collection(name, metric)
+    _check_synthesize_lr(name, lqs, synthesize_lr)
     if metric is not None and (lpips_weights is None or niqe_params is None):
         raise ValueError(f"grl_b200: evaluate: metric={metric!r} scores LPIPS and NIQE and needs lpips_weights and "
                          "niqe_params")
@@ -259,7 +274,8 @@ def evaluate(model, name, gts, lqs=None, keys=None, dataset=None, niqe_params=No
     if distributed:
         lo, hi = sharding.shard_range(n, torch.distributed.get_rank(), torch.distributed.get_world_size())
     clean = clean_images(name, gts[lo:hi], dataset)
-    inputs = model_inputs(name, clean, None if lqs is None else lqs[lo:hi], None if keys is None else keys[lo:hi])
+    inputs = model_inputs(name, clean, None if lqs is None else lqs[lo:hi], None if keys is None else keys[lo:hi],
+                          synthesize_lr)
     outs = restore(model, name, inputs)
     per = [score(name, o, c, niqe_params, metric, lpips_weights) for o, c in zip(outs, clean)]
     return gather_scores(per, names, lo, hi, gts[0].device)

@@ -670,6 +670,75 @@ def luma_host(rgb):
     return out
 
 
+def _resize_factor(scale):
+    """s of imresize's scale = 1 / s, s in {2, 3, 4}."""
+    import math
+    import numbers
+
+    if not isinstance(scale, bool) and isinstance(scale, numbers.Real) and math.isfinite(scale) and scale > 0:
+        s = round(1 / scale)
+        if s in (2, 3, 4) and scale * s == 1:
+            return s
+    raise ValueError(f"grl_b200: imresize supports the scales 1/2, 1/3 and 1/4 (pass 1 / s as the reference does), got "
+                     f"{scale!r}")
+
+
+def imresize(x, scale):
+    """The reference's imresize(img, scale) (utils/matlab_functions.py:92-188, MATLAB's bicubic with antialiasing) for the
+    downscales scale = 1/2, 1/3 and 1/4: x (B, C, H, W) float32 on the GPU, 1 <= C <= 8 -> new (B, C, ceil(H*scale),
+    ceil(W*scale)) float32, not rounded or clipped.  Each pass sums in float64 and rounds once to float32 (csrc/grl_resize.h);
+    the reference's own float32 sums agree to within float32 rounding.  Each side has 1 sample or at least 4, 6 or 7 for
+    s = 2, 3, 4: the reference's symmetric padding fails on the lengths between, and they are refused.  One kernel per 64
+    images."""
+    s = _resize_factor(scale)
+    x = _f32c(x, "x")
+    if x.dim() != 4 or not 1 <= x.shape[1] <= 8:
+        raise RuntimeError(f"grl_b200: imresize needs (B, C, H, W) float32 images with 1 <= C <= 8, got {tuple(x.shape)}")
+    B, C, H, W = x.shape
+    y = torch.empty(B, C, -(-H // s), -(-W // s), device=x.device, dtype=torch.float32)
+    capi.check(capi.lib().grl_imresize_f32(capi.ptr(x), B, C, H, W, s, capi.ptr(y), capi.stream()))
+    return y
+
+
+def imresize_list(images, scale):
+    """imresize of a list of differently sized (H_i, W_i, C) uint8 images on the GPU, all with the same C in {1, 3}, each
+    read as k / 255 (to_tensor) -> list of new (C, ceil(H_i*scale), ceil(W_i*scale)) float32 tensors in input order, what
+    forward_list takes: the SR dataset's online LR image, imresize(modcrop(img_gt) / 255, 1 / s)
+    (data/datasets/restoration_sr.py:127-141), of modcropped images.  One kernel per 64 images."""
+    s = _resize_factor(scale)
+    images = list(images)
+    C = _jpeg_images(images, "imresize_list")
+    if not images:
+        return []
+    srcs = [t.contiguous() for t in images]
+    outs = [torch.empty(C, -(-t.shape[0] // s), -(-t.shape[1] // s), device=t.device, dtype=torch.float32) for t in srcs]
+    capi.check(capi.lib().grl_imresize_u8_list(_image_refs(srcs, capi.IMAGE_U8), _image_refs(outs, capi.IMAGE_F32),
+                                               len(srcs), C, s, capi.stream()))
+    return outs
+
+
+def imresize_host(x, scale):
+    """imresize of (B, C, H, W) float32 CPU images, evaluated by the library's host copy of the same closed forms (tests)."""
+    s = _resize_factor(scale)
+    x = x.float().contiguous()
+    B, C, H, W = x.shape
+    y = torch.empty(B, C, -(-H // s), -(-W // s), dtype=torch.float32)
+    capi.check(capi.lib().grl_imresize_f32_host(ctypes.c_void_p(x.data_ptr()), B, C, H, W, s, ctypes.c_void_p(y.data_ptr())))
+    return y
+
+
+def imresize_taps(n, scale):
+    """(taps, geometry) of a side of length n at imresize's scale (CPU, no device): taps (T,) float32, the weight row every
+    output uses; geometry {"T", "c", "out", "pad_s", "pad_e"}: output o reads inputs s*o + c + k (0-based), k < T, out =
+    ceil(n * scale), and the reference's symmetric pad lengths.  A length the resize refuses raises RuntimeError."""
+    s = _resize_factor(scale)
+    taps = torch.empty(16, dtype=torch.float32)
+    geom = torch.empty(5, dtype=torch.int32)
+    capi.check(capi.lib().grl_imresize_taps_host(int(n), s, ctypes.c_void_p(taps.data_ptr()), ctypes.c_void_p(geom.data_ptr())))
+    g = dict(zip(("T", "c", "out", "pad_s", "pad_e"), geom.tolist()))
+    return taps[: g["T"]].clone(), g
+
+
 def stripe_attention(qkv, anchor, B, tok_grid, anc_grid, heads, scale1, bias1, scale2, bias2, use_mask, out=None):
     """qkv (B, L, 3c) view (stripe half), anchor (B, Ha, Wa, c) -> (B, L, c)."""
     qp, ldq = _token_rows(qkv, "qkv")

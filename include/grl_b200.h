@@ -535,6 +535,27 @@ int grl_luma_u8(const GrlImageRef* src, const GrlImageRef* dst, int n, void* str
 int grl_mosaic_host(const uint8_t* img, int H, int W, float* out);
 int grl_luma_host(const uint8_t* rgb, int64_t n, uint8_t* out);
 
+/* ---- Bicubic downscale (the SR test command's LR input made from the HR image, csrc/resize.cu, csrc/grl_resize.h) -------
+ * The SR dataset's online LR (data/datasets/restoration_sr.py:127-141, the load_lr False branch): imresize(modcrop(img_gt)
+ * / 255, 1 / s), MATLAB's bicubic imresize with antialiasing (utils/matlab_functions.py:92-188), weights and indices of
+ * calculate_weights_indices (:20-88).  s in {2, 3, 4}; output ceil(H / s) x ceil(W / s), float32, neither rounded to 8 bits
+ * nor clipped.  Every output has the same T = 4s taps, each rounded once to float32 from double; the H pass runs first
+ * and stores float32, each pass sums its products in float64 in tap order and rounds once (csrc/grl_resize.h).  Indices
+ * past an edge mirror with the edge sample repeated; a side of one sample pads with that sample.  A side of 2 .. 3, 2 .. 5
+ * or 2 .. 6 samples for s = 2, 3, 4 is shorter than a pad length, where the reference's symmetric copy fails: refused. */
+/* x (B, C, H, W) fp32 -> y (B, C, ceil(H / s), ceil(W / s)) fp32, 1 <= C <= 8.  One kernel per kResizePerLaunch (64)
+ * images; no workspace. */
+int grl_imresize_f32(const float* x, int B, int C, int H, int W, int s, float* y, void* stream);
+/* src[i] (H, W, C) uint8 GRL_IMAGE_U8 (k / 255 at the load, as to_tensor) -> dst[i] (C, ceil(H / s), ceil(W / s)) fp32
+ * GRL_IMAGE_F32 (H, W of the dst ref are the output's), C in {1, 3}. */
+int grl_imresize_u8_list(const GrlImageRef* src, const GrlImageRef* dst, int n, int C, int s, void* stream);
+/* The taps and geometry of a side of length n on the CPU (tests); HOST pointers: taps[16] (the first T used), geometry[5]
+ * = {T, c, out, pad_s, pad_e}: output o reads inputs s o + c + k (0-based), k < T; out = ceil(n / s); pad_s, pad_e the
+ * reference's sym_len_s, sym_len_e.  Refuses the n the device entries refuse. */
+int grl_imresize_taps_host(int n, int s, float* taps, int32_t* geometry);
+/* grl_imresize_f32 on the CPU from the same closed forms (tests); HOST pointers.  Equal to the device bit for bit. */
+int grl_imresize_f32_host(const float* x, int B, int C, int H, int W, int s, float* y);
+
 #ifdef __cplusplus
 }
 #endif

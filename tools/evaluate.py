@@ -1,6 +1,6 @@
 """Score a released checkpoint on one test set, as its test command does (evaluation.evaluate), from image files:
 
-    python tools/evaluate.py CKPT NAME --gt DIR [--lq DIR | --lq-left DIR --lq-right DIR] [--dataset NAME]
+    python tools/evaluate.py CKPT NAME --gt DIR [--lq DIR | --bicubic-lr | --lq-left DIR --lq-right DIR] [--dataset NAME]
                              [--niqe-params FILE] [--precision fp32|fp16|bf16] [--self-ensemble]
                              [--metric restorer_perceptual --lpips-weights FILE]
 
@@ -12,7 +12,9 @@ device.  --metric restorer_perceptual is the test commands' metric= override: PS
 whose collection is restorer, with LPIPS(net="vgg")'s state dict (or torchvision's vgg16 features merged with LPIPS's
 lin weights) from --lpips-weights and NIQE's pristine model from --niqe-params.  The denoising noise is keyed on
 "<test set directory>/<file name>" (evaluation.seed_keys, the reference's img_info[index][0]; --dataset cbsd68 and CBSD68
-name the same set).  Prints one table.
+name the same set).  --bicubic-lr scores an SR checkpoint from HR images alone: each LR input is the bicubic downscale
+of the modcropped HR image made on the device, as the SR dataset's online branch makes it (evaluate's synthesize_lr),
+instead of an LR file from --lq.  Prints one table.
 Under torchrun each process takes its slice of the images and rank 0 prints the gathered means.
 """
 import argparse
@@ -58,6 +60,9 @@ def main():
     ap.add_argument("name", help="configs.RELEASED key of the checkpoint")
     ap.add_argument("--gt", required=True)
     ap.add_argument("--lq")
+    ap.add_argument("--bicubic-lr", action="store_true",
+                    help="SR names: make each LR input from its HR image on the device (MATLAB bicubic, as the SR "
+                         "dataset's online branch) instead of reading --lq")
     ap.add_argument("--lq-left")
     ap.add_argument("--lq-right")
     ap.add_argument("--dataset", default=None, help="the set's name, e.g. CBSD68, live1 (seed keys, gray JPEG luma)")
@@ -110,7 +115,10 @@ def main():
     t0 = time.perf_counter()
     gts = load_dir(args.gt, names, gray)
     lqs = None
-    if r.input == "lq":
+    if args.bicubic_lr and (r.task != "sr" or args.lq):
+        sys.exit("--bicubic-lr makes the LR inputs of an SR checkpoint and takes no --lq"
+                 if r.task == "sr" else f"--bicubic-lr applies to SR checkpoints, not {args.name}")
+    if r.input == "lq" and not args.bicubic_lr:
         if not args.lq:
             sys.exit(f"{args.name} needs --lq")
         lq_names = list_images(args.lq)
@@ -141,7 +149,7 @@ def main():
     torch.cuda.synchronize()
     t1 = time.perf_counter()
     result = evaluation.evaluate(model, args.name, gts, lqs, keys, dataset, args.niqe_params, args.metric,
-                                 args.lpips_weights)
+                                 args.lpips_weights, synthesize_lr=args.bicubic_lr)
     torch.cuda.synchronize()
     t_eval = time.perf_counter() - t1
     if not torch.distributed.is_initialized() or torch.distributed.get_rank() == 0:
