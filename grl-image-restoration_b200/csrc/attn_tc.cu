@@ -34,6 +34,13 @@ namespace tc {
 
 constexpr int kAttnStages = 4;                 // K / V ring depth
 constexpr int kAttnThreads = 2 * 128 + 32;     // two consumer warpgroups (64 query rows each) + 1 producer warp
+// Two CTAs per SM: four consumer warpgroups hide each other's MMA, load and barrier latency.  Registers are allocated
+// per SM sub-partition (16,384 each, a quarter of the resident warps): the 18 warps of two CTAs put 5 warps on one, so
+// ptxas is capped at 16,384 / (5 x 32) rounded down to the allocation granularity of 8, 96 registers per thread.  Three
+// CTAs (27 warps, 7 on one sub-partition) would cap it at 72, where the loop spills its O accumulator (DESIGN 5.2).
+constexpr int kAttnCtasPerSm = 2;
+static_assert(kAttnCtasPerSm * (AttnSmem<64, kAttnStages>::TOTAL + 1024) <= 228 * 1024,
+              "the attention CTAs of one SM (plus the 1 KB the runtime reserves per CTA) must fit in its 228 KB of shared memory");
 
 // OR of `pred` over the 64 threads of named barrier `id` (one warp pair = 32 consecutive query rows)
 __device__ __forceinline__ bool pair_any(bool pred, int id) {
@@ -63,11 +70,13 @@ struct AttnMaps {
 };
 
 template <int KT, int KW, int VAR>
-__global__ void __launch_bounds__(kAttnThreads, 2) attn_tc_kernel(const __grid_constant__ AttnMaps tm, const GrlTcAttn a) {
+__global__ void __launch_bounds__(kAttnThreads, kAttnCtasPerSm) attn_tc_kernel(const __grid_constant__ AttnMaps tm, const GrlTcAttn a) {
   static_assert(KT == 64, "S fragments of m64n64 products: one key tile per product");
   constexpr int NS = kAttnStages;
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  // aligned up to 1024 bytes by an offset from smem_raw, so that the compiler keeps every pointer below in the shared
+  // window (LDS / STS rather than generic loads)
+  uint8_t* smem = smem_raw + ((0u - smem_u32(smem_raw)) & 1023u);
   using S = AttnSmem<KT, NS>;
   uint8_t* Qs = smem;
   uint8_t* Ks = smem + S::OFF_K;
@@ -164,15 +173,21 @@ __global__ void __launch_bounds__(kAttnThreads, 2) attn_tc_kernel(const __grid_c
     }
   } else {
     // =============================================================== warpgroups 0, 1: MMAs + softmax on the fragments
-    const int wg = warp >> 2, wq = warp & 3, tig = tid & 127;
+    // the warpgroup index through a lane-0 shuffle, so that the compiler knows it is warp-uniform: the key-tile loop
+    // then builds its wgmma descriptors with about 20 fewer instructions (2 fewer register-to-uniform moves), for 8-16
+    // more once per CTA
+    const int wg = __shfl_sync(0xffffffffu, warp >> 2, 0), wq = warp & 3, tig = tid & 127;
     if (wg >= nwg) return;
     // accumulator fragment coordinates: rows fr and fr + 8 of the warpgroup's 64, columns 8i + fc, 8i + fc + 1
     const int fr = 16 * wq + (lane >> 2), fc = 2 * (lane & 3);
     // bias:  idx(i, j) = base_i - koff_j  (grl_geometry.h rel_index); table copy c holds T shifted right by c entries
+    // held as one 64-bit register pair: each bias pointer below is then a single 32-bit-index multiply-add from it
+    // (left as a uniform parameter plus a 64-bit index, every address costs a chain of 64-bit adds and shifts)
     const float* bias_h = a.bias + (size_t)h * 4 * a.rows_pad;
+    asm("mov.b64 %0, %0;" : "+l"(bias_h));
     // What the thread's two rows need per tile (bias base, mask region) and at the end (output element offset) is kept
     // in shared memory and read back when used: registers are the budget of two CTAs per SM.
-    int4* row_s = reinterpret_cast<int4*>(smem + S::OFF_ROWS) + tid;                 // base_i[2], q_rid[2]
+    int2* row_s = reinterpret_cast<int2*>(smem + S::OFF_ROWS) + 2 * tid;            // base_i[2], q_rid[2]
     long long* dst_s = reinterpret_cast<long long*>(smem + S::OFF_DST) + 2 * tid;  // output offsets, -1: row >= Nq
     {
       int v[4];
@@ -186,7 +201,8 @@ __global__ void __launch_bounds__(kAttnThreads, 2) attn_tc_kernel(const __grid_c
                    : a.o_dense ? (((long long)bw * a.heads + h) * Nq + qi) * kDP
                                : ((long long)(b * a.gq.H + tq.y) * a.gq.W + tq.x) * a.ldo + a.o_off + h * kDP;
       }
-      *row_s = make_int4(v[0], v[1], v[2], v[3]);
+      row_s[0] = make_int2(v[0], v[1]);
+      row_s[1] = make_int2(v[2], v[3]);
     }
     const bool need_mask = a.use_mask && (wr == nwh - 1 || wc == nww - 1);
     // ones-column: when head_dim < 32 the projection epilogue sets column 31 of every V row to 1, so O[:, 31] =
@@ -195,7 +211,6 @@ __global__ void __launch_bounds__(kAttnThreads, 2) attn_tc_kernel(const __grid_c
     constexpr bool ones = (VAR & 2) != 0;
     // the lazy-rescale decision is shared by 32 consecutive rows: warps 0-1 and 2-3 of the warpgroup (named barriers 1-4)
     const int pair_bar = 1 + 2 * wg + (wq >> 1);
-    const uint32_t q_sa = smem_u32(Qs) + wg * (64 * 64);
 
     float oacc[16];
 #pragma unroll
@@ -206,42 +221,50 @@ __global__ void __launch_bounds__(kAttnThreads, 2) attn_tc_kernel(const __grid_c
       const int buf = t % NS, k0 = t * KT;
       mbar_wait(&kv_full[buf], (t / NS) & 1);
       float s[32];
-      const int4 rw = *row_s;
-      const int base_i[2] = {rw.x, rw.y}, q_rid[2] = {rw.z, rw.w};
+      const int2 rb = row_s[0];  // the region ids are read when the mask needs them
+      const int base_i[2] = {rb.x, rb.y};
       // ---- the bias of this tile (log2 domain) is the accumulator's initial value, so that S_t = bias + Q K_t^T comes
       // out of the MMA without a second set of registers; s[4i + 2j + e] = row fr + 8j, column 8i + fc + e
       if ((KW > 0) && (k0 + KT <= Nk)) {
         // keys kj = k0 + 8i + fc, kj + 1 (kj even) are adjacent in one key row: table entries e0 = base - koff(kj), e0 - 1.
-        // k0 % 64 == 0 and KW % 8 == 0, so koff(kj) = koff(k0 + fc) + R(i) Wt + C(i) with compile-time R, C: one pointer
-        // per row and key row, constant offsets inside it.
+        // k0 % 64 == 0 and KW % 8 == 0, so koff(kj) = koff(k0 + fc) + R(i) Wt + C(i) with compile-time R, C.  Key rows
+        // R and R + 2 lie 2 Wt entries apart, an even distance, so they read the same table copy: one pointer per row j
+        // and key-row parity, the other key rows 2 Wt entries further, the columns at immediate offsets.
         constexpr int KWS = KW > 0 ? KW : 8;
+        constexpr int NR = KWS >= 64 ? 1 : KT / KWS;  // key rows in the tile
         const int e00 = (k0 / KWS) * Wt + (k0 % KWS) + fc;
 #pragma unroll
-        for (int i = 0; i < KT / 8; ++i) {
-          // KWS >= 64: the tile lies inside one key row (k0 % KWS + 63 < KWS); else k0 % KWS == 0
-          const int R = KWS >= 64 ? 0 : 8 * i / KWS, C = KWS >= 64 ? 8 * i : 8 * i % KWS;
+        for (int j = 0; j < 2; ++j) {
+          const float* pr[2];
 #pragma unroll
-          for (int j = 0; j < 2; ++j) {
-            const int er = base_i[j] - e00 - R * Wt;  // e0 of the key row's first pair in this tile
+          for (int r = 0; r < (NR < 2 ? NR : 2); ++r) {
+            const int er = base_i[j] - e00 - r * Wt;  // e0 of key row r's first pair in this tile
             const int cpy = (er + 1) & 1;  // copy in which T[e0 - 1], T[e0] start at an even (8-byte aligned) position
-            const float2 bb = __ldg(reinterpret_cast<const float2*>(bias_h + (cpy * (a.rows_pad + 1) + er - 1 - C)));
+            pr[r] = bias_h + (cpy * (a.rows_pad + 1) + er - 1);
+          }
+#pragma unroll
+          for (int i = 0; i < KT / 8; ++i) {
+            // KWS >= 64: the tile lies inside one key row (k0 % KWS + 63 < KWS); else k0 % KWS == 0
+            const int R = KWS >= 64 ? 0 : 8 * i / KWS, C = KWS >= 64 ? 8 * i : 8 * i % KWS;
+            const float2 bb = __ldg(reinterpret_cast<const float2*>(pr[R & 1] - (R >> 1) * (2 * Wt) - C));
             s[4 * i + 2 * j] = bb.y;
             s[4 * i + 2 * j + 1] = bb.x;
           }
         }
       } else {
+        const float* prow[2] = {bias_h + base_i[0], bias_h + base_i[1]};  // T[base_j - koff] = prow[j][-koff]
 #pragma unroll
         for (int i = 0; i < KT / 8; ++i) {
           const int2 ko = *reinterpret_cast<const int2*>(koff_s + buf * KT + 8 * i + fc);
 #pragma unroll
           for (int j = 0; j < 2; ++j) {
-            s[4 * i + 2 * j] = __ldg(bias_h + base_i[j] - ko.x);
-            s[4 * i + 2 * j + 1] = __ldg(bias_h + base_i[j] - ko.y);
+            s[4 * i + 2 * j] = __ldg(prow[j] - ko.x);
+            s[4 * i + 2 * j + 1] = __ldg(prow[j] - ko.y);
           }
         }
       }
       {  // ---- S_t = bias + Q K_t^T
-        const uint32_t k_sa = smem_u32(Ks + buf * S::KV_BYTES);
+        const uint32_t q_sa = smem_u32(Qs) + wg * (64 * 64), k_sa = smem_u32(Ks + buf * S::KV_BYTES);
         wgmma_fence_regs(s);
         wgmma_fence();
 #pragma unroll
@@ -257,6 +280,8 @@ __global__ void __launch_bounds__(kAttnThreads, 2) attn_tc_kernel(const __grid_c
       }
 
       if (need_mask) {
+        const int2 rq = row_s[1];
+        const int q_rid[2] = {rq.x, rq.y};
 #pragma unroll
         for (int i = 0; i < KT / 8; ++i) {
           const int2 rr = *reinterpret_cast<const int2*>(krid_s + buf * KT + 8 * i + fc);
