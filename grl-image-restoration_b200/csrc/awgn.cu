@@ -3,7 +3,8 @@
 // rounded to float32, bit for bit, from the closed forms of grl_awgn.h.
 //
 // One CTA per image runs that image's MT19937 stream from its seed to its last sample; a launch takes up to
-// kAwgnPerLaunch images, whose descriptors and keys travel by value in the kernel parameters (as in jpeg.cu).  The number
+// kAwgnPerLaunch images, whose records (pointers, size and key) travel by value in the kernel parameters
+// (grl_param_list.cuh).  The number
 // of twists an image needs depends on how many polar candidates are rejected, so only the CTA knows it: no host sync, no
 // workspace.  Per twist of the 624-word state (shared memory, double-buffered so that no pass overwrites a word another
 // thread of that pass still has to read):
@@ -15,35 +16,37 @@
 // pairs write consecutive addresses.
 #include "grl_awgn.h"
 #include "grl_common.cuh"
+#include "grl_param_list.cuh"
 
 namespace grl {
 
 namespace {
 
-constexpr int kAwgnPerLaunch = 64;  // 64 x 56 bytes of descriptors and keys: 3.5 KB of the 4 KB of kernel parameters
+constexpr int kAwgnPerLaunch = 64;
 constexpr int kAwgnThreads = 256, kAwgnWarps = kAwgnThreads / 32;
 constexpr int kPass = kMtN - kMtM;  // 227: the passes are [0, 227), [227, 454), [454, 624)
 static_assert(kPass <= kAwgnThreads && kMtN - 2 * kPass <= kPass && kAwgnPairsPerTwist <= kAwgnThreads,
               "one word / candidate per thread");
 
-struct AwgnList {
-  const uint8_t* src[kAwgnPerLaunch];
-  float* dst[kAwgnPerLaunch];
-  int H[kAwgnPerLaunch], W[kAwgnPerLaunch];
-  uint32_t key[kAwgnPerLaunch][8];
+struct AwgnRecord {  // 56 bytes
+  const uint8_t* src;
+  float* dst;
+  int H, W;
+  uint32_t key[8];
 };
-static_assert(sizeof(AwgnList) + sizeof(int) + sizeof(double) <= 4096, "kernel parameters");
+using AwgnRecords = ParamList<AwgnRecord, kAwgnPerLaunch, sizeof(int) + sizeof(double)>;
 
-__global__ void __launch_bounds__(kAwgnThreads) awgn_kernel(const AwgnList L, int C, double scale) {
+__global__ void __launch_bounds__(kAwgnThreads) awgn_kernel(const AwgnRecords L, int C, double scale) {
   __shared__ uint32_t mt[2][kMtN];  // the state, double-buffered over twists
   __shared__ uint32_t tw[kMtN];     // the current twist's tempered words
   __shared__ uint32_t key[8];
   __shared__ int accepted[kAwgnWarps];
-  const int img = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int plane = L.H[img] * L.W[img], count = C * plane, npairs = (count + 1) >> 1;
-  const uint8_t* src = L.src[img];
-  float* dst = L.dst[img];
-  if (tid < 8) key[tid] = L.key[img][tid];
+  const AwgnRecord& im = L.at[blockIdx.x];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int plane = im.H * im.W, count = C * plane, npairs = (count + 1) >> 1;
+  const uint8_t* src = im.src;
+  float* dst = im.dst;
+  if (tid < 8) key[tid] = im.key[tid];
   __syncthreads();
   if (tid == 0) awgn_mt_seed(mt[0], key);  // a dependent chain of ~1.9k steps
   __syncthreads();
@@ -101,20 +104,18 @@ __global__ void __launch_bounds__(kAwgnThreads) awgn_kernel(const AwgnList L, in
 
 int check_awgn(const GrlImageRef* src, const GrlImageRef* dst, const uint32_t* keys, int n, int C, double scale,
                const char* what) {
-  GRL_REQUIRE(n >= 0 && ((src && dst && keys) || n == 0), "%s: null image list or keys (n = %d)", what, n);
   GRL_REQUIRE(C == 1 || C == 3, "%s: C = %d, a denoising image is gray (C = 1) or RGB (C = 3)", what, C);
   GRL_REQUIRE(isfinite(scale) && scale >= 0.0, "%s: scale %g is not a finite value >= 0", what, scale);
-  for (int i = 0; i < n; ++i) {
-    const GrlImageRef &s = src[i], &d = dst[i];
-    GRL_REQUIRE(s.kind == GRL_IMAGE_U8 && d.kind == GRL_IMAGE_F32, "%s: image %d: kinds %d / %d, need GRL_IMAGE_U8 -> "
-                "GRL_IMAGE_F32", what, i, s.kind, d.kind);
-    GRL_REQUIRE(s.data && d.data, "%s: image %d: null data", what, i);
-    GRL_REQUIRE(s.H >= 1 && s.W >= 1 && s.H == d.H && s.W == d.W, "%s: image %d: sizes %d x %d -> %d x %d", what, i, s.H,
-                s.W, d.H, d.W);
-    GRL_REQUIRE((long long)s.H * s.W * C <= 0x7fffffffLL, "%s: image %d: %d x %d x %d samples is too large", what, i, s.H,
-                s.W, C);
-  }
-  return GRL_OK;
+  const int rc = check_list_args(n, keys != nullptr, "key", what);
+  if (rc != GRL_OK) return rc;
+  return check_u8_pairs(
+      src, dst, n, GRL_IMAGE_F32, [](const GrlImageRef& s) { return make_int2(s.H, s.W); },
+      [&](const GrlImageRef& s, int i) -> int {
+        GRL_REQUIRE((long long)s.H * s.W * C <= 0x7fffffffLL, "%s: image %d: %d x %d x %d samples is too large", what, i,
+                    s.H, s.W, C);
+        return GRL_OK;
+      },
+      what);
 }
 
 }  // namespace
@@ -161,21 +162,19 @@ int grl_awgn_u8(const GrlImageRef* src, const GrlImageRef* dst, const uint32_t* 
                 void* stream) {
   const int rc = check_awgn(src, dst, keys, n, C, scale, "awgn_u8");
   if (rc != GRL_OK) return rc;
-  const cudaStream_t st = (cudaStream_t)stream;
-  AwgnList L;
-  for (int i0 = 0; i0 < n; i0 += kAwgnPerLaunch) {
-    const int m = n - i0 < kAwgnPerLaunch ? n - i0 : kAwgnPerLaunch;
-    for (int j = 0; j < m; ++j) {
-      L.src[j] = static_cast<const uint8_t*>(src[i0 + j].data);
-      L.dst[j] = static_cast<float*>(dst[i0 + j].data);
-      L.H[j] = src[i0 + j].H;
-      L.W[j] = src[i0 + j].W;
-      for (int w = 0; w < 8; ++w) L.key[j][w] = keys[8 * (i0 + j) + w];
-    }
-    awgn_kernel<<<m, kAwgnThreads, 0, st>>>(L, C, scale);
+  const auto add = [&](AwgnRecord& r, int, int i) {
+    r.src = static_cast<const uint8_t*>(src[i].data);
+    r.dst = static_cast<float*>(dst[i].data);
+    r.H = src[i].H;
+    r.W = src[i].W;
+    for (int w = 0; w < 8; ++w) r.key[w] = keys[8 * i + w];
+    return 1LL;
+  };
+  return launch_list<AwgnRecords>(n, add, [&](const AwgnRecords& L, int, int m) -> int {
+    awgn_kernel<<<m, kAwgnThreads, 0, (cudaStream_t)stream>>>(L, C, scale);
     GRL_LAUNCH_CHECK("awgn_kernel");
-  }
-  return GRL_OK;
+    return GRL_OK;
+  });
 }
 
 }  // extern "C"

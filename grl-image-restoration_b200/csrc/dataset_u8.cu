@@ -1,32 +1,34 @@
 // dataset_u8.cu -- the demosaicking command's packed Bayer input and the gray JPEG command's MATLAB luma, made on the
 // device from clean 8-bit RGB images, from the closed forms of grl_dataset_u8.h.
 //
-// Both are pixel maps, so a launch takes up to kDatasetPerLaunch images of any sizes, their descriptors by value in the
-// kernel parameters: blockIdx.y picks the image, the x blocks stride over its work items (a 2 x 2 quad for the mosaic, a
-// pixel for the luma).  Consecutive threads read consecutive source bytes and write consecutive destination elements of
-// each plane.  No workspace, no host sync; a longer list takes several launches on the caller's stream.
+// Both are pixel maps, so a launch takes up to kDatasetPerLaunch images of any sizes, their records by value in the
+// kernel parameters (grl_param_list.cuh): blockIdx.y picks the image, the x blocks stride over its work items (a 2 x 2
+// quad for the mosaic, a pixel for the luma).  Consecutive threads read consecutive source bytes and write consecutive
+// destination elements of each plane.  No workspace, no host sync.
 #include "grl_common.cuh"
 #include "grl_dataset_u8.h"
+#include "grl_param_list.cuh"
 
 namespace grl {
 
 namespace {
 
-constexpr int kDatasetPerLaunch = 128;  // 128 x 24 bytes of descriptors: 3 KB of the 4 KB of kernel parameters
+constexpr int kDatasetPerLaunch = 128;
 constexpr int kDatasetThreads = 256, kDatasetMaxBlocksX = 512;
 
-struct DatasetList {
-  const uint8_t* src[kDatasetPerLaunch];
-  void* dst[kDatasetPerLaunch];
-  int H[kDatasetPerLaunch], W[kDatasetPerLaunch];  // of the source image
+struct DatasetRecord {  // 24 bytes: 128 (source, destination) GrlImageRef pairs would not fit the kernel parameters
+  const uint8_t* src;
+  void* dst;
+  int H, W;  // of the source image
 };
-static_assert(sizeof(DatasetList) <= 4096, "kernel parameters");
+using DatasetRecords = ParamList<DatasetRecord, kDatasetPerLaunch>;
 
-__global__ void __launch_bounds__(kDatasetThreads) mosaic_kernel(const DatasetList L) {
-  const int img = blockIdx.y, W = L.W[img], h = L.H[img] >> 1, w = W >> 1;
+__global__ void __launch_bounds__(kDatasetThreads) mosaic_kernel(const DatasetRecords L) {
+  const DatasetRecord& im = L.at[blockIdx.y];
+  const int W = im.W, h = im.H >> 1, w = W >> 1;
   const long long quads = (long long)h * w;
-  const uint8_t* src = L.src[img];
-  float* dst = static_cast<float*>(L.dst[img]);
+  const uint8_t* src = im.src;
+  float* dst = static_cast<float*>(im.dst);
   for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < quads; q += (long long)gridDim.x * blockDim.x) {
     const int y = (int)(q / w), x = (int)(q - (long long)y * w);
 #pragma unroll
@@ -34,11 +36,11 @@ __global__ void __launch_bounds__(kDatasetThreads) mosaic_kernel(const DatasetLi
   }
 }
 
-__global__ void __launch_bounds__(kDatasetThreads) luma_kernel(const DatasetList L) {
-  const int img = blockIdx.y;
-  const long long n = (long long)L.H[img] * L.W[img];
-  const uint8_t* src = L.src[img];
-  uint8_t* dst = static_cast<uint8_t*>(L.dst[img]);
+__global__ void __launch_bounds__(kDatasetThreads) luma_kernel(const DatasetRecords L) {
+  const DatasetRecord& im = L.at[blockIdx.y];
+  const long long n = (long long)im.H * im.W;
+  const uint8_t* src = im.src;
+  uint8_t* dst = static_cast<uint8_t*>(im.dst);
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
     dst[i] = luma_y(src[3 * i], src[3 * i + 1], src[3 * i + 2]);
 }
@@ -46,36 +48,28 @@ __global__ void __launch_bounds__(kDatasetThreads) luma_kernel(const DatasetList
 // Every image: an (H, W, 3) uint8 source and its destination, (4, H / 2, W / 2) fp32 planes (mosaic) or (H, W, 1) uint8
 // (luma).  An empty destination (a source of one row or column, mosaic) may have a null pointer.
 int check_dataset(const GrlImageRef* src, const GrlImageRef* dst, int n, bool mosaic, const char* what) {
-  GRL_REQUIRE(n >= 0 && ((src && dst) || n == 0), "%s: null image list (n = %d)", what, n);
-  for (int i = 0; i < n; ++i) {
-    const GrlImageRef &s = src[i], &d = dst[i];
-    const int kind = mosaic ? GRL_IMAGE_RGGB : GRL_IMAGE_U8, dh = mosaic ? s.H / 2 : s.H, dw = mosaic ? s.W / 2 : s.W;
-    GRL_REQUIRE(s.kind == GRL_IMAGE_U8 && d.kind == kind, "%s: image %d: kinds %d / %d, need GRL_IMAGE_U8 -> %s", what, i,
-                s.kind, d.kind, mosaic ? "GRL_IMAGE_RGGB" : "GRL_IMAGE_U8");
-    GRL_REQUIRE(s.H >= 1 && s.W >= 1 && d.H == dh && d.W == dw, "%s: image %d: sizes %d x %d -> %d x %d, need %d x %d",
-                what, i, s.H, s.W, d.H, d.W, dh, dw);
-    GRL_REQUIRE((long long)s.H * s.W * 3 <= 0x7fffffffLL, "%s: image %d: %d x %d x 3 bytes is too large", what, i, s.H,
-                s.W);
-    GRL_REQUIRE(s.data && (d.data || (long long)d.H * d.W == 0), "%s: image %d: null data", what, i);
-  }
-  return GRL_OK;
+  return check_u8_pairs(
+      src, dst, n, mosaic ? GRL_IMAGE_RGGB : GRL_IMAGE_U8,
+      [&](const GrlImageRef& s) { return mosaic ? make_int2(s.H / 2, s.W / 2) : make_int2(s.H, s.W); },
+      [&](const GrlImageRef& s, int i) -> int {
+        GRL_REQUIRE((long long)s.H * s.W * 3 <= 0x7fffffffLL, "%s: image %d: %d x %d x 3 bytes is too large", what, i,
+                    s.H, s.W);
+        return GRL_OK;
+      },
+      what);
 }
 
 int launch_dataset(const GrlImageRef* src, const GrlImageRef* dst, int n, bool mosaic, cudaStream_t st) {
-  DatasetList L;
-  for (int i0 = 0; i0 < n; i0 += kDatasetPerLaunch) {
-    const int m = n - i0 < kDatasetPerLaunch ? n - i0 : kDatasetPerLaunch;
-    long long most = 0;
+  const auto add = [&](DatasetRecord& r, int, int i) {
+    r = {static_cast<const uint8_t*>(src[i].data), dst[i].data, src[i].H, src[i].W};
+    return (long long)dst[i].H * dst[i].W;
+  };
+  return launch_list<DatasetRecords>(n, add, [&](const DatasetRecords& L, int, int m) -> int {
+    long long most = 0;  // work items of the launch's largest image
     for (int j = 0; j < m; ++j) {
-      const GrlImageRef &s = src[i0 + j], &d = dst[i0 + j];
-      L.src[j] = static_cast<const uint8_t*>(s.data);
-      L.dst[j] = d.data;
-      L.H[j] = s.H;
-      L.W[j] = s.W;
-      const long long items = (long long)d.H * d.W;
-      most = items > most ? items : most;
+      const int h = mosaic ? L.at[j].H >> 1 : L.at[j].H, w = mosaic ? L.at[j].W >> 1 : L.at[j].W;
+      most = (long long)h * w > most ? (long long)h * w : most;
     }
-    if (most == 0) continue;
     const dim3 grid(ceil_div(most, kDatasetThreads) < kDatasetMaxBlocksX ? ceil_div(most, kDatasetThreads)
                                                                          : kDatasetMaxBlocksX, m);
     if (mosaic) {
@@ -85,8 +79,8 @@ int launch_dataset(const GrlImageRef* src, const GrlImageRef* dst, int n, bool m
       luma_kernel<<<grid, kDatasetThreads, 0, st>>>(L);
       GRL_LAUNCH_CHECK("luma_kernel");
     }
-  }
-  return GRL_OK;
+    return GRL_OK;
+  });
 }
 
 }  // namespace

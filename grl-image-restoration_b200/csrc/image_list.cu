@@ -4,13 +4,14 @@
 // into such a batch and blends the batch's outputs into each image's accumulator (grl_tiles.h).
 //
 // Both are HBM-bound and tiled like image_u8.cu: a CTA of 32 x 8 threads owns a 32 x 32 pixel tile of one image of the
-// list (grid.z = image).  The image descriptors (GrlImageRef) travel by value in the kernel parameters, at most
-// kListPerLaunch per launch, so a call needs no device copy of them.  8-bit pixels are staged in shared memory by
+// list (grid.z = image).  The descriptors (GrlImageRef, GrlTileRef, GrlTileImage) travel by value in the kernel
+// parameters (grl_param_list.cuh), so a call needs no device copy of them.  8-bit pixels are staged in shared memory by
 // grl_pixel_tile.cuh; fp32 planes and packed RGGB planes are read straight from global memory, one thread per output
 // column.
 #include "grl_common.cuh"
 #include "grl_demosaic.h"
 #include "grl_image_u8.h"
+#include "grl_param_list.cuh"
 #include "grl_pixel_tile.cuh"
 #include "grl_tiles.h"
 
@@ -18,21 +19,12 @@ namespace grl {
 
 namespace {
 
-constexpr int kListPerLaunch = 128;  // 128 x 24-byte refs: 3 KB of the 4 KB of kernel parameters
-
-constexpr int kTilesPerLaunch = 96;  // 96 x 40-byte GrlTileRef: 3.75 KB
-constexpr int kBlendPerLaunch = 80;  // 80 x 48-byte GrlTileImage: 3.75 KB
-static_assert(sizeof(GrlTileRef) == 40 && sizeof(GrlTileImage) == 48, "descriptor sizes the per-launch counts assume");
-
-struct ListRefs {
-  GrlImageRef im[kListPerLaunch];
-};
-struct TileRefs {
-  GrlTileRef t[kTilesPerLaunch];
-};
-struct BlendRefs {
-  GrlTileImage im[kBlendPerLaunch];
-};
+// Per launch: 128 x 24-byte GrlImageRef, 96 x 40-byte GrlTileRef or 80 x 48-byte GrlTileImage, and at most a pointer
+// and four ints besides.
+constexpr int kOtherParams = sizeof(float*) + 4 * sizeof(int);
+using ImageRecords = ParamList<GrlImageRef, 128, kOtherParams>;
+using TileRecords = ParamList<GrlTileRef, 96, kOtherParams>;
+using BlendRecords = ParamList<GrlTileImage, 80, kOtherParams>;
 
 // The region a gather pads into one batch entry: a whole image of a list, or the t x t window at (y0, x0) of a tile's
 // source, in the frame the network sees.
@@ -41,13 +33,13 @@ struct Window {
   int y0, x0, h, w;
 };
 template <class Reader>
-__device__ __forceinline__ Window window(const ListRefs& refs, int z) {
-  const GrlImageRef& im = refs.im[z];
+__device__ __forceinline__ Window window(const ImageRecords& refs, int z) {
+  const GrlImageRef& im = refs.at[z];
   return {im, 0, 0, Reader::height(im), Reader::width(im)};
 }
 template <class Reader>
-__device__ __forceinline__ Window window(const TileRefs& refs, int z) {
-  const GrlTileRef& t = refs.t[z];
+__device__ __forceinline__ Window window(const TileRecords& refs, int z) {
+  const GrlTileRef& t = refs.at[z];
   return {t.src, t.y0, t.x0, t.t, t.t};
 }
 
@@ -77,7 +69,7 @@ struct RggbReader {  // (4, h, w) packed RGGB planes of a (2h, 2w) image, demosa
   }
 };
 
-// Refs: ListRefs (whole images) or TileRefs (tile windows).
+// Refs: ImageRecords (whole images) or TileRecords (tile windows).
 template <class Reader, class Refs>
 __global__ void __launch_bounds__(kTile * kTileRows) gather_planes_kernel(const Refs refs, int C, int Hp, int Wp,
                                                                            float* __restrict__ out) {
@@ -119,8 +111,8 @@ __global__ void __launch_bounds__(kTile * kTileRows, kTileMinBlocks)
 
 // y (n, C, Hy, Wy) -> the top-left (H, W) of image z as (C, H, W) fp32 planes
 __global__ void __launch_bounds__(kTile * kTileRows, kTileMinBlocks)
-    crop_planes_kernel(const float* __restrict__ y, int C, int Hy, int Wy, const ListRefs refs) {
-  const GrlImageRef& im = refs.im[blockIdx.z];
+    crop_planes_kernel(const float* __restrict__ y, int C, int Hy, int Wy, const ImageRecords refs) {
+  const GrlImageRef& im = refs.at[blockIdx.z];
   const int H = im.H, W = im.W;
   const int y0 = blockIdx.y * kTile, x = blockIdx.x * kTile + threadIdx.x;
   if (x >= W) return;
@@ -133,9 +125,9 @@ __global__ void __launch_bounds__(kTile * kTileRows, kTileMinBlocks)
 
 // ... as (H, W, C) uint8 = round8(v) (grl_f32_to_u8)
 __global__ void __launch_bounds__(kTile * kTileRows, kTileMinBlocks)
-    crop_u8_kernel(const float* __restrict__ y, int C, int Hy, int Wy, const ListRefs refs) {
+    crop_u8_kernel(const float* __restrict__ y, int C, int Hy, int Wy, const ImageRecords refs) {
   __shared__ PixelTile tile;
-  const GrlImageRef& im = refs.im[blockIdx.z];
+  const GrlImageRef& im = refs.at[blockIdx.z];
   const int H = im.H, W = im.W;
   const int y0 = blockIdx.y * kTile, x0 = blockIdx.x * kTile;
   if (y0 >= H || x0 >= W) return;  // the grid covers the launch's largest image
@@ -167,12 +159,13 @@ int check_image(const GrlImageRef& im, int i, int C, bool gather, int kind, int 
 
 // The checks both list entry points make before anything launches; *kind receives the list's kind.
 int check_list(const GrlImageRef* images, int n, int C, int Hmax, int Wmax, bool gather, int* kind, const char* what) {
-  GRL_REQUIRE(n >= 0 && (images || n == 0), "%s: null image list (n = %d)", what, n);
+  int rc = check_list_args(n, images != nullptr, "image", what);
+  if (rc != GRL_OK) return rc;
   GRL_REQUIRE(C >= 1 && C <= kTileMaxC, "%s: C = %d outside 1..%d", what, C, kTileMaxC);
   GRL_REQUIRE(Hmax >= 1 && Wmax >= 1 && Hmax <= 65535 * kTile, "%s: bad batch size %d x %d", what, Hmax, Wmax);
   *kind = n ? images[0].kind : GRL_IMAGE_F32;
   for (int i = 0; i < n; ++i) {
-    const int rc = check_image(images[i], i, C, gather, *kind, Hmax, Wmax, what);
+    rc = check_image(images[i], i, C, gather, *kind, Hmax, Wmax, what);
     if (rc != GRL_OK) return rc;
   }
   return GRL_OK;
@@ -182,8 +175,8 @@ int check_list(const GrlImageRef* images, int n, int C, int Hmax, int Wmax, bool
 // Every covering tile of a launch, in origin order, is added to the accumulator as E = E + o: the reference adds the
 // tiles one slice add_ at a time, so a pixel's sum is rounded after every tile in that order.  A thread owns one output
 // column of one image and walks kTile / kTileRows rows of it; the tile outputs it reads are rows of the batch's output.
-__global__ void __launch_bounds__(kTile * kTileRows) tile_accumulate_kernel(const float* __restrict__ y, int C, int Hy, int Wy, int s, const BlendRefs refs) {
-  const GrlTileImage& im = refs.im[blockIdx.z];
+__global__ void __launch_bounds__(kTile * kTileRows) tile_accumulate_kernel(const float* __restrict__ y, int C, int Hy, int Wy, int s, const BlendRecords refs) {
+  const GrlTileImage& im = refs.at[blockIdx.z];
   const TileAxis ay = tile_axis(im.H, im.t, im.overlap), ax = tile_axis(im.W, im.t, im.overlap);
   // the tile rows this launch holds of the image and the output rows they cover
   const int kr0 = im.k0 / ax.n, kr1 = (im.k1 - 1) / ax.n;
@@ -220,8 +213,8 @@ __device__ __forceinline__ float tile_count(const TileAxis& ay, const TileAxis& 
 
 // E / W in place (E.div_(W) with a tensor W is an IEEE division).
 __global__ void __launch_bounds__(kTile * kTileRows, kTileMinBlocks)
-    tile_finish_f32_kernel(int C, int s, const BlendRefs refs) {
-  const GrlTileImage& im = refs.im[blockIdx.z];
+    tile_finish_f32_kernel(int C, int s, const BlendRecords refs) {
+  const GrlTileImage& im = refs.at[blockIdx.z];
   const TileAxis ay = tile_axis(im.H, im.t, im.overlap), ax = tile_axis(im.W, im.t, im.overlap);
   const int Ho = im.H * s, Wo = im.W * s, X = blockIdx.x * kTile + threadIdx.x, Yt = blockIdx.y * kTile;
   if (X >= Wo || Yt >= Ho) return;
@@ -235,9 +228,9 @@ __global__ void __launch_bounds__(kTile * kTileRows, kTileMinBlocks)
 
 // ... as (H*s, W*s, C) uint8 = round8(E / W) (grl_f32_to_u8 of the reference's result)
 __global__ void __launch_bounds__(kTile * kTileRows, kTileMinBlocks)
-    tile_finish_u8_kernel(int C, int s, const BlendRefs refs) {
+    tile_finish_u8_kernel(int C, int s, const BlendRecords refs) {
   __shared__ PixelTile tile;
-  const GrlTileImage& im = refs.im[blockIdx.z];
+  const GrlTileImage& im = refs.at[blockIdx.z];
   const TileAxis ay = tile_axis(im.H, im.t, im.overlap), ax = tile_axis(im.W, im.t, im.overlap);
   const int Ho = im.H * s, Wo = im.W * s, Y0 = blockIdx.y * kTile, X0 = blockIdx.x * kTile;
   if (Y0 >= Ho || X0 >= Wo) return;  // the grid covers the launch's largest image
@@ -263,20 +256,54 @@ int check_blend(const GrlTileImage& im, int i, int s, const char* what) {
   return GRL_OK;
 }
 
-ListRefs refs_of(const GrlImageRef* images, int m) {
-  ListRefs refs = {};
-  for (int j = 0; j < m; ++j) refs.im[j] = images[j];
-  return refs;
+// The kTile x kTile tiles of the largest image of a launch's m records at scale s, one grid.z per record.
+template <class List>
+dim3 tile_grid(const List& L, int m, int s) {
+  int H = 1, W = 1;
+  for (int j = 0; j < m; ++j) H = max(H, L.at[j].H), W = max(W, L.at[j].W);
+  return dim3(ceil_div((long long)W * s, kTile), ceil_div((long long)H * s, kTile), m);
 }
-TileRefs refs_of(const GrlTileRef* tiles, int m) {
-  TileRefs refs = {};
-  for (int j = 0; j < m; ++j) refs.t[j] = tiles[j];
-  return refs;
+
+// The pad-gather of n images or tile windows into (n, C, Hp, Wp), every source of `kind`.
+template <class List, class Item>
+int gather(const Item* items, int n, int kind, int C, int Hp, int Wp, float* out, cudaStream_t st) {
+  const auto add = [&](Item& r, int, int i) {
+    r = items[i];
+    return 1LL;
+  };
+  return launch_list<List>(n, add, [&](const List& L, int i0, int m) -> int {
+    const dim3 grid(ceil_div(Wp, kTile), ceil_div(Hp, kTile), m), block(kTile, kTileRows);
+    float* o = out + i0 * (long long)C * Hp * Wp;
+    if (kind == GRL_IMAGE_U8)
+      gather_u8_kernel<List><<<grid, block, 0, st>>>(L, C, Hp, Wp, o);
+    else if (kind == GRL_IMAGE_RGGB)
+      gather_planes_kernel<RggbReader, List><<<grid, block, 0, st>>>(L, C, Hp, Wp, o);
+    else
+      gather_planes_kernel<PlanesReader, List><<<grid, block, 0, st>>>(L, C, Hp, Wp, o);
+    GRL_LAUNCH_CHECK("gather kernel");
+    return GRL_OK;
+  });
 }
-BlendRefs refs_of(const GrlTileImage* images, int m) {
-  BlendRefs refs = {};
-  for (int j = 0; j < m; ++j) refs.im[j] = images[j];
-  return refs;
+
+// The blend of m images: the batch y's tile outputs added to their accumulators, or (finish) E / count.
+int blend(const float* y, int C, int Hy, int Wy, int s, const GrlTileImage* images, int m, bool finish,
+          cudaStream_t st) {
+  const bool u8 = m && images[0].out_u8;
+  const auto add = [&](GrlTileImage& r, int, int i) {
+    r = images[i];
+    return 1LL;
+  };
+  return launch_list<BlendRecords>(m, add, [&](const BlendRecords& L, int, int mm) -> int {
+    const dim3 grid = tile_grid(L, mm, s), block(kTile, kTileRows);
+    if (!finish)
+      tile_accumulate_kernel<<<grid, block, 0, st>>>(y, C, Hy, Wy, s, L);
+    else if (u8)
+      tile_finish_u8_kernel<<<grid, block, 0, st>>>(C, s, L);
+    else
+      tile_finish_f32_kernel<<<grid, block, 0, st>>>(C, s, L);
+    GRL_LAUNCH_CHECK("tile blend kernel");
+    return GRL_OK;
+  });
 }
 
 }  // namespace
@@ -292,25 +319,7 @@ int grl_list_gather(const GrlImageRef* images, int n, int C, int Hp, int Wp, flo
   const int rc = check_list(images, n, C, Hp, Wp, true, &kind, "list_gather");
   if (rc != GRL_OK) return rc;
   GRL_REQUIRE(out || n == 0, "list_gather: null output");
-  const cudaStream_t st = (cudaStream_t)stream;
-  const long long per_image = (long long)C * Hp * Wp;
-  for (int i0 = 0; i0 < n; i0 += kListPerLaunch) {
-    const int m = min(kListPerLaunch, n - i0);
-    const ListRefs refs = refs_of(images + i0, m);
-    const dim3 grid(ceil_div(Wp, kTile), ceil_div(Hp, kTile), m), block(kTile, kTileRows);
-    float* o = out + i0 * per_image;
-    if (kind == GRL_IMAGE_U8) {
-      gather_u8_kernel<ListRefs><<<grid, block, 0, st>>>(refs, C, Hp, Wp, o);
-      GRL_LAUNCH_CHECK("gather_u8_kernel");
-    } else if (kind == GRL_IMAGE_RGGB) {
-      gather_planes_kernel<RggbReader, ListRefs><<<grid, block, 0, st>>>(refs, C, Hp, Wp, o);
-      GRL_LAUNCH_CHECK("gather_planes_kernel<RggbReader>");
-    } else {
-      gather_planes_kernel<PlanesReader, ListRefs><<<grid, block, 0, st>>>(refs, C, Hp, Wp, o);
-      GRL_LAUNCH_CHECK("gather_planes_kernel<PlanesReader>");
-    }
-  }
-  return GRL_OK;
+  return gather<ImageRecords>(images, n, kind, C, Hp, Wp, out, (cudaStream_t)stream);
 }
 
 int grl_list_crop(const float* y, int n, int C, int Hy, int Wy, const GrlImageRef* images, void* stream) {
@@ -319,35 +328,33 @@ int grl_list_crop(const float* y, int n, int C, int Hy, int Wy, const GrlImageRe
   if (rc != GRL_OK) return rc;
   GRL_REQUIRE(y || n == 0, "list_crop: null input");
   const cudaStream_t st = (cudaStream_t)stream;
-  const long long per_image = (long long)C * Hy * Wy;
-  for (int i0 = 0; i0 < n; i0 += kListPerLaunch) {
-    const int m = min(kListPerLaunch, n - i0);
-    const ListRefs refs = refs_of(images + i0, m);
-    int H = 1, W = 1;
-    for (int j = 0; j < m; ++j) H = max(H, refs.im[j].H), W = max(W, refs.im[j].W);
-    const dim3 grid(ceil_div(W, kTile), ceil_div(H, kTile), m), block(kTile, kTileRows);
-    const float* s = y + i0 * per_image;
-    if (kind == GRL_IMAGE_U8) {
-      crop_u8_kernel<<<grid, block, 0, st>>>(s, C, Hy, Wy, refs);
-      GRL_LAUNCH_CHECK("crop_u8_kernel");
-    } else {
-      crop_planes_kernel<<<grid, block, 0, st>>>(s, C, Hy, Wy, refs);
-      GRL_LAUNCH_CHECK("crop_planes_kernel");
-    }
-  }
-  return GRL_OK;
+  const auto add = [&](GrlImageRef& r, int, int i) {
+    r = images[i];
+    return 1LL;
+  };
+  return launch_list<ImageRecords>(n, add, [&](const ImageRecords& L, int i0, int m) -> int {
+    const dim3 grid = tile_grid(L, m, 1), block(kTile, kTileRows);
+    const float* s = y + i0 * (long long)C * Hy * Wy;
+    if (kind == GRL_IMAGE_U8)
+      crop_u8_kernel<<<grid, block, 0, st>>>(s, C, Hy, Wy, L);
+    else
+      crop_planes_kernel<<<grid, block, 0, st>>>(s, C, Hy, Wy, L);
+    GRL_LAUNCH_CHECK("crop kernel");
+    return GRL_OK;
+  });
 }
 
 int grl_tile_gather(const GrlTileRef* tiles, int n, int C, int Hp, int Wp, float* out, void* stream) {
   const char* what = "tile_gather";
-  GRL_REQUIRE(n >= 0 && (tiles || n == 0), "%s: null tile list (n = %d)", what, n);
+  int rc = check_list_args(n, tiles != nullptr, "tile", what);
+  if (rc != GRL_OK) return rc;
   GRL_REQUIRE(C >= 1 && C <= kTileMaxC, "%s: C = %d outside 1..%d", what, C, kTileMaxC);
   GRL_REQUIRE(Hp >= 1 && Wp >= 1 && Hp <= 65535 * kTile, "%s: bad batch size %d x %d", what, Hp, Wp);
   GRL_REQUIRE(out || n == 0, "%s: null output", what);
   const int kind = n ? tiles[0].src.kind : GRL_IMAGE_F32;
   for (int i = 0; i < n; ++i) {
     const GrlTileRef& t = tiles[i];
-    const int rc = check_image(t.src, i, C, true, kind, 0, 0, what);
+    rc = check_image(t.src, i, C, true, kind, 0, 0, what);
     if (rc != GRL_OK) return rc;
     const int k = t.src.kind == GRL_IMAGE_RGGB ? 2 : 1;
     GRL_REQUIRE(t.t >= 1 && t.t <= Hp && t.t <= Wp, "%s: tile %d: side %d outside 1..min(Hp, Wp) = %d", what, i, t.t,
@@ -357,38 +364,21 @@ int grl_tile_gather(const GrlTileRef* tiles, int n, int C, int Hp, int Wp, float
                 "%s: tile %d: window %d x %d at (%d, %d) is outside the %lld x %lld image", what, i, t.t, t.t, t.y0, t.x0,
                 (long long)k * t.src.H, (long long)k * t.src.W);
   }
-  const cudaStream_t st = (cudaStream_t)stream;
-  const long long per_tile = (long long)C * Hp * Wp;
-  for (int i0 = 0; i0 < n; i0 += kTilesPerLaunch) {
-    const int m = min(kTilesPerLaunch, n - i0);
-    const TileRefs refs = refs_of(tiles + i0, m);
-    const dim3 grid(ceil_div(Wp, kTile), ceil_div(Hp, kTile), m), block(kTile, kTileRows);
-    float* o = out + i0 * per_tile;
-    if (kind == GRL_IMAGE_U8) {
-      gather_u8_kernel<TileRefs><<<grid, block, 0, st>>>(refs, C, Hp, Wp, o);
-      GRL_LAUNCH_CHECK("gather_u8_kernel<TileRefs>");
-    } else if (kind == GRL_IMAGE_RGGB) {
-      gather_planes_kernel<RggbReader, TileRefs><<<grid, block, 0, st>>>(refs, C, Hp, Wp, o);
-      GRL_LAUNCH_CHECK("gather_planes_kernel<RggbReader, TileRefs>");
-    } else {
-      gather_planes_kernel<PlanesReader, TileRefs><<<grid, block, 0, st>>>(refs, C, Hp, Wp, o);
-      GRL_LAUNCH_CHECK("gather_planes_kernel<PlanesReader, TileRefs>");
-    }
-  }
-  return GRL_OK;
+  return gather<TileRecords>(tiles, n, kind, C, Hp, Wp, out, (cudaStream_t)stream);
 }
 
 int grl_tile_accumulate(const float* y, int n, int C, int Hy, int Wy, int scale, const GrlTileImage* images, int m,
                         void* stream) {
   const char* what = "tile_accumulate";
-  GRL_REQUIRE(m >= 0 && (images || m == 0), "%s: null image list (m = %d)", what, m);
+  int rc = check_list_args(m, images != nullptr, "image", what);
+  if (rc != GRL_OK) return rc;
   GRL_REQUIRE(C >= 1 && C <= kTileMaxC, "%s: C = %d outside 1..%d", what, C, kTileMaxC);
   GRL_REQUIRE(scale >= 1 && n >= 0 && Hy >= 1 && Wy >= 1, "%s: bad batch (n %d, %d x %d) or scale %d", what, n, Hy, Wy,
               scale);
   GRL_REQUIRE(y || m == 0, "%s: null input", what);
   for (int i = 0; i < m; ++i) {
     const GrlTileImage& im = images[i];
-    const int rc = check_blend(im, i, scale, what);
+    rc = check_blend(im, i, scale, what);
     if (rc != GRL_OK) return rc;
     const long long tiles = (long long)tile_axis(im.H, im.t, im.overlap).n * tile_axis(im.W, im.t, im.overlap).n;
     GRL_REQUIRE(im.k0 >= 0 && im.k0 < im.k1 && im.k1 <= tiles, "%s: image %d: tiles [%d, %d) outside its %lld tiles", what, i,
@@ -399,49 +389,23 @@ int grl_tile_accumulate(const float* y, int n, int C, int Hy, int Wy, int scale,
                 "%s: image %d: tile output %d x %d is bigger than the batch's %d x %d", what, i, im.t * scale, im.t * scale,
                 Hy, Wy);
   }
-  const cudaStream_t st = (cudaStream_t)stream;
-  for (int i0 = 0; i0 < m; i0 += kBlendPerLaunch) {
-    const int mm = min(kBlendPerLaunch, m - i0);
-    const BlendRefs refs = refs_of(images + i0, mm);
-    int H = 1, W = 1;
-    for (int j = 0; j < mm; ++j) H = max(H, refs.im[j].H), W = max(W, refs.im[j].W);
-    const dim3 grid(ceil_div((long long)W * scale, kTile), ceil_div((long long)H * scale, kTile), mm),
-        block(kTile, kTileRows);
-    tile_accumulate_kernel<<<grid, block, 0, st>>>(y, C, Hy, Wy, scale, refs);
-    GRL_LAUNCH_CHECK("tile_accumulate_kernel");
-  }
-  return GRL_OK;
+  return blend(y, C, Hy, Wy, scale, images, m, false, (cudaStream_t)stream);
 }
 
 int grl_tile_finish(const GrlTileImage* images, int m, int C, int scale, void* stream) {
   const char* what = "tile_finish";
-  GRL_REQUIRE(m >= 0 && (images || m == 0), "%s: null image list (m = %d)", what, m);
+  int rc = check_list_args(m, images != nullptr, "image", what);
+  if (rc != GRL_OK) return rc;
   GRL_REQUIRE(C >= 1 && C <= kTileMaxC, "%s: C = %d outside 1..%d", what, C, kTileMaxC);
   GRL_REQUIRE(scale >= 1, "%s: bad scale %d", what, scale);
   const bool u8 = m && images[0].out_u8;
   for (int i = 0; i < m; ++i) {
-    const int rc = check_blend(images[i], i, scale, what);
+    rc = check_blend(images[i], i, scale, what);
     if (rc != GRL_OK) return rc;
     GRL_REQUIRE(!images[i].out_u8 == !u8, "%s: image %d: uint8 output %s, image 0's %s: one output kind per call", what,
                 i, images[i].out_u8 ? "set" : "NULL", u8 ? "set" : "NULL");
   }
-  const cudaStream_t st = (cudaStream_t)stream;
-  for (int i0 = 0; i0 < m; i0 += kBlendPerLaunch) {
-    const int mm = min(kBlendPerLaunch, m - i0);
-    const BlendRefs refs = refs_of(images + i0, mm);
-    int H = 1, W = 1;
-    for (int j = 0; j < mm; ++j) H = max(H, refs.im[j].H), W = max(W, refs.im[j].W);
-    const dim3 grid(ceil_div((long long)W * scale, kTile), ceil_div((long long)H * scale, kTile), mm),
-        block(kTile, kTileRows);
-    if (u8) {
-      tile_finish_u8_kernel<<<grid, block, 0, st>>>(C, scale, refs);
-      GRL_LAUNCH_CHECK("tile_finish_u8_kernel");
-    } else {
-      tile_finish_f32_kernel<<<grid, block, 0, st>>>(C, scale, refs);
-      GRL_LAUNCH_CHECK("tile_finish_f32_kernel");
-    }
-  }
-  return GRL_OK;
+  return blend(nullptr, C, 0, 0, scale, images, m, true, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -2,8 +2,8 @@
 // of 8-bit images: the pixels of a baseline encode at quality q followed by the default decode, bit for bit, from the
 // closed forms of grl_jpeg.h.
 //
-// Two kernels over flattened indices of the whole list (at most kJpegPerLaunch images per launch; the descriptors travel
-// by value in the kernel parameters, as in image_list.cu):
+// Two kernels over flattened indices of the whole list (at most kJpegPerLaunch images per launch, their records by value
+// in the kernel parameters, grl_param_list.cuh; a thread finds its image with record_of):
 //   jpeg_blocks_kernel  one thread per coded 8 x 8 block of every component: loads its samples (clamp-to-edge; a chroma
 //                       block converts and downsamples its 16 x 16 image pixels), then FDCT -> quantise -> dequantise ->
 //                       IDCT.  Gray: the decoded block is the output.  Colour: Y goes to an (H, W) workspace plane, Cb
@@ -14,34 +14,27 @@
 // kernel would redo the halo blocks' DCTs.
 #include "grl_common.cuh"
 #include "grl_jpeg.h"
+#include "grl_param_list.cuh"
 
 namespace grl {
 
 namespace {
 
-constexpr int kJpegPerLaunch = 80;  // 80 x 40 bytes of descriptors + the tables: 3.3 KB of the 4 KB of kernel parameters
+constexpr int kJpegPerLaunch = 80;
 constexpr int kBlockThreads = 128, kPixelThreads = 256;
 
-struct JpegList {
-  const uint8_t* src[kJpegPerLaunch];
-  uint8_t* dst[kJpegPerLaunch];
-  uint8_t* ws[kJpegPerLaunch];       // colour: Y (H, W), then Cb and Cr (h2, w2)
-  int H[kJpegPerLaunch], W[kJpegPerLaunch];
-  int block0[kJpegPerLaunch + 1];    // first block / pixel of image i in the launch's flat index; [m] = the total
-  int pixel0[kJpegPerLaunch + 1];
-  uint8_t qt[2][64];                 // luma, chroma; natural order
+struct JpegRecord {
+  const uint8_t* src;
+  uint8_t* dst;
+  uint8_t* ws;  // colour: Y (H, W), then Cb and Cr (h2, w2)
+  int H, W;
 };
-static_assert(sizeof(JpegList) + 2 * sizeof(int) <= 4096, "kernel parameters");
-
-// The image of flat index t: the last i < m with first[i] <= t.
-__device__ __forceinline__ int find_image(const int* first, int m, int t) {
-  int lo = 0, hi = m - 1;
-  while (lo < hi) {
-    const int mid = (lo + hi + 1) >> 1;
-    if (first[mid] <= t) lo = mid; else hi = mid - 1;
-  }
-  return lo;
-}
+struct JpegLaunch {
+  int block0[kJpegPerLaunch + 1];  // first block / pixel of image i in the launch's flat index; [m] = the total
+  int pixel0[kJpegPerLaunch + 1];
+  uint8_t qt[2][64];               // luma, chroma; natural order
+};
+using JpegRecords = ParamList<JpegRecord, kJpegPerLaunch, sizeof(JpegLaunch) + 2 * sizeof(int)>;
 
 GRL_HD long long blocks_of(int H, int W, int C) {
   const JpegImage im{nullptr, H, W, C};
@@ -54,12 +47,14 @@ GRL_HD long long workspace_of(int H, int W, int C) {
   return C == 3 ? (long long)H * W + 2LL * ((H + 1) >> 1) * ((W + 1) >> 1) : 0;
 }
 
-__global__ void __launch_bounds__(kBlockThreads) jpeg_blocks_kernel(const JpegList L, int m, int C) {
+__global__ void __launch_bounds__(kBlockThreads) jpeg_blocks_kernel(const JpegRecords L, const JpegLaunch X, int m,
+                                                                     int C) {
   const int t = blockIdx.x * kBlockThreads + threadIdx.x;
-  if (t >= L.block0[m]) return;
-  const int i = find_image(L.block0, m, t);
-  const JpegImage im{L.src[i], L.H[i], L.W[i], C};
-  int k = t - L.block0[i], comp = 0;
+  if (t >= X.block0[m]) return;
+  const int i = record_of(X.block0, m, t);
+  const JpegRecord& r = L.at[i];
+  const JpegImage im{r.src, r.H, r.W, C};
+  int k = t - X.block0[i], comp = 0;
   const int nluma = jpeg_blocks_y(im, 0) * jpeg_blocks_x(im, 0);
   if (k >= nluma) {
     const int nc = jpeg_blocks_y(im, 1) * jpeg_blocks_x(im, 1);
@@ -68,39 +63,37 @@ __global__ void __launch_bounds__(kBlockThreads) jpeg_blocks_kernel(const JpegLi
   }
   const int nx = jpeg_blocks_x(im, comp), by = k / nx, bx = k - by * nx;
   const long long plane = (long long)im.H * im.W, cplane = (long long)im.h2() * im.w2();
-  uint8_t* out = C == 1 ? L.dst[i] : L.ws[i] + (comp ? plane + (comp - 1) * cplane : 0);
-  jpeg_component_block(im, comp, by, bx, L.qt[comp ? 1 : 0], out, comp ? im.w2() : im.W);
+  uint8_t* out = C == 1 ? r.dst : r.ws + (comp ? plane + (comp - 1) * cplane : 0);
+  jpeg_component_block(im, comp, by, bx, X.qt[comp ? 1 : 0], out, comp ? im.w2() : im.W);
 }
 
-__global__ void __launch_bounds__(kPixelThreads) jpeg_rgb_kernel(const JpegList L, int m) {
+__global__ void __launch_bounds__(kPixelThreads) jpeg_rgb_kernel(const JpegRecords L, const JpegLaunch X, int m) {
   const int p = blockIdx.x * kPixelThreads + threadIdx.x;
-  if (p >= L.pixel0[m]) return;
-  const int i = find_image(L.pixel0, m, p);
-  const int H = L.H[i], W = L.W[i], k = p - L.pixel0[i], y = k / W, x = k - y * W;
+  if (p >= X.pixel0[m]) return;
+  const int i = record_of(X.pixel0, m, p);
+  const JpegRecord& r = L.at[i];
+  const int H = r.H, W = r.W, k = p - X.pixel0[i], y = k / W, x = k - y * W;
   const long long plane = (long long)H * W, cplane = (long long)((H + 1) >> 1) * ((W + 1) >> 1);
-  const uint8_t* ws = L.ws[i];
+  const uint8_t* ws = r.ws;
   uint8_t rgb[3];
   jpeg_decode_pixel(ws, ws + plane, ws + plane + cplane, H, W, y, x, rgb);
-  uint8_t* d = L.dst[i] + 3LL * k;
+  uint8_t* d = r.dst + 3LL * k;
   d[0] = rgb[0];
   d[1] = rgb[1];
   d[2] = rgb[2];
 }
 
 int check_jpeg(const GrlImageRef* src, const GrlImageRef* dst, int n, int C, int quality, const char* what) {
-  GRL_REQUIRE(n >= 0 && ((src && dst) || n == 0), "%s: null image list (n = %d)", what, n);
   GRL_REQUIRE(C == 1 || C == 3, "%s: C = %d, a JPEG image is gray (C = 1) or RGB (C = 3)", what, C);
   GRL_REQUIRE(quality >= 1 && quality <= 100, "%s: quality %d outside 1..100", what, quality);
-  for (int i = 0; i < n; ++i) {
-    const GrlImageRef &s = src[i], &d = dst[i];
-    GRL_REQUIRE(s.kind == GRL_IMAGE_U8 && d.kind == GRL_IMAGE_U8, "%s: image %d: kinds %d / %d, need GRL_IMAGE_U8", what,
-                i, s.kind, d.kind);
-    GRL_REQUIRE(s.data && d.data, "%s: image %d: null data", what, i);
-    GRL_REQUIRE(s.H >= 1 && s.W >= 1 && s.H == d.H && s.W == d.W, "%s: image %d: sizes %d x %d -> %d x %d", what, i, s.H,
-                s.W, d.H, d.W);
-    GRL_REQUIRE((long long)s.H * s.W <= 0x7fffffffLL / 2, "%s: image %d: %d x %d pixels is too large", what, i, s.H, s.W);
-  }
-  return GRL_OK;
+  return check_u8_pairs(
+      src, dst, n, GRL_IMAGE_U8, [](const GrlImageRef& s) { return make_int2(s.H, s.W); },
+      [&](const GrlImageRef& s, int i) -> int {
+        GRL_REQUIRE((long long)s.H * s.W <= 0x7fffffffLL / 2, "%s: image %d: %d x %d pixels is too large", what, i, s.H,
+                    s.W);
+        return GRL_OK;
+      },
+      what);
 }
 
 }  // namespace
@@ -158,42 +151,31 @@ int grl_jpeg_roundtrip_u8(const GrlImageRef* src, const GrlImageRef* dst, int n,
   GRL_REQUIRE(workspace || need == 0, "jpeg_roundtrip_u8: null workspace");
   if (workspace_bytes < need)
     return fail(GRL_ERR_WORKSPACE, "jpeg_roundtrip_u8: workspace of %zu bytes, need %zu", workspace_bytes, need);
-  JpegList L;
+  JpegLaunch X;
   for (int t = 0; t < 2; ++t)
-    for (int k = 0; k < 64; ++k) L.qt[t][k] = (uint8_t)jpeg_quant(quality, t, k);
+    for (int k = 0; k < 64; ++k) X.qt[t][k] = (uint8_t)jpeg_quant(quality, t, k);
+  X.block0[0] = X.pixel0[0] = 0;
   const cudaStream_t st = (cudaStream_t)stream;
   uint8_t* ws = static_cast<uint8_t*>(workspace);
-  for (int i0 = 0; i0 < n;) {
-    // A launch takes images while its flat block and pixel counts fit an int.
-    int m = 0;
-    long long blocks = 0, pixels = 0;
-    while (i0 + m < n && m < kJpegPerLaunch) {
-      const GrlImageRef& s = src[i0 + m];
-      const long long b = blocks_of(s.H, s.W, C), p = (long long)s.H * s.W;
-      if (m && (blocks + b > 0x7fffffffLL || pixels + p > 0x7fffffffLL)) break;
-      L.src[m] = static_cast<const uint8_t*>(s.data);
-      L.dst[m] = static_cast<uint8_t*>(dst[i0 + m].data);
-      L.ws[m] = ws;
-      L.H[m] = s.H;
-      L.W[m] = s.W;
-      L.block0[m] = (int)blocks;
-      L.pixel0[m] = (int)pixels;
-      ws += workspace_of(s.H, s.W, C);
-      blocks += b;
-      pixels += p;
-      ++m;
-    }
-    L.block0[m] = (int)blocks;
-    L.pixel0[m] = (int)pixels;
-    jpeg_blocks_kernel<<<ceil_div(blocks, kBlockThreads), kBlockThreads, 0, st>>>(L, m, C);
+  const auto add = [&](JpegRecord& r, int j, int i) {
+    const GrlImageRef& s = src[i];
+    const long long blocks = blocks_of(s.H, s.W, C), b = X.block0[j] + blocks, p = X.pixel0[j] + (long long)s.H * s.W;
+    if (j && (b > 0x7fffffffLL || p > 0x7fffffffLL)) return -1LL;  // the launch's flat indices are ints
+    r = {static_cast<const uint8_t*>(s.data), static_cast<uint8_t*>(dst[i].data), ws, s.H, s.W};
+    ws += workspace_of(s.H, s.W, C);
+    X.block0[j + 1] = (int)b;
+    X.pixel0[j + 1] = (int)p;
+    return blocks;
+  };
+  return launch_list<JpegRecords>(n, add, [&](const JpegRecords& L, int, int m) -> int {
+    jpeg_blocks_kernel<<<ceil_div(X.block0[m], kBlockThreads), kBlockThreads, 0, st>>>(L, X, m, C);
     GRL_LAUNCH_CHECK("jpeg_blocks_kernel");
     if (C == 3) {
-      jpeg_rgb_kernel<<<ceil_div(pixels, kPixelThreads), kPixelThreads, 0, st>>>(L, m);
+      jpeg_rgb_kernel<<<ceil_div(X.pixel0[m], kPixelThreads), kPixelThreads, 0, st>>>(L, X, m);
       GRL_LAUNCH_CHECK("jpeg_rgb_kernel");
     }
-    i0 += m;
-  }
-  return GRL_OK;
+    return GRL_OK;
+  });
 }
 
 }  // extern "C"

@@ -6,12 +6,13 @@
 // One CTA per kResizeTH x kResizeTW output tile of one image, all channels in turn.  Per channel the H pass writes the
 // float32 column sums of the tile's output rows over the s (kResizeTW - 1) + T input columns its W pass reads into shared
 // memory; after a barrier the W pass reads its T taps from there.  A launch takes up to kResizePerLaunch images of any
-// sizes: their descriptors and first-tile numbers travel by value in the kernel parameters, and a CTA finds its image by
-// binary search over them.  No workspace, no host sync.
+// sizes: their records and first-tile numbers travel by value in the kernel parameters (grl_param_list.cuh), and a CTA
+// finds its image with record_of.  No workspace, no host sync.
 #include <vector>
 
 #include "grl_common.cuh"
 #include "grl_image_u8.h"
+#include "grl_param_list.cuh"
 #include "grl_resize.h"
 
 namespace grl {
@@ -21,17 +22,20 @@ namespace {
 constexpr int kResizePerLaunch = 64;
 constexpr int kResizeTH = 16, kResizeTW = 32, kResizeThreads = 256;
 
-struct ResizeList {
-  const void* src[kResizePerLaunch];
-  float* dst[kResizePerLaunch];
-  int H[kResizePerLaunch], W[kResizePerLaunch];
+struct ResizeRecord {
+  const void* src;
+  float* dst;
+  int H, W;  // of the source image
+};
+struct ResizeStarts {
   int tile0[kResizePerLaunch + 1];  // image j's tiles are CTAs tile0[j] .. tile0[j + 1] - 1
 };
 struct ResizeTaps {
   float w[kResizeMaxTaps];
 };
+using ResizeRecords =
+    ParamList<ResizeRecord, kResizePerLaunch, sizeof(ResizeStarts) + sizeof(ResizeTaps) + 2 * sizeof(int)>;
 static_assert(kResizeThreads >= 256, "one thread per entry of the k / 255 table");
-static_assert(sizeof(ResizeList) + sizeof(ResizeTaps) + 2 * sizeof(int) <= 4096, "kernel parameters");
 
 // (C, H, W) float32 planes
 struct F32Img {
@@ -59,25 +63,21 @@ __host__ __device__ int resize_tiles(int H, int W, int s) {
 }
 
 template <class Img, int S>
-__global__ void __launch_bounds__(kResizeThreads) imresize_kernel(const ResizeList L, const ResizeTaps taps, int m,
-                                                                   int C) {
+__global__ void __launch_bounds__(kResizeThreads) imresize_kernel(const ResizeRecords L, const ResizeStarts X,
+                                                                   const ResizeTaps taps, int m, int C) {
   constexpr int T = resize_taps_of(S), c0 = resize_offset(S), kCols = S * (kResizeTW - 1) + T;
   __shared__ float t[kResizeTH][kCols];
   __shared__ float unit[256];
   if (threadIdx.x < 256) unit[threadIdx.x] = u8_unit(threadIdx.x);  // read by U8Img after the first barrier only
-  int lo = 0, hi = m - 1;  // the last image whose first tile is <= blockIdx.x
-  while (lo < hi) {
-    const int mid = (lo + hi + 1) >> 1;
-    if (L.tile0[mid] <= (int)blockIdx.x) lo = mid;
-    else hi = mid - 1;
-  }
-  const int H = L.H[lo], W = L.W[lo], h = (H + S - 1) / S, w = (W + S - 1) / S;
-  const int tiles_x = (w + kResizeTW - 1) / kResizeTW, tile = blockIdx.x - L.tile0[lo];
+  const int j = record_of(X.tile0, m, blockIdx.x);
+  const ResizeRecord& im = L.at[j];
+  const int H = im.H, W = im.W, h = (H + S - 1) / S, w = (W + S - 1) / S;
+  const int tiles_x = (w + kResizeTW - 1) / kResizeTW, tile = blockIdx.x - X.tile0[j];
   const int oy0 = tile / tiles_x * kResizeTH, ox0 = tile % tiles_x * kResizeTW;
   const int nh = min(kResizeTH, h - oy0), nw = min(kResizeTW, w - ox0), ncols = S * (nw - 1) + T;
-  const Img img = Img::at(L.src[lo], H, W, C, unit);
+  const Img img = Img::at(im.src, H, W, C, unit);
   __syncthreads();
-  float* dst = L.dst[lo];
+  float* dst = im.dst;
   for (int c = 0; c < C; ++c) {
     for (int i = threadIdx.x; i < nh * ncols; i += kResizeThreads) {
       const int r = i / ncols, xl = i - r * ncols;
@@ -110,49 +110,36 @@ int check_scale(int s, const char* what) {
   return GRL_OK;
 }
 
-template <class Img, int S>
-int launch_chunks(const void* const* src, float* const* dst, const int* H, const int* W, int n, int C, cudaStream_t st) {
+// Runs n images, image i's record from record(i).
+template <class Img, int S, class Record>
+int launch_resize(int n, int C, Record record, cudaStream_t st) {
+  ResizeStarts X;
   ResizeTaps taps;
   resize_taps(S, taps.w);
-  ResizeList L;
-  for (int i0 = 0; i0 < n; i0 += kResizePerLaunch) {
-    const int m = n - i0 < kResizePerLaunch ? n - i0 : kResizePerLaunch;
+  const auto add = [&](ResizeRecord& r, int, int i) {
+    r = record(i);
+    return (long long)resize_tiles(r.H, r.W, S);
+  };
+  return launch_list<ResizeRecords>(n, add, [&](const ResizeRecords& L, int, int m) -> int {
     long long total = 0;
     for (int j = 0; j < m; ++j) {
-      L.src[j] = src[i0 + j];
-      L.dst[j] = dst[i0 + j];
-      L.H[j] = H[i0 + j];
-      L.W[j] = W[i0 + j];
-      L.tile0[j] = (int)total;
-      total += resize_tiles(H[i0 + j], W[i0 + j], S);
+      X.tile0[j] = (int)total;
+      total += resize_tiles(L.at[j].H, L.at[j].W, S);
     }
     GRL_REQUIRE(total <= 0x7fffffffLL, "imresize: %lld tiles in one launch", total);
-    L.tile0[m] = (int)total;
-    if (total == 0) continue;
-    imresize_kernel<Img, S><<<(unsigned)total, kResizeThreads, 0, st>>>(L, taps, m, C);
+    X.tile0[m] = (int)total;
+    imresize_kernel<Img, S><<<(unsigned)total, kResizeThreads, 0, st>>>(L, X, taps, m, C);
     GRL_LAUNCH_CHECK("imresize_kernel");
-  }
-  return GRL_OK;
+    return GRL_OK;
+  });
 }
 
-template <class Img>
-int launch(const void* const* src, float* const* dst, const int* H, const int* W, int n, int C, int s, cudaStream_t st) {
-  if (s == 2) return launch_chunks<Img, 2>(src, dst, H, W, n, C, st);
-  if (s == 3) return launch_chunks<Img, 3>(src, dst, H, W, n, C, st);
-  return launch_chunks<Img, 4>(src, dst, H, W, n, C, st);
+template <class Img, class Record>
+int launch_resize(int n, int C, int s, Record record, cudaStream_t st) {
+  if (s == 2) return launch_resize<Img, 2>(n, C, record, st);
+  if (s == 3) return launch_resize<Img, 3>(n, C, record, st);
+  return launch_resize<Img, 4>(n, C, record, st);
 }
-
-// The host arrays of one call's images.
-struct ResizeRefs {
-  std::vector<const void*> src;
-  std::vector<float*> dst;
-  std::vector<int> H, W;
-  explicit ResizeRefs(int n) : src(n), dst(n), H(n), W(n) {}
-  template <class Img>
-  int launch(int C, int s, cudaStream_t st) const {
-    return grl::launch<Img>(src.data(), dst.data(), H.data(), W.data(), (int)src.size(), C, s, st);
-  }
-};
 
 }  // namespace
 
@@ -212,42 +199,23 @@ int grl_imresize_f32(const float* x, int B, int C, int H, int W, int s, float* y
   GRL_REQUIRE((x && y) || B == 0, "imresize_f32: null argument");
   rc = check_resize_geometry(H, W, C, s, "imresize_f32", 0);
   if (rc != GRL_OK) return rc;
-  if (B == 0) return GRL_OK;
-  ResizeRefs R(B);
   const long long in = (long long)C * H * W, out = (long long)C * ((H + s - 1) / s) * ((W + s - 1) / s);
-  for (int b = 0; b < B; ++b) {
-    R.src[b] = x + b * in;
-    R.dst[b] = y + b * out;
-    R.H[b] = H;
-    R.W[b] = W;
-  }
-  return R.launch<F32Img>(C, s, (cudaStream_t)stream);
+  return launch_resize<F32Img>(B, C, s, [&](int b) { return ResizeRecord{x + b * in, y + b * out, H, W}; },
+                               (cudaStream_t)stream);
 }
 
 int grl_imresize_u8_list(const GrlImageRef* src, const GrlImageRef* dst, int n, int C, int s, void* stream) {
   int rc = check_scale(s, "imresize_u8_list");
   if (rc != GRL_OK) return rc;
-  GRL_REQUIRE(n >= 0 && ((src && dst) || n == 0), "imresize_u8_list: null image list (n = %d)", n);
   GRL_REQUIRE(C == 1 || C == 3, "imresize_u8_list: C = %d, an 8-bit image here is gray (C = 1) or RGB (C = 3)", C);
-  for (int i = 0; i < n; ++i) {
-    const GrlImageRef &a = src[i], &b = dst[i];
-    GRL_REQUIRE(a.kind == GRL_IMAGE_U8 && b.kind == GRL_IMAGE_F32, "imresize_u8_list: image %d: kinds %d / %d, need "
-                "GRL_IMAGE_U8 -> GRL_IMAGE_F32", i, a.kind, b.kind);
-    GRL_REQUIRE(a.data && b.data, "imresize_u8_list: image %d: null data", i);
-    rc = check_resize_geometry(a.H, a.W, C, s, "imresize_u8_list", i);
-    if (rc != GRL_OK) return rc;
-    GRL_REQUIRE(b.H == (a.H + s - 1) / s && b.W == (a.W + s - 1) / s, "imresize_u8_list: image %d: %d x %d -> %d x %d, "
-                "need %d x %d", i, a.H, a.W, b.H, b.W, (a.H + s - 1) / s, (a.W + s - 1) / s);
-  }
-  if (n == 0) return GRL_OK;
-  ResizeRefs R(n);
-  for (int i = 0; i < n; ++i) {
-    R.src[i] = src[i].data;
-    R.dst[i] = static_cast<float*>(dst[i].data);
-    R.H[i] = src[i].H;
-    R.W[i] = src[i].W;
-  }
-  return R.launch<U8Img>(C, s, (cudaStream_t)stream);
+  rc = check_u8_pairs(
+      src, dst, n, GRL_IMAGE_F32, [&](const GrlImageRef& a) { return make_int2((a.H + s - 1) / s, (a.W + s - 1) / s); },
+      [&](const GrlImageRef& a, int i) { return check_resize_geometry(a.H, a.W, C, s, "imresize_u8_list", i); },
+      "imresize_u8_list");
+  if (rc != GRL_OK) return rc;
+  return launch_resize<U8Img>(n, C, s, [&](int i) {
+    return ResizeRecord{src[i].data, static_cast<float*>(dst[i].data), src[i].H, src[i].W};
+  }, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -372,21 +372,33 @@ def _jpeg_quality(quality):
     return quality
 
 
-def _jpeg_images(images, what):
-    """The list checks of jpeg_roundtrip_list and awgn_list: (H, W, C) uint8 on the current CUDA device, one C in
-    {1, 3}."""
+def _u8_images(images, what, channels):
+    """The checks of a list of 8-bit images: (H, W, C) uint8 tensors on the current CUDA device, H, W >= 1, one C in
+    `channels` for the whole list.  Returns that C (None for an empty list)."""
     C = None
     for i, t in enumerate(images):
         if not isinstance(t, torch.Tensor):
             raise ValueError(f"grl_b200: {what}: element {i} is a {type(t).__name__}, not a tensor")
         capi.require_device(t)
-        if t.dtype != torch.uint8 or t.dim() != 3 or t.shape[2] not in (1, 3) or t.shape[0] < 1 or t.shape[1] < 1:
-            raise ValueError(f"grl_b200: {what} needs (H, W, C) uint8 images with C in {{1, 3}}, got element {i}: {t.dtype} "
-                             f"{tuple(t.shape)}")
+        if t.dtype != torch.uint8 or t.dim() != 3 or t.shape[2] not in channels or t.shape[0] < 1 or t.shape[1] < 1:
+            raise ValueError(f"grl_b200: {what} needs (H, W, C) uint8 images with C in {set(channels)}, got element "
+                             f"{i}: {t.dtype} {tuple(t.shape)}")
         if C is not None and t.shape[2] != C:
             raise ValueError(f"grl_b200: {what}: element {i} has {t.shape[2]} channels, element 0 {C}: one C per call")
         C = t.shape[2]
     return C
+
+
+def _u8_batch(img, what, channels):
+    """The checks of a batch of 8-bit images: a (B, H, W, C) uint8 tensor on the current CUDA device, H, W >= 1, C in
+    `channels`.  Returns it contiguous."""
+    if not isinstance(img, torch.Tensor):
+        raise ValueError(f"grl_b200: {what} needs a tensor, got {type(img).__name__}")
+    capi.require_device(img)
+    if img.dtype != torch.uint8 or img.dim() != 4 or img.shape[3] not in channels or min(img.shape[1:3]) < 1:
+        raise ValueError(f"grl_b200: {what} needs (B, H, W, C) uint8 images with C in {set(channels)}, got "
+                         f"{img.dtype} {tuple(img.shape)}")
+    return img.contiguous()
 
 
 def _jpeg_launch(srcs, dsts, C, quality):
@@ -402,13 +414,7 @@ def jpeg_roundtrip(img, quality):
     for byte to cv2.imdecode(cv2.imencode(".jpg", img, [IMWRITE_JPEG_QUALITY, quality])) (colour via BGR, as the dataset
     does): libjpeg's baseline 4:2:0 encode and default decode.  quality: int in 1..100.  Two kernels (one for gray)."""
     quality = _jpeg_quality(quality)
-    if not isinstance(img, torch.Tensor):
-        raise ValueError(f"grl_b200: jpeg_roundtrip needs a tensor, got {type(img).__name__}")
-    capi.require_device(img)
-    if img.dtype != torch.uint8 or img.dim() != 4 or img.shape[3] not in (1, 3) or min(img.shape[1:3]) < 1:
-        raise ValueError(f"grl_b200: jpeg_roundtrip needs (B, H, W, C) uint8 images with C in {{1, 3}}, got {img.dtype} "
-                         f"{tuple(img.shape)}")
-    img = img.contiguous()
+    img = _u8_batch(img, "jpeg_roundtrip", (1, 3))
     out = torch.empty_like(img)
     if img.shape[0]:
         _jpeg_launch(list(img.unbind(0)), list(out.unbind(0)), img.shape[3], quality)
@@ -420,7 +426,7 @@ def jpeg_roundtrip_list(images, quality):
     -> list of new tensors in input order.  The whole list runs in two kernels per 80 images (one for gray)."""
     quality = _jpeg_quality(quality)
     images = list(images)
-    C = _jpeg_images(images, "jpeg_roundtrip_list")
+    C = _u8_images(images, "jpeg_roundtrip_list", (1, 3))
     if not images:
         return []
     srcs = [t.contiguous() for t in images]
@@ -513,14 +519,8 @@ def awgn(img, noise_sigma, seeds):
     real >= 0.  seeds: one per image, a dataset-relative path (through dn_seed) or 8 uint32 words.  The reference's crop
     to multiples of 8 stays with the caller: g[:H // 8 * 8, :W // 8 * 8].  One kernel per 64 images."""
     scale = _awgn_scale(noise_sigma)
-    if not isinstance(img, torch.Tensor):
-        raise ValueError(f"grl_b200: awgn needs a tensor, got {type(img).__name__}")
-    capi.require_device(img)
-    if img.dtype != torch.uint8 or img.dim() != 4 or img.shape[3] not in (1, 3) or min(img.shape[1:3]) < 1:
-        raise ValueError(f"grl_b200: awgn needs (B, H, W, C) uint8 images with C in {{1, 3}}, got {img.dtype} "
-                         f"{tuple(img.shape)}")
+    img = _u8_batch(img, "awgn", (1, 3))
     keys = _awgn_keys(seeds, img.shape[0], "awgn")
-    img = img.contiguous()
     B, H, W, C = img.shape
     out = torch.empty(B, C, H, W, device=img.device, dtype=torch.float32)
     if B:
@@ -534,7 +534,7 @@ def awgn_list(images, noise_sigma, seeds):
     images, one CTA per image."""
     scale = _awgn_scale(noise_sigma)
     images = list(images)
-    C = _jpeg_images(images, "awgn_list")
+    C = _u8_images(images, "awgn_list", (1, 3))
     keys = _awgn_keys(seeds, len(images), "awgn_list")
     if not images:
         return []
@@ -567,26 +567,6 @@ def awgn_log_host(x):
     return out
 
 
-def _rgb_u8_images(images, what):
-    """The list checks of mosaic_list and luma_list: (H, W, 3) uint8 on the current CUDA device."""
-    for i, t in enumerate(images):
-        if not isinstance(t, torch.Tensor):
-            raise ValueError(f"grl_b200: {what}: element {i} is a {type(t).__name__}, not a tensor")
-        capi.require_device(t)
-        if t.dtype != torch.uint8 or t.dim() != 3 or t.shape[2] != 3 or t.shape[0] < 1 or t.shape[1] < 1:
-            raise ValueError(f"grl_b200: {what} needs (H, W, 3) uint8 RGB images, got element {i}: {t.dtype} "
-                             f"{tuple(t.shape)}")
-
-
-def _rgb_u8_batch(img, what):
-    if not isinstance(img, torch.Tensor):
-        raise ValueError(f"grl_b200: {what} needs a tensor, got {type(img).__name__}")
-    capi.require_device(img)
-    if img.dtype != torch.uint8 or img.dim() != 4 or img.shape[3] != 3 or min(img.shape[1:3]) < 1:
-        raise ValueError(f"grl_b200: {what} needs (B, H, W, 3) uint8 RGB images, got {img.dtype} {tuple(img.shape)}")
-    return img.contiguous()
-
-
 def _mosaic_launch(srcs, outs):
     capi.check(capi.lib().grl_mosaic_u8(_image_refs(srcs, capi.IMAGE_U8), _image_refs(outs, capi.IMAGE_RGGB), len(srcs),
                                         capi.stream()))
@@ -597,7 +577,7 @@ def mosaic(img):
     (B, H, W, 3) uint8 RGB images on the GPU -> new (B, 4, H // 2, W // 2) float32 packed RGGB planes (R, G of the even
     rows, G of the odd rows, B), equal bit for bit to to_tensor(mosaic_CFA_Bayer(img[b])[1]); an odd last row or column is
     dropped.  What GRL(input_format="rggb") takes.  One kernel per 128 images."""
-    img = _rgb_u8_batch(img, "mosaic")
+    img = _u8_batch(img, "mosaic", (3,))
     B, H, W, _ = img.shape
     out = torch.empty(B, 4, H // 2, W // 2, device=img.device, dtype=torch.float32)
     if B:
@@ -609,7 +589,7 @@ def mosaic_list(images):
     """mosaic of a list of differently sized (H_i, W_i, 3) uint8 images on the GPU -> list of new (4, H_i // 2, W_i // 2)
     float32 tensors in input order, what GRL(input_format="rggb").forward_list takes.  One kernel per 128 images."""
     images = list(images)
-    _rgb_u8_images(images, "mosaic_list")
+    _u8_images(images, "mosaic_list", (3,))
     if not images:
         return []
     srcs = [t.contiguous() for t in images]
@@ -639,7 +619,7 @@ def luma(img):
     data/datasets/base_image.py:233-241): (B, H, W, 3) uint8 RGB images on the GPU -> new (B, H, W, 1) uint8, equal byte for
     byte to rgb2ycbcr_np(img[b], y_only=True) (MATLAB's rgb2ycbcr luma of k / 255, rounded half to even).  One kernel per
     128 images."""
-    img = _rgb_u8_batch(img, "luma")
+    img = _u8_batch(img, "luma", (3,))
     out = torch.empty(*img.shape[:3], 1, device=img.device, dtype=torch.uint8)
     if img.shape[0]:
         _luma_launch(list(img.unbind(0)), list(out.unbind(0)))
@@ -650,7 +630,7 @@ def luma_list(images):
     """luma of a list of differently sized (H_i, W_i, 3) uint8 images on the GPU -> list of new (H_i, W_i, 1) uint8
     tensors in input order.  One kernel per 128 images."""
     images = list(images)
-    _rgb_u8_images(images, "luma_list")
+    _u8_images(images, "luma_list", (3,))
     if not images:
         return []
     srcs = [t.contiguous() for t in images]
@@ -707,7 +687,7 @@ def imresize_list(images, scale):
     (data/datasets/restoration_sr.py:127-141), of modcropped images.  One kernel per 64 images."""
     s = _resize_factor(scale)
     images = list(images)
-    C = _jpeg_images(images, "imresize_list")
+    C = _u8_images(images, "imresize_list", (1, 3))
     if not images:
         return []
     srcs = [t.contiguous() for t in images]
