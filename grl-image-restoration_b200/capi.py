@@ -82,6 +82,8 @@ _SIGNATURES = {
     "grl_tc_head_pack": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(c_f32), c_f32, c_vp, c_int, c_vp, c_int, c_vp]),
     "grl_tc_head_pack_rggb": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(c_f32), c_f32, c_vp, c_int, c_vp, c_int, c_vp]),
     "grl_tc_avgpool16": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp]),
+    "grl_tc_maxpool16": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp]),
+    "grl_tc_anchor_gather16": (c_int, [c_vp, c_i64] + [c_int] * 8 + [c_vp, c_int, c_vp]),
     "grl_tc_slot_scale": (c_int, [c_vp, c_vp, c_vp, c_int, c_int, c_vp, c_vp]),
     "grl_tc_channel_gate_workspace": (c_sz, [c_int, c_i64, c_int]),
     "grl_tc_channel_gate": (c_int, [c_vp, c_i64, c_int, c_int, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_sz, c_vp]),
@@ -119,6 +121,8 @@ _SIGNATURES = {
     "grl_linear_f32": (c_int, [c_vp, c_i64, c_vp, c_vp, c_vp, c_i64, c_vp, c_i64, c_i64, c_int, c_int, c_int, c_f32, c_vp]),
     "grl_conv3x3_f32": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_f32, c_vp]),
     "grl_avgpool_f32": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp]),
+    "grl_maxpool_f32": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp]),
+    "grl_anchor_gather_f32": (c_int, [c_vp, c_i64] + [c_int] * 8 + [c_vp, c_int, c_vp]),
     "grl_ln_residual_f32": (c_int, [c_vp, c_vp, c_vp, c_vp, c_f32, c_f32, c_vp, c_vp, c_i64, c_vp, c_i64, c_int, c_vp]),
     "grl_channel_gate_workspace": (c_sz, [c_int, c_i64, c_int]),
     "grl_channel_gate_f32": (c_int, [c_vp, c_int, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_sz, c_vp]),

@@ -1,5 +1,5 @@
 // misc_tc.cu -- small memory-bound kernels around the tensor-core path: the network head (from RGB planes or from packed
-// Bayer planes), fp32 -> padded bf16 packing, bf16 average pooling (anchors), channel means of the CAB features, per-block
+// Bayer planes), fp32 -> padded bf16 packing, 16-bit average / max pooling (anchors), channel means of the CAB features, per-block
 // preparation of the attention constants.
 #include "grl_common.cuh"
 #include "grl_demosaic.h"
@@ -33,9 +33,11 @@ __global__ void unpack_bf16_kernel(const uint16_t* __restrict__ x, long long ldx
   y[m * ldy + c] = unpack16_one(x[m * ldx + x_off + c], fmt);
 }
 
-// AvgPool2d(df) on bf16 channels-last data, fp32 accumulation; 8 channels per thread.
-__global__ void avgpool_bf16_kernel(const uint16_t* __restrict__ x, uint16_t* __restrict__ y, int B, int H,
-                                    int W, int Cpad, int df, int fmt) {
+// AvgPool2d(df) / MaxPool2d(df) on 16-bit channels-last data, fp32 accumulation; 8 channels per thread.  Rounding to 16
+// bits is monotone, so the max of the rounded inputs is the rounded fp32 max.
+template <bool MAX>
+__global__ void pool16_kernel(const uint16_t* __restrict__ x, uint16_t* __restrict__ y, int B, int H, int W, int Cpad,
+                              int df, int fmt) {
   const int Ho = H / df, Wo = W / df, per = Cpad / 8;
   long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (long long)B * Ho * Wo * per) return;
@@ -45,7 +47,8 @@ __global__ void avgpool_bf16_kernel(const uint16_t* __restrict__ x, uint16_t* __
   t /= Wo;
   const int yo = (int)(t % Ho);
   const int b = (int)(t / Ho);
-  float s[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  const float s0 = MAX ? -INFINITY : 0.f;
+  float s[8] = {s0, s0, s0, s0, s0, s0, s0, s0};
   for (int dy = 0; dy < df; ++dy)
     for (int dx = 0; dx < df; ++dx) {
       const uint4 raw = *reinterpret_cast<const uint4*>(x + (((long long)b * H + yo * df + dy) * W + xo * df + dx) * Cpad + c0);
@@ -53,14 +56,32 @@ __global__ void avgpool_bf16_kernel(const uint16_t* __restrict__ x, uint16_t* __
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
         const float2 f = unpack16(p[e], fmt);
-        s[2 * e] += f.x;
-        s[2 * e + 1] += f.y;
+        if (MAX) {
+          s[2 * e] = (f.x > s[2 * e] || f.x != f.x) ? f.x : s[2 * e];
+          s[2 * e + 1] = (f.y > s[2 * e + 1] || f.y != f.y) ? f.y : s[2 * e + 1];
+        } else {
+          s[2 * e] += f.x;
+          s[2 * e + 1] += f.y;
+        }
       }
     }
-  const float inv = 1.f / (float)(df * df);
+  const float inv = MAX ? 1.f : 1.f / (float)(df * df);
   *reinterpret_cast<uint4*>(y + i * 8) =
       make_uint4(pack16(s[0] * inv, s[1] * inv, fmt), pack16(s[2] * inv, s[3] * inv, fmt),
                  pack16(s[4] * inv, s[5] * inv, fmt), pack16(s[6] * inv, s[7] * inv, fmt));
+}
+
+static int launch_pool16(const void* x, void* y, int B, int H, int W, int Cpad, int df, int fmt, bool max, cudaStream_t st) {
+  if (check_fmt(fmt)) return GRL_ERR_INVALID;
+  GRL_REQUIRE(df >= 1 && H % df == 0 && W % df == 0 && Cpad % 8 == 0, "pool16: bad shape");
+  long long total = (long long)B * (H / df) * (W / df) * (Cpad / 8);
+  if (total == 0) return GRL_OK;
+  if (max)
+    pool16_kernel<true><<<ceil_div(total, 256), 256, 0, st>>>((const uint16_t*)x, (uint16_t*)y, B, H, W, Cpad, df, fmt);
+  else
+    pool16_kernel<false><<<ceil_div(total, 256), 256, 0, st>>>((const uint16_t*)x, (uint16_t*)y, B, H, W, Cpad, df, fmt);
+  GRL_LAUNCH_CHECK("pool16_kernel");
+  return GRL_OK;
 }
 
 // Network input: check_image_size (reflect pad to a multiple of pad_size, grl.py:479-489) + (x - mean) * img_range
@@ -203,14 +224,11 @@ int grl_tc_head_pack_rggb(const float* cfa4, int B, int h, int w, int Hp, int Wp
 }
 
 int grl_tc_avgpool16(const void* x, void* y, int B, int H, int W, int Cpad, int df, int fmt, void* stream) {
-  if (check_fmt(fmt)) return GRL_ERR_INVALID;
-  GRL_REQUIRE(df >= 1 && H % df == 0 && W % df == 0 && Cpad % 8 == 0, "avgpool_bf16: bad shape");
-  long long total = (long long)B * (H / df) * (W / df) * (Cpad / 8);
-  if (total == 0) return GRL_OK;
-  avgpool_bf16_kernel<<<ceil_div(total, 256), 256, 0, (cudaStream_t)stream>>>((const uint16_t*)x, (uint16_t*)y, B, H, W, Cpad,
-                                                                              df, fmt);
-  GRL_LAUNCH_CHECK("avgpool_bf16_kernel");
-  return GRL_OK;
+  return launch_pool16(x, y, B, H, W, Cpad, df, fmt, false, (cudaStream_t)stream);
+}
+
+int grl_tc_maxpool16(const void* x, void* y, int B, int H, int W, int Cpad, int df, int fmt, void* stream) {
+  return launch_pool16(x, y, B, H, W, Cpad, df, fmt, true, (cudaStream_t)stream);
 }
 
 int grl_tc_slot_scale(const float* ls_w, const float* ls_s1, const float* ls_s2, int hw, int hs, float* out,

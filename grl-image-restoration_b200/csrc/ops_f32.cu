@@ -209,9 +209,10 @@ __global__ void __launch_bounds__(256) gemm_f32_kernel(GemmArgs a) {
 }
 
 // =====================================================================================
-// AvgPool2d(df) on channels-last data (AnchorLinear, mixed_attn_block.py:725,:733).
+// AvgPool2d(df) / MaxPool2d(df) on channels-last data (AnchorLinear, mixed_attn_block.py:723-726,:733).
 // =====================================================================================
-__global__ void avgpool_kernel(const float* __restrict__ x, float* __restrict__ y, int B, int H, int W, int C, int df) {
+template <bool MAX>
+__global__ void pool_kernel(const float* __restrict__ x, float* __restrict__ y, int B, int H, int W, int C, int df) {
   const int Ho = H / df, Wo = W / df;
   long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   long long total = (long long)B * Ho * Wo * C;
@@ -222,10 +223,16 @@ __global__ void avgpool_kernel(const float* __restrict__ x, float* __restrict__ 
   t /= Wo;
   int yo = (int)(t % Ho);
   int b = (int)(t / Ho);
-  float s = 0.f;
+  float s = MAX ? -INFINITY : 0.f;
   for (int dy = 0; dy < df; ++dy)
-    for (int dx = 0; dx < df; ++dx) s += x[(((long long)b * H + yo * df + dy) * W + xo * df + dx) * C + c];
-  y[i] = s / (float)(df * df);
+    for (int dx = 0; dx < df; ++dx) {
+      const float v = x[(((long long)b * H + yo * df + dy) * W + xo * df + dx) * C + c];
+      if (MAX)
+        s = (v > s || v != v) ? v : s;  // a NaN propagates, as in torch's max_pool2d
+      else
+        s += v;
+    }
+  y[i] = MAX ? s : s / (float)(df * df);
 }
 
 // =====================================================================================
@@ -539,13 +546,24 @@ int grl_conv3x3_f32(const float* x, const float* w, const float* b, const float*
   return launch_gemm(a, true, (cudaStream_t)stream);
 }
 
-int grl_avgpool_f32(const float* x, float* y, int B, int H, int W, int C, int df, void* stream) {
-  GRL_REQUIRE(df >= 1 && H % df == 0 && W % df == 0, "avgpool: %dx%d not divisible by %d", H, W, df);
+static int launch_pool(const float* x, float* y, int B, int H, int W, int C, int df, bool max, cudaStream_t st) {
+  GRL_REQUIRE(df >= 1 && H % df == 0 && W % df == 0, "pool: %dx%d not divisible by %d", H, W, df);
   long long total = (long long)B * (H / df) * (W / df) * C;
   if (total == 0) return GRL_OK;
-  avgpool_kernel<<<ceil_div(total, 256), 256, 0, (cudaStream_t)stream>>>(x, y, B, H, W, C, df);
-  GRL_LAUNCH_CHECK("avgpool_kernel");
+  if (max)
+    pool_kernel<true><<<ceil_div(total, 256), 256, 0, st>>>(x, y, B, H, W, C, df);
+  else
+    pool_kernel<false><<<ceil_div(total, 256), 256, 0, st>>>(x, y, B, H, W, C, df);
+  GRL_LAUNCH_CHECK("pool_kernel");
   return GRL_OK;
+}
+
+int grl_avgpool_f32(const float* x, float* y, int B, int H, int W, int C, int df, void* stream) {
+  return launch_pool(x, y, B, H, W, C, df, false, (cudaStream_t)stream);
+}
+
+int grl_maxpool_f32(const float* x, float* y, int B, int H, int W, int C, int df, void* stream) {
+  return launch_pool(x, y, B, H, W, C, df, true, (cudaStream_t)stream);
 }
 
 int grl_ln_residual_f32(const float* x, const float* u, const float* gamma, const float* beta, float eps,

@@ -58,11 +58,10 @@ def linear(x, weight, bias=None, act=ACT_NONE, slope=0.0, res=None, out=None):
 
 
 def pack_conv_weight(weight):
-    """(Cout, Cin, 3, 3) -> (Cout, 9*Cin) with k = (ky*3+kx)*Cin + c (the im2col order of the kernels)."""
+    """(Cout, Cin, kh, kw) -> (Cout, kh*kw*Cin) with k = (ky*kw+kx)*Cin + c: the im2col order of conv3x3 and the patch
+    order of anchor_gather."""
     co, ci, kh, kw = weight.shape
-    if (kh, kw) != (3, 3):
-        raise RuntimeError("grl_b200: only 3x3 convolutions are on this path")
-    return weight.detach().permute(0, 2, 3, 1).reshape(co, 9 * ci).contiguous()
+    return weight.detach().permute(0, 2, 3, 1).reshape(co, kh * kw * ci).contiguous()
 
 
 def conv3x3(x, wpacked, bias=None, act=ACT_NONE, slope=0.0, res=None, out=None):
@@ -70,6 +69,8 @@ def conv3x3(x, wpacked, bias=None, act=ACT_NONE, slope=0.0, res=None, out=None):
     x = _f32c(x, "x")
     B, H, W, Cin = x.shape
     Cout = wpacked.shape[0]
+    if wpacked.shape[1] != 9 * Cin:
+        raise RuntimeError("grl_b200: only 3x3 convolutions are on this path")
     y = out if out is not None else torch.empty(B, H, W, Cout, device=x.device, dtype=torch.float32)
     if res is not None:
         res = _f32c(res, "res")
@@ -78,11 +79,43 @@ def conv3x3(x, wpacked, bias=None, act=ACT_NONE, slope=0.0, res=None, out=None):
     return y
 
 
-def avgpool(x, df, out=None):
+def pool(x, df, mode="avgpool", out=None):
+    """AvgPool2d(df) / MaxPool2d(df) (mode "avgpool" / "maxpool") on channels-last x (B, H, W, C)."""
     x = _f32c(x, "x")
     B, H, W, C = x.shape
     y = out if out is not None else torch.empty(B, H // df, W // df, C, device=x.device, dtype=torch.float32)
-    capi.check(capi.lib().grl_avgpool_f32(capi.ptr(x), capi.ptr(y), B, H, W, C, df, capi.stream()))
+    fn = {"avgpool": capi.lib().grl_avgpool_f32, "maxpool": capi.lib().grl_maxpool_f32}[mode]
+    capi.check(fn(capi.ptr(x), capi.ptr(y), B, H, W, C, df, capi.stream()))
+    return y
+
+
+def avgpool(x, df, out=None):
+    return pool(x, df, "avgpool", out)
+
+
+def gather_size(H, W, ksize, stride, pad):
+    """(Ho, Wo) of a k x k, stride, zero-pad patch grid over an H x W image (nn.Conv2d's output size)."""
+    return (H + 2 * pad - ksize) // stride + 1, (W + 2 * pad - ksize) // stride + 1
+
+
+def anchor_gather(x, C, ksize, stride, pad, row_major, ldy=None, out=None):
+    """Patch rows of channels-last x (B, H, W, ld) (its first C channels; fp32, fp16 or bf16) -> (B*Ho*Wo, ldy) of x's
+    dtype: column tap*C + c holds channel c of patch tap (row-major taps: nn.Conv2d's order; else PatchMerging's column-
+    major order), zero outside the image and in the columns from k*k*C up to ldy (default k*k*C)."""
+    capi.require_device(x)
+    B, H, W, ld = x.shape
+    Ho, Wo = gather_size(H, W, ksize, stride, pad)
+    ldy = ksize * ksize * C if ldy is None else ldy
+    y = out if out is not None else torch.empty(B * Ho * Wo, ldy, device=x.device, dtype=x.dtype)
+    if x.dtype == torch.float32:
+        fn = capi.lib().grl_anchor_gather_f32
+    elif x.dtype in (torch.float16, torch.bfloat16):
+        fn = capi.lib().grl_tc_anchor_gather16
+    else:
+        raise RuntimeError(f"grl_b200: anchor_gather takes fp32 / fp16 / bf16, got {x.dtype}")
+    if y.dtype != x.dtype or not x.is_contiguous() or not y.is_contiguous():
+        raise RuntimeError("grl_b200: anchor_gather needs contiguous operands of one dtype")
+    capi.check(fn(capi.ptr(x), ld, B, H, W, C, ksize, stride, pad, int(bool(row_major)), capi.ptr(y), ldy, capi.stream()))
     return y
 
 

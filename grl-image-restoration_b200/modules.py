@@ -47,18 +47,22 @@ def linear(launch, name, x, lin, act=K.ACT_NONE):
     return y
 
 
-def conv3x3(launch, name, owner, key, x, act=K.ACT_NONE, slope=0.0, res=None):
-    """nn.Conv2d(3x3, stride 1, pad 1) `owner.<key>` on channels-last x (B, H, W, Cin), launched as `name`.  Its
-    (Cout, 9*Cin) im2col-ordered weight is cached on the owner under `key` (a streams.Produced) and re-packed when the
-    weight changes."""
-    conv = owner.get_submodule(key)
-    w = conv.weight
+def packed_conv(owner, key):
+    """The (Cout, kh*kw*Cin) weight of nn.Conv2d `owner.<key>` in K.pack_conv_weight's order, cached on the owner under
+    `key` (a streams.Produced) and re-packed when the weight changes."""
+    w = owner.get_submodule(key).weight
     version = (w.data_ptr(), w._version, w.device)
     cache = owner.__dict__.setdefault("_f32_convs", {})
     if cache.get(key, (None,))[0] != version:
         cache[key] = (version, Produced(K.pack_conv_weight(w)))
-    y = torch.empty(*x.shape[:-1], w.shape[0], device=x.device, dtype=torch.float32)
-    launch.listed(name, K.conv3x3, x, cache[key][1].use(), conv.bias, act, slope, res, out=y)
+    return cache[key][1].use()
+
+
+def conv3x3(launch, name, owner, key, x, act=K.ACT_NONE, slope=0.0, res=None):
+    """nn.Conv2d(3x3, stride 1, pad 1) `owner.<key>` on channels-last x (B, H, W, Cin), launched as `name`."""
+    conv = owner.get_submodule(key)
+    y = torch.empty(*x.shape[:-1], conv.weight.shape[0], device=x.device, dtype=torch.float32)
+    launch.listed(name, K.conv3x3, x, packed_conv(owner, key), conv.bias, act, slope, res, out=y)
     return y
 
 
@@ -122,7 +126,8 @@ class WindowAttention(nn.Module):
         self.shift_size = self.window_size[0] // 2 if window_shift else 0
         self.euclidean_dist = bool(getattr(args, "euclidean_dist", False))
         if self.euclidean_dist:
-            raise NotImplementedError("euclidean_dist is an ablation outside the hot path")
+            raise NotImplementedError("euclidean_dist replaces the attention kernels' cosine similarity; it is not "
+                                      "implemented")
         self.attn_transform = AffineTransform(num_heads)
         self.attn_drop = nn.Dropout(attn_drop)
         self.softmax = nn.Softmax(dim=-1)
@@ -159,7 +164,8 @@ class AnchorStripeAttention(nn.Module):
         self.anchor_window_down_factor = anchor_window_down_factor
         self.euclidean_dist = bool(getattr(args, "euclidean_dist", False))
         if self.euclidean_dist:
-            raise NotImplementedError("euclidean_dist is an ablation outside the hot path")
+            raise NotImplementedError("euclidean_dist replaces the attention kernels' cosine similarity; it is not "
+                                      "implemented")
         self.attn_transform1 = AffineTransform(num_heads)
         self.attn_transform2 = AffineTransform(num_heads)
         self.attn_drop = nn.Dropout(attn_drop)
@@ -197,7 +203,10 @@ class QKVProjection(nn.Module):
     def __init__(self, dim, qkv_bias, proj_type, args):
         super().__init__()
         if proj_type != "linear":
-            raise NotImplementedError(f"qkv_proj_type={proj_type!r}: only 'linear' is on the hot path")
+            # SeparableConv reads args.separable_conv_act (mixed_attn_block.py:655), which the args namespace GRL builds
+            # never sets (grl.py:302-308): the reference cannot construct this projection
+            raise NotImplementedError(f"qkv_proj_type={proj_type!r}: the reference's SeparableConv needs "
+                                      "args.separable_conv_act, which GRL never sets, so no such model exists")
         self.proj_type = proj_type
         self.body = nn.Linear(dim, dim * 3, bias=qkv_bias)
 
@@ -207,14 +216,16 @@ class QKVProjection(nn.Module):
 
 
 class AnchorLinear(nn.Module):
-    """mixed_attn_block.py:714-736: AvgPool2d(df) then Linear(C -> C/2); returns (B, H/df, W/df, C/2)."""
+    """mixed_attn_block.py:714-736: AvgPool2d(df) or MaxPool2d(df) then Linear(C -> C/2); returns (B, H/df, W/df, C/2)."""
 
     def __init__(self, in_channels, out_channels, down_factor, pooling_mode, bias):
         super().__init__()
-        if pooling_mode != "avgpool":
-            raise NotImplementedError(f"anchor pooling {pooling_mode!r}: only 'avgpool' is on the hot path")
         self.down_factor = down_factor
-        self.pooling = nn.AvgPool2d(down_factor, down_factor)
+        self.pooling_mode = pooling_mode
+        if pooling_mode == "maxpool":
+            self.pooling = nn.MaxPool2d(down_factor, down_factor)
+        elif pooling_mode == "avgpool":
+            self.pooling = nn.AvgPool2d(down_factor, down_factor)
         self.reduction = nn.Linear(in_channels, out_channels, bias=bias)
 
     @torch.no_grad()
@@ -222,24 +233,133 @@ class AnchorLinear(nn.Module):
         B, L, C = x.shape
         df = self.down_factor
         pooled = torch.empty(B, x_size[0] // df, x_size[1] // df, C, device=x.device, dtype=torch.float32)
-        launch.run(K.avgpool, x.view(B, x_size[0], x_size[1], C), df, out=pooled)
+        if self.pooling_mode == "avgpool":  # K.avgpool, not K.pool: the released configs' launch listing names it
+            launch.run(K.avgpool, x.view(B, x_size[0], x_size[1], C), df, out=pooled)
+        else:
+            launch.run(K.pool, x.view(B, x_size[0], x_size[1], C), df, self.pooling_mode, out=pooled)
         return linear(launch, name, pooled, self.reduction)
 
 
+class AnchorGather(NamedTuple):
+    """The patch grid of a convolutional anchor stage (K.anchor_gather): k x k patches at `stride`, zero `pad`, taps in
+    nn.Conv2d's row-major order or PatchMerging's column-major one."""
+    ksize: int
+    stride: int
+    pad: int
+    row_major: bool
+
+
+def anchor_gemm(launch, name, x, x_size, gather, weight, bias):
+    """One convolutional anchor stage on x (B, L, C) at x_size: the patch rows of K.anchor_gather, then a K.linear with
+    the (N, tap*C + c) `weight`; returns (B, Ho, Wo, N)."""
+    B, L, C = x.shape
+    Ho, Wo = K.gather_size(*x_size, gather.ksize, gather.stride, gather.pad)
+    cols = torch.empty(B * Ho * Wo, gather.ksize ** 2 * C, device=x.device, dtype=torch.float32)
+    launch.run(K.anchor_gather, x.view(B, *x_size, C), C, *gather, out=cols)
+    y = torch.empty(B, Ho, Wo, weight.shape[0], device=x.device, dtype=torch.float32)
+    launch.listed(name, K.linear, cols, weight, bias, K.ACT_NONE, out=y)
+    return y
+
+
+class PatchMerging(nn.Module):
+    """mixed_attn_block.py:679-711: 2 x 2 space-to-depth (x0 [0::2, 0::2], x1 [1::2, 0::2], x2 [0::2, 1::2],
+    x3 [1::2, 1::2]) then Linear(4 in_dim -> out_dim, no bias); returns (B, H/2, W/2, out_dim)."""
+
+    gather = AnchorGather(2, 2, 0, False)
+
+    def __init__(self, in_dim, out_dim):
+        super().__init__()
+        self.in_dim = in_dim
+        self.out_dim = out_dim
+        self.reduction = nn.Linear(4 * in_dim, out_dim, bias=False)
+
+    def packed(self):
+        """(weight (N, tap*C + c), bias) in K.anchor_gather's column order: the reduction's own."""
+        return self.reduction.weight, self.reduction.bias
+
+    @torch.no_grad()
+    def forward(self, x, x_size, launch=tc.DEVICE, name="anchor"):
+        return anchor_gemm(launch, name, x, x_size, self.gather, *self.packed())
+
+
+class AnchorConv2d(nn.Conv2d):
+    """nn.Conv2d(C, C/2, k, stride, pad) of the "conv2d" anchor projection (mixed_attn_block.py:747-751,:767), on
+    (B, L, C) tokens; returns (B, Ho, Wo, C/2).  Its parameters are the nn.Conv2d's (body.<i>.weight / bias)."""
+
+    @property
+    def gather(self):
+        return AnchorGather(self.kernel_size[0], self.stride[0], self.padding[0], True)
+
+    def packed(self):
+        """(weight (N, tap*C + c), bias) in K.anchor_gather's column order."""
+        return packed_conv(self, ""), self.bias
+
+    @torch.no_grad()
+    def forward(self, x, x_size, launch=tc.DEVICE, name="anchor"):
+        return anchor_gemm(launch, name, x, x_size, self.gather, *self.packed())
+
+
+ANCHOR_PROJ_TYPES = ("avgpool", "maxpool", "conv2d", "patchmerging")
+
+
+def anchor_projection_error(proj_type, one_stage, df):
+    """Why the reference cannot run AnchorProjection(proj_type, one_stage, df) (mixed_attn_block.py:739-785), or None.
+    Its anchors must be (H/df, W/df, C/2) for the stripe attention; the reference builds these bodies and fails in the
+    forward."""
+    if proj_type not in ANCHOR_PROJ_TYPES:
+        return f"anchor_proj_type must be one of {ANCHOR_PROJ_TYPES} (or 'separable_conv'), got {proj_type!r}"
+    if one_stage:
+        if proj_type == "conv2d" and df % 2:
+            return (f"a one-stage conv2d anchor projection with an odd anchor_window_down_factor ({df}) gives H/df + 1 "
+                    "anchor rows (kernel df+1, stride df, padding (df+1)//2)")
+        if proj_type == "patchmerging" and df != 2:
+            return f"a one-stage patchmerging anchor projection halves the size once; anchor_window_down_factor={df} != 2"
+        return None
+    if proj_type.find("pool") >= 0:
+        return (f"anchor_one_stage=False with {proj_type!r} builds an empty body: the anchors keep full resolution and C "
+                "channels")
+    if df < 2 or df & (df - 1):
+        return (f"anchor_one_stage=False runs int(log2(df)) stride-2 stages, which reach H/df only for a power of two "
+                f">= 2; anchor_window_down_factor={df}")
+    return None
+
+
 class AnchorProjection(nn.Module):
-    """mixed_attn_block.py:739-785 (one-stage avgpool variant)."""
+    """mixed_attn_block.py:739-785: one stage (pooling + Linear, a k = df+1 stride-df conv, or PatchMerging), or
+    log2(df) stride-2 stages (3x3 convs or PatchMerging, C -> C/2 then C/2 -> C/2).  Returns (B, H/df, W/df, C/2)."""
 
     def __init__(self, dim, proj_type, one_stage, anchor_window_down_factor, args):
         super().__init__()
-        if not one_stage or proj_type.find("pool") < 0:
-            raise NotImplementedError("only the one-stage avgpool anchor projection is on the hot path")
+        if proj_type == "separable_conv":
+            raise NotImplementedError("anchor_proj_type='separable_conv': the reference's SeparableConv needs "
+                                      "args.separable_conv_act, which GRL never sets, so no such model exists")
+        err = anchor_projection_error(proj_type, one_stage, anchor_window_down_factor)
+        if err is not None:
+            raise ValueError(err)
         self.proj_type = proj_type
-        self.body = nn.ModuleList([AnchorLinear(dim, dim // 2, anchor_window_down_factor, proj_type, True)])
+        self.body = nn.ModuleList([])
+        df = anchor_window_down_factor
+        if one_stage:
+            if proj_type == "patchmerging":
+                self.body.append(PatchMerging(dim, dim // 2))
+            elif proj_type == "conv2d":
+                self.body.append(AnchorConv2d(dim, dim // 2, df + 1, df, (df + 1) // 2))
+            else:
+                self.body.append(AnchorLinear(dim, dim // 2, df, proj_type, True))
+        else:
+            for i in range(int(math.log2(df))):
+                cin = dim if i == 0 else dim // 2
+                self.body.append(PatchMerging(cin, dim // 2) if proj_type == "patchmerging"
+                                 else AnchorConv2d(cin, dim // 2, 3, 2, 1))
 
     def forward(self, x, x_size, launch=tc.DEVICE, name="anchor"):
-        for m in self.body:
-            x = m(x, x_size, launch, name)
-        return x
+        """x (B, L, C) -> (B, H/df, W/df, C/2); stage i of several is launched as "{name}.{i}", the last as `name`."""
+        B = x.shape[0]
+        for i, m in enumerate(self.body):
+            last = i == len(self.body) - 1
+            y = m(x, x_size, launch, name if last else f"{name}.{i}")
+            x, x_size = y.view(B, y.shape[1] * y.shape[2], y.shape[3]), (y.shape[1], y.shape[2])
+        return y
 
 
 class MixedAttention(nn.Module):
@@ -436,11 +556,52 @@ class EfficientMixAttnTransformerBlock(nn.Module):
                 f"self.stripe_type={self.stripe_type}, mlp_ratio={self.mlp_ratio}, res_scale={self.res_scale}")
 
 
+class Linear(nn.Linear):
+    """swin_v1_block.py:457-466: nn.Linear on each pixel of a (B, C, H, W) map (conv_type "linear").  GRL's forwards
+    run it through last_conv (fp32) and tc.last_conv (tensor cores), which list its launch; this forward is for calling
+    the module on its own, like the reference's, and launches K.linear directly."""
+
+    @torch.no_grad()
+    def forward(self, x):
+        B, C, H, W = x.shape
+        y = torch.empty(B, H, W, self.weight.shape[0], device=x.device, dtype=torch.float32)
+        K.linear(x.permute(0, 2, 3, 1).contiguous(), self.weight, self.bias, out=y)
+        return y.permute(0, 3, 1, 2)
+
+
+CONV_TYPES = ("1conv", "3conv", "1conv1x1", "linear")
+
+
 def build_last_conv(conv_type, dim):
-    """swin_v1_block.py:469-485 ('1conv' is what every GRL config uses)."""
-    if conv_type != "1conv":
-        raise NotImplementedError(f"conv_type={conv_type!r}: only '1conv' is on the hot path")
-    return nn.Conv2d(dim, dim, 3, 1, 1)
+    """swin_v1_block.py:469-485: each stage's `conv` and the network's `conv_after_body`."""
+    if conv_type == "1conv":
+        return nn.Conv2d(dim, dim, 3, 1, 1)
+    if conv_type == "3conv":
+        return nn.Sequential(nn.Conv2d(dim, dim // 4, 3, 1, 1), nn.LeakyReLU(negative_slope=0.2, inplace=True),
+                             nn.Conv2d(dim // 4, dim // 4, 1, 1, 0), nn.LeakyReLU(negative_slope=0.2, inplace=True),
+                             nn.Conv2d(dim // 4, dim, 3, 1, 1))
+    if conv_type == "1conv1x1":
+        return nn.Conv2d(dim, dim, 1, 1, 0)
+    if conv_type == "linear":
+        return Linear(dim, dim)
+    raise ValueError(f"conv_type must be one of {CONV_TYPES}, got {conv_type!r}")
+
+
+def last_conv(launch, name, owner, key, x, res=None):
+    """build_last_conv's block `owner.<key>` on channels-last x (B, H, W, C) (+ res), launched as `name` ("3conv": its
+    convs as "{name}.0", ".2", ".4")."""
+    m = owner.get_submodule(key)
+    if isinstance(m, nn.Sequential):
+        t = conv3x3(launch, f"{name}.0", owner, f"{key}.0", x, K.ACT_LEAKY, m[1].negative_slope)
+        u = torch.empty(t.shape, device=x.device, dtype=torch.float32)
+        launch.listed(f"{name}.2", K.linear, t, m[2].weight.view(t.shape[-1], -1), m[2].bias, K.ACT_LEAKY,
+                      m[3].negative_slope, out=u)
+        return conv3x3(launch, f"{name}.4", owner, f"{key}.4", u, res=res)
+    if m.weight.dim() == 4 and m.weight.shape[2] == 3:
+        return conv3x3(launch, name, owner, key, x, res=res)
+    y = torch.empty(*x.shape[:-1], m.weight.shape[0], device=x.device, dtype=torch.float32)
+    launch.listed(name, K.linear, x, m.weight.view(m.weight.shape[0], -1), m.bias, K.ACT_NONE, res=res, out=y)
+    return y
 
 
 class Upsample(nn.Module):
@@ -553,12 +714,15 @@ class TransformerStage(nn.Module):
             res = blk(res, x_size, table_index_mask, launch, f"{name}.block{bi}")
         B, L, C = x.shape
         H, W = x_size
-        return conv3x3(launch, f"{name}.conv", self, "conv", res.view(B, H, W, C), res=x.view(B, H, W, C)).view(B, L, C)
+        return last_conv(launch, f"{name}.conv", self, "conv", res.view(B, H, W, C), res=x.view(B, H, W, C)).view(B, L, C)
 
 
 class GRL(nn.Module):
     """models/networks/grl.py:176-569.  Same constructor kwargs (plus **kwargs swallowing the extra yaml keys),
-    parameter names and call contract as the reference network."""
+    parameter names and call contract as the reference network.  anchor_proj_type ("avgpool", "maxpool", "conv2d",
+    "patchmerging") with anchor_one_stage, and conv_type ("1conv", "3conv", "1conv1x1", "linear") take every value the
+    reference can run; the combinations it cannot run raise ValueError (anchor_projection_error).  out_proj_type is
+    accepted and ignored, as in the reference (its output projection is always nn.Linear)."""
 
     def __init__(self, img_size=64, in_channels=3, out_channels=None, embed_dim=96, upscale=2, img_range=1.0,
                  upsampler="", depths=[6, 6, 6, 6, 6, 6], num_heads_window=[3, 3, 3, 3, 3, 3],
@@ -604,12 +768,11 @@ class GRL(nn.Module):
         self.stripe_size, self.stripe_groups = stripe_size, stripe_groups
         self.pretrained_window_size, self.pretrained_stripe_size = pretrained_window_size, pretrained_stripe_size
         self.anchor_window_down_factor = anchor_window_down_factor
-        if out_proj_type != "linear":
-            raise NotImplementedError("only out_proj_type='linear' is on the hot path")
         if any(int(v) != 0 for v in list(pretrained_window_size) + list(pretrained_stripe_size)):
             # ops.get_relative_coords_table_all divides by the pretrained size when it is > 0 (ops.py:225-271); no released
             # config sets it, and the closed-form tables here always normalise by the current size
-            raise NotImplementedError("pretrained_window_size / pretrained_stripe_size != 0 are not on the hot path")
+            raise NotImplementedError("pretrained_window_size / pretrained_stripe_size != 0 rescale the coordinate "
+                                      "tables, which the kernels compute in closed form for the current size only")
 
         self.conv_first = nn.Conv2d(in_channels, embed_dim, 3, 1, 1)
         self.norm_start = norm_layer(embed_dim)
@@ -962,8 +1125,8 @@ class GRL(nn.Module):
             return conv3x3(launch, name, self, key or name, inp, act, slope, res)
 
         first = conv("conv_first", xc)
-        body = conv("conv_after_body", self.forward_features(first.permute(0, 3, 1, 2), launch).permute(0, 2, 3, 1),
-                    res=first)
+        body = last_conv(launch, "conv_after_body", self, "conv_after_body",
+                         self.forward_features(first.permute(0, 3, 1, 2), launch).permute(0, 2, 3, 1), res=first)
         if self.upsampler == "pixelshuffle":
             t = conv("conv_before_upsample", body, K.ACT_LEAKY, 0.01, key="conv_before_upsample.0")
             y = conv("conv_last", self.upsample.forward_cl(t, launch))

@@ -117,8 +117,9 @@ def _pad_matrix(w, npad, kpad, row_map=None, col_map=None, fmt=0):
     return out.to(DTYPE[fmt]).contiguous()
 
 
-def _pad_vector(b, npad, row_map=None):
-    out = torch.zeros(npad, device=b.device, dtype=torch.float32)
+def _pad_vector(b, npad, row_map=None, device=None):
+    """fp32 (N) -> (npad) with dest row_map[i] <- b[i]; b None (no bias): zeros on `device`."""
+    out = torch.zeros(npad, device=b.device if b is not None else device, dtype=torch.float32)
     if b is not None:
         out[torch.arange(b.numel(), device=b.device) if row_map is None else row_map] = b.detach().float()
     return out
@@ -365,6 +366,12 @@ def avgpool16(x16, out, df):
     capi.check(capi.lib().grl_tc_avgpool16(capi.ptr(x16), capi.ptr(out), B, H, W, cpad, df, fmt_of(x16), capi.stream()))
 
 
+def maxpool16(x16, out, df):
+    """Anchor pooling: the df x df max of 16-bit (B, H, W, cpad) into 16-bit (B, H / df, W / df, cpad) `out`."""
+    B, H, W, cpad = x16.shape
+    capi.check(capi.lib().grl_tc_maxpool16(capi.ptr(x16), capi.ptr(out), B, H, W, cpad, df, fmt_of(x16), capi.stream()))
+
+
 def channel_gate(y16, ld, B, L, C, ca, gate):
     """CAB gate (B, C) fp32 into `gate` from the 16-bit features y16 (B*L, ld); ca: the packed ChannelAttention weights."""
     lib = capi.lib()
@@ -416,14 +423,28 @@ class BlockPlan:
             if on:
                 base = (0 if half == 0 else 3 * hw) + 2 * hh
                 self.b_qkv.view(-1, SLOT)[base:base + hh, SLOT - 1].fill_(1.0)  # fill_: a scalar store would sync
-        # --- anchor projection: dest row = head*32 + e
+        # --- anchor projection: its stages (AnchorProjection.body), each a pooling or a patch gather (K.anchor_gather:
+        # K = taps * C padded to 64) in front of one GEMM.  The last writes the anchors at row head*32 + e (EPI_QKV);
+        # the others write their C/2 channels at a 64-padded pitch (bias epilogue, PatchMerging's bias is zero).
         amap = _slot_rows(0, hs, ds, dev)
-        red = at.anchor.body[0].reduction
         self.n_anc = hs * SLOT
-        self.w_anc = _pad_matrix(red.weight, round_up(self.n_anc, 32), self.cpad, row_map=amap, fmt=fmt)
-        self.b_anc = _pad_vector(red.bias, round_up(self.n_anc, 32), amap)
-        self.anc_scale = torch.ones(hs, device=red.weight.device, dtype=torch.float32)
-        self.df = at.anchor.body[0].down_factor
+        self.anc_scale = torch.ones(hs, device=dev, dtype=torch.float32)
+        self.anc_stages = []
+        cin = C
+        body = list(at.anchor.body)
+        for i, m in enumerate(body):
+            last = i == len(body) - 1
+            if hasattr(m, "pooling_mode"):  # AnchorLinear: kind "avgpool" / "maxpool", geo = the pooling window df
+                kind, w, b, geo, kpad = m.pooling_mode, m.reduction.weight, m.reduction.bias, m.down_factor, self.cpad
+            else:  # AnchorConv2d / PatchMerging: kind "gather", geo = its modules.AnchorGather
+                kind, (w, b), geo = "gather", m.packed(), m.gather
+                kpad = round_up(geo.ksize ** 2 * cin, 64)
+            npad = round_up(self.n_anc, 32) if last else round_up(C // 2, 64)
+            rmap = amap if last else None
+            self.anc_stages.append((kind, geo, _pad_matrix(w, npad, kpad, row_map=rmap, fmt=fmt), _pad_vector(b, npad, rmap, dev),
+                                    cin, kpad, npad))
+            cin = C // 2
+        self.w_anc, self.b_anc = self.anc_stages[-1][2:4]  # the projection that writes the anchors
         # --- output projection: K index = slot*32 + e over [window heads | stripe heads]
         cmap = torch.cat([_slot_rows(0, hw, dw, dev), _slot_rows(hw, hs, ds, dev)])
         self.k_proj = round_up((hw + hs) * SLOT, 64)
@@ -487,14 +508,26 @@ class BlockPlan:
         qkv = _h16(B * L, self.n_qkv, device=dev, fmt=fmt)
         launch.listed(f"{name}.qkv", gemm, x16, self.w_qkv, self.b_qkv, M=B * L, kpad=cpad, npad=self.n_qkv,
                       epi=EPI_QKV, n_store=self.n_qkv, out_bf16=qkv, slot_scale=scales)
-        df = self.df
-        pooled = _h16(B, H // df, W // df, cpad, device=dev, fmt=fmt)
-        launch.run(avgpool16, x16.view(B, H, W, cpad), pooled, df)
-        La = (H // df) * (W // df)
-        n_anc = self.w_anc.shape[0]
-        anchor = _h16(B * La, n_anc, device=dev, fmt=fmt)
-        launch.listed(f"{name}.anchor", gemm, pooled, self.w_anc, self.b_anc, M=B * La, kpad=cpad, npad=n_anc,
-                      epi=EPI_QKV, n_store=n_anc, out_bf16=anchor, slot_scale=self.anc_scale)
+        a16, (h, w) = x16.view(B, H, W, cpad), (H, W)
+        for i, (kind, geo, w_a, b_a, cin, kpad, npad) in enumerate(self.anc_stages):
+            last = i == len(self.anc_stages) - 1
+            if kind != "gather":
+                h, w = h // geo, w // geo
+                rows = _h16(B, h, w, cpad, device=dev, fmt=fmt)
+                launch.run(avgpool16 if kind == "avgpool" else maxpool16, a16, rows, geo)
+            else:
+                h, w = K.gather_size(h, w, geo.ksize, geo.stride, geo.pad)
+                rows = _h16(B * h * w, kpad, device=dev, fmt=fmt)
+                launch.run(K.anchor_gather, a16, cin, *geo, kpad, out=rows)
+            out = _h16(B * h * w, npad, device=dev, fmt=fmt)
+            if last:
+                launch.listed(f"{name}.anchor", gemm, rows, w_a, b_a, M=B * h * w, kpad=kpad, npad=npad, epi=EPI_QKV,
+                              n_store=npad, out_bf16=out, slot_scale=self.anc_scale)
+            else:
+                launch.listed(f"{name}.anchor.{i}", gemm, rows, w_a, b_a, M=B * h * w, kpad=kpad, npad=npad,
+                              epi=EPI_BIAS_ACT, n_store=npad, out_bf16=out)
+            a16 = out.view(B, h, w, npad)
+        anchor = out
         # attention
         merged = _h16(B * L, self.k_proj, device=dev, fmt=fmt, zero=self.k_proj != (hw + hs) * SLOT)
         launches = attention_launches(blk, x_size)
@@ -547,14 +580,20 @@ def block_plan(blk, fmt):
 
 
 class ConvPlan:
-    """One packed 3x3 conv (stage conv / head convs)."""
+    """One packed 3x3 conv (stage conv / head convs), or a 1x1 conv / per-pixel nn.Linear (stage conv types "1conv1x1",
+    "linear" and the middle conv of "3conv": one GEMM over the pixels)."""
 
     def __init__(self, conv, cin_pad, fmt, ps_r=0):
         self.key = (_version_key(conv), fmt, ps_r)
         self.cout = conv.weight.shape[0]
         self.cin_pad, self.ps_r = cin_pad, ps_r
         self.npad = round_up(self.cout, 64)
-        self.w, self.b = pack_conv(conv, cin_pad, self.npad, fmt, ps_r)
+        self.taps = 9 if conv.weight.dim() == 4 and conv.weight.shape[2] == 3 else 1
+        if self.taps == 9:
+            self.w, self.b = pack_conv(conv, cin_pad, self.npad, fmt, ps_r)
+        else:
+            self.w = _pad_matrix(conv.weight.reshape(self.cout, -1), self.npad, cin_pad, fmt=fmt)
+            self.b = _pad_vector(conv.bias, self.npad)
         self.ready = Produced((self.w, self.b))
 
     def run(self, launch, name, x16, *, want16=True, want_f32=False, rows=False, **kw):
@@ -571,8 +610,12 @@ class ConvPlan:
             o16 = torch.empty(*px, self.npad, device=dev, dtype=self.w.dtype)
         if want_f32:
             o32 = torch.empty(*px, self.cout, device=dev, dtype=torch.float32)
-        conv3x3(x16, self.w, self.b, self.cin_pad, self.npad, n_store=self.cout if r else self.npad, n_real=self.cout,
-                out_bf16=o16, out_f32=o32, ps_r=r, launch=launch, name=name, **kw)
+        if self.taps == 1:
+            launch.listed(name, gemm, x16, self.w, self.b, M=B * H * W, kpad=self.cin_pad, npad=self.npad,
+                          epi=EPI_BIAS_ACT, n_store=self.npad, n_real=self.cout, out_bf16=o16, out_f32=o32, **kw)
+        else:
+            conv3x3(x16, self.w, self.b, self.cin_pad, self.npad, n_store=self.cout if r else self.npad,
+                    n_real=self.cout, out_bf16=o16, out_f32=o32, ps_r=r, launch=launch, name=name, **kw)
         return o16, o32
 
 
@@ -584,6 +627,20 @@ def conv_plan(owner, name, conv, cin_pad, fmt, ps_r=0):
         cache[name] = plan
     plan.ready.use()
     return plan
+
+
+def last_conv(owner, key, x16, fmt, launch, name, **kw):
+    """build_last_conv's block `owner.<key>` on x16 (B, H, W, cin_pad), as ConvPlan.run (kw: its outputs and the
+    residual).  "3conv" runs conv3x3 + LeakyReLU, conv1x1 + LeakyReLU (launched as "{name}.0", ".2") at the 64-padded
+    C/4 width, then the last conv with kw as "{name}.4"."""
+    m = owner.get_submodule(key)
+    if isinstance(m, nn.Sequential):
+        t, _ = conv_plan(owner, f"{key}.0", m[0], x16.shape[-1], fmt).run(launch, f"{name}.0", x16, act=K.ACT_LEAKY,
+                                                                          slope=m[1].negative_slope)
+        t, _ = conv_plan(owner, f"{key}.2", m[2], t.shape[-1], fmt).run(launch, f"{name}.2", t, act=K.ACT_LEAKY,
+                                                                        slope=m[3].negative_slope)
+        return conv_plan(owner, f"{key}.4", m[4], t.shape[-1], fmt).run(launch, f"{name}.4", t, **kw)
+    return conv_plan(owner, key, m, x16.shape[-1], fmt).run(launch, name, x16, **kw)
 
 
 @torch.no_grad()
@@ -601,8 +658,8 @@ def stage_forward(stage, x32, x16, x_size, table_index_mask, launch=DEVICE, name
     if r16 is None or r16.dtype != DTYPE[fmt]:
         r16 = _h16(B, L, cpad, device=x32.device, fmt=fmt)
         launch.run(pack_rows, r32.contiguous(), cpad, fmt, out=r16)
-    o16, o32 = conv_plan(stage, "conv", stage.conv, cpad, fmt).run(launch, f"{name}.conv", r16.view(B, H, W, cpad),
-                                                                   want_f32=True, rows=True, res_f32=x32.contiguous())
+    o16, o32 = last_conv(stage, "conv", r16.view(B, H, W, cpad), fmt, launch, f"{name}.conv", want_f32=True, rows=True,
+                         res_f32=x32.contiguous())
     return o32, o16
 
 
@@ -651,7 +708,7 @@ def forward(model, x, rggb=False, launch=DEVICE):
     t = ln(model.norm_end, t)
     t16 = _h16(B, Hp, Wp, cpad, device=dev, fmt=fmt)
     launch.run(pack_rows, t, cpad, fmt, out=t16)
-    body16, _ = conv("conv_after_body", model.conv_after_body, t16, res_f32=f32)
+    body16, _ = last_conv(model, "conv_after_body", t16, fmt, launch, "conv_after_body", res_f32=f32)
     if model.upsampler == "pixelshuffle":
         u16, _ = conv("conv_before_upsample", model.conv_before_upsample[0], body16, act=K.ACT_LEAKY, slope=0.01)
         mods = list(model.upsample.up)

@@ -98,6 +98,15 @@ int grl_conv3x3_f32(const float* x, const float* w, const float* b, const float*
 
 /* AvgPool2d(df, df) on channels-last data (AnchorLinear.pooling, mixed_attn_block.py:725,:733). */
 int grl_avgpool_f32(const float* x, float* y, int B, int H, int W, int C, int df, void* stream);
+/* MaxPool2d(df, df) on channels-last data (AnchorLinear.pooling with pooling_mode "maxpool", mixed_attn_block.py:724). */
+int grl_maxpool_f32(const float* x, float* y, int B, int H, int W, int C, int df, void* stream);
+/* Patch rows of a channels-last image x (B, H, W, C) at row pitch ldx, for the convolutional anchor projections
+ * (nn.Conv2d(C, C/2, k, stride, pad) and PatchMerging, mixed_attn_block.py:679-711,:745-770; the reference runs them with
+ * torch's conv2d / cat + Linear): y (B*Ho*Wo, ldy), Ho = (H + 2 pad - k) / stride + 1,
+ * y[(b,yo,xo), tap*C + c] = x[b, yo*stride - pad + ky, xo*stride - pad + kx, c] (0 outside), 0 for k*k*C <= col < ldy;
+ * tap = ky*k + kx when row_major (nn.Conv2d's weight order), kx*k + ky otherwise (PatchMerging's x0..x3 order). */
+int grl_anchor_gather_f32(const float* x, int64_t ldx, int B, int H, int W, int C, int ksize, int stride, int pad,
+                          int row_major, float* y, int ldy, void* stream);
 
 /* out = (x ? x : 0) + res_scale * LayerNorm(u; gamma, beta, eps) (+ cab_y * cab_gate[b, c])
  * (post-norm residual, mixed_attn_block_efficient.py:543-554; norm_start/norm_end grl.py:494,:501 with x = NULL).
@@ -164,6 +173,12 @@ int grl_tc_head_pack_rggb(const float* cfa4, int B, int h, int w, int Hp, int Wp
                           int Cpad, float* y32, int fmt, void* stream);
 /* AvgPool2d(df) on 16-bit channels-last data (AnchorLinear.pooling, mixed_attn_block.py:725). */
 int grl_tc_avgpool16(const void* x16, void* y16, int B, int H, int W, int Cpad, int df, int fmt, void* stream);
+/* MaxPool2d(df) on 16-bit channels-last data (AnchorLinear.pooling with pooling_mode "maxpool", mixed_attn_block.py:724). */
+int grl_tc_maxpool16(const void* x16, void* y16, int B, int H, int W, int Cpad, int df, int fmt, void* stream);
+/* grl_anchor_gather_f32 on 16-bit operands (either format: the values are copied): the K operand of the anchor
+ * projection's grl_tc_gemm, ldy a multiple of 64. */
+int grl_tc_anchor_gather16(const void* x16, int64_t ldx, int B, int H, int W, int C, int ksize, int stride, int pad,
+                           int row_major, void* y16, int ldy, void* stream);
 /* Per-slot multipliers of the packed qkv layout [win q|k|v][stripe q|k|v] x heads: exp(min(logit_scale, ln100))*log2(e)
  * on window q, stripe q (attn_transform2) and stripe k (attn_transform1); 1 on the other q/k slots; 0 on v slots
  * (mixed_attn_block_efficient.py:39). out: (3*hw + 3*hs) floats. */
